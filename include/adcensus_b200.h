@@ -261,6 +261,18 @@ int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR
 		       const float *imgL, const float *imgR, float *disp,
 		       float *volL, float *volR, adcensus_stream_t stream);
 
+/* Run at (H, W, D) with H <= the created H, W <= the created W, D <= the created D; C and params as created, so that
+ * one pipeline created at the largest shape of a dataset serves every image of it (KITTI widths, Middlebury sizes and
+ * disparity ranges) without allocating.  featL/featR (C,H,W), imgL/imgR (H,W), disp (H,W), volL/volR (D,H,W) or NULL,
+ * all contiguous at the RUN shape.  Same results, bit for bit, as mccnn_pipeline_run on a pipeline created at (C, D, H, W)
+ * with the same params, CBCA mode, SGM layout and overlap mode.  ADCENSUS_ELIMIT if the shape exceeds the created one,
+ * ADCENSUS_EINVAL for H, W or D < 1 or border + 1 > W; nothing is launched then.  Asynchronous on `stream`.
+ * The batch, host and twin-lane entry points (mccnn_pipeline_run_batch / _run_host / _run_host_batch) always run at the
+ * created shape. */
+int mccnn_pipeline_run_shape(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+			     const float *imgL, const float *imgR, float *disp, float *volL, float *volR,
+			     adcensus_stream_t stream);
+
 /* Host-buffer call (what a non-CUDA caller binds): copies inputs H2D, runs,
  * copies disp back, and returns after the result is in disp_host. */
 int mccnn_pipeline_run_host(mccnn_pipeline *p, const float *featL_host, const float *featR_host,

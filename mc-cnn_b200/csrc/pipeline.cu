@@ -76,7 +76,9 @@ struct mccnn_pipeline {
 	// tensor map of the left volume for StereoJoin's TMA store (box {128, 1, disparity chunk})
 	int sj_tm_ok;
 	CUtensorMap sj_tm;
-	// tensor maps of the volume buffers (inputs of the TMA-staged CBCA)
+	// tensor maps of the volume buffers (inputs of the TMA-staged CBCA), all encoded for the run shape
+	// (tm_D, tm_H, tm_W); a run at another shape re-encodes them first (encode_maps), 0 = none valid
+	int tm_D, tm_H, tm_W;
 	int ntm;
 	const float *tm_ptr[6];
 	CUtensorMap tm[6];
@@ -115,17 +117,45 @@ int dev_alloc(void **p, size_t bytes, size_t *acc)
 // longest arm cross() can produce for this preset, and the CBCA support radius
 int pipe_maxlen(const mccnn_pipeline *p) { return p->prm.L1 > 2 ? p->prm.L1 : 2; }
 
+// a map of `buf` as a (tm_D, tm_H, tm_W) volume with rows of tm_W rounded up to 4 floats
 int add_tensor_map(mccnn_pipeline *p, const float *buf)
 {
 	const int halo = pipe_maxlen(p) - 1;
 	if (halo > adc_cbca_tma_max_halo()) return 0;      // such presets run the exact kernels
+	if (!p->tm_D) return 0;                            // no valid shape: the next run encodes every map
 	if (p->ntm >= 6) return ADCENSUS_EINVAL;
 	int bw, bh;
 	adc_cbca_tma_box(halo, &bw, &bh);
-	int rc = adc_tma_encode_volume(&p->tm[p->ntm], buf, p->D, p->H, p->W, p->ld, bw, bh);
+	int rc = adc_tma_encode_volume(&p->tm[p->ntm], buf, p->tm_D, p->tm_H, p->tm_W, (p->tm_W + 3) & ~3, bw, bh);
 	if (rc) return rc;
 	p->tm_ptr[p->ntm++] = buf;
 	return 0;
+}
+
+// (Re-)encode every tensor map for volumes of shape (D, H, W): StereoJoin's store map of the left volume and the CBCA
+// input maps of both volumes (the right one starts D*H*ld floats into `vols`), the ping-pong / accumulator buffers and,
+// in overlap mode, the side stream's.  Kernels already launched are unaffected: each one received its map by value
+// (__grid_constant__) at launch.
+int encode_maps(mccnn_pipeline *p, int D, int H, int W)
+{
+	const int ld = (W + 3) & ~3;
+	const long V = (long)D * H * ld;
+	p->ntm = 0;
+	p->tm_D = D; p->tm_H = H; p->tm_W = W;
+	const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)D};
+	const uint64_t strides[2] = {(uint64_t)ld * 4, (uint64_t)ld * 4 * (uint64_t)H};
+	const uint32_t box[3] = {128u, 1u, (uint32_t)adc_stereo_join_dc(D)};
+	p->sj_tm_ok = adc_tma_encode(&p->sj_tm, p->vols, 3, dims, strides, box) == 0;
+	int rc = 0;
+	for (const float *b : {(const float *)p->vols, (const float *)(p->vols + V), (const float *)p->bufA, (const float *)p->bufC,
+			       (const float *)p->bufA2, (const float *)p->bufC2})
+		if (!rc && b) rc = add_tensor_map(p, b);
+	if (rc) {                                          // leave nothing half-encoded behind
+		p->ntm = 0;
+		p->tm_D = p->tm_H = p->tm_W = 0;
+		p->sj_tm_ok = 0;
+	}
+	return rc;
 }
 
 const CUtensorMap *find_tensor_map(const mccnn_pipeline *p, const float *buf)
@@ -176,16 +206,7 @@ extern "C" int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, 
 	if (!rc) rc = (int)cudaMemset(p->maxlen, 0, sizeof(int));
 	if (!rc) rc = dev_alloc((void **)&p->maps, 8 * p->HW * f, &p->bytes);
 	if (!rc) rc = dev_alloc((void **)&p->sgmtab, p->tab_bytes, &p->bytes);
-	if (!rc) {
-		const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)D};
-		const uint64_t strides[2] = {(uint64_t)p->ld * 4, (uint64_t)p->ld * 4 * (uint64_t)H};
-		const uint32_t box[3] = {128u, 1u, (uint32_t)adc_stereo_join_dc(D)};
-		p->sj_tm_ok = adc_tma_encode(&p->sj_tm, p->vols, 3, dims, strides, box) == 0;
-	}
-	if (!rc) rc = add_tensor_map(p, p->vols);
-	if (!rc) rc = add_tensor_map(p, p->vols + p->V);
-	if (!rc) rc = add_tensor_map(p, p->bufA);
-	if (!rc) rc = add_tensor_map(p, p->bufC);
+	if (!rc) rc = encode_maps(p, D, H, W);
 	p->ks = mccnn_gaussian(params->blur_sigma, nullptr);
 	if (!rc) rc = dev_alloc((void **)&p->gauss, (size_t)p->ks * p->ks * f, &p->bytes);
 	if (!rc) {
@@ -311,17 +332,22 @@ extern "C" int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p) { return
 		if (rc__) return rc__; \
 	} while (0)
 
-extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR,
-				  const float *imgL, const float *imgR, float *disp,
-				  float *volL, float *volR, adcensus_stream_t stream)
+// One run at (H, W, D) <= the created shape: every shape-dependent quantity (row pitch, volume size, the offset of the
+// right volume, map offsets, table sizes, tensor maps) is derived here from the run shape, so the buffers hold exactly
+// what a pipeline created at this shape would hold.
+static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+			   const float *imgL, const float *imgR, float *disp, float *volL, float *volR, cudaStream_t s)
 {
-	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
-	DeviceGuard g(p->device);
-	cudaStream_t s = adc_stream(stream);
-	const int C = p->C, D = p->D, H = p->H, W = p->W, ld = p->ld;
-	const long HW = p->HW, V = p->V;
+	const int C = p->C, ld = (W + 3) & ~3;
+	const long HW = (long)H * W, V = (long)D * H * ld;
 	const mccnn_params &o = p->prm;
 	int nl = 0;
+	// the allocations were sized for the created shape; check the run's needs against them instead of assuming
+	if (V > p->V || HW > p->HW) return ADCENSUS_ELIMIT;
+	if (adc_packed_words(H, W) + adc_packed_hv_words(H, W) > adc_packed_words(p->H, p->W) + adc_packed_hv_words(p->H, p->W))
+		return ADCENSUS_ELIMIT;
+	if (adc_sgm_table_bytes(H, W, D) > p->tab_bytes || adc_sgm_dhw_table_bytes(H, W, D) > p->tab_bytes) return ADCENSUS_ELIMIT;
+	if (p->tm_D != D || p->tm_H != H || p->tm_W != W) STEP(encode_maps(p, D, H, W));
 
 	float *volsL = p->vols, *volsR = p->vols + V;
 	// main.lua:946 (only what :947 leaves); on the fast path StereoJoin's TMA store fills the left volume's invalid entries itself
@@ -446,6 +472,26 @@ extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const f
 	STEP(adcensus_mean2d(m + 6 * HW, p->gauss, disp, H, W, p->ks, o.blur_t, s)); nl += 3;        // :1078
 	p->launches = nl;
 	return 0;
+}
+
+extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR,
+				  const float *imgL, const float *imgR, float *disp,
+				  float *volL, float *volR, adcensus_stream_t stream)
+{
+	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
+	DeviceGuard g(p->device);
+	return pipeline_run_at(p, p->H, p->W, p->D, featL, featR, imgL, imgR, disp, volL, volR, adc_stream(stream));
+}
+
+extern "C" int mccnn_pipeline_run_shape(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+					const float *imgL, const float *imgR, float *disp, float *volL, float *volR,
+					adcensus_stream_t stream)
+{
+	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
+	if (H < 1 || W < 1 || D < 1 || p->prm.border + 1 > W) return ADCENSUS_EINVAL;
+	if (H > p->H || W > p->W || D > p->D) return ADCENSUS_ELIMIT;
+	DeviceGuard g(p->device);
+	return pipeline_run_at(p, H, W, D, featL, featR, imgL, imgR, disp, volL, volR, adc_stream(stream));
 }
 
 static int host_staging(mccnn_pipeline *p)

@@ -76,6 +76,38 @@ def write_bin(path, t):
     np.ascontiguousarray(t, dtype="<f4").tofile(path)
 
 
+def load_net(net_fname, arch):
+    """``torch.load(opt.net_fname, 'ascii')`` (main.lua:893-901) on the host: the :class:`t7.Net` of `net_fname`, which must
+    hold a network of architecture `arch` ('fast' or 'slow')."""
+    from . import t7
+
+    net = t7.load_net(net_fname)
+    if net.arch != arch:
+        raise ValueError("%s holds a '%s' network, arch '%s' was asked for" % (net_fname, net.arch, arch))
+    return net
+
+
+def net_border(net):
+    """fix_border's width for a network (main.lua:382-391, 923): (window - 1) / 2 = the sum of (kW - 1) / 2 over the
+    tower's convolutions (4 for the published 4-layer 3x3 KITTI towers, 5 for Middlebury's 5 layers)."""
+    return sum((w.shape[3] - 1) // 2 for w, _ in net.tower)
+
+
+def make_stages(net, device):
+    """The GPU stages of a loaded network on `device` (a torch.device or index): (FeatureTower, ScorerHead or None) --
+    net_te, and for 'slow' net_te2 (main.lua:894-900)."""
+    import torch
+
+    from .feature_tower import FeatureTower
+    from .scorer_head import ScorerHead
+
+    dev = torch.device("cuda", device) if isinstance(device, int) else device
+    with torch.cuda.device(dev):
+        tower = FeatureTower(net.tower, arch=net.arch, device=dev.index)
+        head = ScorerHead(net.head, device=dev.index) if net.arch == "slow" else None
+    return tower, head
+
+
 def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=None, out_dir=None, device=0,
             net_fname=None, **overrides):
     """``main.lua <dataset> <arch> -a predict -net_fname N -left L -right R -disp_max D`` from the image files on:
@@ -92,11 +124,7 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     if arch in ("fast", "slow") and features is None:                          # decided before any GPU work
         if net_fname is None:
             raise ValueError("arch '%s' needs -net_fname (or, for 'fast', the tower output in `features`)" % arch)
-        from . import t7
-
-        net = t7.load_net(net_fname)                                            # main.lua:893-901
-        if net.arch != arch:
-            raise ValueError("%s holds a '%s' network, arch '%s' was asked for" % (net_fname, net.arch, arch))
+        net = load_net(net_fname, arch)                                         # main.lua:893-901
     elif arch == "slow":
         raise ValueError("arch 'slow' needs -net_fname: the scorer head's weights come with the tower's")
     elif arch not in ("fast", "ad", "census"):
@@ -107,13 +135,9 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     x_batch = torch.from_numpy(batch).to(dev)
     feats = head = None
     if net is not None:
-        from .feature_tower import FeatureTower
-        from .scorer_head import ScorerHead
-
+        tower, head = make_stages(net, dev)
         with torch.cuda.device(dev):
-            feats = FeatureTower(net.tower, arch=arch, device=dev.index).forward(x_batch)      # main.lua:944 / :957
-            if arch == "slow":
-                head = ScorerHead(net.head, device=dev.index)                                  # net_te2, main.lua:896
+            feats = tower.forward(x_batch)                                      # main.lua:944 / :957
     elif arch == "fast":
         feats = torch.as_tensor(features, dtype=torch.float32).to(dev).contiguous()
     opt = pipeline.make_params(dataset, arch, **overrides)

@@ -162,7 +162,8 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
 
 
 class StereoPipeline:
-    """Native fused stereo_predict (mccnn_pipeline_*): buffers allocated once per (C,D,H,W)."""
+    """Native fused stereo_predict (mccnn_pipeline_*): buffers allocated once per (C,D,H,W); :meth:`run` runs at that
+    shape, :meth:`run_shape` at any (H, W, D) that fits inside it."""
 
     def __init__(self, C, D, H, W, params, device=0, cbca_mode=None):
         """``cbca_mode``: "fast" (library default) = constant-work aggregation inside the north star's 1e-4 contract
@@ -228,6 +229,32 @@ class StereoPipeline:
                                                    adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
                                                    adcensus._t(disp, 5, n), vp(volL), vp(volR),
                                                    adcensus._stream(featL))
+        adcensus._check(rc, n)
+        return disp
+
+    def run_shape(self, featL, featR, imgL, imgR, disp_max=None, disp=None, volL=None, volR=None):
+        """:meth:`run` at a smaller shape than the created one (mccnn_pipeline_run_shape): H, W from ``imgL``, D =
+        ``disp_max`` (default: the created D); every tensor must be contiguous at that shape.  Same results, bit for bit,
+        as a pipeline created at this shape, without allocating: one pipeline created at the largest (H, W, D) of a dataset
+        serves all of its images.  Asynchronous on torch's current stream."""
+        n = "mccnn_pipeline_run_shape"
+        if imgL.dim() != 2:
+            raise adcensus.AdcensusError("%s: imgL must be (H, W), got %s" % (n, tuple(imgL.shape)))
+        H, W = imgL.shape
+        D = self.D if disp_max is None else int(disp_max)
+        if disp is None:
+            disp = torch.empty((H, W), device=imgL.device, dtype=torch.float32)
+        want = [("featL", featL, (self.C, H, W)), ("featR", featR, (self.C, H, W)), ("imgR", imgR, (H, W)),
+                ("disp", disp, (H, W)), ("volL", volL, (D, H, W)), ("volR", volR, (D, H, W))]
+        for name, t, shape in want:
+            if t is not None and tuple(t.shape) != shape:
+                raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
+        vp = lambda t, i: adcensus._t(t, i, n) if t is not None else ctypes.c_void_p(0)
+        with torch.cuda.device(imgL.device):
+            rc = adcensus.lib().mccnn_pipeline_run_shape(self._h, H, W, D, adcensus._t(featL, 1, n), adcensus._t(featR, 2, n),
+                                                         adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
+                                                         adcensus._t(disp, 5, n), vp(volL, 6), vp(volR, 7),
+                                                         adcensus._stream(imgL))
         adcensus._check(rc, n)
         return disp
 

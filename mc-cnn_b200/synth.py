@@ -68,3 +68,86 @@ def make_pair(H, W, C, D, seed=0, noise=0.1, block=(16, 48)):
 
     return dict(featL=unit(featL), featR=unit(featR), imgL=standardise(imgL), imgR=standardise(imgR),
                 gt=gt.astype(np.float32))
+
+
+def _standardise(x):
+    return ((x - x.mean()) / x.std(ddof=1)).astype(np.float32)
+
+
+def _scene_views(rng, H, W, D, n_views=2):
+    """(views (n_views, H, W), gt (H, W)): standardised grey views of one natural scene, view 0 the left image, every other
+    view the right image (views 2, 3 ... with their own brightness and noise, like Middlebury's extra exposures / lights).
+    Left pixel x matches right pixel x - gt; gt is piecewise constant in [1, D) and 0 (invalid) on about 10% of the pixels."""
+    dmax = max(2, min(D, W // 3))
+    gy, gx = (H + 15) // 16, (W + 47) // 48
+    gt = np.kron(rng.integers(1, dmax, size=(gy, gx)), np.ones((16, 48), np.int64))[:H, :W]
+    ext = W + D
+    scene = natural_image(rng, H, ext)
+    cols = np.arange(W)[None, :] + D
+    rows = np.arange(H)[:, None]
+    views = [_standardise(scene[rows, cols - gt] + 0.004 * rng.standard_normal((H, W), dtype=np.float32))]
+    for k in range(1, n_views):
+        gain = 1.0 if k == 1 else 0.7 + 0.2 * k
+        views.append(_standardise(gain * scene[:, D:D + W] + 0.004 * k * rng.standard_normal((H, W), dtype=np.float32)))
+    gt = gt.astype(np.float32)
+    gt[rng.random((H, W)) < 0.1] = 0
+    return np.stack(views), gt
+
+
+def write_kitti_set(root, dataset="kitti", n_tr=4, n_te=2, H=48, width=130, widths=(130, 117), seed=0):
+    """A small seeded KITTI set in preprocess_kitti.lua's layout under ``root/data.kitti`` (or ``data.kitti2015``):
+    x0.bin, x1.bin (n, 1, H, width) with row i's first widths[i % len(widths)] columns filled, dispnoc.bin (n_tr, 1, H, width),
+    metadata.bin (n, 3) int32 (img_height = H + 25, img_width, id), tr.bin / te.bin (1-based int64 split of the training
+    rows, te first).  Returns the directory."""
+    from . import dataio
+    import os
+
+    rng = np.random.default_rng(seed)
+    d = os.path.join(root, "data.kitti" if dataset == "kitti" else "data.kitti2015")
+    os.makedirs(d, exist_ok=True)
+    n = n_tr + n_te
+    x0 = np.zeros((n, 1, H, width), np.float32)
+    x1 = np.zeros_like(x0)
+    dispnoc = np.zeros((n_tr, 1, H, width), np.float32)
+    meta = np.zeros((n, 3), np.int32)
+    for i in range(n):
+        w = int(widths[i % len(widths)])
+        assert 1 <= w <= width
+        views, gt = _scene_views(rng, H, w, 32)
+        x0[i, 0, :, :w], x1[i, 0, :, :w] = views
+        if i < n_tr:
+            dispnoc[i, 0, :, :w] = gt
+        meta[i] = (H + 25, w, i if i < n_tr else i - n_tr)
+    perm = rng.permutation(n_tr) + 1
+    n_val = max(1, n_tr // 3)
+    for name, x in (("x0", x0), ("x1", x1), ("dispnoc", dispnoc), ("metadata", meta),
+                    ("te", perm[:n_val].astype(np.int64)), ("tr", perm[n_val:].astype(np.int64))):
+        dataio.tofile(os.path.join(d, name + ".bin"), x)
+    return d
+
+
+def write_mb_set(root, n=6, shapes=((40, 96, 24), (48, 130, 32)), seed=0, rect="imperfect", color="gray"):
+    """A small seeded Middlebury set in preprocess_mb.py's layout under ``root/data.mb.<rect>_<color>``: per image k = 1..n
+    x_<k>_1.bin (views, 1, H, W) (4 views for image 5, else 2) and dispnoc<k>.bin (H, W), meta.bin (n, 3) int32 (H, W,
+    ndisp) with (H, W, ndisp) = shapes[(k - 1) % len(shapes)], te.bin (1-based int64: images 1 .. n // 2) and
+    fname_submit.txt naming the last min(n, 30) images.  Returns the directory."""
+    from . import dataio
+    import os
+
+    assert n >= 5, "the test action reads views 3 and 4 of image 5"
+    rng = np.random.default_rng(seed)
+    d = os.path.join(root, "data.mb.%s_%s" % (rect, color))
+    os.makedirs(d, exist_ok=True)
+    meta = np.zeros((n, 3), np.int32)
+    for k in range(1, n + 1):
+        H, W, ndisp = shapes[(k - 1) % len(shapes)]
+        views, gt = _scene_views(rng, H, W, ndisp, n_views=4 if k == 5 else 2)
+        dataio.tofile(os.path.join(d, "x_%d_1.bin" % k), np.ascontiguousarray(views[:, None]))
+        dataio.tofile(os.path.join(d, "dispnoc%d.bin" % k), gt)
+        meta[k - 1] = (H, W, ndisp)
+    dataio.tofile(os.path.join(d, "meta.bin"), meta)
+    dataio.tofile(os.path.join(d, "te.bin"), np.arange(1, n // 2 + 1, dtype=np.int64))
+    n_sub = min(n, 30)
+    with open(os.path.join(d, "fname_submit.txt"), "w") as f:
+        f.write("\n".join("%s/Synth%d" % ("trainingH" if j < n_sub // 2 else "testH", j) for j in range(n_sub)))
+    return d

@@ -1,0 +1,100 @@
+"""main.lua's command line for a trained network: the non-training actions.
+
+    python tools/run_main.py kitti fast -a test_te -net_fname net/net_kitti_fast_-a_train_all.t7
+    python tools/run_main.py kitti2015 slow -a submit -net_fname N -data_root /data -out out
+    python tools/run_main.py mb census -a test_te -rect imperfect -color gray
+    python tools/run_main.py kitti fast -a time -net_fname N [-tiny]
+    python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70
+
+Option names are main.lua's (-gpu is 1-based as there); -L1 ... -blur_t override the stereo method's preset
+(main.lua:70-295).  Datasets are read relative to -data_root (default: the working directory), as main.lua reads them
+relative to its own.  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
+what each action computes and where it deliberately differs from main.lua.
+"""
+import argparse
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+PRESET_OPTIONS = {"L1": int, "tau1": float, "cbca_i1": int, "cbca_i2": int, "pi1": float, "pi2": float, "sgm_q1": float,
+                  "sgm_q2": float, "alpha1": float, "tau_so": float, "sgm_i": int, "blur_sigma": float, "blur_t": float}
+ACTIONS = ("test_te", "test_all", "submit", "time", "predict")
+
+
+def _flag(v):
+    """main.lua's boolean options: `-tiny` alone, or `-tiny true|false|1|0`"""
+    return str(v).lower() not in ("false", "0", "")
+
+
+def parser():
+    ap = argparse.ArgumentParser(prog="run_main.py", description=__doc__.splitlines()[0])
+    ap.add_argument("dataset", choices=("kitti", "kitti2015", "mb"))
+    ap.add_argument("arch", choices=("fast", "slow", "ad", "census"))
+    ap.add_argument("-a", default="test_te", help="|".join(ACTIONS))
+    ap.add_argument("-net_fname", default="")
+    ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    ap.add_argument("-tiny", nargs="?", const=True, default=False, type=_flag)
+    ap.add_argument("-rect", default="imperfect")
+    ap.add_argument("-color", default="gray")
+    ap.add_argument("-data_root", default=".")
+    ap.add_argument("-out", default="out")
+    ap.add_argument("-left", default="")
+    ap.add_argument("-right", default="")
+    ap.add_argument("-disp_max", type=int, default=None)
+    ap.add_argument("-at", type=int, default=0)
+    for name in ("debug", "use_cache", "make_cache"):
+        ap.add_argument("-" + name, nargs="?", const=True, default=False, type=_flag)
+    ap.add_argument("-sm_terminate", default="")
+    ap.add_argument("-sm_skip", default="")
+    for name, typ in PRESET_OPTIONS.items():
+        ap.add_argument("-" + name, type=typ, default=None)
+    return ap
+
+
+def parse_args(argv=None):
+    """-> (namespace, preset overrides dict).  Refuses what the actions do not implement before any GPU work."""
+    from mccnn_b200 import evaluate
+
+    args = parser().parse_args(argv)
+    if args.a in ("train_tr", "train_all"):
+        raise SystemExit("run_main.py: -a %s (training) is not supported; use a trained net with -net_fname" % args.a)
+    if args.a not in ACTIONS:
+        raise SystemExit("run_main.py: unknown action -a %s (%s)" % (args.a, ", ".join(ACTIONS)))
+    if args.gpu < 1:
+        raise SystemExit("run_main.py: -gpu is 1-based")
+    evaluate.check_options(args.dataset, at=args.at, color=args.color, debug=args.debug, use_cache=args.use_cache,
+                           make_cache=args.make_cache, sm_terminate=args.sm_terminate, sm_skip=args.sm_skip)
+    overrides = {k: getattr(args, k) for k in PRESET_OPTIONS if getattr(args, k) is not None}
+    args.device = args.gpu - 1
+    return args, overrides
+
+
+def main(argv=None):
+    args, overrides = parse_args(argv)
+    import mccnn_b200  # noqa: F401
+    from mccnn_b200 import evaluate, frontend
+
+    if args.a == "predict":
+        if not (args.left and args.right and args.disp_max):
+            raise SystemExit("run_main.py: -a predict needs -left, -right and -disp_max")
+        if args.arch in ("fast", "slow") and args.net_fname:
+            overrides.setdefault("border", frontend.net_border(frontend.load_net(args.net_fname, args.arch)))
+        frontend.predict(args.left, args.right, dataset=args.dataset, arch=args.arch, disp_max=args.disp_max,
+                         out_dir=".", device=args.device, net_fname=args.net_fname or None, **overrides)
+        return 0
+    ev = evaluate.Evaluator(args.dataset, args.arch, net_fname=args.net_fname or None, device=args.device, **overrides)
+    try:
+        if args.a == "time":
+            ev.time(tiny=args.tiny)
+        elif args.a == "submit":
+            ev.submit(data_root=args.data_root, out=args.out, rect=args.rect, color=args.color)
+        else:
+            ev.test(args.a, data_root=args.data_root, rect=args.rect, color=args.color)
+    finally:
+        ev.close()
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
