@@ -490,13 +490,13 @@ extern "C" int mccnn_feature_tower_forward(const mccnn_feature_tower *h, const f
 			if (nterms == 3) {
 				if (!attr_r3[dev & 63]) {
 					rc = (int)cudaFuncSetAttribute(conv3x3_resident_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_SMEM);
-					attr_r3[dev & 63] = true;
+					attr_r3[dev & 63] = !rc;
 				}
 				if (!rc) conv3x3_resident_kernel<3><<<nb, F2_NT, F2_SMEM, s>>>(p, nimg);
 			} else {
 				if (!attr_r1[dev & 63]) {
 					rc = (int)cudaFuncSetAttribute(conv3x3_resident_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_SMEM);
-					attr_r1[dev & 63] = true;
+					attr_r1[dev & 63] = !rc;
 				}
 				if (!rc) conv3x3_resident_kernel<1><<<nb, F2_NT, F2_SMEM, s>>>(p, nimg);
 			}
@@ -507,14 +507,14 @@ extern "C" int mccnn_feature_tower_forward(const mccnn_feature_tower *h, const f
 			if (!attr3[dev & 63]) {
 				rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<3, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
 				if (!rc) rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<3, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				attr3[dev & 63] = true;
+				attr3[dev & 63] = !rc;
 			}
 			if (!rc) ft_launch<3>(p, grid, s);
 		} else {
 			if (!attr1[dev & 63]) {
 				rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
 				if (!rc) rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				attr1[dev & 63] = true;
+				attr1[dev & 63] = !rc;
 			}
 			if (!rc) ft_launch<1>(p, grid, s);
 		}

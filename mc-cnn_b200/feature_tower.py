@@ -49,8 +49,12 @@ class FeatureTower:
         px = adcensus._t(x_batch, 1, n)
         if x_batch.dim() != 4 or x_batch.shape[1] != self.n_in:
             raise adcensus.AdcensusError("%s: expected (N, %d, H, W)" % (n, self.n_in))
+        if x_batch.device != self.device:
+            raise adcensus.AdcensusError("%s: input is on %s, the tower's weights on %s" % (n, x_batch.device, self.device))
         N, _, H, W = x_batch.shape
         out = torch.empty((N, self.fm, H, W), device=x_batch.device, dtype=torch.float32)
-        adcensus._check(adcensus.lib().mccnn_feature_tower_forward(self._h, px, ctypes.c_void_p(out.data_ptr()), N, H, W, nterms,
-                                                                   adcensus._stream(x_batch)), n)
+        with torch.cuda.device(x_batch.device):
+            rc = adcensus.lib().mccnn_feature_tower_forward(self._h, px, ctypes.c_void_p(out.data_ptr()), N, H, W, nterms,
+                                                            adcensus._stream(x_batch))
+        adcensus._check(rc, n)
         return out

@@ -54,11 +54,16 @@ class ScorerHead:
         pL, pR = adcensus._t(featL, 1, n), adcensus._t(featR, 2, n)
         if featL.dim() != 3 or featL.shape != featR.shape or featL.shape[0] != self.fm:
             raise adcensus.AdcensusError("%s: expected two (%d, H, W) tensors" % (n, self.fm))
+        if featL.device != self.device or featR.device != self.device:
+            raise adcensus.AdcensusError("%s: features are on %s and %s, the head's weights on %s"
+                                         % (n, featL.device, featR.device, self.device))
         _, H, W = featL.shape
         vols = []
         for want in (want_left, want_right):
             vols.append(torch.full((1, D, H, W), float("nan"), device=featL.device) if want else None)   # main.lua:962
         vp = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-        adcensus._check(adcensus.lib().mccnn_scorer_head_forward(self._h, pL, pR, vp(vols[0]), vp(vols[1]), H, W, D, nterms,
-                                                                 adcensus._stream(featL)), n)
+        with torch.cuda.device(featL.device):
+            rc = adcensus.lib().mccnn_scorer_head_forward(self._h, pL, pR, vp(vols[0]), vp(vols[1]), H, W, D, nterms,
+                                                          adcensus._stream(featL))
+        adcensus._check(rc, n)
         return vols[0], vols[1]

@@ -52,3 +52,13 @@ def tower_forward(x_batch, layers, normalize=True):
         norm = (h.astype(np.float64) ** 2).sum(1, keepdims=True) + 1e-5           # adcensus.cu:1296
         h = (h / np.sqrt(norm)).astype(np.float32)
     return h
+
+
+def tower_forward_rows(x_batch, layers, y0, y1, normalize=True):
+    """Output rows [y0, y1) of tower_forward at full width, from input rows [y0 - l1, y1 + l1) clipped to the image: each
+    3x3 layer moves the crop's zero padding one row inwards, so the l1 extra rows keep it out of the kept rows.  Lets a
+    full-size image be checked band by band at a fraction of the cost."""
+    H = np.shape(x_batch)[2]
+    l1 = len(layers)
+    a, b = max(0, y0 - l1), min(H, y1 + l1)
+    return tower_forward(np.asarray(x_batch)[:, :, a:b], layers, normalize)[:, :, y0 - a:y1 - a]

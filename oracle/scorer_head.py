@@ -47,6 +47,16 @@ def head_pixels(x, layers):
     return h[0]
 
 
+def head_samples(featL, featR, layers, d, y, x):
+    """The scores at the entries (d, y, x) of the left volume (x >= d): head_pixels on the gathered columns
+    [featL[:, y, x]; featR[:, y, x - d]].  Checks a full-size volume at chosen points without running every disparity."""
+    d, y, x = (np.asarray(v, dtype=np.int64) for v in (d, y, x))
+    if (x < d).any():
+        raise ValueError("head_samples: every entry needs x >= d")
+    cols = np.concatenate([np.asarray(featL)[:, y, x], np.asarray(featR)[:, y, x - d]], axis=0)
+    return head_pixels(cols, layers)
+
+
 def head_volume(featL, featR, D, layers, direction):
     """main.lua:963-978 for one direction: (D,H,W) float32, NaN where x - d < 0 (direction -1, left
     volume) / x + d >= W (direction +1, right volume).  fix_border is applied by the caller."""

@@ -53,6 +53,24 @@ def test_receptive_field_is_the_window():
     assert not np.array_equal(ft.tower_forward(x3, layers, normalize=False)[0, :, 10, 10], base[0, :, 10, 10])
 
 
+def test_rows_equal_the_full_tower_in_every_band():
+    """tower_forward_rows: a full-width band of output rows from a crop with l1 rows of margin equals those rows of the
+    whole image's tower (to float64 summation order), at the top edge, in the middle and at the bottom edge"""
+    rng = np.random.default_rng(4)
+    for l1, normalize in ((3, True), (5, False)):
+        layers = ft.make_weights(rng, l1=l1, fm=8)
+        x = rng.standard_normal((2, 1, 23, 17)).astype(np.float32)
+        full = ft.tower_forward(x, layers, normalize)
+        for y0, y1 in ((0, 3), (0, 1), (9, 14), (20, 23), (22, 23), (0, 23)):
+            got = ft.tower_forward_rows(x, layers, y0, y1, normalize)
+            assert got.shape == (2, 8, y1 - y0, 17)
+            assert np.abs(got - full[:, :, y0:y1]).max() < 1e-6, (l1, y0, y1)
+        # one row less of margin lets the crop's zero padding in
+        y0, y1 = 9, 14
+        short = ft.tower_forward(x[:, :, y0 - l1 + 1:y1 + l1 - 1], layers, normalize)[:, :, l1 - 1:l1 - 1 + y1 - y0]
+        assert np.abs(short - full[:, :, y0:y1]).max() > 1e-3
+
+
 def test_against_the_pytorch_restatement_fixture():
     """tests/golden/feature_tower.npz: the module stack of main.lua:726-749 + Normalize_forward restated in PyTorch (CPU fp32),
     generator oracle/make_feature_tower_golden.py"""

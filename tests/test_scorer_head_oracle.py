@@ -2,6 +2,7 @@
 next hot-path row.  Parity is unpinned (no reference vectors exist); these tests pin the
 restatement to the definition in main.lua:963-978 / SpatialConvolution1_fw.lua."""
 import numpy as np
+import pytest
 
 from oracle import scorer_head as sh
 
@@ -58,6 +59,24 @@ def test_first_layer_splits_into_a_left_and_a_right_half():
     rest = sh.head_pixels(h1.astype(np.float32), [(np.eye(nh2, dtype=np.float32), np.zeros(nh2, np.float32))] + layers[1:])
     want = sh.head_volume(fL, fR, d + 1, layers, -1)[d, :, d:].ravel()
     assert np.abs(rest - want).max() < 1e-5
+
+
+def test_samples_equal_the_volume():
+    """head_samples at chosen (d, y, x) equals head_volume's entries there (to float64 summation order), including x = d
+    and x = W - 1"""
+    rng = np.random.default_rng(3)
+    fm, nh2, l2, H, W, D = 8, 16, 3, 4, 13, 9
+    layers = sh.make_weights(rng, fm, nh2, l2)
+    fL, fR = _feats(rng, fm, H, W), _feats(rng, fm, H, W)
+    vol = sh.head_volume(fL, fR, D, layers, -1)
+    d, y, x = np.nonzero(~np.isnan(vol))                            # every valid entry, in one call
+    assert np.abs(sh.head_samples(fL, fR, layers, d, y, x) - vol[d, y, x]).max() < 1e-6
+    d, y, x = [0, 8, 8, 3], [0, 3, 1, 2], [0, 8, W - 1, 5]           # a few in arbitrary order
+    assert np.abs(sh.head_samples(fL, fR, layers, d, y, x) - vol[d, y, x]).max() < 1e-6
+    # the right image's pixel is x - d: one column off is far from the volume
+    assert np.abs(sh.head_samples(fL, fR, layers, [2, 3], [1, 1], [7, 7]) - vol[[3, 2], [1, 1], [7, 7]]).max() > 1e-4
+    with pytest.raises(ValueError):
+        sh.head_samples(fL, fR, layers, [4], [0], [3])              # x < d has no score
 
 
 def test_against_the_pytorch_restatement_fixture():
