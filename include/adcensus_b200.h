@@ -329,6 +329,37 @@ void mccnn_feature_tower_destroy(mccnn_feature_tower *h);
 int mccnn_feature_tower_forward(const mccnn_feature_tower *h, const float *img, float *out, int nimg, int H, int W,
 				int nterms, adcensus_stream_t stream);
 
+/* ---- KITTI label cleaning and training-sample lists (csrc/preprocess.cu, preprocess_kitti.lua:95-116) ----------------
+ * Stacks are (N, 1, H, W) disparity maps, treated as N*H rows of W columns as the reference does (x = index % W); the three
+ * cleaning operators work in place.  Not registered in the Lua face yet (csrc/lua_face.cu still names them
+ * "not implemented"). */
+
+/* adcensus.remove_nonvisible(y)  adcensus.cu:1723-1745: y[.., x] >= x -> 0 */
+int adcensus_remove_nonvisible(float *y, int N, int H, int W, adcensus_stream_t stream);
+
+/* adcensus.remove_occluded(y)  adcensus.cu:1747-1771: y[.., x] -> 0 if some i >= 1, x + i < W, has i - y[x+i] < -y[x].
+ * Computed as one reverse suffix minimum of j - y[j] per row (DESIGN.md).  PRECONDITION for bit-identity with the reference:
+ * every y is >= 0 and every x - y[x] is exact in fp32 -- true for any map readPNG16 produces (multiples of 1/256 in [0, 256))
+ * with W <= 2^15.  ADCENSUS_ELIMIT for W > 32768. */
+int adcensus_remove_occluded(float *y, int N, int H, int W, adcensus_stream_t stream);
+
+/* adcensus.remove_white(x, y)  adcensus.cu:1773-1796: y -> 0 where x == 255 (x has y's N*H*W elements) */
+int adcensus_remove_white(const float *x, float *y, int N, int H, int W, adcensus_stream_t stream);
+
+/* The sample lists nnz_tr / nnz_te of preprocess_kitti.lua:95-116 in two calls.  disp (n, 1, H, W) training maps (not
+ * modified: the cleaning runs on an on-chip copy), x0 (at least n, 1, H, W) their standardised left images, is_te (n) int32
+ * flags (1: image i is in the validation split te).  Per map: remove_nonvisible, remove_occluded, remove_white(x0[i]); then
+ * every entry d > 0.5 becomes the float row (i + 1, y, x, d) of nnz_te if is_te[i] else nnz_tr, ordered by image, then row,
+ * then column -- make_dataset2's order (adcensus.cu:1900-1929).  Same precondition as adcensus_remove_occluded;
+ * ADCENSUS_ELIMIT for W > 32768 or n*H*W >= 2^31.
+ *   mccnn_kitti_nnz_count writes the two row counts to counts[0] (nnz_tr) and counts[1] (nnz_te), DEVICE int64;
+ *   mccnn_kitti_nnz_fill writes the rows ((rows, 4) float32, 16-byte aligned); rows past cap_tr / cap_te are dropped, and a
+ *   buffer may be NULL when its cap is 0.  Size the buffers with the count call. */
+int mccnn_kitti_nnz_count(const float *disp, const float *x0, const int *is_te, int n, int H, int W, long long *counts,
+			  adcensus_stream_t stream);
+int mccnn_kitti_nnz_fill(const float *disp, const float *x0, const int *is_te, int n, int H, int W, float *nnz_tr,
+			 long long cap_tr, float *nnz_te, long long cap_te, adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

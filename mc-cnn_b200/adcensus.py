@@ -215,6 +215,47 @@ def census(x0, x1, out, direction):
                                      _stream(out)), n)
 
 
+# ---- label cleaning of preprocess_kitti.lua (not in the Lua face yet) --------
+
+def _stack_shape(y):
+    """(N, H, W) of a disparity stack: W = the last size (the reference's size(3) of an (n,1,H,W) tensor), H the one before"""
+    W = y.size(-1) if y.dim() else 1
+    H = y.size(-2) if y.dim() >= 2 else 1
+    return y.numel() // max(1, H * W), H, W
+
+
+def remove_nonvisible(y):
+    """adcensus.remove_nonvisible(y)  adcensus.cu:1735-1745: in place, y >= x (the column index) -> 0"""
+    n = "remove_nonvisible"
+    p = _t(y, 1, n)
+    if y.numel():
+        with torch.cuda.device(y.device):
+            _check(lib().adcensus_remove_nonvisible(p, *_stack_shape(y), _stream(y)), n)
+
+
+def remove_occluded(y):
+    """adcensus.remove_occluded(y)  adcensus.cu:1761-1771: in place; bit-identical to the reference for maps in readPNG16's
+    domain (see adcensus_remove_occluded in include/adcensus_b200.h)"""
+    n = "remove_occluded"
+    p = _t(y, 1, n)
+    if y.numel():
+        with torch.cuda.device(y.device):
+            _check(lib().adcensus_remove_occluded(p, *_stack_shape(y), _stream(y)), n)
+
+
+def remove_white(x, y):
+    """adcensus.remove_white(x, y)  adcensus.cu:1784-1796: in place, y -> 0 where x == 255"""
+    n = "remove_white"
+    px, py = _t(x, 1, n), _t(y, 2, n)
+    if x.numel() != y.numel():
+        raise AdcensusError("bad argument #1 to '%s' (%d elements, y has %d)" % (n, x.numel(), y.numel()))
+    if x.device != y.device:
+        raise AdcensusError("bad argument #1 to '%s' (on %s, y on %s)" % (n, x.device, y.device))
+    if y.numel():
+        with torch.cuda.device(y.device):
+            _check(lib().adcensus_remove_white(px, py, *_stack_shape(y), _stream(y)), n)
+
+
 # ---- the Lua-side tensor ops of stereo_predict ------------------------------
 
 def fill_nan(t):

@@ -126,6 +126,45 @@ def write_kitti_set(root, dataset="kitti", n_tr=4, n_te=2, H=48, width=130, widt
     return d
 
 
+def write_kitti_raw(root, dataset="kitti", n_tr=41, n_te=2, H=375, widths=(1242, 1241, 1224), seed=0, D=64):
+    """A seeded raw KITTI tree as the archives unpack, under ``root/data.kitti/unzip`` (or ``data.kitti2015``):
+    ``{training,testing}/<left>|<right>/%06d_10.png`` (8-bit grey image_0 / image_1 for 'kitti', RGB image_2 / image_3 for
+    'kitti2015') and ``training/<disp_noc>/%06d_10.png`` (disp_noc / disp_noc_0), 16-bit maps of disparity * 256.  Image k
+    of a directory is H x widths[k % len(widths)].  The maps are _scene_views' ground truth (piecewise constant in [1, D),
+    so there are real occlusions where a nearer block lies to the right, and entries d >= x at the left border) plus a
+    per-block slant quantised to 1/256, with about 10% zero (invalid) pixels.  Returns the unzip directory."""
+    import os
+
+    from PIL import Image
+
+    from . import dataio
+
+    rgb = dataset == "kitti2015"
+    names = ("image_2", "image_3", "disp_noc_0") if rgb else ("image_0", "image_1", "disp_noc")
+    unzip = os.path.join(root, "data.kitti2015" if rgb else "data.kitti", "unzip")
+    rng = np.random.default_rng(seed)
+    for sub, n in (("training", n_tr), ("testing", n_te)):
+        for name in names[:2] + ((names[2],) if sub == "training" else ()):
+            os.makedirs(os.path.join(unzip, sub, name), exist_ok=True)
+        for k in range(n):
+            W = int(widths[k % len(widths)])
+            views, gt = _scene_views(rng, H, W, D)
+            fname = "%06d_10.png" % k
+            for v, name in zip(views, names[:2]):
+                byte = lambda a: np.clip(np.rint(128 + 40 * a), 0, 255).astype(np.uint8)
+                if rgb:
+                    tint = rng.uniform(0.8, 1.2, 3)
+                    im = Image.fromarray(np.stack([byte(v * t) for t in tint], axis=2), "RGB")
+                else:
+                    im = Image.fromarray(byte(v), "L")
+                im.save(os.path.join(unzip, sub, name, fname), format="PNG")
+            if sub == "training":
+                slant = np.kron(rng.integers(0, 256, size=((H + 15) // 16, (W + 47) // 48)), np.ones((16, 48), np.int64))
+                frac = (slant[:H, :W] * (np.arange(W)[None, :] % 48) // 48) / np.float32(256)
+                dataio.write_png16(np.where(gt > 0, gt + frac, 0).astype(np.float32), os.path.join(unzip, sub, names[2], fname))
+    return unzip
+
+
 def write_mb_set(root, n=6, shapes=((40, 96, 24), (48, 130, 32)), seed=0, rect="imperfect", color="gray"):
     """A small seeded Middlebury set in preprocess_mb.py's layout under ``root/data.mb.<rect>_<color>``: per image k = 1..n
     x_<k>_1.bin (views, 1, H, W) (4 views for image 5, else 2) and dispnoc<k>.bin (H, W), meta.bin (n, 3) int32 (H, W,
