@@ -56,9 +56,9 @@ int adcensus_StereoJoin(const float *input_L, const float *input_R, float *outpu
 			int C, int D, int H, int W, adcensus_stream_t stream);
 
 /* StereoJoin into PITCHED volumes (D, H, ld), ld % 4 == 0, 16-byte aligned outputs, W even, 8-byte aligned features (else
- * ADCENSUS_EINVAL): 8-byte cp.async operand loads, the left volume leaves through one TMA store per tile.  Same
- * values as adcensus_StereoJoin bit for bit; additionally output_L[d,y,x] = NaN for x < d (the fill of main.lua:946 for
- * the left volume); output_R's entries with x >= W - d are left untouched. */
+ * ADCENSUS_EINVAL), with the kernels the fused pipeline runs.  Same values as adcensus_StereoJoin bit for bit;
+ * additionally output_L[d,y,x] = NaN for x < d (the fill of main.lua:946 for the left volume); output_R's entries with
+ * x >= W - d and the padding columns x >= W of both volumes are left untouched. */
 int mccnn_stereo_join_pitched(const float *input_L, const float *input_R, float *output_L, float *output_R,
 			      int C, int D, int H, int W, int ld, adcensus_stream_t stream);
 
@@ -236,12 +236,11 @@ int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, int W,
 void mccnn_pipeline_destroy(mccnn_pipeline *p);
 size_t mccnn_pipeline_device_bytes(const mccnn_pipeline *p);
 /* CBCA mode of the pipeline's iterations: 1 (default) = constant-work aggregation (mccnn_cbca_fast_pitched: volumes within
- * the north star's 1e-4 of the reference, measured ~1e-6; disparity map identical except at isolated near-ties);
- * 0 = exact, every output bit-identical to the reference.  ADCENSUS_CBCA_EXACT=1 in the environment makes 0 the default.
- * mccnn_pipeline_set_fast_cbca is the older name of the same switch. */
+ * the north star's 1e-4 of the reference, measured ~1e-6; disparity map identical except at isolated near-ties) for presets
+ * whose arms are at most 5 pixels long, the exact kernels for longer arms; 0 = exact, every output bit-identical to the
+ * reference.  ADCENSUS_CBCA_EXACT=1 in the environment makes 0 the default. */
 void mccnn_pipeline_set_cbca_mode(mccnn_pipeline *p, int mode);
 int mccnn_pipeline_get_cbca_mode(const mccnn_pipeline *p);
-void mccnn_pipeline_set_fast_cbca(mccnn_pipeline *p, int on);
 /* SGM data layout inside the pipeline: 0 (default) = permute the pitched volume to (H,W,D) and back around sgm2 like
  * main.lua:1008-1020 (fused /4); 1 = scan the (D,H,ld) layout directly (mccnn_sgm2_dhw, no permutes).  Bit-identical
  * results either way; ADCENSUS_SGM_DHW=1 in the environment makes 1 the default. */

@@ -423,10 +423,8 @@ int launch_win(const uint32_t *a0, const uint32_t *a1, const float *vol, float *
 	// disparities per CTA.  The kernel is issue-bound and balances dynamically, so the chunk size hardly matters; timed on an
 	// H100 through the exact-mode pipeline at 370x1226x228 (ms per pair, two rounds): 8 -> 17.29 / 17.43, 10 -> 17.24 / 17.39,
 	// 14 -> 17.18 / 17.16, 20 -> 17.15 / 17.23.
-	const char *env = getenv("ADCENSUS_CBCA_DCH");   // tuning knob, not part of the ABI
-	int dch = env ? atoi(env) : 14;
-	if (dch < 1) dch = 1;
-	if (dch > CW_DCH_MAX) dch = CW_DCH_MAX;
+	constexpr int dch = 14;
+	static_assert(dch <= CW_DCH_MAX, "right-image arm window too narrow");
 	dim3 grid(adc_div_up(W, CW_TX), adc_div_up(H, CW_TY), adc_div_up(D, dch));
 	cbca_win_kernel<R><<<grid, CW_NT, SMEM, s>>>(a0, a1, vol, out, D, H, W, ld, direction, dch, gate, gate_lo, gate_hi);
 	return 0;

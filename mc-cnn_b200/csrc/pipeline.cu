@@ -27,7 +27,7 @@ int adc_cbca_packed(const uint32_t *pk, const float *x0c, const float *x1c,
 		    const float *vol, float *out, int D, int H, int W, int ld, int direction, int maxlen, cudaStream_t s);
 size_t adc_packed_hv_words(int H, int W);
 int adc_pack_arms_hv(const float *xc, uint32_t *hv, int which, int H, int W, cudaStream_t s);
-int adc_cbca_tma_max_halo();
+int adc_cbca_ws_max_halo();
 void adc_cbca_tma_box(int halo, int *box_w, int *box_h);
 int adc_cbca_tma(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
 		 int halo, cudaStream_t s);
@@ -41,9 +41,7 @@ size_t adc_sgm_dhw_table_bytes(int H, int W, int D);
 int adc_sgm2_dhw(const float *x0, const float *x1, const float *in, float *acc, uint8_t *tab, int H, int W, int ld, int D,
 		 float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction, bool div4, cudaStream_t s);
 int adc_stereo_join(const float *input_L, const float *input_R, float *output_L, float *output_R,
-		    int C, int D, int H, int W, int ldo, int fast, const CUtensorMap *tmL, cudaStream_t s);
-int adc_stereo_join_dc(int D);
-int adc_stereo_join_fast_ok(const float *input_L, const float *input_R, const float *output_L, const float *output_R, int W, int ldo);
+		    int C, int D, int H, int W, int ldo, cudaStream_t s);
 int adc_fill_invalid(float *volL, float *volR, int D, int H, int W, int ld, cudaStream_t s);
 int adc_fix_border(float *vol, int D, int H, int W, int ld, int n, int direction, cudaStream_t s);
 int adc_argmin_pitched(const float *vol, float *disp, int D, int H, int W, int ld, cudaStream_t s);
@@ -73,9 +71,6 @@ struct mccnn_pipeline {
 	float *gauss;     // ks*ks
 	uint8_t *sgmtab;  // SGM penalty-class tables
 	int ks;
-	// tensor map of the left volume for StereoJoin's TMA store (box {128, 1, disparity chunk})
-	int sj_tm_ok;
-	CUtensorMap sj_tm;
 	// tensor maps of the volume buffers (inputs of the TMA-staged CBCA), all encoded for the run shape
 	// (tm_D, tm_H, tm_W); a run at another shape re-encodes them first (encode_maps), 0 = none valid
 	int tm_D, tm_H, tm_W;
@@ -117,11 +112,16 @@ int dev_alloc(void **p, size_t bytes, size_t *acc)
 // longest arm cross() can produce for this preset, and the CBCA support radius
 int pipe_maxlen(const mccnn_pipeline *p) { return p->prm.L1 > 2 ? p->prm.L1 : 2; }
 
+// Constant-work aggregation only for arms <= 5 (the KITTI presets, cbca_ws.cu): with the Middlebury presets' arms of up to
+// 14 pixels the first-generation kernel's float prefixes over 27 x 27 windows reach 1.03e-4 after six iterations (measured,
+// mb slow at 300 x 700 x 128) -- outside the 1e-4 contract -- so those presets run the exact tile kernels in every mode.
+bool pipe_fast_cbca_ok(const mccnn_pipeline *p) { return pipe_maxlen(p) - 1 <= adc_cbca_ws_max_halo(); }
+
 // a map of `buf` as a (tm_D, tm_H, tm_W) volume with rows of tm_W rounded up to 4 floats
 int add_tensor_map(mccnn_pipeline *p, const float *buf)
 {
+	if (!pipe_fast_cbca_ok(p)) return 0;               // such presets run the exact kernels
 	const int halo = pipe_maxlen(p) - 1;
-	if (halo > adc_cbca_tma_max_halo()) return 0;      // such presets run the exact kernels
 	if (!p->tm_D) return 0;                            // no valid shape: the next run encodes every map
 	if (p->ntm >= 6) return ADCENSUS_EINVAL;
 	int bw, bh;
@@ -132,20 +132,15 @@ int add_tensor_map(mccnn_pipeline *p, const float *buf)
 	return 0;
 }
 
-// (Re-)encode every tensor map for volumes of shape (D, H, W): StereoJoin's store map of the left volume and the CBCA
-// input maps of both volumes (the right one starts D*H*ld floats into `vols`), the ping-pong / accumulator buffers and,
-// in overlap mode, the side stream's.  Kernels already launched are unaffected: each one received its map by value
-// (__grid_constant__) at launch.
+// (Re-)encode every tensor map for volumes of shape (D, H, W): the CBCA input maps of both volumes (the right one starts
+// D*H*ld floats into `vols`), the ping-pong / accumulator buffers and, in overlap mode, the side stream's.  Kernels already
+// launched are unaffected: each one received its map by value (__grid_constant__) at launch.
 int encode_maps(mccnn_pipeline *p, int D, int H, int W)
 {
 	const int ld = (W + 3) & ~3;
 	const long V = (long)D * H * ld;
 	p->ntm = 0;
 	p->tm_D = D; p->tm_H = H; p->tm_W = W;
-	const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)D};
-	const uint64_t strides[2] = {(uint64_t)ld * 4, (uint64_t)ld * 4 * (uint64_t)H};
-	const uint32_t box[3] = {128u, 1u, (uint32_t)adc_stereo_join_dc(D)};
-	p->sj_tm_ok = adc_tma_encode(&p->sj_tm, p->vols, 3, dims, strides, box) == 0;
 	int rc = 0;
 	for (const float *b : {(const float *)p->vols, (const float *)(p->vols + V), (const float *)p->bufA, (const float *)p->bufC,
 			       (const float *)p->bufA2, (const float *)p->bufC2})
@@ -153,7 +148,6 @@ int encode_maps(mccnn_pipeline *p, int D, int H, int W)
 	if (rc) {                                          // leave nothing half-encoded behind
 		p->ntm = 0;
 		p->tm_D = p->tm_H = p->tm_W = 0;
-		p->sj_tm_ok = 0;
 	}
 	return rc;
 }
@@ -261,7 +255,6 @@ extern "C" size_t mccnn_pipeline_device_bytes(const mccnn_pipeline *p) { return 
 // 1 (default) constant-work aggregation within the 1e-4 contract (cbca_tma.cu); 0 exact, bit-identical to the reference
 extern "C" void mccnn_pipeline_set_cbca_mode(mccnn_pipeline *p, int mode) { if (p) p->cbca_mode = mode ? 1 : 0; }
 extern "C" int mccnn_pipeline_get_cbca_mode(const mccnn_pipeline *p) { return p ? p->cbca_mode : -1; }
-extern "C" void mccnn_pipeline_set_fast_cbca(mccnn_pipeline *p, int on) { mccnn_pipeline_set_cbca_mode(p, on); }
 // 0 (default): permute to (H,W,D) for sgm2 like main.lua:1008; 1: scan (D,H,ld) directly (sgm_dhw.cu).  Same results.
 extern "C" void mccnn_pipeline_set_sgm_layout(mccnn_pipeline *p, int dhw) { if (p) p->sgm_dhw = dhw ? 1 : 0; }
 static void overlap_release(mccnn_pipeline *p)
@@ -350,12 +343,8 @@ static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *
 	if (p->tm_D != D || p->tm_H != H || p->tm_W != W) STEP(encode_maps(p, D, H, W));
 
 	float *volsL = p->vols, *volsR = p->vols + V;
-	// main.lua:946 (only what :947 leaves); on the fast path StereoJoin's TMA store fills the left volume's invalid entries itself
-	// (opt-in: on an H100 at the bench size the pipeline takes 11.59 ms per pair with it against 10.99 ms without: ADCENSUS_SJ_FAST=1)
-	static const bool sj_fast_env = getenv("ADCENSUS_SJ_FAST") && atoi(getenv("ADCENSUS_SJ_FAST"));
-	const bool sj_fast = sj_fast_env && p->sj_tm_ok && adc_stereo_join_fast_ok(featL, featR, volsL, volsR, W, ld);
-	STEP(adc_fill_invalid(sj_fast ? nullptr : volsL, volsR, D, H, W, ld, s)); nl += 1;
-	STEP(adc_stereo_join(featL, featR, volsL, volsR, C, D, H, W, ld, sj_fast, sj_fast ? &p->sj_tm : nullptr, s)); nl += 1;   // :947
+	STEP(adc_fill_invalid(volsL, volsR, D, H, W, ld, s)); nl += 1;                                 // main.lua:946 (only what :947 leaves)
+	STEP(adc_stereo_join(featL, featR, volsL, volsR, C, D, H, W, ld, s)); nl += 1;                  // :947
 	STEP(adc_fix_border(volsL, D, H, W, ld, o.border, -1, s));                                    // :948
 	STEP(adc_fix_border(volsR, D, H, W, ld, o.border, 1, s)); nl += o.border ? 2 : 0;             // :949
 
@@ -365,13 +354,7 @@ static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *
 	// fix_border copies column W-n-1 over the border columns: for D > W - n - 1 that column holds NaN at "valid"
 	// positions, which only the tap-by-tap generic kernel treats like the reference (NaN only where a tap is NaN)
 	const bool nan_in_valid = o.border > 0 && D > W - o.border - 1;
-	// constant-work aggregation only for arms <= 5 (the KITTI presets, cbca_ws.cu): with the Middlebury presets' arms of up to
-	// 14 pixels the first-generation kernel's float prefixes over 27 x 27 windows reach 1.03e-4 after six iterations (measured,
-	// mb slow at 300 x 700 x 128) -- outside the 1e-4 contract -- so those presets run the exact tile kernels in every mode
-	// (ADCENSUS_CBCA_FAST_LONG=1 overrides)
-	static const bool fast_long = getenv("ADCENSUS_CBCA_FAST_LONG") && atoi(getenv("ADCENSUS_CBCA_FAST_LONG"));
-	const int fast_halo = fast_long ? adc_cbca_tma_max_halo() : 4;
-	const bool tma = p->cbca_mode && !nan_in_valid && maxlen - 1 <= fast_halo && p->ntm > 0;
+	const bool tma = p->cbca_mode && !nan_in_valid && pipe_fast_cbca_ok(p) && p->ntm > 0;
 	uint32_t *hv = p->packed + adc_packed_words(H, W);
 	if (ncbca > 0) {
 		STEP(adcensus_cross(imgL, p->x0c, H, W, o.L1, o.tau1, s));

@@ -1,4 +1,5 @@
-"""Time StereoJoin at the bench size (L2 flushed between launches): pitched fast path vs the operator on contiguous tensors."""
+"""Time StereoJoin at the bench size (L2 flushed between launches): the pitched form the fused pipeline runs vs the operator
+on contiguous tensors."""
 import argparse
 import ctypes
 import os
