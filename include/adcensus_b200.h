@@ -359,6 +359,41 @@ int mccnn_kitti_nnz_count(const float *disp, const float *x0, const int *is_te, 
 int mccnn_kitti_nnz_fill(const float *disp, const float *x0, const int *is_te, int n, int H, int W, float *nnz_tr,
 			 long long cap_tr, float *nnz_te, long long cap_te, adcensus_stream_t stream);
 
+/* ---- Middlebury views, halving, masks and training-sample lists (csrc/preprocess_mb.cu, preprocess_mb.py) ---------------
+ * All pointers are DEVICE pointers; images are 8-bit (n, H, W, 3) in R, G, B order (a grey file replicated to three
+ * channels, as cv2.imread does). */
+
+/* read_im (preprocess_mb.py:85-97) on n views: out (n, nchannel, H, W) float32.  nchannel 1: cv2's BGR2GRAY,
+ * fma(R, .299, fma(B, .114, G * .587)) in fp32; 3: the R, G, B planes.  Then (x - mean) / std exactly as numpy's float32
+ * x.mean() and x.std() (pairwise sums in memory order, pixels with interleaved channels): bit-identical.  n <= 65535,
+ * H * W * 3 < 2^31 (else ADCENSUS_ELIMIT). */
+int mccnn_mb_views(const unsigned char *rgb, float *out, int n, int H, int W, int nchannel, adcensus_stream_t stream);
+
+/* `convert X -resize 50%` restated, NOT bit-pinned against ImageMagick: (n, H, W, 3) -> (n, H/2, W/2, 3).  Lanczos-3
+ * L(t) = sinc(t) sinc(t/3); output x reads source 2x-5 .. 2x+6 with weights L((j + 0.5 - (2x + 1)) / 2), taps outside the
+ * image dropped and the rest renormalised; rows first, then columns, in fp32; rounded half up, clamped to [0, 255].  H and
+ * W must be even (ADCENSUS_EINVAL otherwise). */
+int mccnn_mb_half_image(const unsigned char *in, unsigned char *out, int n, int H, int W, adcensus_stream_t stream);
+
+/* load_pfm(.., True) (preprocess_mb.py:13-26) on n top-down maps: out (n, H/2, W/2) = the second smallest of each 2x2 block
+ * of in / 2 in np.sort's order (-inf < finite < inf < NaN).  H and W must be even. */
+int mccnn_mb_half_disp(const float *in, float *out, int n, int H, int W, adcensus_stream_t stream);
+
+/* `computemask d0 [d0y] d1 -1` restated, NOT pinned against the MiddEval3 SDK: mask (H, W) bytes = 0 where d0 is not
+ * finite; else x1 = floor(x - d0 + 0.5), y1 = floor(y + d0y + 0.5) (d0y may be NULL: 0), in fp64; 128 when (x1, y1) is
+ * outside the frame (or d0y not finite) or when not |d0 - d1[y1, x1]| <= 1 (inf and NaN on the right fail); else 255. */
+int mccnn_mb_mask(const float *d0, const float *d0y, const float *d1, int H, int W, unsigned char *mask,
+		  adcensus_stream_t stream);
+
+/* The training rows of one map (preprocess_mb.py:177-182) in two calls:
+ *   mccnn_mb_nnz_count writes the number of mask == 255 pixels to *count (DEVICE int64);
+ *   mccnn_mb_nnz_fill writes dispnoc (H, W) = d0 where mask == 255, else 0, and the float rows (image, y, x, d0) of those
+ *   pixels in row-major order to nnz ((rows, 4) float32, 16-byte aligned); rows past cap are dropped, nnz may be NULL when
+ *   cap is 0.  image is 1-based, <= 2^24. */
+int mccnn_mb_nnz_count(const unsigned char *mask, int H, int W, long long *count, adcensus_stream_t stream);
+int mccnn_mb_nnz_fill(const float *d0, const unsigned char *mask, int H, int W, int image, float *dispnoc, float *nnz,
+		      long long cap, adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

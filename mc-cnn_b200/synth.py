@@ -190,3 +190,154 @@ def write_mb_set(root, n=6, shapes=((40, 96, 24), (48, 130, 32)), seed=0, rect="
     with open(os.path.join(d, "fname_submit.txt"), "w") as f:
         f.write("\n".join("%s/Synth%d" % ("trainingH" if j < n_sub // 2 else "testH", j) for j in range(n_sub)))
     return d
+
+
+MB_SUBMIT_NAMES = ("Adirondack", "ArtL", "Jadeplant", "Motorcycle", "MotorcycleE", "Piano", "PianoL", "Pipes", "Playroom",
+                   "Playtable", "PlaytableP", "Recycle", "Shelves", "Teddy", "Vintage")
+
+
+def _mb_right_map(rng, d0, p_bad=0.05):
+    """a right-view map consistent with d0 where it is finite (d1[y, round(x - d0)] = d0 + small noise), a few entries off
+    by more than a pixel, inf elsewhere"""
+    H, W = d0.shape
+    d1 = np.full((H, W), np.inf, np.float32)
+    ys, xs = np.nonzero(np.isfinite(d0))
+    x1 = np.floor(xs - d0[ys, xs] + 0.5).astype(np.int64)
+    ok = (x1 >= 0) & (x1 < W)
+    noise = rng.uniform(-0.4, 0.4, ok.sum()).astype(np.float32)
+    noise[rng.random(ok.sum()) < p_bad] += np.float32(3)
+    d1[ys[ok], x1[ok]] = d0[ys[ok], xs[ok]] + noise
+    return d1
+
+
+def write_mb_raw(root, n2014=11, full=(80, 192), half_size=(40, 96), D=48, seed=0):
+    """A seeded raw Middlebury tree as preprocess_mb.py expects it under ``root/data.mb/unzip``:
+
+    * n2014 2014 scenes ``scenes2014/datasets/Scene<k>-{perfect,imperfect}`` of full x full RGB PNG views (im0, im1, im1E,
+      im1L; ``ambient/L<l>/im<c>e<e>.png`` with 1-3 lights and exposure counts cycling through 2, 3, 5, 6, 7, 8, the two
+      cameras of some scenes differing), calib.txt (ndisp = D), float PFMs disp0 / disp1 / disp0y (inf holes, a NaN, a
+      vertical offset of up to 0.7 px).  Scene 2 carries ``.H.png`` caches for all its views and a ``disp1.pfm.H.pfm``;
+      scene 5 caches im0 and im1 only.  Caches are decimated (every other pixel), so they differ from a real halving;
+    * 2006 Aloe and Baby1, 2005 Art (and Books, which has no disp1.png and is skipped), ``HalfSize/<s>/Illum<l>/Exp<e>/
+      view{1,5}.png`` and 8-bit disp1 / disp5 (value 2 d, 0 invalid);
+    * 2003 conesH and teddyH (PPM views, PGM maps of 2 d);
+    * 2001 tsukuba (PPM views, truedisp of 16 d, nonocc.png), map (PGM views, maps of 8 d with real 0 disparities) and
+      sawtooth (PPM, maps of 8 d);
+    * MiddEval3 ``trainingH`` and ``testH``, 15 pairs each.
+    Smaller scenes are half_size.  Returns the unzip directory."""
+    import os
+
+    from PIL import Image
+
+    from . import dataio
+
+    rng = np.random.default_rng(seed)
+    unzip = os.path.join(root, "data.mb", "unzip")
+    data = os.path.join(unzip, "vision.middlebury.edu", "stereo", "data")
+
+    def byte(v):
+        return np.clip(np.rint(128 + 40 * v), 0, 255).astype(np.uint8)
+
+    def rgb(v):
+        return np.stack([byte(v * t) for t in rng.uniform(0.8, 1.2, 3)], axis=2)
+
+    def save(a, *p):
+        path = os.path.join(*p)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        Image.fromarray(a).save(path)
+        return path
+
+    def pfm(m, *p):
+        path = os.path.join(*p)
+        dataio.write_pfm(np.flipud(np.asarray(m, np.float32)), path)
+        return path
+
+    def calib(ndisp, *p):
+        os.makedirs(os.path.join(*p), exist_ok=True)
+        with open(os.path.join(*p, "calib.txt"), "w") as f:
+            f.write("cam0=[1 0 0; 0 1 0; 0 0 1]\ndoffs=0\nbaseline=100\nwidth=1\nheight=1\nndisp=%d\nisint=0\n" % ndisp)
+
+    exps = (2, 3, 5, 6, 7, 8)
+    H, W = full
+    for k in range(n2014):
+        name = "Scene%02d" % k
+        views, gt = _scene_views(rng, H, W, D, n_views=4)
+        for kind in ("imperfect", "perfect"):
+            base = os.path.join(data, "scenes2014", "datasets", "%s-%s" % (name, kind))
+            calib(D, base)
+            for v, f in zip(views, ("im0.png", "im1.png", "im1E.png", "im1L.png")):
+                p = save(rgb(v), base, f)
+                if kind == "imperfect" and (k == 2 or (k == 5 and f in ("im0.png", "im1.png"))):
+                    save(np.asarray(Image.open(p))[::2, ::2].copy(), p + ".H.png")
+            n_exp = exps[k % len(exps)]
+            n_exp_other = n_exp + (1 if k % 3 == 0 else 0)            # the other camera has one more: min(max) wins
+            for light in range(1 + k % 3):
+                for cam, ne in ((0, n_exp), (1, n_exp_other)):
+                    for e in range(ne):
+                        v = views[cam] * (0.6 + 0.1 * e) + 0.05 * light
+                        p = save(rgb(v), base, "ambient", "L%d" % (light + 1), "im%de%d.png" % (cam, e))
+                        if kind == "imperfect" and k == 2:
+                            save(np.asarray(Image.open(p))[::2, ::2].copy(), p + ".H.png")
+            d0 = np.where(gt > 0, gt + rng.uniform(0, 1, gt.shape), np.inf).astype(np.float32)
+            d0[3, 5] = np.nan
+            d1 = _mb_right_map(rng, d0)
+            dy = rng.uniform(-0.7, 0.7, gt.shape).astype(np.float32)
+            pfm(d0, base, "disp0.pfm")
+            p1 = pfm(d1, base, "disp1.pfm")
+            pfm(dy, base, "disp0y.pfm")
+            if kind == "imperfect" and k == 2:
+                pfm(np.where(np.isfinite(d1[::2, ::2]), d1[::2, ::2] / 2, np.inf), p1 + ".H.pfm")
+
+    h, w = half_size
+
+    def grey_map(gt, scale, zero_invalid=True):
+        return np.clip(np.where(gt > 0, gt * scale, 0) if zero_invalid else gt * scale, 0, 255).astype(np.uint8)
+
+    for year, scenes in ((2006, ("Aloe", "Baby1")), (2005, ("Art", "Books"))):
+        for s in scenes:
+            base = os.path.join(data, "scenes%d" % year, "HalfSize", s)
+            views, gt = _scene_views(rng, h, w, D // 2)
+            for light in range(3):
+                for e in range(3):
+                    for v, f in zip(views, ("view1.png", "view5.png")):
+                        save(rgb(v * (0.7 + 0.15 * e) + 0.1 * light), base, "Illum%d" % (light + 1), "Exp%d" % e, f)
+            if s != "Books":
+                save(grey_map(gt, 2), base, "disp1.png")
+            d1 = _mb_right_map(rng, np.where(gt > 0, gt, np.inf).astype(np.float32))
+            save(grey_map(np.where(np.isfinite(d1), np.rint(d1 * 2) / 2, 0), 2), base, "disp5.png")
+
+    for s in ("conesH", "teddyH"):
+        base = os.path.join(data, "scenes2003", s)
+        views, gt = _scene_views(rng, h, w, D // 2)
+        save(rgb(views[0]), base, "im2.ppm")
+        save(rgb(views[1]), base, "im6.ppm")
+        save(grey_map(gt, 2), base, "disp2.pgm")
+        d1 = _mb_right_map(rng, np.where(gt > 0, gt, np.inf).astype(np.float32))
+        save(grey_map(np.where(np.isfinite(d1), np.rint(d1 * 2) / 2, 0), 2), base, "disp6.pgm")
+
+    base1 = os.path.join(data, "scenes2001", "data")
+    views, gt = _scene_views(rng, h, w, 15)
+    base = os.path.join(base1, "tsukuba")
+    save(rgb(views[0]), base, "scene1.row3.col3.ppm")
+    save(rgb(views[1]), base, "scene1.row3.col4.ppm")
+    save(grey_map(gt, 16), base, "truedisp.row3.col3.pgm")
+    save(np.where(rng.random(gt.shape) < 0.8, 255, 0).astype(np.uint8), base, "nonocc.png")
+    for s, names in (("map", ("im0.pgm", "im1.pgm", "disp0.pgm", "disp1.pgm")),
+                     ("sawtooth", ("im2.ppm", "im6.ppm", "disp2.pgm", "disp6.pgm"))):
+        base = os.path.join(base1, s)
+        views, gt = _scene_views(rng, h, w, 24)
+        gt[:, : w // 4] = 0                                           # 0 is a real disparity in 2001 maps
+        for v, f in zip(views, names[:2]):
+            save(byte(v) if s == "map" else rgb(v), base, f)
+        save(grey_map(gt, 8, zero_invalid=False), base, names[2])
+        d1 = _mb_right_map(rng, gt.astype(np.float32), p_bad=0.1)
+        save(grey_map(np.where(np.isfinite(d1), np.rint(d1 * 8) / 8, 0), 8, zero_invalid=False), base, names[3])
+
+    for sub, suffix in (("trainingH", "H"), ("testH", "T")):
+        for s in MB_SUBMIT_NAMES:
+            base = os.path.join(unzip, "MiddEval3", sub, s + (suffix if sub == "testH" else ""))
+            views, _ = _scene_views(rng, h, w, D // 2)
+            calib(D // 2, base)
+            save(rgb(views[0]), base, "im0.png")
+            save(rgb(views[1]), base, "im1.png")
+    return unzip
