@@ -252,6 +252,14 @@ void mccnn_pipeline_set_sgm_layout(mccnn_pipeline *p, int dhw);
 int mccnn_pipeline_set_overlap(mccnn_pipeline *p, int mode);
 /* number of kernel launches one run issues (for bench.py's gpu_launches) */
 int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p);
+/* Re-targets a created pipeline to another parameter set without allocating its volumes again (a parameter search runs
+ * many sets over the same images).  Checked like mccnn_pipeline_create (ADCENSUS_EINVAL; border + 1 must not exceed the
+ * created W).  HOST-SYNCHRONOUS: waits for all work enqueued on the pipeline's device before anything an enqueued run reads
+ * changes.  The Gaussian buffer grows only when blur_sigma needs a larger kernel (sigma 10 -> 61 x 61).  Applies to every
+ * twin lane of the batch entry points that exists; lanes created later inherit the new parameters.  Every later run gives
+ * the same bits as a pipeline created with these parameters, in the same CBCA mode, SGM layout and overlap mode.  On an
+ * error (a CUDA error, or no memory for a larger Gaussian) the pipeline must be re-targeted again or destroyed. */
+int mccnn_pipeline_set_params(mccnn_pipeline *p, const mccnn_params *params);
 
 /* Device-resident inputs: featL/featR (C,H,W) unit-norm tower outputs, imgL/imgR
  * (H,W) standardised images.  disp (H,W) device; volL/volR (D,H,W) device or NULL
@@ -271,6 +279,17 @@ int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR
 int mccnn_pipeline_run_shape(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
 			     const float *imgL, const float *imgR, float *disp, float *volL, float *volR,
 			     adcensus_stream_t stream);
+
+/* The chain of mccnn_pipeline_run_shape from given cost volumes on: volL / volR (D,H,W) contiguous at the run shape, what
+ * main.lua holds at :986 -- NaN where the reference leaves its fill, fix_border (:948-949 / :981) already applied by the
+ * caller (the fast net's StereoJoin volumes, the scorer head's, or adcensus_ad / adcensus_census outputs).  They are copied
+ * into the private pitched buffers (not modified), then cross / CBCA / SGM / ... run exactly as in mccnn_pipeline_run_shape,
+ * same bits for the same volumes.  volR may be NULL when lr_check == 0 and outR == NULL (Middlebury: only direction -1 is
+ * consumed, main.lua:954-955).  imgL/imgR/disp (H,W); outL/outR (D,H,W) or NULL.  Shape limits and error codes as
+ * mccnn_pipeline_run_shape; ADCENSUS_EINVAL also for a NULL volR that is needed.  Asynchronous on `stream`. */
+int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
+			       const float *imgL, const float *imgR, float *disp, float *outL, float *outR,
+			       adcensus_stream_t stream);
 
 /* Host-buffer call (what a non-CUDA caller binds): copies inputs H2D, runs,
  * copies disp back, and returns after the result is in disp_host. */

@@ -68,9 +68,9 @@ struct mccnn_pipeline {
 	uint32_t *packed; // packed arm lengths of both images: bytes (exact kernels) + H/V words (constant-work kernel)
 	int *maxlen;
 	float *maps;      // 8HW: disparity maps and stage outputs
-	float *gauss;     // ks*ks
+	float *gauss;     // ks*ks of the current blur_sigma, in a buffer of ks_alloc*ks_alloc floats
 	uint8_t *sgmtab;  // SGM penalty-class tables
-	int ks;
+	int ks, ks_alloc;
 	// tensor maps of the volume buffers (inputs of the TMA-staged CBCA), all encoded for the run shape
 	// (tm_D, tm_H, tm_W); a run at another shape re-encodes them first (encode_maps), 0 = none valid
 	int tm_D, tm_H, tm_W;
@@ -165,14 +165,45 @@ struct DeviceGuard {
 	~DeviceGuard() { cudaSetDevice(prev); }
 };
 
+// the parameter checks shared by create and set_params; W = the created width
+bool params_ok(const mccnn_params *o, int W)
+{
+	return o->cbca_i1 >= 0 && o->cbca_i2 >= 0 && o->sgm_i >= 0 && o->border >= 0 && o->border + 1 <= W;
+}
+
+// gaussian(blur_sigma) (main.lua:1078 gaussian(opt.blur_sigma):cuda()) into p->gauss; the buffer grows only when the kernel
+// does not fit the one allocated.  Synchronous: the caller makes sure no enqueued run still reads the buffer.
+int load_gauss(mccnn_pipeline *p, double sigma)
+{
+	const int ks = mccnn_gaussian(sigma, nullptr);
+	const size_t f = sizeof(float);
+	if (ks > p->ks_alloc) {
+		if (p->gauss) {
+			cudaFree(p->gauss);
+			p->bytes -= (size_t)p->ks_alloc * p->ks_alloc * f;
+			p->gauss = nullptr;
+			p->ks_alloc = 0;
+		}
+		int rc = dev_alloc((void **)&p->gauss, (size_t)ks * ks * f, &p->bytes);
+		if (rc) return rc;
+		p->ks_alloc = ks;
+	}
+	float *hk = (float *)malloc((size_t)ks * ks * f);
+	if (!hk) return ADCENSUS_EINVAL;
+	mccnn_gaussian(sigma, hk);
+	int rc = (int)cudaMemcpy(p->gauss, hk, (size_t)ks * ks * f, cudaMemcpyHostToDevice);
+	free(hk);
+	if (!rc) p->ks = ks;
+	return rc;
+}
+
 }  // namespace
 
 extern "C" int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, int W, const mccnn_params *params, int device)
 {
 	if (!out || !params || C < 1 || D < 1 || H < 1 || W < 1) return ADCENSUS_EINVAL;
 	if (C > 128 || D > ADCENSUS_MAX_DISP) return ADCENSUS_ELIMIT;
-	if (params->cbca_i1 < 0 || params->cbca_i2 < 0 || params->sgm_i < 0 || params->border < 0 || params->border + 1 > W)
-		return ADCENSUS_EINVAL;
+	if (!params_ok(params, W)) return ADCENSUS_EINVAL;
 	DeviceGuard g(device);
 	mccnn_pipeline *p = new (std::nothrow) mccnn_pipeline();
 	if (!p) return ADCENSUS_EINVAL;
@@ -201,14 +232,7 @@ extern "C" int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, 
 	if (!rc) rc = dev_alloc((void **)&p->maps, 8 * p->HW * f, &p->bytes);
 	if (!rc) rc = dev_alloc((void **)&p->sgmtab, p->tab_bytes, &p->bytes);
 	if (!rc) rc = encode_maps(p, D, H, W);
-	p->ks = mccnn_gaussian(params->blur_sigma, nullptr);
-	if (!rc) rc = dev_alloc((void **)&p->gauss, (size_t)p->ks * p->ks * f, &p->bytes);
-	if (!rc) {
-		float *hk = (float *)malloc((size_t)p->ks * p->ks * f);
-		mccnn_gaussian(params->blur_sigma, hk);  // main.lua:1078 gaussian(opt.blur_sigma):cuda()
-		rc = (int)cudaMemcpy(p->gauss, hk, (size_t)p->ks * p->ks * f, cudaMemcpyHostToDevice);
-		free(hk);
-	}
+	if (!rc) rc = load_gauss(p, params->blur_sigma);
 	if (rc) {
 		mccnn_pipeline_destroy(p);
 		return rc;
@@ -319,34 +343,74 @@ extern "C" int mccnn_pipeline_set_overlap(mccnn_pipeline *p, int mode)
 
 extern "C" int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p) { return p ? p->launches : 0; }
 
+// Re-targets the pipeline (and every twin lane) to another parameter set.  What create derived from the parameters is
+// derived again: the Gaussian (main.lua:1078) and the tensor maps, whose box and very existence depend on the arm bound
+// max(L1, 2) -- the maps are dropped here and the next run encodes them for its shape, as after a shape change.
+extern "C" int mccnn_pipeline_set_params(mccnn_pipeline *p, const mccnn_params *params)
+{
+	if (!p || !params || !params_ok(params, p->W)) return ADCENSUS_EINVAL;
+	DeviceGuard g(p->device);
+	ADC_CUDA(cudaDeviceSynchronize());                 // enqueued runs read the Gaussian and the parameters' kernel choice
+	for (mccnn_pipeline *q = p; q; q = q->twin) {
+		int rc = load_gauss(q, params->blur_sigma);
+		if (rc) return rc;
+		q->prm = *params;
+		q->ntm = 0;
+		q->tm_D = q->tm_H = q->tm_W = 0;
+	}
+	return 0;
+}
+
 #define STEP(call)                 \
 	do {                       \
 		int rc__ = (call); \
 		if (rc__) return rc__; \
 	} while (0)
 
-// One run at (H, W, D) <= the created shape: every shape-dependent quantity (row pitch, volume size, the offset of the
-// right volume, map offsets, table sizes, tensor maps) is derived here from the run shape, so the buffers hold exactly
-// what a pipeline created at this shape would hold.
-static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
-			   const float *imgL, const float *imgR, float *disp, float *volL, float *volR, cudaStream_t s)
+// A run at (H, W, D) <= the created shape: every shape-dependent quantity (row pitch, volume size, the offset of the
+// right volume, map offsets, table sizes, tensor maps) is derived from the run shape, so the buffers hold exactly
+// what a pipeline created at this shape would hold.  run_fits checks the shape against the allocations and encodes the
+// tensor maps for it; then the volumes are built (run_build_volumes) or copied in (mccnn_pipeline_run_volumes), and
+// run_chain takes them from cross/CBCA to the disparity map.
+static int run_fits(mccnn_pipeline *p, int H, int W, int D)
 {
-	const int C = p->C, ld = (W + 3) & ~3;
+	const int ld = (W + 3) & ~3;
 	const long HW = (long)H * W, V = (long)D * H * ld;
-	const mccnn_params &o = p->prm;
-	int nl = 0;
 	// the allocations were sized for the created shape; check the run's needs against them instead of assuming
 	if (V > p->V || HW > p->HW) return ADCENSUS_ELIMIT;
 	if (adc_packed_words(H, W) + adc_packed_hv_words(H, W) > adc_packed_words(p->H, p->W) + adc_packed_hv_words(p->H, p->W))
 		return ADCENSUS_ELIMIT;
 	if (adc_sgm_table_bytes(H, W, D) > p->tab_bytes || adc_sgm_dhw_table_bytes(H, W, D) > p->tab_bytes) return ADCENSUS_ELIMIT;
 	if (p->tm_D != D || p->tm_H != H || p->tm_W != W) STEP(encode_maps(p, D, H, W));
+	return 0;
+}
 
+// main.lua:946-949: both cost volumes of the pair into the private pitched buffers; returns the number of kernel launches
+static int run_build_volumes(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR, cudaStream_t s,
+			     int *launches)
+{
+	const int C = p->C, ld = (W + 3) & ~3;
+	const long V = (long)D * H * ld;
+	const mccnn_params &o = p->prm;
+	int nl = 0;
 	float *volsL = p->vols, *volsR = p->vols + V;
 	STEP(adc_fill_invalid(volsL, volsR, D, H, W, ld, s)); nl += 1;                                 // main.lua:946 (only what :947 leaves)
 	STEP(adc_stereo_join(featL, featR, volsL, volsR, C, D, H, W, ld, s)); nl += 1;                  // :947
 	STEP(adc_fix_border(volsL, D, H, W, ld, o.border, -1, s));                                    // :948
 	STEP(adc_fix_border(volsR, D, H, W, ld, o.border, 1, s)); nl += o.border ? 2 : 0;             // :949
+	*launches = nl;
+	return 0;
+}
+
+// main.lua:986-1082 from the two volumes in the private buffers (the right one only when it is consumed); nl = the
+// launches that built them
+static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, const float *imgR, float *disp, float *volL,
+		     float *volR, int nl, cudaStream_t s)
+{
+	const int ld = (W + 3) & ~3;
+	const long HW = (long)H * W, V = (long)D * H * ld;
+	const mccnn_params &o = p->prm;
+	float *volsL = p->vols, *volsR = p->vols + V;
 
 	// cross arms: identical for both directions (main.lua:993-996 recomputes them)
 	const int maxlen = pipe_maxlen(p);       // bound on the arm length cross() can produce
@@ -455,6 +519,35 @@ static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *
 	STEP(adcensus_mean2d(m + 6 * HW, p->gauss, disp, H, W, p->ks, o.blur_t, s)); nl += 3;        // :1078
 	p->launches = nl;
 	return 0;
+}
+
+static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+			   const float *imgL, const float *imgR, float *disp, float *volL, float *volR, cudaStream_t s)
+{
+	int nl = 0;
+	STEP(run_fits(p, H, W, D));
+	STEP(run_build_volumes(p, H, W, D, featL, featR, s, &nl));
+	return run_chain(p, H, W, D, imgL, imgR, disp, volL, volR, nl, s);
+}
+
+extern "C" int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
+					  const float *imgL, const float *imgR, float *disp, float *outL, float *outR,
+					  adcensus_stream_t stream)
+{
+	if (!p || !volL || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
+	if (!volR && (p->prm.lr_check || outR)) return ADCENSUS_EINVAL;       // direction +1 is run: it needs its volume
+	if (H < 1 || W < 1 || D < 1 || p->prm.border + 1 > W) return ADCENSUS_EINVAL;
+	if (H > p->H || W > p->W || D > p->D) return ADCENSUS_ELIMIT;
+	DeviceGuard g(p->device);
+	cudaStream_t s = adc_stream(stream);
+	STEP(run_fits(p, H, W, D));
+	const int ld = (W + 3) & ~3;
+	const long V = (long)D * H * ld;
+	const size_t row = (size_t)W * sizeof(float), pitch = (size_t)ld * sizeof(float);
+	ADC_CUDA(cudaMemcpy2DAsync(p->vols, pitch, volL, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
+	if (p->prm.lr_check || outR)                                           // only then is the right volume read
+		ADC_CUDA(cudaMemcpy2DAsync(p->vols + V, pitch, volR, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
+	return run_chain(p, H, W, D, imgL, imgR, disp, outL, outR, 0, s);
 }
 
 extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR,

@@ -206,6 +206,14 @@ class StereoPipeline:
         """True: sgm2 scans the (D,H,ld) layout directly (csrc/sgm_dhw.cu); False (default): permutes around sgm2 as main.lua does"""
         adcensus.lib().mccnn_pipeline_set_sgm_layout(self._h, int(bool(dhw)))
 
+    def set_params(self, params):
+        """Re-target the pipeline to another :class:`Params` (mccnn_pipeline_set_params): later runs give the bits of a
+        pipeline created with them.  Waits for the work enqueued on the pipeline's device."""
+        if not isinstance(params, Params):
+            raise adcensus.AdcensusError("mccnn_pipeline_set_params: a pipeline.Params expected, got %s" % type(params).__name__)
+        adcensus._check(adcensus.lib().mccnn_pipeline_set_params(self._h, ctypes.byref(params)), "mccnn_pipeline_set_params")
+        self.params = params
+
     @property
     def device_bytes(self):
         return adcensus.lib().mccnn_pipeline_device_bytes(self._h)
@@ -251,6 +259,35 @@ class StereoPipeline:
                                                          adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
                                                          adcensus._t(disp, 5, n), vp(volL, 6), vp(volR, 7),
                                                          adcensus._stream(imgL))
+        adcensus._check(rc, n)
+        return disp
+
+    def run_volumes(self, volL, volR, imgL, imgR, disp_max=None, disp=None, outL=None, outR=None):
+        """The chain of :meth:`run_shape` from given cost volumes (mccnn_pipeline_run_volumes): volL / volR (D, H, W) or
+        (1, D, H, W) device tensors as main.lua holds them at :986 (NaN fill, fix_border applied); they are not modified.
+        ``volR`` may be None when the parameters have no LR check and ``outR`` is None.  H, W from ``imgL``, D = ``disp_max``
+        (default: the created D).  Asynchronous on torch's current stream."""
+        n = "mccnn_pipeline_run_volumes"
+        if imgL.dim() != 2:
+            raise adcensus.AdcensusError("%s: imgL must be (H, W), got %s" % (n, tuple(imgL.shape)))
+        H, W = imgL.shape
+        D = self.D if disp_max is None else int(disp_max)
+        if disp is None:
+            disp = torch.empty((H, W), device=imgL.device, dtype=torch.float32)
+        vol = lambda t: t[0] if t is not None and t.dim() == 4 and t.shape[0] == 1 else t
+        volL, volR = vol(volL), vol(volR)
+        want = [("volL", volL, (D, H, W)), ("volR", volR, (D, H, W)), ("imgR", imgR, (H, W)), ("disp", disp, (H, W)),
+                ("outL", outL, (D, H, W)), ("outR", outR, (D, H, W))]
+        for name, t, shape in want:
+            if t is not None and tuple(t.shape) != shape:
+                raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
+        if volR is None and (self.params.lr_check or outR is not None):
+            raise adcensus.AdcensusError("%s: volR is needed (LR check or outR)" % n)
+        vp = lambda t, i: adcensus._t(t, i, n) if t is not None else ctypes.c_void_p(0)
+        ptrs = (adcensus._t(volL, 1, n), vp(volR, 2), adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
+                adcensus._t(disp, 5, n), vp(outL, 6), vp(outR, 7))
+        with torch.cuda.device(imgL.device):
+            rc = adcensus.lib().mccnn_pipeline_run_volumes(self._h, H, W, D, *ptrs, adcensus._stream(imgL))
         adcensus._check(rc, n)
         return disp
 
