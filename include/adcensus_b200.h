@@ -378,6 +378,25 @@ int mccnn_kitti_nnz_count(const float *disp, const float *x0, const int *is_te, 
 int mccnn_kitti_nnz_fill(const float *disp, const float *x0, const int *is_te, int n, int H, int W, float *nnz_tr,
 			 long long cap_tr, float *nnz_te, long long cap_te, adcensus_stream_t stream);
 
+/* ---- the image front end of main.lua -a predict and predict_kitti.lua's error (csrc/frontend.cu) ------------------------
+ * All pointers are DEVICE pointers. */
+
+/* frontend.make_batch (main.lua:1085-1100) on one pair: left / right the decoded 8-bit views, (H, W) grey (nch 1) or (H, W, 3)
+ * interleaved R, G, B (nch 3, through image.rgb2y); x_batch (2, 1, H, W) float32, bit-identical to frontend.make_batch.
+ * Y = 0.299 R, + 0.587 G, + 0.114 B, each product and sum rounded in fp32.  Per view, frontend.standardise: m = sum(y) / n,
+ * y' = y + f32(-m) in fp32, m2 = sum(y') / n, var = sum((y' - m2)^2) / (n - 1), out = y' / f32(sqrt(var)), every sum
+ * numpy's pairwise float64 sum over the view in memory order.  stats (2, 3) float64 receives (m, m2, var) per view: a
+ * constant view has var == 0 (its x_batch plane is then not finite) and the caller must refuse it, as standardise does.
+ * H * W >= 2 (else ADCENSUS_EINVAL), H * W * nch < 2^31 (else ADCENSUS_ELIMIT). */
+int mccnn_frontend_batch(const unsigned char *left, const unsigned char *right, int nch, int H, int W, float *x_batch,
+			 double *stats, adcensus_stream_t stream);
+
+/* dataio.bad_pixel_rate's counts for one map (predict_kitti.lua:62-70): disp (H, W) float32, gt (H, W) the PNG16 ground
+ * truth as stored (uint16, disparity * 256, 0 = invalid).  counts[0] = #(gt != 0 and |gt / 256 - disp| > err_at) in fp32
+ * (a NaN disparity is not bad), counts[1] = #(gt != 0); DEVICE int64, overwritten.  The error is counts[0] / counts[1]. */
+int mccnn_kitti_error_count(const float *disp, const unsigned short *gt, int H, int W, float err_at, long long *counts,
+			    adcensus_stream_t stream);
+
 /* ---- Middlebury views, halving, masks and training-sample lists (csrc/preprocess_mb.cu, preprocess_mb.py) ---------------
  * All pointers are DEVICE pointers; images are 8-bit (n, H, W, 3) in R, G, B order (a grey file replicated to three
  * channels, as cv2.imread does). */

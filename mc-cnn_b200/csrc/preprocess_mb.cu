@@ -4,7 +4,8 @@
 //   (x - x.mean()) / x.std() exactly as numpy computes it in float32: numpy's pairwise sum over the array in memory order
 //   (pixels, channels interleaved for rgb), the two quotients by the element count in float64 rounded to float32 (numpy
 //   divides a float32 by an intp), a float32 sqrt and IEEE float32 subtraction and division.  One thread per leaf of the
-//   pairwise tree (<= 128 elements), then the fixed combine tree, one block per view: deterministic, bit-identical.
+//   pairwise tree (<= 128 elements), then the fixed combine tree, one block per view (pairwise.cuh): deterministic,
+//   bit-identical.
 // * mccnn_mb_half_image: `convert X -resize 50%` restated (Lanczos-3, renormalised at the border, fp32, rounded half up).
 //   ImageMagick is not pinned: this is a restatement of its documented filter, not a bit-for-bit copy.
 // * mccnn_mb_half_disp: load_pfm(.., True) (:13-26): x / 2, then the second smallest of each 2x2 block in np.sort order.
@@ -18,11 +19,10 @@
 #include <vector>
 
 #include "common.cuh"
+#include "pairwise.cuh"
 
 namespace {
 
-constexpr int LEAF = 128;                 // numpy's PW_BLOCKSIZE
-constexpr int COMBINE_THREADS = 1024;
 constexpr int ROW_THREADS = 256;
 constexpr int ROW_WARPS = ROW_THREADS / 32;
 constexpr int SCAN_THREADS = 1024;
@@ -47,59 +47,33 @@ __device__ __forceinline__ float element(const unsigned char *v, long i, float m
 	return __fmul_rn(d, d);
 }
 
-// numpy's pairwise_sum below PW_BLOCKSIZE: sequential under 8 elements, else eight strided accumulators combined as
-// ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)) and the remainder added in turn
+// element i of view `view` minus its mean and squared when SQUARE: the terms of np.mean / np.std's pairwise sums
 template <int C, bool SQUARE>
-__global__ void leaf_kernel(const unsigned char *__restrict__ rgb, long view_bytes, const int2 *__restrict__ leaves, int nleaf,
-			    int nval, float *__restrict__ val, const float *__restrict__ stats)
-{
-	const int k = blockIdx.x * blockDim.x + threadIdx.x;
-	if (k >= nleaf) return;
-	const int view = blockIdx.y;
-	const unsigned char *v = rgb + view * view_bytes;
-	const float m = SQUARE ? stats[2 * view] : 0.f;
-	const long a = leaves[k].x;
-	const int n = leaves[k].y;
-	float res = 0.f;
-	if (n < 8) {
-		for (int i = 0; i < n; i++) res = __fadd_rn(res, element<C, SQUARE>(v, a + i, m));
-	} else {
-		float r[8];
-#pragma unroll
-		for (int j = 0; j < 8; j++) r[j] = element<C, SQUARE>(v, a + j, m);
-		const int body = n - n % 8;
-		for (int i = 8; i < body; i += 8) {
-#pragma unroll
-			for (int j = 0; j < 8; j++) r[j] = __fadd_rn(r[j], element<C, SQUARE>(v, a + i + j, m));
-		}
-		res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-				__fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-		for (int i = body; i < n; i++) res = __fadd_rn(res, element<C, SQUARE>(v, a + i, m));
+struct ViewElem {
+	const unsigned char *rgb;
+	long view_bytes;
+	const float *stats;
+	__device__ float operator()(int view, long i) const
+	{
+		return element<C, SQUARE>(rgb + view * view_bytes, i, SQUARE ? stats[2 * view] : 0.f);
 	}
-	val[(long)view * nval + k] = res;
-}
+};
 
-// The internal nodes sorted by height: level h (1..) holds the nodes lev_off[h-1] .. lev_off[h]-1 (ids nleaf + index), each
-// the float32 sum of its two children.  The root is the last node.  Then stats[2 view] = mean or stats[2 view + 1] = std.
+// stats[2 view] = the mean, or stats[2 view + 1] = the std when SQUARE: the sum / count in float64 rounded to float32 (numpy
+// divides a float32 by an intp), then a float32 sqrt
 template <bool SQUARE>
-__global__ void __launch_bounds__(COMBINE_THREADS) combine_kernel(const int2 *__restrict__ child, const int *__restrict__ lev_off,
-								  int nlev, int nleaf, int nval, float *__restrict__ val,
-								  float *__restrict__ stats, long count)
-{
-	float *v = val + (long)blockIdx.x * nval;
-	for (int h = 0; h < nlev; h++) {
-		for (int k = lev_off[h] + threadIdx.x; k < lev_off[h + 1]; k += COMBINE_THREADS)
-			v[nleaf + k] = __fadd_rn(v[child[k].x], v[child[k].y]);
-		__syncthreads();
-	}
-	if (threadIdx.x == 0) {
-		const float s = (float)((double)v[nval - 1] / (double)count);     // float32 / intp in float64, rounded to float32
+struct ViewFinish {
+	float *stats;
+	long count;
+	__device__ void operator()(int view, float sum) const
+	{
+		const float s = (float)((double)sum / (double)count);
 		if (SQUARE)
-			stats[2 * blockIdx.x + 1] = __fsqrt_rn(s);
+			stats[2 * view + 1] = __fsqrt_rn(s);
 		else
-			stats[2 * blockIdx.x] = s;
+			stats[2 * view] = s;
 	}
-}
+};
 
 template <int C>
 __global__ void normalise_kernel(const unsigned char *__restrict__ rgb, float *__restrict__ out, const float *__restrict__ stats,
@@ -117,80 +91,16 @@ __global__ void normalise_kernel(const unsigned char *__restrict__ rgb, float *_
 	}
 }
 
-// numpy's pairwise split: n > 128 -> [0, n2) and [n2, n), n2 = n / 2 rounded down to a multiple of 8
-struct PairwiseTree {
-	std::vector<int2> leaves;                   // (start, length)
-	std::vector<std::vector<int4>> levels;      // per height - 1: (left height, left index, right height, right index)
-
-	// returns (height, index within that height); height 0 = leaf
-	int2 build(long a, long n)
-	{
-		if (n <= LEAF) {
-			leaves.push_back(make_int2((int)a, (int)n));
-			return make_int2(0, (int)leaves.size() - 1);
-		}
-		long n2 = n / 2;
-		n2 -= n2 % 8;
-		const int2 l = build(a, n2), r = build(a + n2, n - n2);
-		const int h = (l.x > r.x ? l.x : r.x) + 1;
-		if ((int)levels.size() < h) levels.resize(h);
-		levels[h - 1].push_back(make_int4(l.x, l.y, r.x, r.y));
-		return make_int2(h, (int)levels[h - 1].size() - 1);
-	}
-};
-
-int pairwise_stats(const unsigned char *rgb, int n, long hw, int C, float *stats, cudaStream_t s)
+template <int C>
+int pairwise_stats(const unsigned char *rgb, int n, long hw, float *stats, cudaStream_t s)
 {
-	const long count = hw * C;
-	PairwiseTree t;
-	t.build(0, count);
-	const int nleaf = (int)t.leaves.size();
-	std::vector<int> lev_off(1, 0);
-	for (auto &l : t.levels) lev_off.push_back(lev_off.back() + (int)l.size());
-	const int ninner = lev_off.back(), nlev = (int)t.levels.size();
-	std::vector<int2> child(ninner);
-	auto id = [&](int h, int k) { return h == 0 ? k : nleaf + lev_off[h - 1] + k; };
-	for (int h = 1; h <= nlev; h++)
-		for (size_t k = 0; k < t.levels[h - 1].size(); k++) {
-			const int4 c = t.levels[h - 1][k];
-			child[lev_off[h - 1] + k] = make_int2(id(c.x, c.y), id(c.z, c.w));
-		}
-	const int nval = nleaf + ninner;
-
-	const size_t b_leaves = sizeof(int2) * nleaf, b_child = sizeof(int2) * (ninner + 1),
-		     b_lev = sizeof(int) * lev_off.size(), b_val = sizeof(float) * (size_t)nval * n;
-	char *scratch = nullptr;
-	int rc = adc_scratch_alloc((void **)&scratch, b_leaves + b_child + b_lev + b_val, s);
-	if (rc) return rc;
-	int2 *d_leaves = (int2 *)scratch, *d_child = (int2 *)(scratch + b_leaves);
-	int *d_lev = (int *)(scratch + b_leaves + b_child);
-	float *d_val = (float *)(scratch + b_leaves + b_child + b_lev);
-	// pageable sources: cudaMemcpyAsync returns once they are staged, so the vectors may go out of scope
-	cudaError_t e = cudaMemcpyAsync(d_leaves, t.leaves.data(), b_leaves, cudaMemcpyHostToDevice, s);
-	if (e == cudaSuccess && ninner)
-		e = cudaMemcpyAsync(d_child, child.data(), sizeof(int2) * ninner, cudaMemcpyHostToDevice, s);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d_lev, lev_off.data(), b_lev, cudaMemcpyHostToDevice, s);
-	if (e == cudaSuccess) {
-		const dim3 grid((nleaf + 255) / 256, n);
-		const long view_bytes = hw * 3;
-		for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {
-			if (C == 1 && pass == 0)
-				leaf_kernel<1, false><<<grid, 256, 0, s>>>(rgb, view_bytes, d_leaves, nleaf, nval, d_val, stats);
-			else if (C == 1)
-				leaf_kernel<1, true><<<grid, 256, 0, s>>>(rgb, view_bytes, d_leaves, nleaf, nval, d_val, stats);
-			else if (pass == 0)
-				leaf_kernel<3, false><<<grid, 256, 0, s>>>(rgb, view_bytes, d_leaves, nleaf, nval, d_val, stats);
-			else
-				leaf_kernel<3, true><<<grid, 256, 0, s>>>(rgb, view_bytes, d_leaves, nleaf, nval, d_val, stats);
-			if (pass == 0)
-				combine_kernel<false><<<n, COMBINE_THREADS, 0, s>>>(d_child, d_lev, nlev, nleaf, nval, d_val, stats, count);
-			else
-				combine_kernel<true><<<n, COMBINE_THREADS, 0, s>>>(d_child, d_lev, nlev, nleaf, nval, d_val, stats, count);
-			e = cudaPeekAtLastError();
-		}
-	}
-	int rf = adc_scratch_free(scratch, s);
-	return e != cudaSuccess ? (int)e : rf;
+	const long count = hw * C, view_bytes = hw * 3;
+	pairwise::Sum<float> t;
+	int rc = t.init(count, n, s);
+	if (!rc) rc = t.sum(ViewElem<C, false>{rgb, view_bytes, stats}, ViewFinish<false>{stats, count});
+	if (!rc) rc = t.sum(ViewElem<C, true>{rgb, view_bytes, stats}, ViewFinish<true>{stats, count});
+	const int rf = t.release();
+	return rc ? rc : rf;
 }
 
 // ---- halving ------------------------------------------------------------------------------------------------------
@@ -422,7 +332,7 @@ extern "C" int mccnn_mb_views(const unsigned char *rgb, float *out, int n, int H
 	float *stats = nullptr;
 	int rc = adc_scratch_alloc((void **)&stats, sizeof(float) * 2 * n, s);
 	if (rc) return rc;
-	rc = pairwise_stats(rgb, n, hw, nchannel, stats, s);
+	rc = nchannel == 1 ? pairwise_stats<1>(rgb, n, hw, stats, s) : pairwise_stats<3>(rgb, n, hw, stats, s);
 	if (!rc) {
 		const dim3 grid((unsigned)std::min<long>((hw + 255) / 256, 4096), n);
 		if (nchannel == 1)

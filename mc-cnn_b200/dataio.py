@@ -53,14 +53,19 @@ def tofile(fname, x):
     open(fname + ".dim", "w").write("\n".join(map(str, x.shape)))
 
 
-def read_png16(fname):
-    """adcensus.cu:1670-1686: 16-bit grey PNG -> float32 (H,W), 0 stays 0 (invalid), else value / 256"""
+def read_png16_raw(fname):
+    """the stored uint16 (H,W) values of a 16-bit grey PNG (disparity * 256, 0 = invalid)"""
     from PIL import Image
 
     with Image.open(fname) as im:
         if im.mode not in ("I;16", "I;16B", "I"):
             raise ValueError("%s: 16-bit grey PNG expected, got mode %s" % (fname, im.mode))
-        v = np.asarray(im).astype(np.uint16)
+        return np.asarray(im).astype(np.uint16)
+
+
+def read_png16(fname):
+    """adcensus.cu:1670-1686: 16-bit grey PNG -> float32 (H,W), 0 stays 0 (invalid), else value / 256"""
+    v = read_png16_raw(fname)
     return np.where(v == 0, np.float32(0.0), v.astype(np.float32) / np.float32(256.0)).astype(np.float32)
 
 

@@ -17,19 +17,28 @@ import os
 import numpy as np
 
 
-def load_image(path):
-    """``image.load(path, nil, 'byte'):float()``: (C,H,W) float32 with the byte values 0..255
-    (C = 1 for grey files, 3 for colour; an alpha channel is dropped)."""
+def load_bytes(path):
+    """The decoded 8-bit image of ``image.load(path, nil, 'byte')``: (H, W) uint8 for grey files, (H, W, 3) interleaved R, G, B
+    for colour (an alpha channel is dropped); a 16-bit file keeps its high byte."""
     from PIL import Image
 
     with Image.open(path) as im:
         if im.mode in ("I;16", "I;16B", "I"):            # 16-bit grey: 'byte' loading keeps the high byte
-            a = (np.asarray(im, dtype=np.uint32) >> 8).astype(np.float32)[None]
-        elif im.mode in ("L", "1", "P", "LA"):
-            a = np.asarray(im.convert("L"), dtype=np.uint8).astype(np.float32)[None]
-        else:
-            a = np.asarray(im.convert("RGB"), dtype=np.uint8).astype(np.float32).transpose(2, 0, 1)
-    return np.ascontiguousarray(a)
+            a = np.asarray(im, dtype=np.uint32) >> 8
+            if a.size and a.max() > 255:
+                raise ValueError("%s: more than 16 bits per pixel" % path)
+            return a.astype(np.uint8)
+        if im.mode in ("L", "1", "P", "LA"):
+            return np.array(im.convert("L"), dtype=np.uint8)
+        return np.array(im.convert("RGB"), dtype=np.uint8)
+
+
+def load_image(path):
+    """``image.load(path, nil, 'byte'):float()``: (C,H,W) float32 with the byte values 0..255
+    (C = 1 for grey files, 3 for colour; an alpha channel is dropped)."""
+    a = load_bytes(path)
+    a = a[None] if a.ndim == 2 else a.transpose(2, 0, 1)
+    return np.ascontiguousarray(a.astype(np.float32))
 
 
 def rgb2y(x):
@@ -69,6 +78,41 @@ def make_batch(left, right):
         out.append(standardise(a))                                              # :1094-1095
     assert out[0].shape == out[1].shape, "the two views must have the same size"
     return np.ascontiguousarray(np.stack(out))                                  # :1097-1100
+
+
+def make_batch_cuda(left, right, device=0):
+    """:func:`make_batch` on the GPU (csrc/frontend.cu, mccnn_frontend_batch), bit-identical to it: `left` / `right` the decoded
+    views as :func:`load_bytes` returns them, (H, W) or (H, W, 3) uint8 numpy arrays or torch tensors (host or device), both
+    grey or both colour.  Only the bytes are copied to `device` (a torch.device or index); returns x_batch (2,1,H,W) CUDA
+    float32.  Waits for the two views' statistics and refuses a constant view, as :func:`standardise` does."""
+    import ctypes
+
+    import torch
+
+    from .adcensus import _check, _stream, lib
+
+    dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+    views = [v if isinstance(v, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(v)) for v in (left, right)]
+    for name, v in zip(("left", "right"), views):
+        if v.dtype != torch.uint8 or not (v.dim() == 2 or (v.dim() == 3 and v.size(2) == 3)):
+            raise ValueError("%s view: (H, W) or (H, W, 3) uint8 expected, got %s %s" % (name, v.dtype, tuple(v.shape)))
+    if views[0].shape != views[1].shape:
+        raise ValueError("the two views must have the same size and channels, got %s and %s"
+                         % (tuple(views[0].shape), tuple(views[1].shape)))
+    H, W = views[0].shape[:2]
+    nch = 1 if views[0].dim() == 2 else 3
+    with torch.cuda.device(dev):
+        views = [v.to(dev).contiguous() for v in views]
+        x_batch = torch.empty((2, 1, H, W), dtype=torch.float32, device=dev)
+        stats = torch.empty((2, 3), dtype=torch.float64, device=dev)
+        p = lambda t: ctypes.c_void_p(t.data_ptr())
+        _check(lib().mccnn_frontend_batch(p(views[0]), p(views[1]), nch, H, W, p(x_batch), p(stats), _stream(x_batch)),
+               "mccnn_frontend_batch")
+        var = stats[:, 2].cpu()
+    for name, v in zip(("left", "right"), var.tolist()):
+        if not v > 0:
+            raise ValueError("%s view: constant image (standardise needs a non-zero variance)" % name)
+    return x_batch
 
 
 def write_bin(path, t):

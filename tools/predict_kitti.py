@@ -1,0 +1,69 @@
+"""predict_kitti.lua: a trained net over every full-size raw KITTI pair, in one process per GPU.
+
+    python tools/predict_kitti.py test   kitti     -net_fname net/net_kitti_fast_-a_train_all.t7 -data_root /data
+    python tools/predict_kitti.py submit kitti2015 -net_fname N -data_root /data -out out [-arch fast|slow|census|ad] \\
+        [-disp_max 228] [-gpu 1]
+    torchrun --nproc-per-node 8 tools/predict_kitti.py test kitti -net_fname N -data_root /data
+
+`test` prints ``i<TAB>err`` for every training pair (0-based), then the mean 3-pixel error; `submit` writes
+``out/%06d_10.png`` (kitti) or ``out/disp_0/%06d_10.png`` (kitti2015) for every testing pair and prints its index.  The raw
+archives are read from ``<data_root>/data.kitti/unzip`` or ``data.kitti2015/unzip``, as preprocess_kitti.py reads them.
+-gpu is 1-based as in main.lua.  Under torchrun each process takes the GPU of its LOCAL_RANK and the pairs are shared
+round-robin; the output is the one a single process prints.  See mc-cnn_b200/predict_kitti.py.
+"""
+import argparse
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def parser():
+    ap = argparse.ArgumentParser(prog="predict_kitti.py", description=__doc__.splitlines()[0])
+    ap.add_argument("action", choices=("test", "submit"))
+    ap.add_argument("dataset", choices=("kitti", "kitti2015"))
+    ap.add_argument("-net_fname", default="")
+    ap.add_argument("-arch", choices=("fast", "slow", "census", "ad"), default="fast")
+    ap.add_argument("-data_root", default=".")
+    ap.add_argument("-out", default="out")
+    ap.add_argument("-disp_max", type=int, default=228)
+    ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    return ap
+
+
+def parse_args(argv=None):
+    """Refuses what cannot run before any file or GPU is touched."""
+    args = parser().parse_args(argv)
+    if args.arch in ("fast", "slow") and not args.net_fname:
+        raise SystemExit("predict_kitti.py: arch '%s' needs -net_fname" % args.arch)
+    if args.disp_max < 1:
+        raise SystemExit("predict_kitti.py: -disp_max must be at least 1")
+    if args.gpu < 1:
+        raise SystemExit("predict_kitti.py: -gpu is 1-based")
+    return args
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    import torch.distributed as dist
+
+    import mccnn_b200  # noqa: F401
+    from mccnn_b200.predict_kitti import predict_kitti
+
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    device = args.gpu - 1
+    if world > 1:
+        # only two counts (or one index) per pair cross between processes: gloo on the host is enough
+        dist.init_process_group("gloo")
+        device = int(os.environ.get("LOCAL_RANK", "0"))
+    try:
+        predict_kitti(args.action, args.dataset, net_fname=args.net_fname or None, arch=args.arch, data_root=args.data_root,
+                      out=args.out, disp_max=args.disp_max, device=device)
+    finally:
+        if world > 1:
+            dist.destroy_process_group()
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
