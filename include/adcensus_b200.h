@@ -432,6 +432,67 @@ int mccnn_mb_nnz_count(const unsigned char *mask, int H, int W, long long *count
 int mccnn_mb_nnz_fill(const float *d0, const unsigned char *mask, int H, int W, int image, float *dispnoc, float *nnz,
 		      long long cap, adcensus_stream_t stream);
 
+/* ---- training of the fast architecture (csrc/train.cu, train.py; main.lua:602-890) ------------------------------------
+ * Patches are ws x ws, ws = 1 + 2 l1; a batch of bs pairs is N = 2 bs patches, sample i owning patches 4i .. 4i + 3
+ * (main.lua:843-846).  Pointers may be host or device unless noted (copies use cudaMemcpyDefault). */
+
+/* One patch of make_patch (main.lua:607-619): m the forward 2x3 matrix as stored in the FloatTensor, contrast and
+ * brightness as float, image the 0-based index into X0 / X1 ((n_img, 1, H, W) float32), view 0 = X0, 1 = X1. */
+typedef struct {
+	float m[6];
+	float contrast, brightness;
+	int image, view;
+} mccnn_warp;
+
+/* The sampler alone: out (n, ws, ws) = warpAffine(X[image], m, (ws, ws), INTER_CUBIC, BORDER_CONSTANT 0) * contrast +
+ * brightness, bit-identical to OpenCV's float path as oracle/train.py restates it.  DEVICE pointers; an image index
+ * outside [0, n_img) gives a NaN patch. */
+int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n, int ws,
+		       float *out, adcensus_stream_t stream);
+
+typedef struct mccnn_trainer mccnn_trainer;
+
+/* net_tr of arch 'fast' (l1 valid 3x3 convolutions 1 -> fm -> .. -> fm, ReLU between them, Normalize2, StereoJoin1) with
+ * Margin2(margin, pow) and momentum `mom`, for batches of bs pairs, sampling from the DEVICE images X0 / X1 (kept by the
+ * caller for the trainer's lifetime).  Parameters, momenta and gradients are one flat fp32 vector each: per layer W
+ * (fm, cin, 3, 3) then b (fm), layer 1 first; all start at 0.  `chunk` bounds the steps of one mccnn_trainer_run,
+ * `loss_cap` the per-step losses kept between two mccnn_trainer_reset_losses.  The step is captured once into a CUDA graph
+ * of mccnn_trainer_launches_per_step kernels; it has no floating-point atomics, so equal inputs give equal bits.
+ * bs even, l1 <= 8, fm <= 128 (else ADCENSUS_ELIMIT, also when a patch's activations exceed shared memory). */
+int mccnn_trainer_create(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom, const float *X0,
+			 const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
+			 adcensus_stream_t stream);
+int mccnn_trainer_destroy(mccnn_trainer *h);
+
+/* nsteps <= chunk training steps: warps (nsteps, N) mccnn_warp (pinned host or device; it must stay unchanged until the
+ * copy has run on `stream`), then per step the sampler, forward, backward and the update with the scalar (float)(-lr).
+ * Each step's loss (Margin2's mean) goes to the next entry of the loss buffer.  Asynchronous. */
+int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr, adcensus_stream_t stream);
+
+/* One step from given patches ((N, 1, ws, ws) float32) instead of the sampler. */
+int mccnn_trainer_step_patches(mccnn_trainer *h, const float *patches, double lr, adcensus_stream_t stream);
+
+/* The trainer's buffers, for get / set (set: PARAMS and MOMENTA only) and the tests.  Sizes in floats from
+ * mccnn_trainer_size.  TOWER: every layer's output, layer k (N, fm, s_k, s_k) after the previous layers, s_k = ws - 2k, post
+ * ReLU except the last; DZ: the gradient of the loss wrt each layer's pre-activation output, same layout; NORM (N) = sum of
+ * squares + 1e-5; NORMALIZED (N, fm); JOIN (bs); JOIN_GRAD (bs) Margin2's gradInput / (bs / 2); HINGE (bs / 2);
+ * NORM_GRAD_OUT (N, fm) the gradient wrt Normalize2's output; LOSS (loss_cap). */
+enum {
+	MCCNN_TRAIN_PARAMS, MCCNN_TRAIN_MOMENTA, MCCNN_TRAIN_GRADS, MCCNN_TRAIN_PATCHES, MCCNN_TRAIN_TOWER, MCCNN_TRAIN_NORM,
+	MCCNN_TRAIN_NORMALIZED, MCCNN_TRAIN_JOIN, MCCNN_TRAIN_JOIN_GRAD, MCCNN_TRAIN_HINGE, MCCNN_TRAIN_NORM_GRAD_OUT,
+	MCCNN_TRAIN_DZ, MCCNN_TRAIN_LOSS, MCCNN_TRAIN_NBUF
+};
+long long mccnn_trainer_size(mccnn_trainer *h, int what);
+int mccnn_trainer_get(mccnn_trainer *h, int what, float *dst, adcensus_stream_t stream);
+int mccnn_trainer_set(mccnn_trainer *h, int what, const float *src, adcensus_stream_t stream);
+/* the next step's loss goes to entry 0 of the loss buffer */
+int mccnn_trainer_reset_losses(mccnn_trainer *h, adcensus_stream_t stream);
+int mccnn_trainer_launches_per_step(mccnn_trainer *h);
+
+/* HOST helper: the swaps i = i0 .. i0 + k - 1 of THTensor_(randperm) on perm (n) int64: swap perm[i] and
+ * perm[i + draws[j] % (n - i)], draws the generator's 32-bit outputs in order (i0 + k <= n - 1). */
+int mccnn_randperm_swaps(long long *perm, long long n, long long i0, const unsigned *draws, long long k);
+
 #ifdef __cplusplus
 }
 #endif

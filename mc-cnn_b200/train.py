@@ -1,0 +1,459 @@
+"""main.lua's ``-a train_tr`` / ``-a train_all`` (main.lua:602-890) for the fast architecture on KITTI 2012 / 2015.
+
+    opt = options("kitti", lr=0.002)                                   # main.lua's presets (:34-49, :206-262) + overrides
+    fname = train("kitti", "train_tr", opt, data_root=".", seed=42)   # 14 epochs, net/net_<cmd_str>.t7, then test_te
+
+Per step (bs / 2 samples of four ws x ws patches, ws = 1 + 2 l1): the host draws the augmentation parameters and builds each
+patch's float 2x3 matrix as make_patch does (:607-619); the GPU (csrc/train.cu) warps the patches out of the device-resident
+X0 / X1 (OpenCV's cubic warpAffine, restated bit for bit), runs net_tr forward and backward with Margin2 and applies the
+momentum update, as one CUDA graph.  The host builds the next chunk of steps while the GPU runs the current one, and reads
+the per-step losses once per epoch.
+
+Random numbers: one Torch7 stream, ``torch.manualSeed(seed)`` (:340) -- MT19937 after init_genrand(seed), which numpy's
+``MT19937._legacy_seeding`` reproduces -- consumed as main.lua consumes it: ``torch.randperm(#nnz)`` once (:657), each
+convolution's reset() (weight then bias, U(-1/sqrt(9 cin), +1/sqrt(9 cin)) in double, stored as float), then per sample the
+torch.uniform calls of :791-818 in order, each r / 2^32 * (b - a) + a in double (the flip draws only with -hflip / -vflip 1).
+Torch7 is not available to compare against, so parity with Torch7 itself is **unpinned**, as in :mod:`preprocess`; the stream
+is pinned against ``preprocess.MT19937`` and the line-by-line restatement in oracle/train.py.
+
+Deliberate deviations from main.lua:
+
+* only arch 'fast' and datasets kitti / kitti2015; ``-at 1``, ``-subset`` < 1 and ``-debug`` are refused;
+* the net file goes to ``<data_root>/net/`` and an existing file is refused; the file name is built from main.lua's options
+  only (``-data_root`` and ``-out`` are not part of it);
+* Margin2's loss is the hinge terms summed in order, then divided by bs / 2 (Torch7's ``mean`` reduces in another order),
+  and the convolutions accumulate in another order than cuDNN: both are fp32.
+"""
+import ctypes
+import math
+import os
+import time
+
+import numpy as np
+
+from . import evaluate
+
+EPOCHS = 14                                  # main.lua:779
+LR_DROP_EPOCH = 12                           # :783-785
+CHUNK = 256                                  # steps per host -> device copy of the warp parameters
+TWO32 = 1.0 / 4294967296.0
+
+# main.lua:34-49 (KITTI augmentation) and :206-262 (arch 'fast', kitti / kitti2015: the same training options)
+AUGMENT = dict(hflip=0, vflip=0, rotate=7.0, hscale=0.9, scale=1.0, trans=0.0, hshear=0.1, brightness=0.7, contrast=1.3,
+               d_vtrans=0.0, d_rotate=0.0, d_hscale=1.0, d_hshear=0.0, d_brightness=0.3, d_contrast=1.0)
+NET = dict(at=0, m=0.2, pow=1, l1=4, fm=64, ks=3, lr=0.002, bs=128, mom=0.9, true1=1.0, false1=4.0, false2=10.0)
+WARP_DTYPE = np.dtype([("m", "<f4", (6,)), ("contrast", "<f4"), ("brightness", "<f4"), ("image", "<i4"), ("view", "<i4")])
+TRAIN_PARAMS, TRAIN_MOMENTA, TRAIN_GRADS, TRAIN_PATCHES, TRAIN_TOWER, TRAIN_NORM, TRAIN_NORMALIZED, TRAIN_JOIN, \
+    TRAIN_JOIN_GRAD, TRAIN_HINGE, TRAIN_NORM_GRAD_OUT, TRAIN_DZ, TRAIN_LOSS = range(13)
+
+
+def options(dataset, arch="fast", **overrides):
+    """main.lua's training options for (dataset, arch) with `overrides`; refuses what this module does not train"""
+    if dataset == "mb":
+        raise ValueError("dataset mb: Middlebury training (the light and exposure sampler) is not supported")
+    if dataset not in ("kitti", "kitti2015"):
+        raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
+    if arch != "fast":
+        raise ValueError("arch %s: only the fast architecture can be trained" % arch)
+    o = dict(AUGMENT, **NET)
+    for k, v in overrides.items():
+        if k not in o:
+            raise ValueError("unknown training option -%s" % k)
+        o[k] = type(o[k])(v)
+    check(o)
+    return o
+
+
+def check(o):
+    """main.lua's asserts (:797, :810) and the limits of csrc/train.cu and the inference feature tower"""
+    if o["at"]:
+        raise ValueError("-at 1 (the combined KITTI 2012 + 2015 training set) is not supported")
+    if o["ks"] != 3:
+        raise ValueError("-ks %d: only 3x3 kernels are supported" % o["ks"])
+    if not 1 <= o["l1"] <= 8:
+        raise ValueError("-l1 %d: 1 to 8 layers are supported" % o["l1"])
+    if o["fm"] < 16 or o["fm"] > 128 or o["fm"] % 16:
+        raise ValueError("-fm %d: the feature tower runs 16 to 128 planes in steps of 16" % o["fm"])
+    if o["bs"] < 2 or o["bs"] % 2:
+        raise ValueError("-bs %d: the batch size must be even and at least 2" % o["bs"])
+    if o["pow"] not in (1, 2):
+        raise ValueError("-pow %d: Margin2 takes pow 1 or 2" % o["pow"])
+    if not (o["hscale"] <= 1 and o["scale"] <= 1):
+        raise ValueError("-hscale and -scale must be <= 1 (main.lua:797)")
+    if not (o["contrast"] >= 1 and o["d_contrast"] >= 1):
+        raise ValueError("-contrast and -d_contrast must be >= 1 (main.lua:810)")
+
+
+def steps_per_epoch(n, bs):
+    """the iterations of ``for t = 1, n - bs/2, bs/2`` (main.lua:789)"""
+    h = bs // 2
+    return max(0, (n - h - 1) // h + 1) if n - h >= 1 else 0
+
+
+def lr_at(lr, epoch):
+    """opt.lr during `epoch` (1-based): divided by 10 from epoch 12 on (main.lua:783-785)"""
+    return lr / 10 if epoch >= LR_DROP_EPOCH else lr
+
+
+def cmd_str(dataset, args):
+    """save_net's name stem (main.lua:344-347): dataset_arch then '_' + each further argument"""
+    return "_".join([dataset, "fast"] + list(args))
+
+
+def net_lines(o):
+    """print_net(net_tr) (main.lua:542-564, 751)"""
+    out = []
+    for i in range(o["l1"]):
+        out.append("conv(in=%d, out=%d, k=%d)" % (1 if i == 0 else o["fm"], o["fm"], o["ks"]))
+        if i < o["l1"] - 1:
+            out.append("cudnn.ReLU")
+    return out + ["nn.Normalize2", "nn.StereoJoin1"]
+
+
+def epoch_line(epoch, err, lr, seconds):
+    """``print(epoch, err_tr / err_tr_cnt, opt.lr, sys.clock() - time)`` (main.lua:880)"""
+    return "\t".join(evaluate.lua_num(v) for v in (epoch, err, lr, seconds))
+
+
+class Stream:
+    """Torch7's generator after ``torch.manualSeed(seed)``: numpy's MT19937 with init_genrand seeding."""
+
+    def __init__(self, seed):
+        self.bg = np.random.MT19937()
+        self.bg._legacy_seeding(seed)
+
+    def raw(self, n):
+        return self.bg.random_raw(n).astype(np.uint32)
+
+    def uniform(self, n, a, b):
+        return self.raw(n) * TWO32 * (b - a) + a
+
+
+def randperm(stream, n):
+    """``torch.randperm(n)`` as 1-based int64 (THTensor_(randperm): n - 1 swaps, one draw each)"""
+    from .adcensus import _check, lib
+
+    perm = np.arange(n, dtype=np.int64)
+    step = 1 << 22
+    for i0 in range(0, max(n - 1, 0), step):
+        k = min(step, n - 1 - i0)
+        d = np.ascontiguousarray(stream.raw(k))
+        _check(lib().mccnn_randperm_swaps(perm.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(n), ctypes.c_longlong(i0),
+                                          d.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(k)), "randperm")
+    return perm + 1
+
+
+def init_weights(stream, l1, fm, n_in=1, ks=3):
+    """each convolution's reset() in order -> [(W (fm, cin, ks, ks), b (fm,))] float32"""
+    out = []
+    for i in range(l1):
+        cin = n_in if i == 0 else fm
+        stdv = 1 / math.sqrt(ks * ks * cin)
+        w = stream.uniform(fm * cin * ks * ks, -stdv, stdv).astype(np.float32).reshape(fm, cin, ks, ks)
+        b = stream.uniform(fm, -stdv, stdv).astype(np.float32)
+        out.append((w, b))
+    return out
+
+
+def draw_params(stream, o, n):
+    """the torch.uniform calls of main.lua:791-818 for n samples -> dict of float64 arrays (n,) (scale, trans pairs as
+    two arrays)"""
+    cols = ["d_pos", "d_neg", "neg", "s", "hscale"] + (["hflip"] if o["hflip"] == 1 else []) + \
+        (["vflip"] if o["vflip"] == 1 else []) + ["hshear", "trans0", "trans1", "phi", "brightness", "contrast",
+                                                  "d_hscale", "d_hshear", "d_vtrans", "d_rotate", "d_brightness",
+                                                  "d_contrast"]
+    r = stream.raw(n * len(cols)).reshape(n, len(cols)).astype(np.float64) * TWO32
+    c = {k: r[:, j] for j, k in enumerate(cols)}
+    u = lambda k, a, b: c[k] * (b - a) + a
+    p = {}
+    p["d_pos"] = u("d_pos", -o["true1"], o["true1"])
+    d_neg = u("d_neg", o["false1"], o["false2"])
+    p["d_neg"] = np.where(c["neg"] < 0.5, -d_neg, d_neg)
+    s = u("s", o["scale"], 1)
+    sc0, sc1 = s * u("hscale", o["hscale"], 1), s
+    if o["hflip"] == 1:
+        sc0 = np.where(c["hflip"] < 0.5, -sc0, sc0)
+    if o["vflip"] == 1:
+        sc1 = np.where(c["vflip"] < 0.5, -sc1, sc1)
+    p["scale"] = (sc0, sc1)
+    p["hshear"] = u("hshear", -o["hshear"], o["hshear"])
+    p["trans"] = (u("trans0", -o["trans"], o["trans"]), u("trans1", -o["trans"], o["trans"]))
+    p["phi"] = u("phi", -o["rotate"] * math.pi / 180, o["rotate"] * math.pi / 180)
+    p["brightness"] = u("brightness", -o["brightness"], o["brightness"])
+    p["contrast"] = u("contrast", 1 / o["contrast"], o["contrast"])
+    p["scale_"] = (p["scale"][0] * u("d_hscale", o["d_hscale"], 1), p["scale"][1])
+    p["hshear_"] = p["hshear"] + u("d_hshear", -o["d_hshear"], o["d_hshear"])
+    p["trans_"] = (p["trans"][0], p["trans"][1] + u("d_vtrans", -o["d_vtrans"], o["d_vtrans"]))
+    p["phi_"] = p["phi"] + u("d_rotate", -o["d_rotate"] * math.pi / 180, o["d_rotate"] * math.pi / 180)
+    p["brightness_"] = p["brightness"] + u("d_brightness", -o["d_brightness"], o["d_brightness"])
+    p["contrast_"] = p["contrast"] * u("d_contrast", 1 / o["d_contrast"], o["d_contrast"])
+    return p
+
+
+def _mul32(a, b):
+    """main.lua:603-605 on arrays"""
+    return [a[0] * b[0] + a[1] * b[3], a[0] * b[1] + a[1] * b[4], a[0] * b[2] + a[1] * b[5] + a[2],
+            a[3] * b[0] + a[4] * b[3], a[3] * b[1] + a[4] * b[4], a[3] * b[2] + a[4] * b[5] + a[5]]
+
+
+def patch_matrices(ws, dim3, dim4, scale, phi, trans, hshear):
+    """make_patch's matrix (main.lua:608-616) for arrays of patches -> (n, 6) float32"""
+    m = [1, 0, -dim4, 0, 1, -dim3]
+    m = _mul32([1, 0, trans[0], 0, 1, trans[1]], m)
+    m = _mul32([scale[0], 0, 0, 0, scale[1], 0], m)
+    c = np.array([math.cos(v) for v in phi])
+    s = np.array([math.sin(v) for v in phi])
+    m = _mul32([c, s, 0, -s, c, 0], m)
+    m = _mul32([1, hshear, 0, 0, 1, 0], m)
+    m = _mul32([1, 0, (ws - 1) / 2, 0, 1, (ws - 1) / 2], m)
+    n = len(dim3)
+    return np.stack([np.broadcast_to(np.asarray(v, np.float64), (n,)) for v in m], 1).astype(np.float32)
+
+
+def make_warps(p, rows, ws):
+    """main.lua:820-846: the (4 n,) mccnn_warp records of n samples from their parameters `p` and nnz rows (n, 4)
+    (image 1-based, dim3, dim4, d)"""
+    rows = np.asarray(rows, np.float32).astype(np.float64)
+    n = len(rows)
+    img, dim3, dim4, d = rows[:, 0], rows[:, 1], rows[:, 2], rows[:, 3]
+    a = (p["scale"], p["phi"], p["trans"], p["hshear"])
+    b = (p["scale_"], p["phi_"], p["trans_"], p["hshear_"])
+    out = np.zeros((n, 4), WARP_DTYPE)
+    out["m"][:, 0] = out["m"][:, 2] = patch_matrices(ws, dim3, dim4, *a)
+    out["m"][:, 1] = patch_matrices(ws, dim3, dim4 - d + p["d_pos"], *b)
+    out["m"][:, 3] = patch_matrices(ws, dim3, dim4 - d + p["d_neg"], *b)
+    for j, (c, br) in enumerate([(p["contrast"], p["brightness"]), (p["contrast_"], p["brightness_"])] * 2):
+        out["contrast"][:, j] = c.astype(np.float32)
+        out["brightness"][:, j] = br.astype(np.float32)
+    out["image"] = (img.astype(np.int64) - 1)[:, None]
+    out["view"] = np.array([0, 1, 0, 1], np.int32)[None]
+    return out.reshape(-1)
+
+
+def sample_patches(X0, X1, warps, ws):
+    """the sampler alone (mccnn_train_sample): X0 / X1 (n_img, 1, H, W) CUDA float32, warps a WARP_DTYPE array ->
+    (len(warps), ws, ws) CUDA float32"""
+    import torch
+
+    from .adcensus import _check, _stream, _t, lib
+
+    name = "sample_patches"
+    p0, p1 = _t(X0, 1, name), _t(X1, 2, name)
+    if X0.shape != X1.shape or X0.dim() != 4 or X0.shape[1] != 1:
+        raise ValueError("%s: X0 and X1 must both be (n, 1, H, W)" % name)
+    n_img, _, H, W = X0.shape
+    w = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(X0.device)
+    out = torch.empty((len(warps), ws, ws), dtype=torch.float32, device=X0.device)
+    with torch.cuda.device(X0.device):
+        _check(lib().mccnn_train_sample(p0, p1, n_img, H, W, ctypes.c_void_p(w.data_ptr()), len(warps), ws,
+                                        ctypes.c_void_p(out.data_ptr()), _stream(out)), name)
+    return out
+
+
+class Trainer:
+    """csrc/train.cu's trainer: net_tr + Margin2 + the momentum update on `device`, sampling from X0 / X1 (CUDA)."""
+
+    def __init__(self, o, X0, X1, chunk=CHUNK, loss_cap=1, device=None):
+        import torch
+
+        from .adcensus import _check, _stream, _t, lib
+
+        self.o, self.chunk = o, chunk
+        self.dev = X0.device if device is None else torch.device("cuda", device)
+        self.l1, self.fm, self.bs = o["l1"], o["fm"], o["bs"]
+        self.ws = 1 + 2 * self.l1
+        self.N = 2 * self.bs
+        self._keep = (X0, X1)
+        n_img, _, H, W = X0.shape
+        self._h = ctypes.c_void_p()
+        with torch.cuda.device(self.dev):
+            self.stream = torch.cuda.current_stream(self.dev)
+            _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, ctypes.c_float(o["m"]),
+                                              o["pow"], ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
+                                              _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
+                                              _stream(X0)), "mccnn_trainer_create")
+        self.launches_per_step = lib().mccnn_trainer_launches_per_step(self._h)
+
+    def close(self):
+        from .adcensus import lib
+
+        if getattr(self, "_h", None):
+            lib().mccnn_trainer_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _s(self):
+        return ctypes.c_void_p(self.stream.cuda_stream)
+
+    def size(self, what):
+        from .adcensus import lib
+
+        lib().mccnn_trainer_size.restype = ctypes.c_longlong
+        return int(lib().mccnn_trainer_size(self._h, what))
+
+    def get(self, what):
+        """a copy of one of the trainer's buffers (TRAIN_*) as a CUDA float32 tensor"""
+        import torch
+
+        from .adcensus import _check, lib
+
+        out = torch.empty(self.size(what), dtype=torch.float32, device=self.dev)
+        _check(lib().mccnn_trainer_get(self._h, what, ctypes.c_void_p(out.data_ptr()), self._s()), "mccnn_trainer_get")
+        return out
+
+    def set(self, what, src):
+        import torch
+
+        from .adcensus import _check, lib
+
+        t = torch.as_tensor(src, dtype=torch.float32).reshape(-1).to(self.dev).contiguous()
+        if t.numel() != self.size(what):
+            raise ValueError("Trainer.set: %d values for a buffer of %d" % (t.numel(), self.size(what)))
+        _check(lib().mccnn_trainer_set(self._h, what, ctypes.c_void_p(t.data_ptr()), self._s()), "mccnn_trainer_set")
+        self.stream.synchronize()
+
+    def set_layers(self, layers):
+        self.set(TRAIN_PARAMS, flatten(layers))
+
+    def layers(self, what=TRAIN_PARAMS):
+        return unflatten(self.get(what).cpu().numpy(), self.l1, self.fm)
+
+    def run(self, warps, lr):
+        """len(warps) / N steps (<= chunk) from a WARP_DTYPE array (pinned host or CUDA uint8 tensor, or numpy)"""
+        import torch
+
+        from .adcensus import _check, lib
+
+        if isinstance(warps, np.ndarray):
+            warps = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(self.dev)
+        nsteps = warps.numel() // (WARP_DTYPE.itemsize * self.N)
+        _check(lib().mccnn_trainer_run(self._h, ctypes.c_void_p(warps.data_ptr()), nsteps, ctypes.c_double(lr), self._s()),
+               "mccnn_trainer_run")
+        return warps
+
+    def step_patches(self, patches, lr):
+        import torch
+
+        from .adcensus import _check, lib
+
+        t = torch.as_tensor(patches, dtype=torch.float32).to(self.dev).contiguous()
+        if t.numel() != self.N * self.ws * self.ws:
+            raise ValueError("step_patches: (%d, 1, %d, %d) patches expected" % (self.N, self.ws, self.ws))
+        _check(lib().mccnn_trainer_step_patches(self._h, ctypes.c_void_p(t.data_ptr()), ctypes.c_double(lr), self._s()),
+               "mccnn_trainer_step_patches")
+        self._last = t
+
+    def reset_losses(self):
+        from .adcensus import _check, lib
+
+        _check(lib().mccnn_trainer_reset_losses(self._h, self._s()), "mccnn_trainer_reset_losses")
+
+
+def flatten(layers):
+    return np.concatenate([np.concatenate([np.asarray(w, np.float32).reshape(-1), np.asarray(b, np.float32).reshape(-1)])
+                           for w, b in layers])
+
+
+def unflatten(v, l1, fm):
+    out, o = [], 0
+    for i in range(l1):
+        cin = 1 if i == 0 else fm
+        w = v[o:o + fm * cin * 9].reshape(fm, cin, 3, 3)
+        o += fm * cin * 9
+        out.append((w.copy(), v[o:o + fm].copy()))
+        o += fm
+    return out
+
+
+def load_nnz(data, action, data_root):
+    d = os.path.join(data_root, "data.kitti" if data.dataset == "kitti" else "data.kitti2015")
+    nnz = evaluate._fromfile(os.path.join(d, "nnz_tr.bin"))
+    if action == "train_all":                                                    # main.lua:650-654
+        nnz = np.concatenate([nnz, evaluate._fromfile(os.path.join(d, "nnz_te.bin"))])
+    nnz = np.ascontiguousarray(nnz, np.float32).reshape(-1, 4)
+    if len(nnz) and not (nnz[:, 0].min() >= 1 and nnz[:, 0].max() <= len(data.X0)):
+        raise ValueError("%s: nnz rows name images outside 1 .. %d" % (d, len(data.X0)))
+    return nnz
+
+
+def net_path(data_root, dataset, args):
+    return os.path.join(data_root, "net", "net_%s.t7" % cmd_str(dataset, args))
+
+
+def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS):
+    """main.lua:602-890 for arch 'fast': returns the saved net's file name.  `args` are main.lua's arguments after
+    dataset and arch (for the file name), `stereo` the stereo method's overrides for the evaluation that follows;
+    `log` receives the printed lines."""
+    import torch
+
+    from . import t7
+
+    if action not in ("train_tr", "train_all"):
+        raise ValueError("action must be train_tr or train_all, got %r" % (action,))
+    check(o)
+    fname = net_path(data_root, dataset, args)
+    if os.path.exists(fname):
+        raise FileExistsError("%s already exists; remove it first" % fname)
+    if action == "train_all" and os.path.isdir(out) and any(f != ".empty" for f in os.listdir(out)):
+        raise ValueError("submit: output directory %s is not empty" % out)
+    data = evaluate.load_data(dataset, data_root)
+    nnz = load_nnz(data, action, data_root)
+    stream = Stream(seed)                                                        # main.lua:340
+    perm = randperm(stream, len(nnz))                                            # :657
+    layers = init_weights(stream, o["l1"], o["fm"])                              # :726-736
+    for line in net_lines(o):
+        log(line)
+    h = o["bs"] // 2
+    nsteps = steps_per_epoch(len(nnz), o["bs"])
+    dev = torch.device("cuda", device)
+    with torch.cuda.device(dev):
+        X0 = torch.from_numpy(np.ascontiguousarray(data.X0, np.float32)).to(dev)
+        X1 = torch.from_numpy(np.ascontiguousarray(data.X1, np.float32)).to(dev)
+        tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
+        try:
+            tr.set_layers(layers)
+            rec = WARP_DTYPE.itemsize * tr.N
+            pinned = [torch.empty(CHUNK * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+            events = [None, None]
+            t0 = time.time()
+            lr = o["lr"]
+            for epoch in range(1, epochs + 1):
+                if epoch == LR_DROP_EPOCH:
+                    lr = lr / 10
+                tr.reset_losses()
+                for k, s0 in enumerate(range(0, nsteps, CHUNK)):
+                    n = min(CHUNK, nsteps - s0)
+                    rows = nnz[perm[s0 * h:(s0 + n) * h] - 1]                  # perm[t + i - 1], :820
+                    warps = make_warps(draw_params(stream, o, n * h), rows, tr.ws)
+                    b = k % 2
+                    if events[b] is not None:
+                        events[b].synchronize()
+                    pinned[b][:n * rec].numpy()[:] = warps.view(np.uint8)
+                    tr.run(pinned[b][:n * rec], lr)
+                    events[b] = torch.cuda.Event()
+                    events[b].record(tr.stream)
+                losses = tr.get(TRAIN_LOSS)[:nsteps].cpu().numpy().astype(np.float64)
+                ok = (losses >= 0) & (losses < 100)                              # :861-866
+                for v in losses[~ok]:
+                    log("WARNING! err=%f" % v)
+                err = np.cumsum(losses[ok])[-1] / ok.sum() if ok.any() else float("nan")
+                log(epoch_line(epoch, err, lr, time.time() - t0))
+            trained = tr.layers()
+        finally:
+            tr.close()
+    os.makedirs(os.path.dirname(fname), exist_ok=True)
+    t7.save_net(fname, trained, opt=dict(o, a=action, seed=seed, gpu=device + 1))   # :883, save_net(0)
+    ev = evaluate.Evaluator(dataset, "fast", net_fname=fname, device=device, **(stereo or {}))
+    try:
+        if action == "train_tr":                                                 # :884-888
+            ev.test("test_te", data_root=data_root, data=data)
+        else:
+            ev.submit(data_root=data_root, out=out, data=data)
+    finally:
+        ev.close()
+    return fname

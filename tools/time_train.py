@@ -1,0 +1,160 @@
+"""Measure the training step of the fast architecture (csrc/train.cu) on a synthetic full-size KITTI 2012 set.
+
+    python tools/time_train.py [-steps 2000] [-gpu 1] [-json out.json]
+
+The set is 389 views of 350 x 1242 per side on the device and 1,048,576 nnz rows, at main.lua's kitti presets (l1 4, fm 64,
+bs 128).  Reported, each after a warm-up:
+
+* device:   the captured step alone, warp parameters already on the device (steps/s, samples/s = steps/s * bs / 2);
+* driver:   as train.train runs it: the host draws and builds each chunk of parameters while the GPU runs the previous one;
+* baseline: the same step written with torch autograd / cuDNN in fp32 (conv2d, the Normalize2 / StereoJoin1 / Margin2 formulas,
+  the momentum update as main.lua:871-874) on patches from the same sampler, TF32 off.
+
+The card's name and power limit are printed with the numbers.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+import numpy as np  # noqa: E402
+
+
+def card():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=30)
+        return r.stdout.strip().splitlines()[0]
+    except Exception as e:  # noqa: BLE001
+        return "unknown (%s)" % e
+
+
+def baseline_step(x, params, vel, o, lr):
+    import torch
+
+    F = torch.nn.functional
+    h = x
+    for i in range(o["l1"]):
+        h = F.conv2d(h, params[2 * i], params[2 * i + 1])
+        if i < o["l1"] - 1:
+            h = torch.relu(h)
+    h = h / ((h * h).sum(1, keepdim=True) + 1e-5).sqrt()
+    s = (h[0::2] * h[1::2]).sum(1).reshape(-1)
+    f = torch.clamp(s[1::2] - s[0::2] + o["m"], min=0)
+    loss = f.mean() if o["pow"] == 1 else (0.5 * f * f).mean()
+    grads = torch.autograd.grad(loss, params)
+    with torch.no_grad():
+        for p, v, g in zip(params, vel, grads):
+            v.mul_(o["mom"]).add_(g, alpha=-lr)
+            p.add_(v)
+    return loss
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("-steps", type=int, default=2000)
+    ap.add_argument("-gpu", type=int, default=1)
+    ap.add_argument("-json", default="")
+    args = ap.parse_args(argv)
+    import torch
+
+    import mccnn_b200  # noqa: F401
+    from mccnn_b200 import train
+
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    dev = torch.device("cuda", args.gpu - 1)
+    torch.cuda.set_device(dev)
+    o = train.options("kitti")
+    n_img, H, W, rows = 389, 350, 1242, 1 << 20
+    g = torch.Generator(device=dev).manual_seed(0)
+    X0 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
+    X1 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
+    rng = np.random.default_rng(0)
+    nnz = np.stack([rng.integers(1, n_img + 1, rows), rng.integers(0, H, rows), rng.integers(0, W, rows),
+                    rng.uniform(1, 200, rows)], 1).astype(np.float32)
+    s = train.Stream(42)
+    perm = train.randperm(s, rows)
+    chunk = train.CHUNK
+    tr = train.Trainer(o, X0, X1, chunk=chunk, loss_cap=args.steps + 4 * chunk, device=dev.index)
+    tr.set_layers(train.init_weights(s, o["l1"], o["fm"]))
+    h = o["bs"] // 2
+    res = dict(card=card(), launches_per_step=tr.launches_per_step, steps=args.steps)
+
+    def warps_for(s0, n):
+        r = nnz[perm[(s0 * h) % (rows - n * h):][:n * h] - 1]
+        return train.make_warps(train.draw_params(s, o, n * h), r, tr.ws)
+
+    # device: parameters already on the device
+    dw = torch.from_numpy(warps_for(0, chunk).view(np.uint8)).to(dev)
+    tr.run(dw, o["lr"])
+    torch.cuda.synchronize()
+    n = 0
+    t0 = time.perf_counter()
+    while n < args.steps:
+        tr.run(dw, o["lr"])
+        n += chunk
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    res["device_steps_per_s"] = n / dt
+    res["device_samples_per_s"] = n * h / dt
+
+    # driver: host-built chunks through two pinned buffers, as train.train does
+    rec = train.WARP_DTYPE.itemsize * tr.N
+    pinned = [torch.empty(chunk * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+    ev = [None, None]
+    n = 0
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    k = 0
+    while n < args.steps:
+        w = warps_for(n, chunk)
+        b = k % 2
+        if ev[b] is not None:
+            ev[b].synchronize()
+        pinned[b].numpy()[:] = w.view(np.uint8)
+        tr.run(pinned[b], o["lr"])
+        ev[b] = torch.cuda.Event()
+        ev[b].record(tr.stream)
+        n += chunk
+        k += 1
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    res["driver_steps_per_s"] = n / dt
+    res["driver_samples_per_s"] = n * h / dt
+    t = time.perf_counter()
+    warps_for(0, chunk)
+    res["host_build_s_per_step"] = (time.perf_counter() - t) / chunk
+
+    # baseline: torch autograd / cuDNN on the sampler's patches
+    layers = tr.layers()
+    params = []
+    for w, b_ in layers:
+        params += [torch.from_numpy(w).to(dev).requires_grad_(), torch.from_numpy(b_).to(dev).requires_grad_()]
+    vel = [torch.zeros_like(p) for p in params]
+    x = tr.get(train.TRAIN_PATCHES).reshape(tr.N, 1, tr.ws, tr.ws)
+    for _ in range(50):
+        baseline_step(x, params, vel, o, o["lr"])
+    torch.cuda.synchronize()
+    nb = max(200, args.steps // 4)
+    t0 = time.perf_counter()
+    for _ in range(nb):
+        baseline_step(x, params, vel, o, o["lr"])
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    res["baseline_steps_per_s"] = nb / dt
+    res["baseline_samples_per_s"] = nb * h / dt
+    tr.close()
+    print(json.dumps(res, indent=1))
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(res, f, indent=1)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
