@@ -472,15 +472,32 @@ int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, dou
 /* One step from given patches ((N, 1, ws, ws) float32) instead of the sampler. */
 int mccnn_trainer_step_patches(mccnn_trainer *h, const float *patches, double lr, adcensus_stream_t stream);
 
+/* net_tr of arch 'slow' (main.lua:663-677): l1 valid 3x3 convolutions 1 -> fm -> .. -> fm with a ReLU after every one,
+ * Reshape(bs, 2 fm) (row r = the features of patches 2r and 2r + 1), l2 x [Linear(in, nh2), ReLU], Linear(nh2, 1), Sigmoid,
+ * then BCECriterion2 against the targets 0, 1, 0, 1, ... (main.lua:848-849), with momentum `mom`.  The parameter vector
+ * holds the tower's layers as for 'fast', then per Linear W (out, in) followed by b (out), in main.lua's order.  fp32 on
+ * the CUDA cores with fixed reduction orders and no floating-point atomics.  The handle works with every mccnn_trainer_*
+ * call; the loss of a step is BCECriterion2's output.  l1 1..8, fm a multiple of 16 up to 128, l2 1..4, nh2 128, 256 or
+ * 384 (else ADCENSUS_ELIMIT). */
+int mccnn_trainer_create_slow(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom, const float *X0,
+			      const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
+			      adcensus_stream_t stream);
+
 /* The trainer's buffers, for get / set (set: PARAMS and MOMENTA only) and the tests.  Sizes in floats from
  * mccnn_trainer_size.  TOWER: every layer's output, layer k (N, fm, s_k, s_k) after the previous layers, s_k = ws - 2k, post
- * ReLU except the last; DZ: the gradient of the loss wrt each layer's pre-activation output, same layout; NORM (N) = sum of
- * squares + 1e-5; NORMALIZED (N, fm); JOIN (bs); JOIN_GRAD (bs) Margin2's gradInput / (bs / 2); HINGE (bs / 2);
- * NORM_GRAD_OUT (N, fm) the gradient wrt Normalize2's output; LOSS (loss_cap). */
+ * ReLU except the last ('fast') or post ReLU ('slow'); DZ: the gradient of the loss wrt each layer's pre-activation output,
+ * same layout; LOSS (loss_cap).
+ * 'fast' only: NORM (N) = sum of squares + 1e-5; NORMALIZED (N, fm); JOIN (bs); JOIN_GRAD (bs) Margin2's gradInput /
+ * (bs / 2); HINGE (bs / 2); NORM_GRAD_OUT (N, fm) the gradient wrt Normalize2's output.
+ * 'slow' only: ROWS (bs, 2 fm) the reshaped rows (a view of TOWER's last layer); FC each Linear's output, the hidden ones
+ * (bs, nh2) after their ReLU, then the last one's (bs) before the Sigmoid; SIGMOID (bs); BCE_GRAD (bs) the criterion's
+ * gradInput; ROWS_GRAD (bs, 2 fm) the gradient arriving at the tower (wrt its last ReLU's output).
+ * An id that does not apply to the handle's arch: size -1, get ADCENSUS_EINVAL. */
 enum {
 	MCCNN_TRAIN_PARAMS, MCCNN_TRAIN_MOMENTA, MCCNN_TRAIN_GRADS, MCCNN_TRAIN_PATCHES, MCCNN_TRAIN_TOWER, MCCNN_TRAIN_NORM,
 	MCCNN_TRAIN_NORMALIZED, MCCNN_TRAIN_JOIN, MCCNN_TRAIN_JOIN_GRAD, MCCNN_TRAIN_HINGE, MCCNN_TRAIN_NORM_GRAD_OUT,
-	MCCNN_TRAIN_DZ, MCCNN_TRAIN_LOSS, MCCNN_TRAIN_NBUF
+	MCCNN_TRAIN_DZ, MCCNN_TRAIN_LOSS, MCCNN_TRAIN_ROWS, MCCNN_TRAIN_FC, MCCNN_TRAIN_SIGMOID, MCCNN_TRAIN_BCE_GRAD,
+	MCCNN_TRAIN_ROWS_GRAD, MCCNN_TRAIN_NBUF
 };
 long long mccnn_trainer_size(mccnn_trainer *h, int what);
 int mccnn_trainer_get(mccnn_trainer *h, int what, float *dst, adcensus_stream_t stream);

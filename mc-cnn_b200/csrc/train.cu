@@ -15,8 +15,13 @@
 //     update_kernel      v = v * mom; v = v + (-lr) * g; p = p + v, each operation rounded; the loss (the hinge terms
 //                        summed in order / (bs / 2)) goes to the per-step loss buffer.
 //   No floating-point atomics anywhere: a step is a pure function of its inputs, bit for bit.
+// * Arch 'slow' (main.lua:663-677 + BCECriterion2): the same sampler, graph, chunked warp parameters and update_kernel;
+//   the tower, the Linear layers and their backward passes are gemm_kernel launches (see below), then slow_head_kernel
+//   and wgrad_reduce_kernel.  The fast kernels above are not shared with it.
 #include <math.h>
 #include <stdlib.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 
@@ -311,6 +316,233 @@ __global__ void update_kernel(float *__restrict__ P, float *__restrict__ V, cons
 	}
 }
 
+// ---- arch 'slow' (main.lua:663-677): the tower with a ReLU after every layer, Reshape(bs, 2 fm), l2 x [Linear, ReLU],
+// Linear(nh2, 1), Sigmoid, BCECriterion2.  Every convolution and Linear, forward and backward, is one tiled fp32 GEMM
+// (gemm_kernel) whose operands are read through an implicit-im2col functor; each output is one thread's fmaf chain in
+// ascending k, and the weight gradients of the tower are split over k into partial sums added in split order.
+constexpr int L2MAX = 4;
+constexpr int BM = 64, BN = 64, BK = 16, GT = 256;  // gemm_kernel: 64 x 64 tiles, 4 x 4 outputs per thread
+
+template <class Op>
+__global__ void __launch_bounds__(GT) gemm_kernel(Op op)
+{
+	__shared__ __align__(16) float As[BK][BM + 4], Bs[BK][BN + 4];
+	const int t = threadIdx.x, tx = t % 16, ty = t / 16;
+	const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+	const int k0 = blockIdx.z * op.kchunk, k1 = min(op.K, k0 + op.kchunk);
+	float acc[4][4];
+#pragma unroll
+	for (int i = 0; i < 4; i++)
+#pragma unroll
+		for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
+	for (int kb = k0; kb < k1; kb += BK) {
+#pragma unroll
+		for (int i = 0; i < BM * BK / GT; i++) {
+			const int e = t + GT * i, m = e / BK, k = e % BK;
+			As[k][m] = m0 + m < op.M && kb + k < k1 ? op.a(m0 + m, kb + k) : 0.f;
+		}
+#pragma unroll
+		for (int i = 0; i < BN * BK / GT; i++) {
+			const int e = t + GT * i, k = e / BN, n = e % BN;
+			Bs[k][n] = n0 + n < op.N && kb + k < k1 ? op.b(kb + k, n0 + n) : 0.f;
+		}
+		__syncthreads();
+#pragma unroll
+		for (int k = 0; k < BK; k++) {
+			const float4 a = *(const float4 *)&As[k][ty * 4], b = *(const float4 *)&Bs[k][tx * 4];
+			const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+			for (int i = 0; i < 4; i++)
+#pragma unroll
+				for (int j = 0; j < 4; j++) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+		}
+		__syncthreads();
+	}
+#pragma unroll
+	for (int i = 0; i < 4; i++)
+#pragma unroll
+		for (int j = 0; j < 4; j++) {
+			const int m = m0 + ty * 4 + i, n = n0 + tx * 4 + j;
+			if (m < op.M && n < op.N) op.store(m, n, acc[i][j], blockIdx.z);
+		}
+}
+
+// layer forward: out[n][co][y][x] = ReLU(sum_{ci,ky,kx} W[co][ci][ky][kx] in[n][ci][y+ky][x+kx] + b[co]);
+// rows co, columns (n, y, x), k = (ci, ky, kx)
+struct ConvFwd {
+	int M, N, K, kchunk, cin, si, so;
+	const float *__restrict__ in, *__restrict__ w, *__restrict__ bias;
+	float *__restrict__ out;
+	__device__ float a(int m, int k) const { return __ldg(w + (long)m * K + k); }
+	__device__ float b(int k, int c) const
+	{
+		const int P = so * so, n = c / P, p = c % P, ci = k / 9, tap = k % 9;
+		return in[((long)n * cin + ci) * si * si + (p / so + tap / 3) * si + p % so + tap % 3];
+	}
+	__device__ void store(int m, int c, float acc, int) const
+	{
+		const int P = so * so, n = c / P, p = c % P;
+		out[((long)n * M + m) * P + p] = fmaxf(acc + __ldg(bias + m), 0.f);
+	}
+};
+
+// gradient through layer k's weights and layer k - 1's ReLU: rows ci, columns (n, y, x) of layer k's input, k = (co, ky, kx)
+struct ConvBwdData {
+	int M, N, K, kchunk, fm, si, so;
+	const float *__restrict__ w, *__restrict__ dz, *__restrict__ act;
+	float *__restrict__ dst;
+	__device__ float a(int m, int k) const { return __ldg(w + ((long)(k / 9) * fm + m) * 9 + k % 9); }
+	__device__ float b(int k, int c) const
+	{
+		const int Pi = si * si, n = c / Pi, p = c % Pi, co = k / 9, tap = k % 9;
+		const int y = p / si - tap / 3, x = p % si - tap % 3;
+		return y >= 0 && y < so && x >= 0 && x < so ? dz[((long)n * fm + co) * so * so + y * so + x] : 0.f;
+	}
+	__device__ void store(int m, int c, float acc, int) const
+	{
+		const int Pi = si * si;
+		const long i = ((long)(c / Pi) * fm + m) * Pi + c % Pi;
+		dst[i] = act[i] > 0.f ? acc : 0.f;
+	}
+};
+
+// layer k's weight and bias gradient, split over k: rows co, columns (ci, ky, kx) and a last column of ones (the bias),
+// k = (n, y, x); split z writes its partial sums to part (nsplit, M, N)
+struct ConvWgrad {
+	int M, N, K, kchunk, cin, si, so;
+	const float *__restrict__ dz, *__restrict__ in;
+	float *__restrict__ part;
+	__device__ float a(int m, int k) const
+	{
+		const int P = so * so;
+		return dz[((long)(k / P) * M + m) * P + k % P];
+	}
+	__device__ float b(int k, int c) const
+	{
+		if (c == N - 1) return 1.f;
+		const int P = so * so, n = k / P, p = k % P, ci = c / 9, tap = c % 9;
+		return in[((long)n * cin + ci) * si * si + (p / so + tap / 3) * si + p % so + tap % 3];
+	}
+	__device__ void store(int m, int c, float acc, int z) const { part[((long)z * M + m) * N + c] = acc; }
+};
+
+// Linear + ReLU: Y (bs, out) = ReLU(X (bs, in) W^T + b)
+struct FcFwd {
+	int M, N, K, kchunk;
+	const float *__restrict__ x, *__restrict__ w, *__restrict__ bias;
+	float *__restrict__ y;
+	__device__ float a(int m, int k) const { return x[(long)m * K + k]; }
+	__device__ float b(int k, int c) const { return __ldg(w + (long)c * K + k); }
+	__device__ void store(int m, int c, float acc, int) const { y[(long)m * N + c] = fmaxf(acc + __ldg(bias + c), 0.f); }
+};
+
+// Linear's input gradient dZ (bs, out) W -> through the previous ReLU (mask = its output); the first Linear also writes
+// the reshape's gradient (raw, no mask)
+struct FcBwdData {
+	int M, N, K, kchunk;
+	const float *__restrict__ dz, *__restrict__ w, *__restrict__ mask;
+	float *__restrict__ dst, *__restrict__ raw;
+	__device__ float a(int m, int k) const { return dz[(long)m * K + k]; }
+	__device__ float b(int k, int c) const { return __ldg(w + (long)k * N + c); }
+	__device__ void store(int m, int c, float acc, int) const
+	{
+		const long i = (long)m * N + c;
+		if (raw) raw[i] = acc;
+		dst[i] = mask[i] > 0.f ? acc : 0.f;
+	}
+};
+
+// Linear's weight and bias gradient: rows out, columns in and a last column of ones, k = the batch row
+struct FcWgrad {
+	int M, N, K, kchunk;
+	const float *__restrict__ dz, *__restrict__ x;
+	float *__restrict__ gw, *__restrict__ gb;
+	__device__ float a(int m, int k) const { return dz[(long)k * M + m]; }
+	__device__ float b(int k, int c) const { return c == N - 1 ? 1.f : x[(long)k * (N - 1) + c]; }
+	__device__ void store(int m, int c, float acc, int) const
+	{
+		if (c == N - 1) gb[m] = acc;
+		else gw[(long)m * (N - 1) + c] = acc;
+	}
+};
+
+// Linear(nh2, 1) + Sigmoid + BCECriterion2 (targets 0, 1, 0, 1, ...: main.lua:848-849) and back to the last hidden
+// Linear's pre-ReLU gradient, plus the last Linear's weight and bias gradient; one block
+__global__ void slow_head_kernel(int bs, int nh2, const float *__restrict__ X, const float *__restrict__ w,
+				 const float *__restrict__ b, float *__restrict__ z, float *__restrict__ sig,
+				 float *__restrict__ gin, float *__restrict__ term, float *__restrict__ dzo,
+				 float *__restrict__ dz, float *__restrict__ gw, float *__restrict__ gb, float *__restrict__ loss)
+{
+	const float eps = 1e-12f, n = (float)bs;
+	const int lane = threadIdx.x % 32, warp = threadIdx.x / 32, nwarp = blockDim.x / 32;
+	for (int r = warp; r < bs; r += nwarp) {
+		float acc = 0.f;
+		for (int k = lane; k < nh2; k += 32) acc = fmaf(X[(long)r * nh2 + k], w[k], acc);
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+		if (lane == 0) {
+			const float zr = acc + b[0], y = 1.f / (1.f + expf(-zr)), t = (float)(r & 1);
+			z[r] = zr;
+			sig[r] = y;
+			// updateOutput: term3 = (log(x + eps) * t + log(1 - x + eps) * (1 - t)) / n
+			const float t1 = 1.f - t, t2 = __fmul_rn(logf(__fadd_rn(__fsub_rn(1.f, y), eps)), t1);
+			term[r] = __fdiv_rn(__fadd_rn(__fmul_rn(logf(__fadd_rn(y, eps)), t), t2), n);
+			// updateGradInput: -((t / (x + eps) - (1 - t) / (1 - x + eps)) / n)
+			const float g1 = __fdiv_rn(t1, __fadd_rn(__fsub_rn(1.f, y), eps));
+			const float g = -__fdiv_rn(__fsub_rn(__fdiv_rn(t, __fadd_rn(y, eps)), g1), n);
+			gin[r] = g;
+			dzo[r] = __fmul_rn(__fmul_rn(g, __fsub_rn(1.f, y)), y);          // Sigmoid backward
+		}
+	}
+	__syncthreads();
+	for (int k = threadIdx.x; k < nh2; k += blockDim.x) {
+		float acc = 0.f;
+		for (int r = 0; r < bs; r++) acc = fmaf(dzo[r], X[(long)r * nh2 + k], acc);
+		gw[k] = acc;
+	}
+	for (long i = threadIdx.x; i < (long)bs * nh2; i += blockDim.x) {
+		const int r = (int)(i / nh2), k = (int)(i % nh2);
+		dz[i] = X[i] > 0.f ? __fmul_rn(dzo[r], w[k]) : 0.f;
+	}
+	if (threadIdx.x == 0) {
+		float s = 0.f, l = 0.f;
+		for (int r = 0; r < bs; r++) {
+			s = __fadd_rn(s, dzo[r]);
+			l = __fadd_rn(l, term[r]);
+		}
+		gb[0] = s;
+		*loss = -l;                                                          // -term3:sum()
+	}
+}
+
+struct SlowLayout {
+	int l2, nh2, nsplit[LMAX], kchunk[LMAX];
+	long fwoff[L2MAX + 1], fboff[L2MAX + 1];  // the Linear layers' W (out, in), b (out) in the parameter vector
+	long poff[LMAX];                          // each tower layer's partial sums in the split-k workspace
+};
+
+// the tower's weight and bias gradients: the partial sums of the splits, added in split order
+__global__ void wgrad_reduce_kernel(Layout L, SlowLayout S, const float *__restrict__ part, float *__restrict__ G)
+{
+	const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= L.boff[L.l1 - 1] + L.fm) return;
+	int k = 0;
+	while (i >= L.boff[k] + L.fm) k++;
+	const int cin9 = (k ? L.fm : 1) * 9, N = cin9 + 1;
+	const long co = i < L.boff[k] ? (i - L.woff[k]) / cin9 : i - L.boff[k];
+	const int c = i < L.boff[k] ? (int)((i - L.woff[k]) % cin9) : cin9;
+	const float *p = part + S.poff[k] + co * N + c;
+	float s = p[0];
+	for (int z = 1; z < S.nsplit[k]; z++) s = __fadd_rn(s, p[(long)z * L.fm * N]);
+	G[i] = s;
+}
+
+template <class Op>
+void launch_gemm(const Op &op, int nsplit, cudaStream_t s)
+{
+	gemm_kernel<Op><<<dim3(adc_div_up(op.N, BN), adc_div_up(op.M, BM), nsplit), GT, 0, s>>>(op);
+}
+
 }  // namespace
 
 struct mccnn_trainer {
@@ -326,7 +558,61 @@ struct mccnn_trainer {
 	mccnn_warp *warps;
 	cudaStream_t cap;
 	cudaGraphExec_t full, body;
+	// arch 'slow' only
+	int slow;
+	SlowLayout S;
+	float *rows, *fc, *sig, *bce_grad, *rows_grad, *fc_dz, *term, *dzo, *part, *bce_loss;
 };
+
+static int enqueue_slow(mccnn_trainer *h, cudaStream_t s)
+{
+	const Layout &L = h->L;
+	const SlowLayout &S = h->S;
+	const int bs = L.N / 2, fm = L.fm, nh2 = S.nh2, l2 = S.l2;
+	for (int k = 0; k < L.l1; k++) {                                         // tower forward
+		const int cin = k ? fm : 1, si = L.ws - 2 * k, so = si - 2;
+		const ConvFwd op{fm, L.N * so * so, cin * 9, cin * 9, cin, si, so, k ? h->act + L.aoff[k - 1] : h->X,
+				 h->P + L.woff[k], h->P + L.boff[k], h->act + L.aoff[k]};
+		launch_gemm(op, 1, s);
+	}
+	const float *x = h->rows;
+	for (int j = 0; j < l2; j++) {                                           // Linear + ReLU
+		const int in = j ? nh2 : 2 * fm;
+		const FcFwd op{bs, nh2, in, in, x, h->P + S.fwoff[j], h->P + S.fboff[j], h->fc + (long)j * bs * nh2};
+		launch_gemm(op, 1, s);
+		x = op.y;
+	}
+	slow_head_kernel<<<1, 512, 0, s>>>(bs, nh2, x, h->P + S.fwoff[l2], h->P + S.fboff[l2], h->fc + (long)l2 * bs * nh2,
+					  h->sig, h->bce_grad, h->term, h->dzo, h->fc_dz + (long)(l2 - 1) * bs * nh2,
+					  h->G + S.fwoff[l2], h->G + S.fboff[l2], h->bce_loss);
+	for (int j = l2 - 1; j >= 0; j--) {                                      // Linear backward
+		const int in = j ? nh2 : 2 * fm;
+		const float *dz = h->fc_dz + (long)j * bs * nh2, *xj = j ? h->fc + (long)(j - 1) * bs * nh2 : h->rows;
+		const FcBwdData op{bs, in, nh2, nh2, dz, h->P + S.fwoff[j], xj,
+				   j ? h->fc_dz + (long)(j - 1) * bs * nh2 : h->dz + L.aoff[L.l1 - 1], j ? nullptr : h->rows_grad};
+		launch_gemm(op, 1, s);
+		const FcWgrad og{nh2, in + 1, bs, bs, dz, xj, h->G + S.fwoff[j], h->G + S.fboff[j]};
+		launch_gemm(og, 1, s);
+	}
+	for (int k = L.l1 - 1; k >= 1; k--) {                                    // tower backward
+		const int so = L.ws - 2 * (k + 1), si = so + 2;
+		const ConvBwdData op{fm, L.N * si * si, fm * 9, fm * 9, fm, si, so, h->P + L.woff[k], h->dz + L.aoff[k],
+				     h->act + L.aoff[k - 1], h->dz + L.aoff[k - 1]};
+		launch_gemm(op, 1, s);
+	}
+	for (int k = 0; k < L.l1; k++) {                                         // tower weight gradients, split over k
+		const int cin = k ? fm : 1, so = L.ws - 2 * (k + 1);
+		const ConvWgrad op{fm, cin * 9 + 1, L.N * so * so, S.kchunk[k], cin, so + 2, so, h->dz + L.aoff[k],
+				   k ? h->act + L.aoff[k - 1] : h->X, h->part + S.poff[k]};
+		launch_gemm(op, S.nsplit[k], s);
+	}
+	const long ntower = L.boff[L.l1 - 1] + fm;
+	wgrad_reduce_kernel<<<adc_div_up(ntower, 256), 256, 0, s>>>(L, S, h->part, h->G);
+	update_kernel<<<adc_div_up(h->nparam, 256), 256, 0, s>>>(h->P, h->V, h->G, h->nparam, h->mom, h->neg_lr, h->bce_loss, 1,
+								 h->loss, h->loss_cap, h->ctr);
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
 
 static int enqueue_step(mccnn_trainer *h, cudaStream_t s, bool sample)
 {
@@ -337,6 +623,7 @@ static int enqueue_step(mccnn_trainer *h, cudaStream_t s, bool sample)
 		train_sample_kernel<<<adc_div_up(tot, 128), 128, 0, s>>>(h->X0, h->X1, h->n_img, h->H, h->W, h->warps, h->ctr, L.N,
 								       ws, h->X);
 	}
+	if (h->slow) return enqueue_slow(h, s);
 	tower_fwd_kernel<<<L.N, 256, h->smem, s>>>(L, h->X, h->P, h->act, h->bufsz);
 	head_kernel<<<L.N / 4, 4 * L.fm, 0, s>>>(L, h->act, h->margin, h->pow2, h->norm, h->nout, h->join, h->gjoin, h->hinge,
 						  h->gout, h->dz);
@@ -362,20 +649,34 @@ static int capture(mccnn_trainer *h, bool sample, cudaGraphExec_t *exec)
 	return (int)ei;
 }
 
+// the trainer's buffers by id: the public MCCNN_TRAIN_* ids, then the slow step's internal ones (id >= MCCNN_TRAIN_NBUF).
+// nullptr for an id that does not apply to the handle's arch.
+enum { TRAIN_FC_DZ = MCCNN_TRAIN_NBUF, TRAIN_TERM, TRAIN_DZO, TRAIN_PART, TRAIN_BCE_LOSS, TRAIN_NALL };
+
 static float **train_buffer(mccnn_trainer *h, int what, long *count)
 {
 	const Layout &L = h->L;
-	const long N = L.N, fm = L.fm;
-	struct { float **p; long n; } t[] = {
-		{&h->P, h->nparam}, {&h->V, h->nparam}, {&h->G, h->nparam}, {&h->X, N * L.ws * L.ws},
-		{&h->act, L.aoff[L.l1 - 1] + N * fm}, {&h->norm, N}, {&h->nout, N * fm}, {&h->join, N / 2},
-		{&h->gjoin, N / 2}, {&h->hinge, N / 4}, {&h->gout, N * fm}, {&h->dz, L.aoff[L.l1 - 1] + N * fm},
-		{&h->loss, h->loss_cap},
+	const SlowLayout &S = h->S;
+	const long N = L.N, fm = L.fm, bs = N / 2, nh2 = S.nh2;
+	const int F = !h->slow, Sl = h->slow;
+	struct { float **p; long n; int ok; } t[] = {
+		{&h->P, h->nparam, 1}, {&h->V, h->nparam, 1}, {&h->G, h->nparam, 1}, {&h->X, N * L.ws * L.ws, 1},
+		{&h->act, L.aoff[L.l1 - 1] + N * fm, 1}, {&h->norm, N, F}, {&h->nout, N * fm, F}, {&h->join, N / 2, F},
+		{&h->gjoin, N / 2, F}, {&h->hinge, N / 4, F}, {&h->gout, N * fm, F}, {&h->dz, L.aoff[L.l1 - 1] + N * fm, 1},
+		{&h->loss, h->loss_cap, 1},
+		{&h->rows, bs * 2 * fm, Sl}, {&h->fc, S.l2 * bs * nh2 + bs, Sl}, {&h->sig, bs, Sl}, {&h->bce_grad, bs, Sl},
+		{&h->rows_grad, bs * 2 * fm, Sl},
+		{&h->fc_dz, S.l2 * bs * nh2, Sl}, {&h->term, bs, Sl}, {&h->dzo, bs, Sl},
+		{&h->part, Sl ? S.poff[L.l1 - 1] + (long)S.nsplit[L.l1 - 1] * fm * (fm * 9 + 1) : 0, Sl}, {&h->bce_loss, 1, Sl},
 	};
-	if (what < 0 || what >= (int)(sizeof(t) / sizeof(t[0]))) return nullptr;
+	static_assert(sizeof(t) / sizeof(t[0]) == TRAIN_NALL, "one entry per buffer id");
+	if (what < 0 || what >= TRAIN_NALL || !t[what].ok) return nullptr;
 	*count = t[what].n;
 	return t[what].p;
 }
+
+// ROWS is a view of the tower's last layer (N, fm, 1, 1) = (bs, 2 fm), not an allocation of its own
+static bool owned(int what) { return what != MCCNN_TRAIN_ROWS; }
 
 extern "C" int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n,
 				  int ws, float *out, adcensus_stream_t stream)
@@ -398,7 +699,10 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	if (h->body) cudaGraphExecDestroy(h->body);
 	if (h->cap) cudaStreamDestroy(h->cap);
 	long n;
-	for (int what = 0; what < MCCNN_TRAIN_NBUF; what++) cudaFree(*train_buffer(h, what, &n));
+	for (int what = 0; what < TRAIN_NALL; what++) {
+		float **p = train_buffer(h, what, &n);
+		if (p && owned(what)) cudaFree(*p);
+	}
 	cudaFree(h->neg_lr);
 	cudaFree(h->ctr);
 	cudaFree(h->warps);
@@ -407,17 +711,14 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	return 0;
 }
 
-extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
-				    const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap,
-				    int device, adcensus_stream_t stream)
+static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2, int bs, float margin, int pow, float mom,
+		  const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
+		  adcensus_stream_t stream)
 {
-	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || n_img < 1 || H < 1 ||
-	    W < 1 || chunk < 1 || loss_cap < 1)
-		return ADCENSUS_EINVAL;
-	if (l1 > LMAX || fm > 128 || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
 	*out = nullptr;
 	mccnn_trainer *h = (mccnn_trainer *)calloc(1, sizeof(mccnn_trainer));
 	if (!h) return ADCENSUS_EINVAL;
+	h->slow = slow;
 	Layout &L = h->L;
 	L.l1 = l1; L.fm = fm; L.ws = 1 + 2 * l1; L.N = 2 * bs;
 	long off = 0, aoff = 0;
@@ -426,6 +727,26 @@ extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs,
 		L.woff[k] = off; off += (long)fm * cin * 9;
 		L.boff[k] = off; off += fm;
 		L.aoff[k] = aoff; aoff += (long)L.N * fm * s * s;
+	}
+	if (slow) {
+		SlowLayout &S = h->S;
+		S.l2 = l2; S.nh2 = nh2;
+		for (int j = 0; j <= l2; j++) {
+			const int in = j ? nh2 : 2 * fm, o = j < l2 ? nh2 : 1;
+			S.fwoff[j] = off; off += (long)o * in;
+			S.fboff[j] = off; off += o;
+		}
+		// split k so that each weight-gradient GEMM has about 256 blocks of at least 256 k each; the split depends on the
+		// shapes only, so the summation order (and the bits) do not depend on the device
+		long poff = 0;
+		for (int k = 0; k < l1; k++) {
+			const int cin = k ? fm : 1, s = L.ws - 2 * (k + 1), K = L.N * s * s;
+			const int tiles = adc_div_up(fm, BM) * adc_div_up(cin * 9 + 1, BN);
+			const int want = std::max(1, std::min(adc_div_up(256, tiles), adc_div_up(K, 256)));
+			S.kchunk[k] = adc_div_up(adc_div_up(K, want), BK) * BK;
+			S.nsplit[k] = adc_div_up(K, S.kchunk[k]);
+			S.poff[k] = poff; poff += (long)S.nsplit[k] * fm * (cin * 9 + 1);
+		}
 	}
 	h->nparam = off;
 	h->bufsz = L.ws * L.ws;
@@ -440,15 +761,19 @@ extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs,
 	int rc = (int)cudaSetDevice(device);
 	int optin = 0;
 	if (!rc) rc = (int)cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
-	if (!rc && h->smem > optin) rc = ADCENSUS_ELIMIT;
-	if (!rc) rc = (int)cudaFuncSetAttribute(tower_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
-	if (!rc) rc = (int)cudaFuncSetAttribute(tower_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
-	for (int what = 0; what < MCCNN_TRAIN_NBUF && !rc; what++) {
+	if (!slow) {
+		if (!rc && h->smem > optin) rc = ADCENSUS_ELIMIT;
+		if (!rc) rc = (int)cudaFuncSetAttribute(tower_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+		if (!rc) rc = (int)cudaFuncSetAttribute(tower_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+	}
+	for (int what = 0; what < TRAIN_NALL && !rc; what++) {
 		long n;
 		float **p = train_buffer(h, what, &n);
+		if (!p || !owned(what)) continue;
 		rc = (int)cudaMalloc((void **)p, (size_t)n * sizeof(float));
 		if (!rc) rc = (int)cudaMemsetAsync(*p, 0, (size_t)n * sizeof(float), adc_stream(stream));
 	}
+	if (slow) h->rows = h->act + L.aoff[l1 - 1];
 	if (!rc) rc = (int)cudaMalloc((void **)&h->neg_lr, sizeof(float));
 	if (!rc) rc = (int)cudaMemsetAsync(h->neg_lr, 0, sizeof(float), adc_stream(stream));
 	if (!rc) rc = (int)cudaMalloc((void **)&h->ctr, 2 * sizeof(int));
@@ -466,6 +791,30 @@ extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs,
 	}
 	*out = h;
 	return 0;
+}
+
+extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
+				    const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap,
+				    int device, adcensus_stream_t stream)
+{
+	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || n_img < 1 || H < 1 ||
+	    W < 1 || chunk < 1 || loss_cap < 1)
+		return ADCENSUS_EINVAL;
+	if (l1 > LMAX || fm > 128 || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
+	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, X0, X1, n_img, H, W, chunk, loss_cap, device, stream);
+}
+
+extern "C" int mccnn_trainer_create_slow(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
+					 const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap,
+					 int device, adcensus_stream_t stream)
+{
+	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || n_img < 1 || H < 1 ||
+	    W < 1 || chunk < 1 || loss_cap < 1)
+		return ADCENSUS_EINVAL;
+	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) || H > 32767 ||
+	    W > 32767 || (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31))
+		return ADCENSUS_ELIMIT;
+	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, X0, X1, n_img, H, W, chunk, loss_cap, device, stream);
 }
 
 static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
@@ -512,14 +861,14 @@ extern "C" int mccnn_trainer_step_patches(mccnn_trainer *h, const float *patches
 extern "C" long long mccnn_trainer_size(mccnn_trainer *h, int what)
 {
 	long n = 0;
-	if (!h || !train_buffer(h, what, &n)) return -1;
+	if (!h || what >= MCCNN_TRAIN_NBUF || !train_buffer(h, what, &n)) return -1;
 	return n;
 }
 
 extern "C" int mccnn_trainer_get(mccnn_trainer *h, int what, float *dst, adcensus_stream_t stream)
 {
 	long n = 0;
-	float **p = h ? train_buffer(h, what, &n) : nullptr;
+	float **p = h && what < MCCNN_TRAIN_NBUF ? train_buffer(h, what, &n) : nullptr;
 	if (!p || !dst) return ADCENSUS_EINVAL;
 	return (int)cudaMemcpyAsync(dst, *p, (size_t)n * sizeof(float), cudaMemcpyDefault, adc_stream(stream));
 }
@@ -540,7 +889,8 @@ extern "C" int mccnn_trainer_reset_losses(mccnn_trainer *h, adcensus_stream_t st
 
 extern "C" int mccnn_trainer_launches_per_step(mccnn_trainer *h)
 {
-	return h ? 5 + h->L.l1 : -1;
+	if (!h) return -1;
+	return h->slow ? 3 + 3 * h->L.l1 + 3 * h->S.l2 : 5 + h->L.l1;
 }
 
 extern "C" int mccnn_randperm_swaps(long long *perm, long long n, long long i0, const unsigned *draws, long long k)

@@ -1,7 +1,9 @@
-"""main.lua's ``-a train_tr`` / ``-a train_all`` (main.lua:602-890) for the fast architecture on KITTI 2012 / 2015.
+"""main.lua's ``-a train_tr`` / ``-a train_all`` (main.lua:602-890) for the fast and slow architectures on KITTI 2012 / 2015.
 
     opt = options("kitti", lr=0.002)                                   # main.lua's presets (:34-49, :206-262) + overrides
     fname = train("kitti", "train_tr", opt, data_root=".", seed=42)   # 14 epochs, net/net_<cmd_str>.t7, then test_te
+    opt = options("kitti", "slow")                                     # arch 'slow' (:70-114): l2, nh2; no -m / -pow
+    fname = train("kitti", "train_all", opt, args=["-a", "train_all"])  # ... then submit
 
 Per step (bs / 2 samples of four ws x ws patches, ws = 1 + 2 l1): the host draws the augmentation parameters and builds each
 patch's float 2x3 matrix as make_patch does (:607-619); the GPU (csrc/train.cu) warps the patches out of the device-resident
@@ -16,13 +18,20 @@ torch.uniform calls of :791-818 in order, each r / 2^32 * (b - a) + a in double 
 Torch7 is not available to compare against, so parity with Torch7 itself is **unpinned**, as in :mod:`preprocess`; the stream
 is pinned against ``preprocess.MT19937`` and the line-by-line restatement in oracle/train.py.
 
+Arch 'slow' (net_tr of main.lua:663-677, BCECriterion2): the stream is consumed as randperm, net_tr's constructors (each
+convolution's reset(), then each nn.Linear's: weight (out, in) in order, then bias, U(-1/sqrt(in), +1/sqrt(in))), then
+net_te's l1 convolutions constructed anew -- their reset() draws are thrown away when the weights are tied (:697-724), but
+they advance the stream; SpatialConvolution1_fw draws nothing -- then the per-sample draws as for 'fast'.  This order is
+read from the sources; parity with Torch7 is unpinned, and it is pinned against oracle/train_slow.py.
+
 Deliberate deviations from main.lua:
 
-* only arch 'fast' and datasets kitti / kitti2015; ``-at 1``, ``-subset`` < 1 and ``-debug`` are refused;
+* only archs 'fast' and 'slow' and datasets kitti / kitti2015; ``-at 1``, ``-subset`` < 1 and ``-debug`` are refused;
 * the net file goes to ``<data_root>/net/`` and an existing file is refused; the file name is built from main.lua's options
   only (``-data_root`` and ``-out`` are not part of it);
 * Margin2's loss is the hinge terms summed in order, then divided by bs / 2 (Torch7's ``mean`` reduces in another order),
-  and the convolutions accumulate in another order than cuDNN: both are fp32.
+  BCECriterion2's ``sum`` is taken in row order, and the convolutions and Linear layers accumulate in another order than
+  cuDNN / cuBLAS: all are fp32.
 """
 import ctypes
 import math
@@ -42,9 +51,13 @@ TWO32 = 1.0 / 4294967296.0
 AUGMENT = dict(hflip=0, vflip=0, rotate=7.0, hscale=0.9, scale=1.0, trans=0.0, hshear=0.1, brightness=0.7, contrast=1.3,
                d_vtrans=0.0, d_rotate=0.0, d_hscale=1.0, d_hshear=0.0, d_brightness=0.3, d_contrast=1.0)
 NET = dict(at=0, m=0.2, pow=1, l1=4, fm=64, ks=3, lr=0.002, bs=128, mom=0.9, true1=1.0, false1=4.0, false2=10.0)
+# main.lua:70-84 (arch 'slow', kitti / kitti2015)
+NET_SLOW = dict(at=0, l1=4, fm=112, ks=3, l2=4, nh2=384, lr=0.003, bs=128, mom=0.9, true1=1.0, false1=4.0, false2=10.0)
+PRESETS = {"fast": NET, "slow": NET_SLOW}
 WARP_DTYPE = np.dtype([("m", "<f4", (6,)), ("contrast", "<f4"), ("brightness", "<f4"), ("image", "<i4"), ("view", "<i4")])
 TRAIN_PARAMS, TRAIN_MOMENTA, TRAIN_GRADS, TRAIN_PATCHES, TRAIN_TOWER, TRAIN_NORM, TRAIN_NORMALIZED, TRAIN_JOIN, \
     TRAIN_JOIN_GRAD, TRAIN_HINGE, TRAIN_NORM_GRAD_OUT, TRAIN_DZ, TRAIN_LOSS = range(13)
+TRAIN_ROWS, TRAIN_FC, TRAIN_SIGMOID, TRAIN_BCE_GRAD, TRAIN_ROWS_GRAD = range(13, 18)      # arch 'slow' only
 
 
 def options(dataset, arch="fast", **overrides):
@@ -53,19 +66,23 @@ def options(dataset, arch="fast", **overrides):
         raise ValueError("dataset mb: Middlebury training (the light and exposure sampler) is not supported")
     if dataset not in ("kitti", "kitti2015"):
         raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
-    if arch != "fast":
-        raise ValueError("arch %s: only the fast architecture can be trained" % arch)
-    o = dict(AUGMENT, **NET)
+    if arch not in PRESETS:
+        raise ValueError("arch %s: only the fast and slow architectures can be trained" % arch)
+    o = dict(AUGMENT, **PRESETS[arch])
     for k, v in overrides.items():
         if k not in o:
-            raise ValueError("unknown training option -%s" % k)
+            raise ValueError("-%s is not a training option of arch %s" % (k, arch))
         o[k] = type(o[k])(v)
     check(o)
     return o
 
 
+def arch_of(o):
+    return "slow" if "l2" in o else "fast"
+
+
 def check(o):
-    """main.lua's asserts (:797, :810) and the limits of csrc/train.cu and the inference feature tower"""
+    """main.lua's asserts (:797, :810) and the limits of csrc/train.cu and the inference feature tower / scorer head"""
     if o["at"]:
         raise ValueError("-at 1 (the combined KITTI 2012 + 2015 training set) is not supported")
     if o["ks"] != 3:
@@ -76,8 +93,12 @@ def check(o):
         raise ValueError("-fm %d: the feature tower runs 16 to 128 planes in steps of 16" % o["fm"])
     if o["bs"] < 2 or o["bs"] % 2:
         raise ValueError("-bs %d: the batch size must be even and at least 2" % o["bs"])
-    if o["pow"] not in (1, 2):
+    if "pow" in o and o["pow"] not in (1, 2):
         raise ValueError("-pow %d: Margin2 takes pow 1 or 2" % o["pow"])
+    if "l2" in o and not 1 <= o["l2"] <= 4:
+        raise ValueError("-l2 %d: the scorer head runs 1 to 4 hidden layers" % o["l2"])
+    if "nh2" in o and o["nh2"] not in (128, 256, 384):
+        raise ValueError("-nh2 %d: the scorer head runs 128, 256 or 384 units" % o["nh2"])
     if not (o["hscale"] <= 1 and o["scale"] <= 1):
         raise ValueError("-hscale and -scale must be <= 1 (main.lua:797)")
     if not (o["contrast"] >= 1 and o["d_contrast"] >= 1):
@@ -95,13 +116,21 @@ def lr_at(lr, epoch):
     return lr / 10 if epoch >= LR_DROP_EPOCH else lr
 
 
-def cmd_str(dataset, args):
+def cmd_str(dataset, args, arch="fast"):
     """save_net's name stem (main.lua:344-347): dataset_arch then '_' + each further argument"""
-    return "_".join([dataset, "fast"] + list(args))
+    return "_".join([dataset, arch] + list(args))
 
 
 def net_lines(o):
-    """print_net(net_tr) (main.lua:542-564, 751)"""
+    """print_net(net_tr) (main.lua:542-564, 751); for 'slow' the other modules as the nn of that era prints them (unpinned)"""
+    if arch_of(o) == "slow":
+        out = []
+        for i in range(o["l1"]):
+            out += ["conv(in=%d, out=%d, k=%d)" % (1 if i == 0 else o["fm"], o["fm"], o["ks"]), "cudnn.ReLU"]
+        out.append("nn.Reshape(%dx%d)" % (o["bs"], 2 * o["fm"]))
+        for i in range(o["l2"]):
+            out += ["nn.Linear(%d -> %d)" % (2 * o["fm"] if i == 0 else o["nh2"], o["nh2"]), "cudnn.ReLU"]
+        return out + ["nn.Linear(%d -> 1)" % o["nh2"], "cudnn.Sigmoid"]
     out = []
     for i in range(o["l1"]):
         out.append("conv(in=%d, out=%d, k=%d)" % (1 if i == 0 else o["fm"], o["fm"], o["ks"]))
@@ -153,6 +182,28 @@ def init_weights(stream, l1, fm, n_in=1, ks=3):
         b = stream.uniform(fm, -stdv, stdv).astype(np.float32)
         out.append((w, b))
     return out
+
+
+def init_linear(stream, n_in, n_out):
+    """nn.Linear(n_in, n_out):reset(): weight (out, in) then bias, U(-1/sqrt(in), +1/sqrt(in)) -> (W, b) float32"""
+    stdv = 1 / math.sqrt(n_in)
+    w = stream.uniform(n_out * n_in, -stdv, stdv).astype(np.float32).reshape(n_out, n_in)
+    return w, stream.uniform(n_out, -stdv, stdv).astype(np.float32)
+
+
+def init_slow(stream, o):
+    """arch 'slow': net_tr's constructors, then net_te's convolutions, whose draws are thrown away (main.lua:663-695)
+    -> (tower, head)"""
+    tower = init_weights(stream, o["l1"], o["fm"])
+    head = [init_linear(stream, 2 * o["fm"] if i == 0 else o["nh2"], o["nh2"]) for i in range(o["l2"])]
+    head.append(init_linear(stream, o["nh2"], 1))
+    init_weights(stream, o["l1"], o["fm"])
+    return tower, head
+
+
+def init_net(stream, o):
+    """the reset() draws of either arch -> (tower, head); head None for 'fast'"""
+    return init_slow(stream, o) if arch_of(o) == "slow" else (init_weights(stream, o["l1"], o["fm"]), None)
 
 
 def draw_params(stream, o, n):
@@ -251,7 +302,8 @@ def sample_patches(X0, X1, warps, ws):
 
 
 class Trainer:
-    """csrc/train.cu's trainer: net_tr + Margin2 + the momentum update on `device`, sampling from X0 / X1 (CUDA)."""
+    """csrc/train.cu's trainer: net_tr + Margin2 ('fast') or + BCECriterion2 ('slow', when `o` has l2) and the momentum
+    update on `device`, sampling from X0 / X1 (CUDA)."""
 
     def __init__(self, o, X0, X1, chunk=CHUNK, loss_cap=1, device=None):
         import torch
@@ -260,7 +312,9 @@ class Trainer:
 
         self.o, self.chunk = o, chunk
         self.dev = X0.device if device is None else torch.device("cuda", device)
+        self.arch = arch_of(o)
         self.l1, self.fm, self.bs = o["l1"], o["fm"], o["bs"]
+        self.l2, self.nh2 = o.get("l2"), o.get("nh2")
         self.ws = 1 + 2 * self.l1
         self.N = 2 * self.bs
         self._keep = (X0, X1)
@@ -268,10 +322,16 @@ class Trainer:
         self._h = ctypes.c_void_p()
         with torch.cuda.device(self.dev):
             self.stream = torch.cuda.current_stream(self.dev)
-            _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, ctypes.c_float(o["m"]),
-                                              o["pow"], ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
-                                              _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
-                                              _stream(X0)), "mccnn_trainer_create")
+            if self.arch == "slow":
+                _check(lib().mccnn_trainer_create_slow(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2, self.bs,
+                                                       ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
+                                                       _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
+                                                       _stream(X0)), "mccnn_trainer_create_slow")
+            else:
+                _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, ctypes.c_float(o["m"]),
+                                                  o["pow"], ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
+                                                  _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
+                                                  _stream(X0)), "mccnn_trainer_create")
         self.launches_per_step = lib().mccnn_trainer_launches_per_step(self._h)
 
     def close(self):
@@ -317,11 +377,18 @@ class Trainer:
         _check(lib().mccnn_trainer_set(self._h, what, ctypes.c_void_p(t.data_ptr()), self._s()), "mccnn_trainer_set")
         self.stream.synchronize()
 
-    def set_layers(self, layers):
-        self.set(TRAIN_PARAMS, flatten(layers))
+    def set_layers(self, layers, head=None):
+        self.set(TRAIN_PARAMS, flatten(list(layers) + list(head or [])))
 
     def layers(self, what=TRAIN_PARAMS):
+        """the tower's (W, b) of the parameters, momenta or gradients"""
         return unflatten(self.get(what).cpu().numpy(), self.l1, self.fm)
+
+    def net(self, what=TRAIN_PARAMS):
+        """(tower, head) of the parameters, momenta or gradients; head None for 'fast'"""
+        v = self.get(what).cpu().numpy()
+        tower = unflatten(v, self.l1, self.fm)
+        return tower, (unflatten_head(v, self.l1, self.fm, self.l2, self.nh2) if self.arch == "slow" else None)
 
     def run(self, warps, lr):
         """len(warps) / N steps (<= chunk) from a WARP_DTYPE array (pinned host or CUDA uint8 tensor, or numpy)"""
@@ -370,6 +437,19 @@ def unflatten(v, l1, fm):
     return out
 
 
+def unflatten_head(v, l1, fm, l2, nh2):
+    """the Linear layers' (W (out, in), b (out,)) after the tower's parameters"""
+    o = sum(fm * (1 if i == 0 else fm) * 9 + fm for i in range(l1))
+    out = []
+    for j in range(l2 + 1):
+        n_in, n_out = 2 * fm if j == 0 else nh2, nh2 if j < l2 else 1
+        w = v[o:o + n_out * n_in].reshape(n_out, n_in)
+        o += n_out * n_in
+        out.append((w.copy(), v[o:o + n_out].copy()))
+        o += n_out
+    return out
+
+
 def load_nnz(data, action, data_root):
     d = os.path.join(data_root, "data.kitti" if data.dataset == "kitti" else "data.kitti2015")
     nnz = evaluate._fromfile(os.path.join(d, "nnz_tr.bin"))
@@ -381,12 +461,12 @@ def load_nnz(data, action, data_root):
     return nnz
 
 
-def net_path(data_root, dataset, args):
-    return os.path.join(data_root, "net", "net_%s.t7" % cmd_str(dataset, args))
+def net_path(data_root, dataset, args, arch="fast"):
+    return os.path.join(data_root, "net", "net_%s.t7" % cmd_str(dataset, args, arch))
 
 
 def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS):
-    """main.lua:602-890 for arch 'fast': returns the saved net's file name.  `args` are main.lua's arguments after
+    """main.lua:602-890 for arch 'fast' or 'slow' (as `o` was made): returns the saved net's file name.  `args` are main.lua's arguments after
     dataset and arch (for the file name), `stereo` the stereo method's overrides for the evaluation that follows;
     `log` receives the printed lines."""
     import torch
@@ -396,7 +476,8 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     if action not in ("train_tr", "train_all"):
         raise ValueError("action must be train_tr or train_all, got %r" % (action,))
     check(o)
-    fname = net_path(data_root, dataset, args)
+    arch = arch_of(o)
+    fname = net_path(data_root, dataset, args, arch)
     if os.path.exists(fname):
         raise FileExistsError("%s already exists; remove it first" % fname)
     if action == "train_all" and os.path.isdir(out) and any(f != ".empty" for f in os.listdir(out)):
@@ -405,7 +486,7 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     nnz = load_nnz(data, action, data_root)
     stream = Stream(seed)                                                        # main.lua:340
     perm = randperm(stream, len(nnz))                                            # :657
-    layers = init_weights(stream, o["l1"], o["fm"])                              # :726-736
+    tower, head = init_net(stream, o)                                            # :663-736
     for line in net_lines(o):
         log(line)
     h = o["bs"] // 2
@@ -416,7 +497,7 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
         X1 = torch.from_numpy(np.ascontiguousarray(data.X1, np.float32)).to(dev)
         tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
         try:
-            tr.set_layers(layers)
+            tr.set_layers(tower, head)
             rec = WARP_DTYPE.itemsize * tr.N
             pinned = [torch.empty(CHUNK * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
             events = [None, None]
@@ -443,12 +524,12 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
                     log("WARNING! err=%f" % v)
                 err = np.cumsum(losses[ok])[-1] / ok.sum() if ok.any() else float("nan")
                 log(epoch_line(epoch, err, lr, time.time() - t0))
-            trained = tr.layers()
+            tower, head = tr.net()
         finally:
             tr.close()
     os.makedirs(os.path.dirname(fname), exist_ok=True)
-    t7.save_net(fname, trained, opt=dict(o, a=action, seed=seed, gpu=device + 1))   # :883, save_net(0)
-    ev = evaluate.Evaluator(dataset, "fast", net_fname=fname, device=device, **(stereo or {}))
+    t7.save_net(fname, tower, head, opt=dict(o, a=action, seed=seed, gpu=device + 1))   # :883, save_net(0)
+    ev = evaluate.Evaluator(dataset, arch, net_fname=fname, device=device, **(stereo or {}))
     try:
         if action == "train_tr":                                                 # :884-888
             ev.test("test_te", data_root=data_root, data=data)

@@ -1,6 +1,6 @@
-"""Measure the training step of the fast architecture (csrc/train.cu) on a synthetic full-size KITTI 2012 set.
+"""Measure the training step of the fast or slow architecture (csrc/train.cu) on a synthetic full-size KITTI 2012 set.
 
-    python tools/time_train.py [-steps 2000] [-gpu 1] [-json out.json]
+    python tools/time_train.py [-arch fast|slow] [-steps 2000] [-gpu 1] [-json out.json]
 
 The set is 389 views of 350 x 1242 per side on the device and 1,048,576 nnz rows, at main.lua's kitti presets (l1 4, fm 64,
 bs 128).  Reported, each after a warm-up:
@@ -10,6 +10,8 @@ bs 128).  Reported, each after a warm-up:
 * baseline: the same step written with torch autograd / cuDNN in fp32 (conv2d, the Normalize2 / StereoJoin1 / Margin2 formulas,
   the momentum update as main.lua:871-874) on patches from the same sampler, TF32 off.
 
+With -arch slow (l1 4, fm 112, l2 4, nh2 384, bs 128) the baseline is net_tr + BCECriterion2 + the update in autograd, and
+the device and baseline runs alternate three times in the one call (each round is reported, then the medians).
 The card's name and power limit are printed with the numbers.
 """
 import argparse
@@ -54,11 +56,36 @@ def baseline_step(x, params, vel, o, lr):
     return loss
 
 
+def baseline_step_slow(x, params, vel, o, lr):
+    import torch
+
+    F = torch.nn.functional
+    h = x
+    for i in range(o["l1"]):
+        h = torch.relu(F.conv2d(h, params[2 * i], params[2 * i + 1]))
+    h = h.reshape(o["bs"], -1)
+    k = 2 * o["l1"]
+    for j in range(o["l2"] + 1):
+        h = F.linear(h, params[k + 2 * j], params[k + 2 * j + 1])
+        if j < o["l2"]:
+            h = torch.relu(h)
+    y = torch.sigmoid(h).reshape(-1)
+    t = torch.arange(o["bs"], device=x.device).remainder(2).float()
+    loss = -((torch.log(y + 1e-12) * t + torch.log(1 - y + 1e-12) * (1 - t)) / o["bs"]).sum()
+    grads = torch.autograd.grad(loss, params)
+    with torch.no_grad():
+        for p, v, g in zip(params, vel, grads):
+            v.mul_(o["mom"]).add_(g, alpha=-lr)
+            p.add_(v)
+    return loss
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("-steps", type=int, default=2000)
     ap.add_argument("-gpu", type=int, default=1)
     ap.add_argument("-json", default="")
+    ap.add_argument("-arch", choices=("fast", "slow"), default="fast")
     args = ap.parse_args(argv)
     import torch
 
@@ -69,7 +96,7 @@ def main(argv=None):
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda", args.gpu - 1)
     torch.cuda.set_device(dev)
-    o = train.options("kitti")
+    o = train.options("kitti", args.arch)
     n_img, H, W, rows = 389, 350, 1242, 1 << 20
     g = torch.Generator(device=dev).manual_seed(0)
     X0 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
@@ -81,9 +108,11 @@ def main(argv=None):
     perm = train.randperm(s, rows)
     chunk = train.CHUNK
     tr = train.Trainer(o, X0, X1, chunk=chunk, loss_cap=args.steps + 4 * chunk, device=dev.index)
-    tr.set_layers(train.init_weights(s, o["l1"], o["fm"]))
+    tr.set_layers(*train.init_net(s, o))
     h = o["bs"] // 2
     res = dict(card=card(), launches_per_step=tr.launches_per_step, steps=args.steps)
+    if args.arch == "slow":
+        res["arch"] = "slow"
 
     def warps_for(s0, n):
         r = nnz[perm[(s0 * h) % (rows - n * h):][:n * h] - 1]
@@ -93,15 +122,18 @@ def main(argv=None):
     dw = torch.from_numpy(warps_for(0, chunk).view(np.uint8)).to(dev)
     tr.run(dw, o["lr"])
     torch.cuda.synchronize()
-    n = 0
-    t0 = time.perf_counter()
-    while n < args.steps:
-        tr.run(dw, o["lr"])
-        n += chunk
-    torch.cuda.synchronize()
-    dt = time.perf_counter() - t0
-    res["device_steps_per_s"] = n / dt
-    res["device_samples_per_s"] = n * h / dt
+
+    def device_rate():
+        n = 0
+        t0 = time.perf_counter()
+        while n < args.steps:
+            tr.run(dw, o["lr"])
+            n += chunk
+        torch.cuda.synchronize()
+        return n / (time.perf_counter() - t0)
+
+    res["device_steps_per_s"] = device_rate()
+    res["device_samples_per_s"] = res["device_steps_per_s"] * h
 
     # driver: host-built chunks through two pinned buffers, as train.train does
     rec = train.WARP_DTYPE.itemsize * tr.N
@@ -131,23 +163,37 @@ def main(argv=None):
     res["host_build_s_per_step"] = (time.perf_counter() - t) / chunk
 
     # baseline: torch autograd / cuDNN on the sampler's patches
-    layers = tr.layers()
+    tower, head = tr.net()
     params = []
-    for w, b_ in layers:
+    for w, b_ in tower + (head or []):
         params += [torch.from_numpy(w).to(dev).requires_grad_(), torch.from_numpy(b_).to(dev).requires_grad_()]
     vel = [torch.zeros_like(p) for p in params]
     x = tr.get(train.TRAIN_PATCHES).reshape(tr.N, 1, tr.ws, tr.ws)
+    step = baseline_step_slow if args.arch == "slow" else baseline_step
     for _ in range(50):
-        baseline_step(x, params, vel, o, o["lr"])
+        step(x, params, vel, o, o["lr"])
     torch.cuda.synchronize()
     nb = max(200, args.steps // 4)
-    t0 = time.perf_counter()
-    for _ in range(nb):
-        baseline_step(x, params, vel, o, o["lr"])
-    torch.cuda.synchronize()
-    dt = time.perf_counter() - t0
-    res["baseline_steps_per_s"] = nb / dt
-    res["baseline_samples_per_s"] = nb * h / dt
+
+    def baseline_rate():
+        t0 = time.perf_counter()
+        for _ in range(nb):
+            step(x, params, vel, o, o["lr"])
+        torch.cuda.synchronize()
+        return nb / (time.perf_counter() - t0)
+
+    res["baseline_steps_per_s"] = baseline_rate()
+    res["baseline_samples_per_s"] = res["baseline_steps_per_s"] * h
+    if args.arch == "slow":                                     # alternate the two in this one call
+        rounds = [(res["device_steps_per_s"], res["baseline_steps_per_s"])]
+        for _ in range(2):
+            rounds.append((device_rate(), baseline_rate()))
+        res["rounds_device_baseline_steps_per_s"] = rounds
+        res["device_steps_per_s"] = float(np.median([r[0] for r in rounds]))
+        res["baseline_steps_per_s"] = float(np.median([r[1] for r in rounds]))
+        res["device_samples_per_s"] = res["device_steps_per_s"] * h
+        res["baseline_samples_per_s"] = res["baseline_steps_per_s"] * h
+        res["device_ms_per_step"] = 1e3 / res["device_steps_per_s"]
     tr.close()
     print(json.dumps(res, indent=1))
     if args.json:

@@ -7,6 +7,7 @@ Option names and defaults are main.lua's (-gpu is 1-based as there): the network
 -mom -true1 -false1 -false2 -m -pow), the augmentation options (-hflip ... -d_contrast) and the stereo method's overrides of
 run_main.py (-L1 ... -blur_t) for the evaluation that follows.  The net goes to <data_root>/net/net_<cmd_str>.t7, named from
 main.lua's arguments.  Everything the trainer does not implement is refused before any GPU work; see mc-cnn_b200/train.py.
+The slow architecture is trained by tools/train_slow.py, which shares this parser.
 """
 import argparse
 import os
@@ -19,10 +20,10 @@ from run_main import PRESET_OPTIONS, _flag  # noqa: E402
 TOOL_ONLY = ("-data_root", "-out")
 
 
-def parser():
+def parser(prog="train.py", description=__doc__.splitlines()[0]):
     from mccnn_b200 import train
 
-    ap = argparse.ArgumentParser(prog="train.py", description=__doc__.splitlines()[0])
+    ap = argparse.ArgumentParser(prog=prog, description=description)
     ap.add_argument("dataset", choices=("kitti", "kitti2015", "mb"))
     ap.add_argument("arch", choices=("fast", "slow", "ad", "census"))
     ap.add_argument("-a", default="train_tr")
@@ -32,7 +33,7 @@ def parser():
     ap.add_argument("-out", default="out")
     ap.add_argument("-subset", type=float, default=1)
     ap.add_argument("-debug", nargs="?", const=True, default=False, type=_flag)
-    for name, v in dict(train.AUGMENT, **train.NET).items():
+    for name, v in {**train.AUGMENT, **train.NET, **train.NET_SLOW}.items():
         ap.add_argument("-" + name, type=type(v), default=None)
     for name, typ in PRESET_OPTIONS.items():
         ap.add_argument("-" + name, type=typ, default=None)
@@ -52,39 +53,50 @@ def main_args(argv):
     return out
 
 
-def parse_args(argv=None):
-    """-> (namespace, training options, stereo overrides).  Refuses what the trainer does not implement."""
+# the tools and the architecture each trains; the other one is named in the refusal
+TOOLS = {"fast": "train.py", "slow": "train_slow.py"}
+
+
+def parse_args(argv=None, arch="fast"):
+    """-> (namespace, training options, stereo overrides).  Refuses what the trainer does not implement, and every arch
+    but `arch`."""
     from mccnn_b200 import train
 
+    prog = TOOLS[arch]
     argv = list(sys.argv[1:] if argv is None else argv)
-    args = parser().parse_args(argv)
+    args = parser(prog).parse_args(argv)
+    if args.arch != arch:
+        other = [TOOLS[a] for a in TOOLS if a == args.arch]
+        raise SystemExit("%s: arch %s: only the %s architecture can be trained by this tool%s"
+                         % (prog, args.arch, arch, "; use %s" % other[0] if other else ""))
     if args.a not in ("train_tr", "train_all"):
-        raise SystemExit("train.py: -a %s is not a training action (train_tr, train_all); see run_main.py" % args.a)
+        raise SystemExit("%s: -a %s is not a training action (train_tr, train_all); see run_main.py" % (prog, args.a))
     if args.gpu < 1:
-        raise SystemExit("train.py: -gpu is 1-based")
+        raise SystemExit("%s: -gpu is 1-based" % prog)
     if args.subset < 1:
-        raise SystemExit("train.py: -subset %s is not supported (the whole training set is used)" % args.subset)
+        raise SystemExit("%s: -subset %s is not supported (the whole training set is used)" % (prog, args.subset))
     if args.debug:
-        raise SystemExit("train.py: -debug (a net file per epoch) is not supported")
-    given = {k: getattr(args, k) for k in dict(train.AUGMENT, **train.NET) if getattr(args, k) is not None}
+        raise SystemExit("%s: -debug (a net file per epoch) is not supported" % prog)
+    names = {**train.AUGMENT, **train.NET, **train.NET_SLOW}
+    given = {k: getattr(args, k) for k in names if getattr(args, k) is not None}
     try:
         o = train.options(args.dataset, args.arch, **given)
     except ValueError as e:
-        raise SystemExit("train.py: %s" % e)
+        raise SystemExit("%s: %s" % (prog, e))
     stereo = {k: getattr(args, k) for k in PRESET_OPTIONS if getattr(args, k) is not None}
     args.device = args.gpu - 1
     args.argv = argv
     return args, o, stereo
 
 
-def main(argv=None):
-    args, o, stereo = parse_args(argv)
+def main(argv=None, arch="fast"):
+    args, o, stereo = parse_args(argv, arch)
     import mccnn_b200  # noqa: F401
     from mccnn_b200 import train
 
-    fname = train.net_path(args.data_root, args.dataset, main_args(args.argv))
+    fname = train.net_path(args.data_root, args.dataset, main_args(args.argv), arch)
     if os.path.exists(fname):
-        raise SystemExit("train.py: %s already exists; remove it first" % fname)
+        raise SystemExit("%s: %s already exists; remove it first" % (TOOLS[arch], fname))
     print(" ".join(args.argv) + " ", flush=True)                                  # main.lua:6-9
     train.train(args.dataset, args.a, o, args=main_args(args.argv), data_root=args.data_root, seed=args.seed,
                 device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True))
