@@ -13,7 +13,7 @@
  * Conventions
  *   - every pointer is a DEVICE pointer to contiguous float32 (the reference
  *     ignores strides: raw THCudaTensor_data + sizes);
- *   - shapes: features (C,H,W); cost volumes (D,H,W); SGM volumes (H,W,D); `*_pitched` / `*_dhw` entry points take
+ *   - shapes: features (C,H,W); cost volumes (D,H,W); SGM volumes (H,W,D); `*_pitched` entry points take
  *     (D,H,ld) volumes with a row pitch ld (the fused pipeline's private layout);
  *     images / disparity maps (H,W); cross arms (4,H,W);
  *   - `stream` is a cudaStream_t (0 = legacy default stream, what the
@@ -114,14 +114,6 @@ int mccnn_cbca_fast_pitched_packed(const void *hv, const float *vol_in, float *v
 int adcensus_sgm2(const float *x0, const float *x1, const float *input, float *output, float *tmp,
 		  int H, int W, int D, float pi1, float pi2, float tau_so, float alpha1,
 		  float sgm_q1, float sgm_q2, int direction, adcensus_stream_t stream);
-
-/* sgm2 on pitched (D, H, ld) volumes, no permutes (csrc/sgm_dhw.cu): output = sum of the four directional costs of
- * input (right, left, down, up: the reference's accumulation order, bit-identical values), times 1/4 when div4 != 0
- * (main.lua:1008-1020 in one call).  ld % 4 == 0, ld >= W rounded up to 4, 16-byte aligned bases; output need not be
- * initialised and its padding columns receive unspecified values. */
-int mccnn_sgm2_dhw(const float *x0, const float *x1, const float *input, float *output,
-		   int H, int W, int ld, int D, float pi1, float pi2, float tau_so, float alpha1,
-		   float sgm_q1, float sgm_q2, int direction, int div4, adcensus_stream_t stream);
 
 /* Band-wise sgm2 for the row-band / column-band multi-GPU split: x0, x1 are the FULL Ht x Wt images,
  * input/output this GPU's band volume (H,W,D) at image offset (yoff, xoff); pass_mask selects scan
@@ -241,14 +233,11 @@ size_t mccnn_pipeline_device_bytes(const mccnn_pipeline *p);
  * reference.  ADCENSUS_CBCA_EXACT=1 in the environment makes 0 the default. */
 void mccnn_pipeline_set_cbca_mode(mccnn_pipeline *p, int mode);
 int mccnn_pipeline_get_cbca_mode(const mccnn_pipeline *p);
-/* SGM data layout inside the pipeline: 0 (default) = permute the pitched volume to (H,W,D) and back around sgm2 like
- * main.lua:1008-1020 (fused /4); 1 = scan the (D,H,ld) layout directly (mccnn_sgm2_dhw, no permutes).  Bit-identical
- * results either way; ADCENSUS_SGM_DHW=1 in the environment makes 1 the default. */
-void mccnn_pipeline_set_sgm_layout(mccnn_pipeline *p, int dhw);
-/* opt-in: run the two directions of main.lua:955 concurrently (0 = off: one stream, 4V of volume buffers;
- * 1 = direction -1 on a side stream with its own 2V + tables, started when direction +1 reaches its SGM phase;
- * 2 = additionally the permute / SGM phases on high-priority streams).  Results are identical in every mode
- * (same kernels, same data); only the schedule and the memory footprint change.  Returns 0 or an error. */
+/* Schedule of the two directions of main.lua:955.  1 or 2 (the default, set at create time when the extra buffers fit):
+ * concurrent -- direction -1 on a side stream with its own 2V + tables, started when direction +1 reaches its SGM phase,
+ * and the permute / SGM phases on high-priority streams.  0: sequential on one stream, 4V of volume buffers instead of 6V.
+ * Results are identical in every mode (same kernels, same data); only the schedule and the memory footprint change.
+ * Returns 0 or an error. */
 int mccnn_pipeline_set_overlap(mccnn_pipeline *p, int mode);
 /* number of kernel launches one run issues (for bench.py's gpu_launches) */
 int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p);
@@ -257,7 +246,7 @@ int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p);
  * created W).  HOST-SYNCHRONOUS: waits for all work enqueued on the pipeline's device before anything an enqueued run reads
  * changes.  The Gaussian buffer grows only when blur_sigma needs a larger kernel (sigma 10 -> 61 x 61).  Applies to every
  * twin lane of the batch entry points that exists; lanes created later inherit the new parameters.  Every later run gives
- * the same bits as a pipeline created with these parameters, in the same CBCA mode, SGM layout and overlap mode.  On an
+ * the same bits as a pipeline created with these parameters, in the same CBCA mode and overlap mode.  On an
  * error (a CUDA error, or no memory for a larger Gaussian) the pipeline must be re-targeted again or destroyed. */
 int mccnn_pipeline_set_params(mccnn_pipeline *p, const mccnn_params *params);
 
@@ -272,7 +261,7 @@ int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR
  * one pipeline created at the largest shape of a dataset serves every image of it (KITTI widths, Middlebury sizes and
  * disparity ranges) without allocating.  featL/featR (C,H,W), imgL/imgR (H,W), disp (H,W), volL/volR (D,H,W) or NULL,
  * all contiguous at the RUN shape.  Same results, bit for bit, as mccnn_pipeline_run on a pipeline created at (C, D, H, W)
- * with the same params, CBCA mode, SGM layout and overlap mode.  ADCENSUS_ELIMIT if the shape exceeds the created one,
+ * with the same params, CBCA mode and overlap mode.  ADCENSUS_ELIMIT if the shape exceeds the created one,
  * ADCENSUS_EINVAL for H, W or D < 1 or border + 1 > W; nothing is launched then.  Asynchronous on `stream`.
  * The batch, host and twin-lane entry points (mccnn_pipeline_run_batch / _run_host / _run_host_batch) always run at the
  * created shape. */
@@ -310,7 +299,7 @@ int mccnn_pipeline_run_host_batch(mccnn_pipeline *p, int n, const float *const *
 int adcensus_trim_scratch(void);
 
 /* n device-resident pairs (arrays of n device pointers each), ordered on `stream` as a whole.  Pairs alternate between two
- * lanes (two buffer sets on internal streams, created on first use; ADCENSUS_LANES=1 disables the second lane), so that one
+ * lanes (two buffer sets on internal streams, created on first use; one lane if the second does not fit), so that one
  * pair's low-occupancy post-processing tail overlaps the next pair's volume kernels.  Results identical to n calls of
  * mccnn_pipeline_run. */
 int mccnn_pipeline_run_batch(mccnn_pipeline *p, int n, const float *const *featL, const float *const *featR,

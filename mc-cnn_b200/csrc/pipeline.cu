@@ -37,9 +37,6 @@ int adc_sgm2(const float *x0, const float *x1, const float *in, float *out, uint
 	     bool zero_out, cudaStream_t s);
 int adc_transpose_dhw_pitched_to_hwd(const float *in, float *out, int D, int H, int W, int ld, cudaStream_t s);
 int adc_transpose_hwd_to_dhw_pitched_div4(const float *in, float *out, int D, int H, int W, int ld, cudaStream_t s);
-size_t adc_sgm_dhw_table_bytes(int H, int W, int D);
-int adc_sgm2_dhw(const float *x0, const float *x1, const float *in, float *acc, uint8_t *tab, int H, int W, int ld, int D,
-		 float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction, bool div4, cudaStream_t s);
 int adc_stereo_join(const float *input_L, const float *input_R, float *output_L, float *output_R,
 		    int C, int D, int H, int W, int ldo, cudaStream_t s);
 int adc_fill_invalid(float *volL, float *volR, int D, int H, int W, int ld, cudaStream_t s);
@@ -58,7 +55,6 @@ struct mccnn_pipeline {
 	size_t bytes;
 	int launches;
 	int cbca_mode;    // 1 = constant-work aggregation (default, 1e-4 contract), 0 = exact (bit-identical to the reference)
-	int sgm_dhw;      // 1 = scan the (D,H,ld) layout directly (sgm_dhw.cu, no permutes); 0 (default) = permute to (H,W,D) like main.lua:1008
 	size_t tab_bytes;
 	// device buffers
 	float *vols;      // 2V: [0] left volume, [1] right volume (main.lua:946)
@@ -80,7 +76,7 @@ struct mccnn_pipeline {
 	// direction overlap (mccnn_pipeline_set_overlap): the two directions of main.lua:955 are independent
 	// until the LR check, so the second one runs on a side stream with its own ping-pong / SGM buffers,
 	// started when the first reaches its SGM phase.
-	int overlap;      // 0 off, 1 two streams, 2 additionally the SGM phases on high-priority streams
+	int overlap;      // 0 off; otherwise two streams, the SGM phases on high-priority streams
 	float *bufA2, *bufC2;
 	uint8_t *sgmtab2;
 	cudaStream_t side_stream, hi_stream[2];
@@ -215,10 +211,7 @@ extern "C" int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, 
 	p->V = (long)D * H * p->ld;
 	const char *ex = getenv("ADCENSUS_CBCA_EXACT");
 	p->cbca_mode = (ex && atoi(ex)) ? 0 : 1;
-	const char *sd = getenv("ADCENSUS_SGM_DHW");
-	p->sgm_dhw = (sd && atoi(sd)) ? 1 : 0;
 	p->tab_bytes = adc_sgm_table_bytes(H, W, D);
-	if (adc_sgm_dhw_table_bytes(H, W, D) > p->tab_bytes) p->tab_bytes = adc_sgm_dhw_table_bytes(H, W, D);
 	int rc = 0;
 	const size_t f = sizeof(float);
 	if (!rc) rc = dev_alloc((void **)&p->vols, 2 * p->V * f, &p->bytes);
@@ -238,16 +231,9 @@ extern "C" int mccnn_pipeline_create(mccnn_pipeline **out, int C, int D, int H, 
 		return rc;
 	}
 	*out = p;
-	// Default schedule: the two directions overlapped (mode 2), 6V of volume buffers instead of 4V; if the
-	// extra buffers do not fit, the sequential schedule is kept (same results).  ADCENSUS_OVERLAP overrides.
-	const char *e = getenv("ADCENSUS_OVERLAP");
-	const int mode = e ? atoi(e) : 2;
-	rc = mccnn_pipeline_set_overlap(p, mode);
-	if (rc && e) {                                     // an explicit request that cannot be met is an error
-		*out = nullptr;
-		mccnn_pipeline_destroy(p);
-		return rc;
-	}
+	// Default schedule: the two directions overlapped, 6V of volume buffers instead of 4V; if the extra buffers do not
+	// fit, the sequential schedule is kept (same results).
+	mccnn_pipeline_set_overlap(p, 2);
 	return 0;
 }
 
@@ -279,8 +265,6 @@ extern "C" size_t mccnn_pipeline_device_bytes(const mccnn_pipeline *p) { return 
 // 1 (default) constant-work aggregation within the 1e-4 contract (cbca_tma.cu); 0 exact, bit-identical to the reference
 extern "C" void mccnn_pipeline_set_cbca_mode(mccnn_pipeline *p, int mode) { if (p) p->cbca_mode = mode ? 1 : 0; }
 extern "C" int mccnn_pipeline_get_cbca_mode(const mccnn_pipeline *p) { return p ? p->cbca_mode : -1; }
-// 0 (default): permute to (H,W,D) for sgm2 like main.lua:1008; 1: scan (D,H,ld) directly (sgm_dhw.cu).  Same results.
-extern "C" void mccnn_pipeline_set_sgm_layout(mccnn_pipeline *p, int dhw) { if (p) p->sgm_dhw = dhw ? 1 : 0; }
 static void overlap_release(mccnn_pipeline *p)
 {
 	const size_t f = sizeof(float);
@@ -380,7 +364,7 @@ static int run_fits(mccnn_pipeline *p, int H, int W, int D)
 	if (V > p->V || HW > p->HW) return ADCENSUS_ELIMIT;
 	if (adc_packed_words(H, W) + adc_packed_hv_words(H, W) > adc_packed_words(p->H, p->W) + adc_packed_hv_words(p->H, p->W))
 		return ADCENSUS_ELIMIT;
-	if (adc_sgm_table_bytes(H, W, D) > p->tab_bytes || adc_sgm_dhw_table_bytes(H, W, D) > p->tab_bytes) return ADCENSUS_ELIMIT;
+	if (adc_sgm_table_bytes(H, W, D) > p->tab_bytes) return ADCENSUS_ELIMIT;
 	if (p->tm_D != D || p->tm_H != H || p->tm_W != W) STEP(encode_maps(p, D, H, W));
 	return 0;
 }
@@ -452,24 +436,17 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		}
 		if (k == 0 && p->overlap) STEP((int)cudaEventRecord(p->ev_stagger, ds));                 // the other direction may start
 		cudaStream_t ss = ds;                                                                    // stream of the SGM phase
-		if (p->overlap == 2 && o.sgm_i > 0) {
+		if (p->overlap && o.sgm_i > 0) {
 			ss = p->hi_stream[k];
 			STEP((int)cudaEventRecord(p->ev_hi_in[k], ds));
 			STEP((int)cudaStreamWaitEvent(ss, p->ev_hi_in[k], 0));
 		}
 		for (int it = 0; it < o.sgm_i; it++) {                                                   // :1008-1020
-			if (p->sgm_dhw) {                                                                    // no permutes: (D,H,ld) scans
-				STEP(adc_sgm2_dhw(imgL, imgR, cur, acc, tab, H, W, ld, D, o.pi1, o.pi2, o.tau_so, o.alpha1,
-						  o.sgm_q1, o.sgm_q2, direction, /*div4=*/true, ss));              // :1014-1016, :1020
-				float *t = cur; cur = acc; acc = t;
-				nl += 5;
-			} else {
-				STEP(adc_transpose_dhw_pitched_to_hwd(cur, spare, D, H, W, ld, ss));             // :1008
-				STEP(adc_sgm2(imgL, imgR, spare, acc, tab, H, W, D, o.pi1, o.pi2, o.tau_so, o.alpha1,
-					      o.sgm_q1, o.sgm_q2, direction, /*zero_out=*/true, ss));                // :1014-1016
-				STEP(adc_transpose_hwd_to_dhw_pitched_div4(acc, cur, D, H, W, ld, ss));          // :1017-1020
-				nl += 7;
-			}
+			STEP(adc_transpose_dhw_pitched_to_hwd(cur, spare, D, H, W, ld, ss));                 // :1008
+			STEP(adc_sgm2(imgL, imgR, spare, acc, tab, H, W, D, o.pi1, o.pi2, o.tau_so, o.alpha1,
+				      o.sgm_q1, o.sgm_q2, direction, /*zero_out=*/true, ss));                    // :1014-1016
+			STEP(adc_transpose_hwd_to_dhw_pitched_div4(acc, cur, D, H, W, ld, ss));              // :1017-1020
+			nl += 7;
 		}
 		if (ss != ds) {
 			STEP((int)cudaEventRecord(p->ev_hi_out[k], ss));
@@ -589,13 +566,12 @@ static int host_staging(mccnn_pipeline *p)
 	return rc;
 }
 
-// the extra lanes (see struct): a chain of twins created on first use with the same parameters and modes.  ADCENSUS_LANES
-// (1..4, default 2) sets the number of lanes; lane 0 is the pipeline itself.
+// the extra lanes (see struct): a chain of twins created on first use with the same parameters and modes; lane 0 is the
+// pipeline itself.
+static const int BATCH_LANES = 2;
 static int batch_lanes(mccnn_pipeline *p, mccnn_pipeline **lane, int want)
 {
-	static const int lanes_env = getenv("ADCENSUS_LANES") ? atoi(getenv("ADCENSUS_LANES")) : 2;
-	int nl = lanes_env < 1 ? 1 : (lanes_env > 4 ? 4 : lanes_env);
-	if (nl > want) nl = want;
+	const int nl = want < BATCH_LANES ? want : BATCH_LANES;
 	lane[0] = p;
 	int n = 1;
 	for (mccnn_pipeline *q = p; n < nl; n++) {
@@ -609,7 +585,6 @@ static int batch_lanes(mccnn_pipeline *p, mccnn_pipeline **lane, int want)
 		}
 		q = q->twin;
 		q->cbca_mode = p->cbca_mode;
-		q->sgm_dhw = p->sgm_dhw;
 		if (q->overlap != p->overlap) mccnn_pipeline_set_overlap(q, p->overlap);
 		lane[n] = q;
 	}
@@ -653,7 +628,7 @@ extern "C" int mccnn_pipeline_run_host_batch(mccnn_pipeline *p, int n, const flo
 	for (int i = 0; i < n; i++)
 		if (!featL_host[i] || !featR_host[i] || !imgL_host[i] || !imgR_host[i] || !disp_host[i]) return ADCENSUS_EINVAL;
 	DeviceGuard g(p->device);
-	mccnn_pipeline *lane[4];
+	mccnn_pipeline *lane[BATCH_LANES];
 	const int nl = batch_lanes(p, lane, n > 1 ? n : 1);
 	for (int l = 0; l < nl; l++) STEP(host_staging(lane[l]));
 	for (int i = 0; i < n; i++)
@@ -676,7 +651,7 @@ extern "C" int mccnn_pipeline_run_batch(mccnn_pipeline *p, int n, const float *c
 		if (!featL[i] || !featR[i] || !imgL[i] || !imgR[i] || !disp[i]) return ADCENSUS_EINVAL;
 	DeviceGuard g(p->device);
 	cudaStream_t s = adc_stream(stream);
-	mccnn_pipeline *lane[4];
+	mccnn_pipeline *lane[BATCH_LANES];
 	const int nl = batch_lanes(p, lane, n > 1 ? n : 1);
 	if (nl == 1) {
 		for (int i = 0; i < n; i++) STEP(mccnn_pipeline_run(p, featL[i], featR[i], imgL[i], imgR[i], disp[i], nullptr, nullptr, s));

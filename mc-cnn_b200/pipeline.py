@@ -188,8 +188,9 @@ class StereoPipeline:
         except Exception:
             pass
 
-    def set_overlap(self, mode=1):
-        """Run the two directions concurrently on two streams (mccnn_pipeline_set_overlap); results are unchanged."""
+    def set_overlap(self, mode=2):
+        """1 or 2 (the default): run the two directions concurrently on two streams; 0: sequentially on one stream, with
+        less device memory (mccnn_pipeline_set_overlap).  Results are unchanged."""
         adcensus._check(adcensus.lib().mccnn_pipeline_set_overlap(self._h, int(mode)), "mccnn_pipeline_set_overlap")
 
     def set_cbca_mode(self, mode):
@@ -201,10 +202,6 @@ class StereoPipeline:
     @property
     def cbca_mode(self):
         return "fast" if adcensus.lib().mccnn_pipeline_get_cbca_mode(self._h) else "exact"
-
-    def set_sgm_layout(self, dhw):
-        """True: sgm2 scans the (D,H,ld) layout directly (csrc/sgm_dhw.cu); False (default): permutes around sgm2 as main.lua does"""
-        adcensus.lib().mccnn_pipeline_set_sgm_layout(self._h, int(bool(dhw)))
 
     def set_params(self, params):
         """Re-target the pipeline to another :class:`Params` (mccnn_pipeline_set_params): later runs give the bits of a

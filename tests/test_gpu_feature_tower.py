@@ -1,11 +1,8 @@
 """GPU parity of the in-library feature tower (csrc/feature_tower.cu) against the CPU oracle (oracle/feature_tower.py, pinned to
 the PyTorch restatement of main.lua:726-749 by tests/golden/feature_tower.npz).  Bar: 1e-4, absolute for the unit-norm
 features of the fast architecture, scaled by max(1, |want|) for the slow one; plain bf16 operands (nterms = 1): 5e-2."""
-import json
 import math
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -17,8 +14,6 @@ import mccnn_b200  # noqa: E402,F401
 from mccnn_b200 import adcensus, feature_tower  # noqa: E402
 from oracle import feature_tower as oft  # noqa: E402
 from oracle import tower_head_cases as cases  # noqa: E402
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def cu(a):
@@ -149,30 +144,6 @@ def test_full_size(name, seed, fm, l1, arch, H, W, crop, band):
     t.close()
     del out, xd
     _free_device_memory()
-
-
-def test_ring_kernel_at_64_planes():
-    """ADCENSUS_TOWER_RESIDENT=0 sends fm = 64 through the ring kernel (N = 64, two passes of five and four taps).  The knob is
-    read once per process, so the run is a subprocess."""
-    code = "\n".join([
-        "import json, sys",
-        "sys.path.insert(0, %r)" % ROOT,
-        "import numpy as np, torch",
-        "import mccnn_b200",
-        "from mccnn_b200 import feature_tower",
-        "from oracle import tower_head_cases as cases",
-        "layers, x = cases.tower_case(31, 1, 64, 4, 2, 9, 300)",
-        "want = cases.tower_want(x, layers, 'fast')",
-        "t = feature_tower.FeatureTower(layers, arch='fast')",
-        "err = {n: float(np.abs(t.forward(torch.from_numpy(x).cuda(), nterms=n).cpu().numpy() - want).max()) for n in (3, 1)}",
-        "print(json.dumps(err))",
-    ])
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=dict(os.environ, ADCENSUS_TOWER_RESIDENT="0"),
-                       capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
-    err = json.loads(r.stdout.strip().splitlines()[-1])
-    assert err["3"] <= 1e-4 and err["1"] <= 5e-2, err
-    print("ring kernel at fm 64: max err %.3g (nterms 3), %.3g (nterms 1)" % (err["3"], err["1"]))
 
 
 def test_side_stream_gives_the_same_bits():

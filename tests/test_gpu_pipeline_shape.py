@@ -1,7 +1,8 @@
 """GPU: one StereoPipeline created at the largest shape runs smaller shapes (mccnn_pipeline_run_shape) with the same
-results, bit for bit, as a pipeline created at each shape -- in both CBCA modes, both SGM layouts and overlap modes 0 and 2
--- and a plain run afterwards still reproduces the created shape's result.  The preset (accurate_cbca4) has CBCA blocks
-before and after SGM, so the TMA-staged CBCA's tensor maps are re-encoded for every shape change."""
+results, bit for bit, as a pipeline created at each shape -- in both CBCA modes and overlap modes 0 and 2 -- and a plain
+run afterwards still reproduces the created shape's result.  The accurate_cbca4 preset has CBCA blocks before and after
+SGM, so the TMA-staged CBCA's tensor maps are re-encoded for every shape change; mb slow's arms of up to 14 pixels run the
+exact CBCA kernels in both modes, with no tensor maps at all."""
 import ctypes
 
 import numpy as np
@@ -24,9 +25,8 @@ def _inputs(h, w, d, seed):
     return t(p["featL"]), t(p["featR"]), t(p["imgL"]), t(p["imgR"])
 
 
-def _configure(sp, cbca, dhw, overlap):
+def _configure(sp, cbca, overlap):
     sp.set_cbca_mode(cbca)
-    sp.set_sgm_layout(dhw)
     sp.set_overlap(overlap)
 
 
@@ -36,10 +36,10 @@ def _outputs(h, w, d):
             torch.full((d, h, w), nan, device="cuda"))
 
 
-def _fresh(shape, ins, cbca, dhw, overlap):
+def _fresh(shape, ins, opt, cbca, overlap):
     h, w, d = shape
-    sp = pipeline.StereoPipeline(C, d, h, w, OPT)
-    _configure(sp, cbca, dhw, overlap)
+    sp = pipeline.StereoPipeline(C, d, h, w, opt)
+    _configure(sp, cbca, overlap)
     disp, vl, vr = _outputs(h, w, d)
     sp.run(*ins, disp=disp, volL=vl, volR=vr)
     torch.cuda.synchronize()
@@ -55,13 +55,14 @@ def _same(got, want, what):
 
 
 @pytest.mark.parametrize("overlap", [0, 2])
-@pytest.mark.parametrize("dhw", [False, True])
 @pytest.mark.parametrize("cbca", ["fast", "exact"])
-def test_run_shape_matches_a_pipeline_of_that_shape(cbca, dhw, overlap):
+@pytest.mark.parametrize("dataset,arch", [("kitti", "accurate_cbca4"), ("mb", "slow")])
+def test_run_shape_matches_a_pipeline_of_that_shape(dataset, arch, cbca, overlap):
+    opt = pipeline.make_params(dataset, arch)
     inputs = {s: _inputs(*s, seed=7 * s[0] + s[1] + s[2]) for s in SHAPES}
-    want = {s: _fresh(s, inputs[s], cbca, dhw, overlap) for s in SHAPES}
-    sp = pipeline.StereoPipeline(C, D, H, W, OPT)
-    _configure(sp, cbca, dhw, overlap)
+    want = {s: _fresh(s, inputs[s], opt, cbca, overlap) for s in SHAPES}
+    sp = pipeline.StereoPipeline(C, D, H, W, opt)
+    _configure(sp, cbca, overlap)
     first = None
     for s in SHAPES + SHAPES[::-1][1:]:                        # interleaved: every shape change re-encodes the maps
         h, w, d = s

@@ -21,7 +21,7 @@ ap.add_argument("--D", type=int, default=228)
 ap.add_argument("--H", type=int, default=370)
 ap.add_argument("--W", type=int, default=1226)
 ap.add_argument("--C", type=int, default=64)
-ap.add_argument("--batch", action="store_true", help="one mccnn_pipeline_run_batch call for all iterations (lanes: ADCENSUS_LANES)")
+ap.add_argument("--batch", action="store_true", help="one mccnn_pipeline_run_batch call for all iterations")
 a = ap.parse_args()
 dev = torch.device("cuda:0")
 opt = pipeline.make_params("kitti", a.preset)
@@ -47,6 +47,6 @@ else:
         sp.run(fL, fR, iL, iR)
 e1.record()
 torch.cuda.synchronize()
-print("preset=%s lanes=%s cbca=%s overlap=%s ms_per_pair=%.4f launches=%d" % (a.preset, (os.environ.get("ADCENSUS_LANES", "2") if a.batch else "-"), sp.cbca_mode,
-                                                                    a.overlap, e0.elapsed_time(e1) / a.iters, sp.launches_per_run))
+print("preset=%s batch=%d cbca=%s overlap=%s ms_per_pair=%.4f launches=%d" % (a.preset, a.batch, sp.cbca_mode, a.overlap,
+                                                                            e0.elapsed_time(e1) / a.iters, sp.launches_per_run))
 sp.close()
