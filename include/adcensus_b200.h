@@ -426,18 +426,33 @@ int mccnn_mb_nnz_fill(const float *d0, const unsigned char *mask, int H, int W, 
  * (main.lua:843-846).  Pointers may be host or device unless noted (copies use cudaMemcpyDefault). */
 
 /* One patch of make_patch (main.lua:607-619): m the forward 2x3 matrix as stored in the FloatTensor, contrast and
- * brightness as float, image the 0-based index into X0 / X1 ((n_img, 1, H, W) float32), view 0 = X0, 1 = X1. */
+ * brightness as float, image the 0-based index into the trainer's pair table (for the X0 / X1 creators: into X0 / X1,
+ * (n_img, 1, H, W) float32), view 0 = the pair's x0, 1 = its x1. */
 typedef struct {
 	float m[6];
 	float contrast, brightness;
 	int image, view;
 } mccnn_warp;
 
+/* One stereo pair the sampler reads: two DEVICE float32 planes of H x W (row-major, contiguous), 1 <= H, W <= 32767.
+ * Pairs of one table may differ in size (Middlebury: one pair per image, light and exposure; main.lua:828-841). */
+typedef struct {
+	const float *x0, *x1;
+	int H, W;
+} mccnn_train_pair;
+
 /* The sampler alone: out (n, ws, ws) = warpAffine(X[image], m, (ws, ws), INTER_CUBIC, BORDER_CONSTANT 0) * contrast +
  * brightness, bit-identical to OpenCV's float path as oracle/train.py restates it.  DEVICE pointers; an image index
- * outside [0, n_img) gives a NaN patch. */
+ * outside [0, n_img) gives a NaN patch.  Runs mccnn_train_sample_pairs' kernel on the table {X0[i], X1[i], H, W}. */
 int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n, int ws,
 		       float *out, adcensus_stream_t stream);
+
+/* The sampler on a DEVICE table of n_pairs pairs: the source of warps[i] is pairs[image].x0 (view 0) or .x1 (view 1), and
+ * its constant-0 border is that pair's own H x W.  A pair index outside [0, n_pairs) gives a NaN patch.  The table is
+ * read back to the host once to check it (ADCENSUS_EINVAL for a null plane or a size < 1, ADCENSUS_ELIMIT above 32767),
+ * so the call waits for `stream`. */
+int mccnn_train_sample_pairs(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws, float *out,
+			     adcensus_stream_t stream);
 
 typedef struct mccnn_trainer mccnn_trainer;
 
@@ -472,6 +487,18 @@ int mccnn_trainer_create_slow(mccnn_trainer **h, int l1, int fm, int l2, int nh2
 			      const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
 			      adcensus_stream_t stream);
 
+/* The two creators above on a table of stereo pairs instead of X0 / X1: `pairs` is a HOST array of n_pairs records, copied
+ * into trainer-owned device memory; the planes it points to are kept by the caller for the trainer's lifetime.  A warp's
+ * image is an index into this table.  mccnn_trainer_create[_slow] build the table {X0 + i H W, X1 + i H W, H, W} and call
+ * these, so both give the same bits from the same planes.  Each pair's planes non-null and H, W >= 1 (else
+ * ADCENSUS_EINVAL), H, W <= 32767 (else ADCENSUS_ELIMIT); the other limits are the creators'. */
+int mccnn_trainer_create_pairs(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom,
+			       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
+			       adcensus_stream_t stream);
+int mccnn_trainer_create_slow_pairs(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom,
+				    const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
+				    adcensus_stream_t stream);
+
 /* The trainer's buffers, for get / set (set: PARAMS and MOMENTA only) and the tests.  Sizes in floats from
  * mccnn_trainer_size.  TOWER: every layer's output, layer k (N, fm, s_k, s_k) after the previous layers, s_k = ws - 2k, post
  * ReLU except the last ('fast') or post ReLU ('slow'); DZ: the gradient of the loss wrt each layer's pre-activation output,
@@ -498,6 +525,14 @@ int mccnn_trainer_launches_per_step(mccnn_trainer *h);
 /* HOST helper: the swaps i = i0 .. i0 + k - 1 of THTensor_(randperm) on perm (n) int64: swap perm[i] and
  * perm[i + draws[j] % (n - i)], draws the generator's 32-bit outputs in order (i0 + k <= n - 1). */
 int mccnn_randperm_swaps(long long *perm, long long n, long long i0, const unsigned *draws, long long k);
+
+/* HOST helper: the sample boundaries of main.lua:791-841 for dataset mb in a buffer of the generator's 32-bit outputs.
+ * A sample is `base` words (the torch.uniform calls of :791-818), then light, exp, the d_exp test, exp_ only when that
+ * test passes (raw / 2^32 < d_exp in double), then the d_light test: base + 4 or base + 5 words.  Walks from raw[0]
+ * and writes the first word of each whole sample to starts, at most `cap` of them; *count gets their number and *used
+ * the words they take (the words from *used on belong to the next sample). */
+int mccnn_mb_sample_starts(const unsigned *raw, long long n_raw, int base, double d_exp, long long *starts, long long cap,
+			   long long *count, long long *used);
 
 #ifdef __cplusplus
 }

@@ -4,6 +4,8 @@
 //   constant 0 border, restated operation by operation: the float 2x3 matrix inverted in double, source coordinates on
 //   AB_BITS = 10 fixed point rounded to the 1/32-pixel grid, the float cubic table (A = -0.75), interior taps summed row by
 //   row, border taps summed one by one onto 0; then * contrast + brightness in fp32.  Bit-identical to oracle/train.py.
+//   It reads a table of stereo pairs (mccnn_train_pair), each with its own H x W: KITTI's (n_img, 1, H, W) stacks become
+//   one pair per image, Middlebury gives one pair per (image, light, exposure).
 // * One training step (net_tr + Margin2 + the momentum update, main.lua:852-874) in fp32 on the CUDA cores, five kernels
 //   plus one per layer, captured once into a CUDA graph:
 //     tower_fwd_kernel   one block per patch, every layer's activations in shared memory (and kept in global memory);
@@ -22,6 +24,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "common.cuh"
 
@@ -52,7 +55,8 @@ __device__ __forceinline__ void cubic_coeffs(float x, float c[4])
 
 __device__ __forceinline__ int sat_short(int v) { return min(32767, max(-32768, v)); }
 
-__global__ void train_sample_kernel(const float *__restrict__ X0, const float *__restrict__ X1, int n_img, int H, int W,
+// the source of each patch is pairs[w.image].x0 or .x1, with that pair's own H x W (and so its own constant-0 border)
+__global__ void train_sample_kernel(const mccnn_train_pair *__restrict__ pairs, int n_pairs,
 				    const mccnn_warp *__restrict__ warps, const int *__restrict__ slot, int n, int ws,
 				    float *__restrict__ out)
 {
@@ -62,8 +66,10 @@ __global__ void train_sample_kernel(const float *__restrict__ X0, const float *_
 	const int p = (int)(id / np), y = (int)(id % np) / ws, x = (int)(id % np) % ws;
 	const mccnn_warp w = warps[(slot ? (long)*slot * n : 0) + p];
 	float *dst = out + id;
-	if (w.image < 0 || w.image >= n_img) { *dst = adc_nan(); return; }
-	const float *src = (w.view ? X1 : X0) + (long)w.image * H * W;
+	if (w.image < 0 || w.image >= n_pairs) { *dst = adc_nan(); return; }
+	const mccnn_train_pair pr = pairs[w.image];
+	const int H = pr.H, W = pr.W;
+	const float *src = w.view ? pr.x1 : pr.x0;
 
 	// warpAffine: invert the forward matrix in double
 	double M0 = w.m[0], M1 = w.m[1], M2 = w.m[2], M3 = w.m[3], M4 = w.m[4], M5 = w.m[5];
@@ -547,11 +553,11 @@ void launch_gemm(const Op &op, int nsplit, cudaStream_t s)
 
 struct mccnn_trainer {
 	Layout L;
-	int device, bufsz, smem, chunk, loss_cap, n_img, H, W;
+	int device, bufsz, smem, chunk, loss_cap, n_pairs;
 	long nparam;
 	float margin, mom;
 	int pow2;
-	const float *X0, *X1;
+	mccnn_train_pair *pairs;                 // device copy of the creator's table
 	float *P, *V, *G, *X, *act, *dz, *norm, *nout, *join, *gjoin, *hinge, *gout, *loss, *neg_lr;
 	float neg_lr_host;
 	int *ctr;
@@ -620,8 +626,7 @@ static int enqueue_step(mccnn_trainer *h, cudaStream_t s, bool sample)
 	const int ws = L.ws;
 	if (sample) {
 		const long tot = (long)L.N * ws * ws;
-		train_sample_kernel<<<adc_div_up(tot, 128), 128, 0, s>>>(h->X0, h->X1, h->n_img, h->H, h->W, h->warps, h->ctr, L.N,
-								       ws, h->X);
+		train_sample_kernel<<<adc_div_up(tot, 128), 128, 0, s>>>(h->pairs, h->n_pairs, h->warps, h->ctr, L.N, ws, h->X);
 	}
 	if (h->slow) return enqueue_slow(h, s);
 	tower_fwd_kernel<<<L.N, 256, h->smem, s>>>(L, h->X, h->P, h->act, h->bufsz);
@@ -678,15 +683,60 @@ static float **train_buffer(mccnn_trainer *h, int what, long *count)
 // ROWS is a view of the tower's last layer (N, fm, 1, 1) = (bs, 2 fm), not an allocation of its own
 static bool owned(int what) { return what != MCCNN_TRAIN_ROWS; }
 
+// the table {X0 + i H W, X1 + i H W, H, W} of the (n_img, 1, H, W) creators
+static std::vector<mccnn_train_pair> stacked_pairs(const float *X0, const float *X1, int n_img, int H, int W)
+{
+	std::vector<mccnn_train_pair> t(n_img);
+	for (int i = 0; i < n_img; i++) t[i] = {X0 + (long)i * H * W, X1 + (long)i * H * W, H, W};
+	return t;
+}
+
+static int check_pairs(const mccnn_train_pair *pairs, int n_pairs)
+{
+	if (!pairs || n_pairs < 1) return ADCENSUS_EINVAL;
+	for (int i = 0; i < n_pairs; i++) {
+		const mccnn_train_pair &p = pairs[i];
+		if (!p.x0 || !p.x1 || p.H < 1 || p.W < 1) return ADCENSUS_EINVAL;
+		if (p.H > 32767 || p.W > 32767) return ADCENSUS_ELIMIT;
+	}
+	return 0;
+}
+
+static int launch_sample(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws, float *out,
+			 cudaStream_t s)
+{
+	train_sample_kernel<<<adc_div_up((long)n * ws * ws, 128), 128, 0, s>>>(pairs, n_pairs, warps, nullptr, n, ws, out);
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
 extern "C" int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n,
 				  int ws, float *out, adcensus_stream_t stream)
 {
 	if (!X0 || !X1 || !warps || !out || n_img < 1 || H < 1 || W < 1 || n < 1 || ws < 1) return ADCENSUS_EINVAL;
 	if ((long)n * ws * ws >= (1l << 31) || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
 	cudaStream_t s = adc_stream(stream);
-	train_sample_kernel<<<adc_div_up((long)n * ws * ws, 128), 128, 0, s>>>(X0, X1, n_img, H, W, warps, nullptr, n, ws, out);
-	ADC_CHECK_LAUNCH();
-	return 0;
+	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
+	mccnn_train_pair *d = nullptr;
+	ADC_CUDA(cudaMallocAsync((void **)&d, t.size() * sizeof(mccnn_train_pair), s));
+	// from pageable memory: the call returns once `t` has been read
+	int rc = (int)cudaMemcpyAsync(d, t.data(), t.size() * sizeof(mccnn_train_pair), cudaMemcpyHostToDevice, s);
+	if (!rc) rc = launch_sample(d, n_img, warps, n, ws, out, s);
+	const int rf = (int)cudaFreeAsync(d, s);
+	return rc ? rc : rf;
+}
+
+extern "C" int mccnn_train_sample_pairs(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws,
+					float *out, adcensus_stream_t stream)
+{
+	if (!pairs || n_pairs < 1 || !warps || !out || n < 1 || ws < 1) return ADCENSUS_EINVAL;
+	if ((long)n * ws * ws >= (1l << 31)) return ADCENSUS_ELIMIT;
+	cudaStream_t s = adc_stream(stream);
+	std::vector<mccnn_train_pair> t(n_pairs);
+	ADC_CUDA(cudaMemcpyAsync(t.data(), pairs, t.size() * sizeof(mccnn_train_pair), cudaMemcpyDeviceToHost, s));
+	ADC_CUDA(cudaStreamSynchronize(s));
+	const int rc = check_pairs(t.data(), n_pairs);
+	return rc ? rc : launch_sample(pairs, n_pairs, warps, n, ws, out, s);
 }
 
 extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
@@ -706,14 +756,14 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	cudaFree(h->neg_lr);
 	cudaFree(h->ctr);
 	cudaFree(h->warps);
+	cudaFree(h->pairs);
 	cudaSetDevice(prev);
 	free(h);
 	return 0;
 }
 
 static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2, int bs, float margin, int pow, float mom,
-		  const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
-		  adcensus_stream_t stream)
+		  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, adcensus_stream_t stream)
 {
 	*out = nullptr;
 	mccnn_trainer *h = (mccnn_trainer *)calloc(1, sizeof(mccnn_trainer));
@@ -753,8 +803,8 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	for (int k = 1; k < l1; k++) h->bufsz = h->bufsz > fm * (L.ws - 2 * k) * (L.ws - 2 * k) ? h->bufsz
 											   : fm * (L.ws - 2 * k) * (L.ws - 2 * k);
 	h->smem = 2 * h->bufsz * (int)sizeof(float);
-	h->device = device; h->chunk = chunk; h->loss_cap = loss_cap; h->n_img = n_img; h->H = H; h->W = W;
-	h->margin = margin; h->mom = mom; h->pow2 = pow == 2; h->X0 = X0; h->X1 = X1;
+	h->device = device; h->chunk = chunk; h->loss_cap = loss_cap; h->n_pairs = n_pairs;
+	h->margin = margin; h->mom = mom; h->pow2 = pow == 2;
 	h->neg_lr_host = 0.f;
 	int prev = 0;
 	cudaGetDevice(&prev);
@@ -780,6 +830,8 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, 2 * sizeof(int), adc_stream(stream));
 	if (!rc) rc = (int)cudaMalloc((void **)&h->warps, (size_t)chunk * L.N * sizeof(mccnn_warp));
 	if (!rc) rc = (int)cudaMemsetAsync(h->warps, 0, (size_t)chunk * L.N * sizeof(mccnn_warp), adc_stream(stream));
+	if (!rc) rc = (int)cudaMalloc((void **)&h->pairs, (size_t)n_pairs * sizeof(mccnn_train_pair));
+	if (!rc) rc = (int)cudaMemcpy(h->pairs, pairs, (size_t)n_pairs * sizeof(mccnn_train_pair), cudaMemcpyHostToDevice);
 	if (!rc) rc = (int)cudaStreamCreateWithFlags(&h->cap, cudaStreamNonBlocking);
 	if (!rc) rc = capture(h, true, &h->full);
 	if (!rc) rc = capture(h, false, &h->body);
@@ -801,7 +853,8 @@ extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs,
 	    W < 1 || chunk < 1 || loss_cap < 1)
 		return ADCENSUS_EINVAL;
 	if (l1 > LMAX || fm > 128 || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
-	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, X0, X1, n_img, H, W, chunk, loss_cap, device, stream);
+	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
+	return mccnn_trainer_create_pairs(out, l1, fm, bs, margin, pow, mom, t.data(), n_img, chunk, loss_cap, device, stream);
 }
 
 extern "C" int mccnn_trainer_create_slow(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
@@ -811,10 +864,35 @@ extern "C" int mccnn_trainer_create_slow(mccnn_trainer **out, int l1, int fm, in
 	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || n_img < 1 || H < 1 ||
 	    W < 1 || chunk < 1 || loss_cap < 1)
 		return ADCENSUS_EINVAL;
-	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) || H > 32767 ||
-	    W > 32767 || (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31))
+	if (H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
+	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
+	return mccnn_trainer_create_slow_pairs(out, l1, fm, l2, nh2, bs, mom, t.data(), n_img, chunk, loss_cap, device, stream);
+}
+
+extern "C" int mccnn_trainer_create_pairs(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
+					  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
+					  adcensus_stream_t stream)
+{
+	if (!out || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || chunk < 1 || loss_cap < 1)
+		return ADCENSUS_EINVAL;
+	const int rc = check_pairs(pairs, n_pairs);
+	if (rc) return rc;
+	if (l1 > LMAX || fm > 128) return ADCENSUS_ELIMIT;
+	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, pairs, n_pairs, chunk, loss_cap, device, stream);
+}
+
+extern "C" int mccnn_trainer_create_slow_pairs(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
+					       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
+					       adcensus_stream_t stream)
+{
+	if (!out || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || chunk < 1 || loss_cap < 1)
+		return ADCENSUS_EINVAL;
+	const int rc = check_pairs(pairs, n_pairs);
+	if (rc) return rc;
+	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) ||
+	    (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31))
 		return ADCENSUS_ELIMIT;
-	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, X0, X1, n_img, H, W, chunk, loss_cap, device, stream);
+	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, pairs, n_pairs, chunk, loss_cap, device, stream);
 }
 
 static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
@@ -902,5 +980,21 @@ extern "C" int mccnn_randperm_swaps(long long *perm, long long n, long long i0, 
 		perm[i] = perm[i + z];
 		perm[i + z] = t;
 	}
+	return 0;
+}
+
+extern "C" int mccnn_mb_sample_starts(const unsigned *raw, long long n_raw, int base, double d_exp, long long *starts,
+				      long long cap, long long *count, long long *used)
+{
+	if ((!raw && n_raw) || n_raw < 0 || base < 0 || cap < 0 || (!starts && cap) || !count || !used) return ADCENSUS_EINVAL;
+	long long pos = 0, k = 0;
+	while (k < cap && pos + base + 4 <= n_raw) {
+		const int extra = raw[pos + base + 2] * (1.0 / 4294967296.0) < d_exp;     // torch.uniform() < opt.d_exp
+		if (pos + base + 4 + extra > n_raw) break;
+		starts[k++] = pos;
+		pos += base + 4 + extra;
+	}
+	*count = k;
+	*used = pos;
 	return 0;
 }

@@ -1,4 +1,5 @@
-"""main.lua's ``-a train_tr`` / ``-a train_all`` (main.lua:602-890) for the fast and slow architectures on KITTI 2012 / 2015.
+"""main.lua's ``-a train_tr`` / ``-a train_all`` (main.lua:602-890) for the fast and slow architectures on KITTI 2012 / 2015
+and Middlebury.
 
     opt = options("kitti", lr=0.002)                                   # main.lua's presets (:34-49, :206-262) + overrides
     fname = train("kitti", "train_tr", opt, data_root=".", seed=42)   # 14 epochs, net/net_<cmd_str>.t7, then test_te
@@ -24,9 +25,19 @@ net_te's l1 convolutions constructed anew -- their reset() draws are thrown away
 they advance the stream; SpatialConvolution1_fw draws nothing -- then the per-sample draws as for 'fast'.  This order is
 read from the sources; parity with Torch7 is unpinned, and it is pinned against oracle/train_slow.py.
 
+Dataset mb (main.lua:455-491, 828-841): the training images are every light group ``x_<i>_<j>.bin``, j >= 2, of the
+images the nnz rows name, one device pair per (image, light, exposure) in a table the sampler reads (:class:`MbTrainSet`,
+``mccnn_trainer_create_pairs``).  After the uniforms of :791-818 each sample draws light, exp, the d_exp test, exp_ only
+when that test passes, then the d_light test, so a sample takes a variable number of words: ``mccnn_mb_sample_starts``
+finds the boundaries in a buffer of raw words, numpy gathers the columns (:func:`draw_params_mb`), and the words drawn past
+the last sample of a chunk go back to the stream, so chunked building gives the records building everything at once gives.
+``torch.random()`` is taken to be one 32-bit output, like each uniform; pinned against oracle/train_mb.py, not Torch7.
+Only grey sets (``-color gray``) are trained.
+
 Deliberate deviations from main.lua:
 
-* only archs 'fast' and 'slow' and datasets kitti / kitti2015; ``-at 1``, ``-subset`` < 1 and ``-debug`` are refused;
+* only archs 'fast' and 'slow' and datasets kitti / kitti2015 / mb; ``-at 1``, ``-subset`` < 1, ``-debug`` and (mb)
+  ``-color rgb`` are refused;
 * the net file goes to ``<data_root>/net/`` and an existing file is refused; the file name is built from main.lua's options
   only (``-data_root`` and ``-out`` are not part of it);
 * Margin2's loss is the hinge terms summed in order, then divided by bs / 2 (Torch7's ``mean`` reduces in another order),
@@ -40,7 +51,7 @@ import time
 
 import numpy as np
 
-from . import evaluate
+from . import dataio, evaluate
 
 EPOCHS = 14                                  # main.lua:779
 LR_DROP_EPOCH = 12                           # :783-785
@@ -54,7 +65,17 @@ NET = dict(at=0, m=0.2, pow=1, l1=4, fm=64, ks=3, lr=0.002, bs=128, mom=0.9, tru
 # main.lua:70-84 (arch 'slow', kitti / kitti2015)
 NET_SLOW = dict(at=0, l1=4, fm=112, ks=3, l2=4, nh2=384, lr=0.003, bs=128, mom=0.9, true1=1.0, false1=4.0, false2=10.0)
 PRESETS = {"fast": NET, "slow": NET_SLOW}
+# main.lua:50-66 (Middlebury augmentation), :263-280 (arch 'fast', mb) and :115-131 (arch 'slow', mb); -ds is stored and,
+# as in main.lua, has no effect
+AUGMENT_MB = dict(hflip=0, vflip=0, rotate=28.0, hscale=0.8, scale=0.8, trans=0.0, hshear=0.1, brightness=1.3, contrast=1.1,
+                  d_vtrans=1.0, d_rotate=3.0, d_hscale=0.9, d_hshear=0.3, d_brightness=0.7, d_contrast=1.1)
+MB_DRAWS = dict(ds=2001, d_exp=0.2, d_light=0.2)
+NET_MB = dict(m=0.2, pow=1, **MB_DRAWS, l1=5, fm=64, ks=3, lr=0.002, bs=128, mom=0.9, true1=0.5, false1=1.5, false2=6.0)
+NET_SLOW_MB = dict(**MB_DRAWS, l1=5, fm=112, ks=3, l2=3, nh2=384, lr=0.003, bs=128, mom=0.9, true1=0.5, false1=1.5,
+                   false2=18.0)
+PRESETS_MB = {"fast": NET_MB, "slow": NET_SLOW_MB}
 WARP_DTYPE = np.dtype([("m", "<f4", (6,)), ("contrast", "<f4"), ("brightness", "<f4"), ("image", "<i4"), ("view", "<i4")])
+PAIR_DTYPE = np.dtype([("x0", "<u8"), ("x1", "<u8"), ("H", "<i4"), ("W", "<i4")])      # mccnn_train_pair
 TRAIN_PARAMS, TRAIN_MOMENTA, TRAIN_GRADS, TRAIN_PATCHES, TRAIN_TOWER, TRAIN_NORM, TRAIN_NORMALIZED, TRAIN_JOIN, \
     TRAIN_JOIN_GRAD, TRAIN_HINGE, TRAIN_NORM_GRAD_OUT, TRAIN_DZ, TRAIN_LOSS = range(13)
 TRAIN_ROWS, TRAIN_FC, TRAIN_SIGMOID, TRAIN_BCE_GRAD, TRAIN_ROWS_GRAD = range(13, 18)      # arch 'slow' only
@@ -62,13 +83,11 @@ TRAIN_ROWS, TRAIN_FC, TRAIN_SIGMOID, TRAIN_BCE_GRAD, TRAIN_ROWS_GRAD = range(13,
 
 def options(dataset, arch="fast", **overrides):
     """main.lua's training options for (dataset, arch) with `overrides`; refuses what this module does not train"""
-    if dataset == "mb":
-        raise ValueError("dataset mb: Middlebury training (the light and exposure sampler) is not supported")
-    if dataset not in ("kitti", "kitti2015"):
-        raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
+    if dataset not in ("kitti", "kitti2015", "mb"):
+        raise ValueError("dataset must be 'kitti', 'kitti2015' or 'mb', got %r" % (dataset,))
     if arch not in PRESETS:
         raise ValueError("arch %s: only the fast and slow architectures can be trained" % arch)
-    o = dict(AUGMENT, **PRESETS[arch])
+    o = dict(AUGMENT_MB, **PRESETS_MB[arch]) if dataset == "mb" else dict(AUGMENT, **PRESETS[arch])
     for k, v in overrides.items():
         if k not in o:
             raise ValueError("-%s is not a training option of arch %s" % (k, arch))
@@ -83,7 +102,7 @@ def arch_of(o):
 
 def check(o):
     """main.lua's asserts (:797, :810) and the limits of csrc/train.cu and the inference feature tower / scorer head"""
-    if o["at"]:
+    if o.get("at"):
         raise ValueError("-at 1 (the combined KITTI 2012 + 2015 training set) is not supported")
     if o["ks"] != 3:
         raise ValueError("-ks %d: only 3x3 kernels are supported" % o["ks"])
@@ -150,9 +169,17 @@ class Stream:
     def __init__(self, seed):
         self.bg = np.random.MT19937()
         self.bg._legacy_seeding(seed)
+        self.carry = np.zeros(0, np.uint32)      # words drawn ahead and handed back (see unread)
 
     def raw(self, n):
-        return self.bg.random_raw(n).astype(np.uint32)
+        if not len(self.carry):
+            return self.bg.random_raw(n).astype(np.uint32)
+        head, self.carry = self.carry[:n], self.carry[n:]
+        return np.concatenate([head, self.bg.random_raw(n - len(head)).astype(np.uint32)])
+
+    def unread(self, words):
+        """hand back words that were drawn but not used: the next raw() returns them first"""
+        self.carry = np.concatenate([np.asarray(words, np.uint32), self.carry])
 
     def uniform(self, n, a, b):
         return self.raw(n) * TWO32 * (b - a) + a
@@ -206,14 +233,25 @@ def init_net(stream, o):
     return init_slow(stream, o) if arch_of(o) == "slow" else (init_weights(stream, o["l1"], o["fm"]), None)
 
 
-def draw_params(stream, o, n):
-    """the torch.uniform calls of main.lua:791-818 for n samples -> dict of float64 arrays (n,) (scale, trans pairs as
-    two arrays)"""
-    cols = ["d_pos", "d_neg", "neg", "s", "hscale"] + (["hflip"] if o["hflip"] == 1 else []) + \
+def uniform_columns(o):
+    """the torch.uniform calls of main.lua:791-818 for one sample, in order"""
+    return ["d_pos", "d_neg", "neg", "s", "hscale"] + (["hflip"] if o["hflip"] == 1 else []) + \
         (["vflip"] if o["vflip"] == 1 else []) + ["hshear", "trans0", "trans1", "phi", "brightness", "contrast",
                                                   "d_hscale", "d_hshear", "d_vtrans", "d_rotate", "d_brightness",
                                                   "d_contrast"]
-    r = stream.raw(n * len(cols)).reshape(n, len(cols)).astype(np.float64) * TWO32
+
+
+def draw_params(stream, o, n):
+    """the torch.uniform calls of main.lua:791-818 for n samples -> dict of float64 arrays (n,) (scale, trans pairs as
+    two arrays)"""
+    cols = uniform_columns(o)
+    return params_from_words(stream.raw(n * len(cols)).reshape(n, len(cols)), o)
+
+
+def params_from_words(words, o):
+    """main.lua:791-818 from each sample's uniform words (n, len(uniform_columns(o))) uint32 -> dict as draw_params"""
+    cols = uniform_columns(o)
+    r = words.astype(np.float64) * TWO32
     c = {k: r[:, j] for j, k in enumerate(cols)}
     u = lambda k, a, b: c[k] * (b - a) + a
     p = {}
@@ -241,6 +279,45 @@ def draw_params(stream, o, n):
     return p
 
 
+def mb_sample_starts(raw, base, d_exp, cap):
+    """mccnn_mb_sample_starts: (first word of each of the first <= cap whole samples, words they take)"""
+    from .adcensus import _check, lib
+
+    raw = np.ascontiguousarray(raw, np.uint32)
+    starts = np.zeros(cap, np.int64)
+    count, used = ctypes.c_longlong(), ctypes.c_longlong()
+    _check(lib().mccnn_mb_sample_starts(raw.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(len(raw)), base,
+                                        ctypes.c_double(d_exp), starts.ctypes.data_as(ctypes.c_void_p),
+                                        ctypes.c_longlong(cap), ctypes.byref(count), ctypes.byref(used)),
+           "mccnn_mb_sample_starts")
+    return starts[:count.value], used.value
+
+
+def draw_params_mb(stream, o, n_light, n_exp):
+    """main.lua:791-841 for dataset mb, for len(n_light) samples whose images have n_light light groups j >= 2 and n_exp
+    exposures in each -> (draw_params' dict, light, exp, light_, exp_ as int64 arrays, 1-based as in main.lua).
+
+    A sample takes base + 4 or base + 5 words (exp_ is drawn only when the d_exp test passes), so the boundaries are found
+    by a walk over the raw words (mccnn_mb_sample_starts); the words drawn past the last sample go back to `stream`.
+    torch.random() is taken to be one 32-bit word, as for the uniforms."""
+    n_light, n_exp = np.asarray(n_light, np.int64), np.asarray(n_exp, np.int64)
+    n = len(n_light)
+    base = len(uniform_columns(o))
+    raw = stream.raw(n * (base + 5))                                              # enough for n samples
+    starts, used = mb_sample_starts(raw, base, o["d_exp"], n)
+    assert len(starts) == n
+    stream.unread(raw[used:])
+    p = params_from_words(raw[starts[:, None] + np.arange(base)], o)
+    w = lambda k: raw[starts + base + k].astype(np.int64)
+    light = w(0) % n_light + 2                                                    # :829
+    exp = w(1) % n_exp + 1                                                        # :830
+    t_exp = w(2) * TWO32 < o["d_exp"]                                             # :833
+    exp_ = np.where(t_exp, w(3) % n_exp + 1, exp)                                 # :834
+    t_light = raw[starts + base + 3 + t_exp].astype(np.float64) * TWO32 < o["d_light"]   # :836
+    light_ = np.where(t_light, np.maximum(2, light - 1), light)                   # :837
+    return p, light, exp, light_, exp_
+
+
 def _mul32(a, b):
     """main.lua:603-605 on arrays"""
     return [a[0] * b[0] + a[1] * b[3], a[0] * b[1] + a[1] * b[4], a[0] * b[2] + a[1] * b[5] + a[2],
@@ -261,9 +338,10 @@ def patch_matrices(ws, dim3, dim4, scale, phi, trans, hshear):
     return np.stack([np.broadcast_to(np.asarray(v, np.float64), (n,)) for v in m], 1).astype(np.float32)
 
 
-def make_warps(p, rows, ws):
+def make_warps(p, rows, ws, pairs=None):
     """main.lua:820-846: the (4 n,) mccnn_warp records of n samples from their parameters `p` and nnz rows (n, 4)
-    (image 1-based, dim3, dim4, d)"""
+    (image 1-based, dim3, dim4, d).  The patches read image - 1 of X0 / X1, or with `pairs` = (left, right) (n,) pair
+    indices (Middlebury) pair left's x0 and pair right's x1."""
     rows = np.asarray(rows, np.float32).astype(np.float64)
     n = len(rows)
     img, dim3, dim4, d = rows[:, 0], rows[:, 1], rows[:, 2], rows[:, 3]
@@ -276,7 +354,10 @@ def make_warps(p, rows, ws):
     for j, (c, br) in enumerate([(p["contrast"], p["brightness"]), (p["contrast_"], p["brightness_"])] * 2):
         out["contrast"][:, j] = c.astype(np.float32)
         out["brightness"][:, j] = br.astype(np.float32)
-    out["image"] = (img.astype(np.int64) - 1)[:, None]
+    if pairs is None:
+        out["image"] = (img.astype(np.int64) - 1)[:, None]
+    else:
+        out["image"] = np.stack([pairs[0], pairs[1], pairs[0], pairs[1]], 1)
     out["view"] = np.array([0, 1, 0, 1], np.int32)[None]
     return out.reshape(-1)
 
@@ -301,33 +382,80 @@ def sample_patches(X0, X1, warps, ws):
     return out
 
 
+def pair_table(planes):
+    """[(x0, x1)] CUDA float32 (H, W) contiguous planes -> PAIR_DTYPE array (the planes must outlive every use)"""
+    import torch
+
+    t = np.zeros(len(planes), PAIR_DTYPE)
+    for i, (a, b) in enumerate(planes):
+        if a.shape != b.shape or a.dim() != 2 or not (a.is_contiguous() and b.is_contiguous()) or \
+                a.dtype != torch.float32 or b.dtype != torch.float32 or not (a.is_cuda and b.is_cuda):
+            raise ValueError("pair %d: x0 and x1 must be contiguous CUDA float32 (H, W) planes of one shape" % i)
+        t[i] = (a.data_ptr(), b.data_ptr(), a.shape[0], a.shape[1])
+    return t
+
+
+def sample_patches_pairs(planes, warps, ws):
+    """the sampler alone on a table of pairs (mccnn_train_sample_pairs): planes [(x0, x1)] CUDA float32 (H, W) planes,
+    sizes free per pair, warps a WARP_DTYPE array whose image is a pair index -> (len(warps), ws, ws) CUDA float32"""
+    import torch
+
+    from .adcensus import _check, _stream, lib
+
+    dev = planes[0][0].device
+    table = torch.from_numpy(pair_table(planes).view(np.uint8)).to(dev)
+    w = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(dev)
+    out = torch.empty((len(warps), ws, ws), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _check(lib().mccnn_train_sample_pairs(ctypes.c_void_p(table.data_ptr()), len(planes), ctypes.c_void_p(w.data_ptr()),
+                                              len(warps), ws, ctypes.c_void_p(out.data_ptr()), _stream(out)),
+               "sample_patches_pairs")
+    return out
+
+
 class Trainer:
     """csrc/train.cu's trainer: net_tr + Margin2 ('fast') or + BCECriterion2 ('slow', when `o` has l2) and the momentum
-    update on `device`, sampling from X0 / X1 (CUDA)."""
+    update on `device`, sampling from X0 / X1 (CUDA), or with `planes` = [(x0, x1)] CUDA (H, W) planes from that table of
+    stereo pairs (a warp's image is then a pair index)."""
 
-    def __init__(self, o, X0, X1, chunk=CHUNK, loss_cap=1, device=None):
+    def __init__(self, o, X0=None, X1=None, chunk=CHUNK, loss_cap=1, device=None, planes=None):
         import torch
 
         from .adcensus import _check, _stream, _t, lib
 
         self.o, self.chunk = o, chunk
-        self.dev = X0.device if device is None else torch.device("cuda", device)
+        src = X0 if planes is None else planes[0][0]
+        self.dev = src.device if device is None else torch.device("cuda", device)
         self.arch = arch_of(o)
         self.l1, self.fm, self.bs = o["l1"], o["fm"], o["bs"]
         self.l2, self.nh2 = o.get("l2"), o.get("nh2")
         self.ws = 1 + 2 * self.l1
         self.N = 2 * self.bs
-        self._keep = (X0, X1)
-        n_img, _, H, W = X0.shape
+        self._keep = (X0, X1, planes)
         self._h = ctypes.c_void_p()
         with torch.cuda.device(self.dev):
             self.stream = torch.cuda.current_stream(self.dev)
-            if self.arch == "slow":
+            if planes is not None:
+                t = pair_table(planes)
+                tp = t.ctypes.data_as(ctypes.c_void_p)
+                if self.arch == "slow":
+                    _check(lib().mccnn_trainer_create_slow_pairs(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2,
+                                                                 self.bs, ctypes.c_float(o["mom"]), tp, len(t), chunk,
+                                                                 loss_cap, self.dev.index, _stream(src)),
+                           "mccnn_trainer_create_slow_pairs")
+                else:
+                    _check(lib().mccnn_trainer_create_pairs(ctypes.byref(self._h), self.l1, self.fm, self.bs,
+                                                            ctypes.c_float(o["m"]), o["pow"], ctypes.c_float(o["mom"]), tp,
+                                                            len(t), chunk, loss_cap, self.dev.index, _stream(src)),
+                           "mccnn_trainer_create_pairs")
+            elif self.arch == "slow":
+                n_img, _, H, W = X0.shape
                 _check(lib().mccnn_trainer_create_slow(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2, self.bs,
                                                        ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
                                                        _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
                                                        _stream(X0)), "mccnn_trainer_create_slow")
             else:
+                n_img, _, H, W = X0.shape
                 _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, ctypes.c_float(o["m"]),
                                                   o["pow"], ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
                                                   _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
@@ -461,14 +589,117 @@ def load_nnz(data, action, data_root):
     return nnz
 
 
+def _dims(path):
+    """the dimensions in `path`.dim, after checking that the data, .dim and .type files exist"""
+    for p in (path, path + ".dim", path + ".type"):
+        if not os.path.exists(p):
+            raise FileNotFoundError("missing data file %s" % p)
+    with open(path + ".dim") as f:
+        return [int(float(v)) for v in f.read().split()]
+
+
+class MbTrainSet:
+    """The training images of data.mb.<rect>_gray/ (main.lua:455-491): the nnz rows of `action` (nnz_tr, plus nnz_te for
+    train_all) and, for every image they name, its light groups x_<i>_<j>.bin, j >= 2, each (n_exp, 2, 1, H, W).
+
+    Everything is checked on the host from the .dim files, before any GPU work: a missing file, a row naming an image
+    with no light group j >= 2 (main.lua:829 would take % 0), and an image whose light groups hold unequal exposure
+    counts (:834-840 index light_ with an exposure drawn for light).  :meth:`upload` then refuses a set whose planes do
+    not fit in the device's free memory, and copies each group file to the device once.  Pair (image, light, exp) is
+    index ``first[image] + (light - 2) n_exp[image] + exp - 1``: x0 = group[exp - 1, 0], x1 = group[exp - 1, 1]."""
+
+    def __init__(self, data_root=".", rect="imperfect", action="train_tr"):
+        self.dir = d = os.path.join(data_root, "data.mb.%s_gray" % rect)
+        nnz = evaluate._fromfile(os.path.join(d, "nnz_tr.bin"))
+        if action == "train_all":                                                # main.lua:650-654
+            nnz = np.concatenate([nnz, evaluate._fromfile(os.path.join(d, "nnz_te.bin"))])
+        self.nnz = np.ascontiguousarray(nnz, np.float32).reshape(-1, 4)
+        n_img = len(evaluate._fromfile(os.path.join(d, "meta.bin")))
+        imgs = np.unique(self.nnz[:, 0]).astype(np.int64)
+        if len(imgs) and not (imgs[0] >= 1 and imgs[-1] <= n_img):
+            raise ValueError("%s: nnz rows name images outside 1 .. %d" % (d, n_img))
+        self.groups = []                                                         # (image, light, path, dims)
+        self.nbytes = 0
+        counts = {}
+        for i in imgs:
+            exps = []
+            j = 2
+            while os.path.exists(os.path.join(d, "x_%d_%d.bin.dim" % (i, j))):
+                p = os.path.join(d, "x_%d_%d.bin" % (i, j))
+                dims = _dims(p)
+                if len(dims) != 5 or dims[0] < 1 or dims[1] != 2 or dims[2] != 1 or min(dims[3:]) < 1:
+                    raise ValueError("%s: a light group must be (n_exp, 2, 1, H, W), the .dim says %s" % (p, dims))
+                self.groups.append((int(i), j, p, dims))
+                self.nbytes += 4 * int(np.prod(dims))
+                exps.append(dims[0])
+                j += 1
+            if not exps:
+                raise ValueError("%s: nnz rows name image %d, which has no light group x_%d_2.bin (main.lua:829 would "
+                                 "take %% 0)" % (d, i, i))
+            if len(set(exps)) != 1:
+                raise ValueError("%s: image %d's light groups hold unequal exposure counts %s (main.lua:834-840 index "
+                                 "light_ with an exposure drawn for light)" % (d, i, exps))
+            counts[int(i)] = (len(exps), exps[0])
+        self._index(n_img, counts)
+
+    @classmethod
+    def from_counts(cls, nnz, counts):
+        """the draws and pair indices of a set whose planes are built elsewhere (tools/time_train.py): counts
+        {image: (light groups, exposures)}, pairs in the same order as :meth:`upload`'s"""
+        self = cls.__new__(cls)
+        self.dir, self.nnz, self.groups, self.nbytes = None, np.ascontiguousarray(nnz, np.float32).reshape(-1, 4), [], 0
+        self._index(max(counts), counts)
+        return self
+
+    def _index(self, n_img, counts):
+        self.n_light = np.zeros(n_img + 1, np.int64)                            # by 1-based image
+        self.n_exp = np.zeros(n_img + 1, np.int64)
+        self.first = np.full(n_img + 1, -1, np.int64)
+        n_pairs = 0
+        for i in sorted(counts):
+            self.n_light[i], self.n_exp[i] = counts[i]
+            self.first[i] = n_pairs
+            n_pairs += counts[i][0] * counts[i][1]
+        self.n_pairs = n_pairs
+
+    def pair_index(self, img, light, exp):
+        """(image, light, exp), 1-based as in main.lua (arrays or scalars) -> the 0-based pair index"""
+        img = np.asarray(img, np.int64)
+        return self.first[img] + (np.asarray(light) - 2) * self.n_exp[img] + np.asarray(exp) - 1
+
+    def check_fits(self, free):
+        if self.nbytes > free:
+            raise MemoryError("%s: the training planes need %d bytes on the device, %d are free" % (self.dir, self.nbytes,
+                                                                                                      free))
+
+    def upload(self, device):
+        """-> [(x0, x1)] CUDA (H, W) planes in pair order, views of one device tensor per group file"""
+        import torch
+
+        dev = torch.device("cuda", device)
+        self.check_fits(torch.cuda.mem_get_info(dev)[0])
+        planes = []
+        for _, _, p, dims in self.groups:
+            g = torch.from_numpy(np.ascontiguousarray(dataio.fromfile(p), np.float32).reshape(dims)).to(dev)
+            planes += [(g[e, 0, 0], g[e, 1, 0]) for e in range(dims[0])]
+        return planes
+
+    def warps(self, stream, o, rows, ws):
+        """main.lua:791-846 for the samples of nnz `rows` -> WARP_DTYPE records naming pairs"""
+        img = rows[:, 0].astype(np.int64)
+        p, light, exp, light_, exp_ = draw_params_mb(stream, o, self.n_light[img], self.n_exp[img])
+        return make_warps(p, rows, ws, pairs=(self.pair_index(img, light, exp), self.pair_index(img, light_, exp_)))
+
+
 def net_path(data_root, dataset, args, arch="fast"):
     return os.path.join(data_root, "net", "net_%s.t7" % cmd_str(dataset, args, arch))
 
 
-def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS):
+def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS,
+          rect="imperfect"):
     """main.lua:602-890 for arch 'fast' or 'slow' (as `o` was made): returns the saved net's file name.  `args` are main.lua's arguments after
     dataset and arch (for the file name), `stereo` the stereo method's overrides for the evaluation that follows;
-    `log` receives the printed lines."""
+    `log` receives the printed lines.  For dataset mb the set is data.mb.<rect>_gray (see :class:`MbTrainSet`)."""
     import torch
 
     from . import t7
@@ -482,8 +713,10 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
         raise FileExistsError("%s already exists; remove it first" % fname)
     if action == "train_all" and os.path.isdir(out) and any(f != ".empty" for f in os.listdir(out)):
         raise ValueError("submit: output directory %s is not empty" % out)
-    data = evaluate.load_data(dataset, data_root)
-    nnz = load_nnz(data, action, data_root)
+    data = evaluate.load_data(dataset, data_root, rect)
+    mb = MbTrainSet(data_root, rect, action) if dataset == "mb" else None
+    nnz = mb.nnz if mb else load_nnz(data, action, data_root)
+    planes = mb.upload(device) if mb else None
     stream = Stream(seed)                                                        # main.lua:340
     perm = randperm(stream, len(nnz))                                            # :657
     tower, head = init_net(stream, o)                                            # :663-736
@@ -493,9 +726,14 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     nsteps = steps_per_epoch(len(nnz), o["bs"])
     dev = torch.device("cuda", device)
     with torch.cuda.device(dev):
-        X0 = torch.from_numpy(np.ascontiguousarray(data.X0, np.float32)).to(dev)
-        X1 = torch.from_numpy(np.ascontiguousarray(data.X1, np.float32)).to(dev)
-        tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
+        if mb:
+            tr = Trainer(o, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device, planes=planes)
+            build = lambda n, rows: mb.warps(stream, o, rows, tr.ws)                                      # :791-846
+        else:
+            X0 = torch.from_numpy(np.ascontiguousarray(data.X0, np.float32)).to(dev)
+            X1 = torch.from_numpy(np.ascontiguousarray(data.X1, np.float32)).to(dev)
+            tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
+            build = lambda n, rows: make_warps(draw_params(stream, o, n * h), rows, tr.ws)
         try:
             tr.set_layers(tower, head)
             rec = WARP_DTYPE.itemsize * tr.N
@@ -510,7 +748,7 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
                 for k, s0 in enumerate(range(0, nsteps, CHUNK)):
                     n = min(CHUNK, nsteps - s0)
                     rows = nnz[perm[s0 * h:(s0 + n) * h] - 1]                  # perm[t + i - 1], :820
-                    warps = make_warps(draw_params(stream, o, n * h), rows, tr.ws)
+                    warps = build(n, rows)
                     b = k % 2
                     if events[b] is not None:
                         events[b].synchronize()
@@ -527,8 +765,12 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
             tower, head = tr.net()
         finally:
             tr.close()
+    if mb:                                                                       # the training planes are not needed now
+        del planes, tr
+        torch.cuda.empty_cache()
     os.makedirs(os.path.dirname(fname), exist_ok=True)
-    t7.save_net(fname, tower, head, opt=dict(o, a=action, seed=seed, gpu=device + 1))   # :883, save_net(0)
+    extra = dict(rect=rect, color="gray") if mb else {}
+    t7.save_net(fname, tower, head, opt=dict(o, a=action, seed=seed, gpu=device + 1, **extra))   # :883, save_net(0)
     ev = evaluate.Evaluator(dataset, arch, net_fname=fname, device=device, **(stereo or {}))
     try:
         if action == "train_tr":                                                 # :884-888

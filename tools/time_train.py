@@ -1,6 +1,10 @@
 """Measure the training step of the fast or slow architecture (csrc/train.cu) on a synthetic full-size KITTI 2012 set.
 
-    python tools/time_train.py [-arch fast|slow] [-steps 2000] [-gpu 1] [-json out.json]
+    python tools/time_train.py [-arch fast|slow] [-dataset kitti|mb] [-steps 2000] [-gpu 1] [-json out.json]
+
+With -dataset mb the presets are main.lua's mb ones (l1 5; fm 64 'fast', 112 'slow') and the set is a synthetic ragged
+Middlebury set on the device (see mb_shapes: 50 images, one pair per image, light and exposure, 1,048,576 nnz rows); the
+host build is the mb draw builder (MbTrainSet.warps), and the pair count and the bytes of the planes are reported.
 
 The set is 389 views of 350 x 1242 per side on the device and 1,048,576 nnz rows, at main.lua's kitti presets (l1 4, fm 64,
 bs 128).  Reported, each after a warm-up:
@@ -33,6 +37,19 @@ def card():
         return r.stdout.strip().splitlines()[0]
     except Exception as e:  # noqa: BLE001
         return "unknown (%s)" % e
+
+
+def mb_shapes(rng):
+    """a synthetic Middlebury training set of realistic size: 20 scenes of about 1000 x 1450 with 3 to 6 lights of 3
+    exposures (the 2014 half-size scenes) and 30 of about 550 x 690 with 3 x 3 (2006 / 2005 HalfSize and smaller)
+    -> ([(H, W)] per image, {image: (lights, exposures)})"""
+    sizes, counts = [], {}
+    for k in range(50):
+        big = k < 20
+        sizes.append((int(rng.integers(950, 1050)), int(rng.integers(1350, 1500))) if big else
+                     (int(rng.integers(500, 600)), int(rng.integers(640, 740))))
+        counts[k + 1] = (int(rng.integers(3, 7)) if big else 3, 3)
+    return sizes, counts
 
 
 def baseline_step(x, params, vel, o, lr):
@@ -86,6 +103,7 @@ def main(argv=None):
     ap.add_argument("-gpu", type=int, default=1)
     ap.add_argument("-json", default="")
     ap.add_argument("-arch", choices=("fast", "slow"), default="fast")
+    ap.add_argument("-dataset", choices=("kitti", "mb"), default="kitti")
     args = ap.parse_args(argv)
     import torch
 
@@ -96,26 +114,49 @@ def main(argv=None):
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda", args.gpu - 1)
     torch.cuda.set_device(dev)
-    o = train.options("kitti", args.arch)
-    n_img, H, W, rows = 389, 350, 1242, 1 << 20
+    o = train.options(args.dataset, args.arch)
+    rows = 1 << 20
     g = torch.Generator(device=dev).manual_seed(0)
-    X0 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
-    X1 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
     rng = np.random.default_rng(0)
-    nnz = np.stack([rng.integers(1, n_img + 1, rows), rng.integers(0, H, rows), rng.integers(0, W, rows),
-                    rng.uniform(1, 200, rows)], 1).astype(np.float32)
+    extra = {}
+    if args.dataset == "mb":
+        sizes, counts = mb_shapes(rng)
+        img = rng.integers(1, len(sizes) + 1, rows)
+        hw = np.array(sizes)[img - 1]
+        nnz = np.stack([img, rng.integers(0, hw[:, 0]), rng.integers(0, hw[:, 1]), rng.uniform(1, 140, rows)],
+                       1).astype(np.float32)
+        mb = train.MbTrainSet.from_counts(nnz, counts)
+        planes = []
+        for i, (hh, ww) in enumerate(sizes, 1):                   # MbTrainSet.upload's order: image, light, exposure
+            for _ in range(counts[i][0]):
+                grp = torch.randn((counts[i][1], 2, hh, ww), device=dev, generator=g)
+                planes += [(grp[e, 0], grp[e, 1]) for e in range(counts[i][1])]
+        extra = dict(pairs=len(planes), images=len(sizes),
+                     plane_bytes=sum(2 * a.numel() * 4 for a, _ in planes))
+        X0 = X1 = None
+    else:
+        n_img, H, W = 389, 350, 1242
+        X0 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
+        X1 = torch.randn((n_img, 1, H, W), device=dev, generator=g)
+        nnz = np.stack([rng.integers(1, n_img + 1, rows), rng.integers(0, H, rows), rng.integers(0, W, rows),
+                        rng.uniform(1, 200, rows)], 1).astype(np.float32)
+        planes = None
     s = train.Stream(42)
     perm = train.randperm(s, rows)
     chunk = train.CHUNK
-    tr = train.Trainer(o, X0, X1, chunk=chunk, loss_cap=args.steps + 4 * chunk, device=dev.index)
+    tr = train.Trainer(o, X0, X1, chunk=chunk, loss_cap=args.steps + 4 * chunk, device=dev.index, planes=planes)
     tr.set_layers(*train.init_net(s, o))
     h = o["bs"] // 2
     res = dict(card=card(), launches_per_step=tr.launches_per_step, steps=args.steps)
     if args.arch == "slow":
         res["arch"] = "slow"
+    if args.dataset == "mb":
+        res.update(dataset="mb", **extra)
 
     def warps_for(s0, n):
         r = nnz[perm[(s0 * h) % (rows - n * h):][:n * h] - 1]
+        if args.dataset == "mb":
+            return mb.warps(s, o, r, tr.ws)
         return train.make_warps(train.draw_params(s, o, n * h), r, tr.ws)
 
     # device: parameters already on the device

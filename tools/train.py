@@ -7,7 +7,8 @@ Option names and defaults are main.lua's (-gpu is 1-based as there): the network
 -mom -true1 -false1 -false2 -m -pow), the augmentation options (-hflip ... -d_contrast) and the stereo method's overrides of
 run_main.py (-L1 ... -blur_t) for the evaluation that follows.  The net goes to <data_root>/net/net_<cmd_str>.t7, named from
 main.lua's arguments.  Everything the trainer does not implement is refused before any GPU work; see mc-cnn_b200/train.py.
-The slow architecture is trained by tools/train_slow.py, which shares this parser.
+The slow architecture is trained by tools/train_slow.py, and both architectures on Middlebury by tools/train_mb.py; both
+share this parser.
 """
 import argparse
 import os
@@ -20,9 +21,14 @@ from run_main import PRESET_OPTIONS, _flag  # noqa: E402
 TOOL_ONLY = ("-data_root", "-out")
 
 
-def parser(prog="train.py", description=__doc__.splitlines()[0]):
+def _names(mb):
+    """the training options a tool accepts: KITTI's, plus main.lua's mb-only -ds -d_exp -d_light for the Middlebury tool"""
     from mccnn_b200 import train
 
+    return {**train.AUGMENT, **train.NET, **train.NET_SLOW, **(train.MB_DRAWS if mb else {})}
+
+
+def parser(prog="train.py", description=__doc__.splitlines()[0], mb=False):
     ap = argparse.ArgumentParser(prog=prog, description=description)
     ap.add_argument("dataset", choices=("kitti", "kitti2015", "mb"))
     ap.add_argument("arch", choices=("fast", "slow", "ad", "census"))
@@ -33,7 +39,10 @@ def parser(prog="train.py", description=__doc__.splitlines()[0]):
     ap.add_argument("-out", default="out")
     ap.add_argument("-subset", type=float, default=1)
     ap.add_argument("-debug", nargs="?", const=True, default=False, type=_flag)
-    for name, v in {**train.AUGMENT, **train.NET, **train.NET_SLOW}.items():
+    if mb:
+        ap.add_argument("-rect", choices=("perfect", "imperfect"), default="imperfect")
+        ap.add_argument("-color", default="gray")
+    for name, v in _names(mb).items():
         ap.add_argument("-" + name, type=type(v), default=None)
     for name, typ in PRESET_OPTIONS.items():
         ap.add_argument("-" + name, type=typ, default=None)
@@ -53,22 +62,36 @@ def main_args(argv):
     return out
 
 
-# the tools and the architecture each trains; the other one is named in the refusal
+# the KITTI tools and the architecture each trains; the other one is named in the refusal.  train_mb.py trains both
+# architectures on Middlebury (arch None below).
 TOOLS = {"fast": "train.py", "slow": "train_slow.py"}
+MB_TOOL = "train_mb.py"
 
 
 def parse_args(argv=None, arch="fast"):
     """-> (namespace, training options, stereo overrides).  Refuses what the trainer does not implement, and every arch
-    but `arch`."""
+    but `arch` (arch None: the Middlebury tool, fast or slow on dataset mb only)."""
     from mccnn_b200 import train
 
-    prog = TOOLS[arch]
+    mb = arch is None
+    prog = MB_TOOL if mb else TOOLS[arch]
     argv = list(sys.argv[1:] if argv is None else argv)
-    args = parser(prog).parse_args(argv)
-    if args.arch != arch:
+    args = parser(prog, mb=mb).parse_args(argv)
+    if mb:
+        if args.dataset != "mb":
+            raise SystemExit("%s: dataset %s: this tool trains on Middlebury (mb); use train.py or train_slow.py"
+                             % (prog, args.dataset))
+        if args.arch not in TOOLS:
+            raise SystemExit("%s: arch %s: only the fast and slow architectures can be trained" % (prog, args.arch))
+        if args.color != "gray":
+            raise SystemExit("%s: -color %s is not supported: three-plane images need a 3-plane first layer in the "
+                             "trainer, the feature tower and the evaluation; only -color gray is" % (prog, args.color))
+    elif args.arch != arch:
         other = [TOOLS[a] for a in TOOLS if a == args.arch]
         raise SystemExit("%s: arch %s: only the %s architecture can be trained by this tool%s"
                          % (prog, args.arch, arch, "; use %s" % other[0] if other else ""))
+    elif args.dataset == "mb":
+        raise SystemExit("%s: dataset mb: Middlebury training is done by %s" % (prog, MB_TOOL))
     if args.a not in ("train_tr", "train_all"):
         raise SystemExit("%s: -a %s is not a training action (train_tr, train_all); see run_main.py" % (prog, args.a))
     if args.gpu < 1:
@@ -77,8 +100,7 @@ def parse_args(argv=None, arch="fast"):
         raise SystemExit("%s: -subset %s is not supported (the whole training set is used)" % (prog, args.subset))
     if args.debug:
         raise SystemExit("%s: -debug (a net file per epoch) is not supported" % prog)
-    names = {**train.AUGMENT, **train.NET, **train.NET_SLOW}
-    given = {k: getattr(args, k) for k in names if getattr(args, k) is not None}
+    given = {k: getattr(args, k) for k in _names(mb) if getattr(args, k) is not None}
     try:
         o = train.options(args.dataset, args.arch, **given)
     except ValueError as e:
@@ -94,12 +116,22 @@ def main(argv=None, arch="fast"):
     import mccnn_b200  # noqa: F401
     from mccnn_b200 import train
 
-    fname = train.net_path(args.data_root, args.dataset, main_args(args.argv), arch)
+    prog = MB_TOOL if arch is None else TOOLS[arch]
+    fname = train.net_path(args.data_root, args.dataset, main_args(args.argv), args.arch)
     if os.path.exists(fname):
-        raise SystemExit("%s: %s already exists; remove it first" % (TOOLS[arch], fname))
+        raise SystemExit("%s: %s already exists; remove it first" % (prog, fname))
+    rect = {"rect": args.rect} if arch is None else {}
+    if arch is None:                                                              # refuse a bad set before printing
+        try:
+            train.MbTrainSet(args.data_root, args.rect, args.a)
+        except (OSError, ValueError) as e:
+            raise SystemExit("%s: %s" % (prog, e))
     print(" ".join(args.argv) + " ", flush=True)                                  # main.lua:6-9
-    train.train(args.dataset, args.a, o, args=main_args(args.argv), data_root=args.data_root, seed=args.seed,
-                device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True))
+    try:
+        train.train(args.dataset, args.a, o, args=main_args(args.argv), data_root=args.data_root, seed=args.seed,
+                    device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True), **rect)
+    except MemoryError as e:                                                      # the mb planes do not fit
+        raise SystemExit("%s: %s" % (prog, e))
     return 0
 
 
