@@ -218,7 +218,30 @@ typedef struct mccnn_params {
 	float blur_t;
 	int border;    /* fix_border n (4 for the 4-layer 3x3 tower, main.lua:382-391,923) */
 	int lr_check;  /* 1: kitti / kitti2015 (main.lua:1054); 0: mb */
+	/* main.lua's -sm_terminate / -sm_skip (main.lua:953-1082): an MCCNN_SM_* code each, 0 = the full chain.  A step
+	 * runs while no earlier -sm_terminate step has been passed and it is not the skipped one; terminate occlusion /
+	 * mismatch and skip occlusion act only with the LR check.  When the chain stops early, disp receives the map
+	 * main.lua returns (the 0-based argmin of the left volume for terminate cnn / cbca1 / sgm / cbca2). */
+	int sm_terminate;  /* MCCNN_SM_CNN .. MCCNN_SM_MEDIAN */
+	int sm_skip;       /* MCCNN_SM_CBCA, _SGM, _OCCLUSION, _SUBPIXEL, _MEDIAN, _BILATERAL */
 } mccnn_params;
+
+/* Stage codes of mccnn_params.sm_terminate / sm_skip, named after main.lua's option values.  Terminate accepts cnn, cbca1,
+ * sgm, cbca2, occlusion, mismatch, subpixel_enchancement and median; skip accepts cbca, sgm, occlusion,
+ * subpixel_enchancement, median and bilateral.  Any other code is refused (ADCENSUS_EINVAL). */
+enum {
+	MCCNN_SM_NONE = 0,
+	MCCNN_SM_CNN = 1,        /* terminate: the argmin of the raw volume */
+	MCCNN_SM_CBCA1 = 2,      /* terminate: after cross + the first CBCA block */
+	MCCNN_SM_SGM = 3,        /* terminate / skip: SGM */
+	MCCNN_SM_CBCA2 = 4,      /* terminate: after the second CBCA block */
+	MCCNN_SM_OCCLUSION = 5,  /* terminate / skip (both interpolations): LR check only */
+	MCCNN_SM_MISMATCH = 6,   /* terminate: LR check only */
+	MCCNN_SM_SUBPIXEL = 7,   /* terminate / skip: subpixel_enchancement */
+	MCCNN_SM_MEDIAN = 8,     /* terminate / skip: median2d */
+	MCCNN_SM_BILATERAL = 9,  /* skip: mean2d */
+	MCCNN_SM_CBCA = 10       /* skip: the cross arms and both CBCA blocks */
+};
 
 typedef struct mccnn_pipeline mccnn_pipeline;
 
@@ -239,7 +262,7 @@ int mccnn_pipeline_get_cbca_mode(const mccnn_pipeline *p);
  * Results are identical in every mode (same kernels, same data); only the schedule and the memory footprint change.
  * Returns 0 or an error. */
 int mccnn_pipeline_set_overlap(mccnn_pipeline *p, int mode);
-/* number of kernel launches one run issues (for bench.py's gpu_launches) */
+/* number of kernel launches the last run issued (for bench.py's gpu_launches); fewer when sm_terminate / sm_skip drop steps */
 int mccnn_pipeline_launches_per_run(const mccnn_pipeline *p);
 /* Re-targets a created pipeline to another parameter set without allocating its volumes again (a parameter search runs
  * many sets over the same images).  Checked like mccnn_pipeline_create (ADCENSUS_EINVAL; border + 1 must not exceed the

@@ -161,10 +161,54 @@ struct DeviceGuard {
 	~DeviceGuard() { cudaSetDevice(prev); }
 };
 
+bool terminate_ok(int c) { return c >= MCCNN_SM_NONE && c <= MCCNN_SM_MEDIAN; }
+bool skip_ok(int c)
+{
+	return c == MCCNN_SM_NONE || c == MCCNN_SM_SGM || c == MCCNN_SM_OCCLUSION || c == MCCNN_SM_SUBPIXEL || c == MCCNN_SM_MEDIAN ||
+	       c == MCCNN_SM_BILATERAL || c == MCCNN_SM_CBCA;
+}
+
 // the parameter checks shared by create and set_params; W = the created width
 bool params_ok(const mccnn_params *o, int W)
 {
-	return o->cbca_i1 >= 0 && o->cbca_i2 >= 0 && o->sgm_i >= 0 && o->border >= 0 && o->border + 1 <= W;
+	return o->cbca_i1 >= 0 && o->cbca_i2 >= 0 && o->sgm_i >= 0 && o->border >= 0 && o->border + 1 <= W &&
+	       terminate_ok(o->sm_terminate) && skip_ok(o->sm_skip);
+}
+
+// Which steps of main.lua:953-1082 run under -sm_terminate / -sm_skip: sm_active starts true, a step runs while it is true
+// and the step is not the skipped one, and passing the terminate step clears it.  The LR-check steps and their terminate
+// names exist only for kitti (lr_check).
+struct Stages {
+	bool cbca1, sgm, cbca2, occlusion, mismatch, subpixel, median, bilateral;
+};
+
+Stages stages_of(const mccnn_params &o)
+{
+	const int T = o.sm_terminate, S = o.sm_skip;
+	Stages st;
+	bool active = T != MCCNN_SM_CNN;                                                          // :988
+	st.cbca1 = active && S != MCCNN_SM_CBCA;                                                  // :992
+	active = active && T != MCCNN_SM_CBCA1;                                                   // :1005
+	st.sgm = active && S != MCCNN_SM_SGM;                                                     // :1007
+	active = active && T != MCCNN_SM_SGM;                                                     // :1031
+	st.cbca2 = active && S != MCCNN_SM_CBCA;                                                  // :1033
+	active = active && T != MCCNN_SM_CBCA2;                                                   // :1040
+	st.occlusion = o.lr_check && active && S != MCCNN_SM_OCCLUSION;                           // :1057
+	if (o.lr_check) active = active && T != MCCNN_SM_OCCLUSION;                              // :1060
+	st.mismatch = o.lr_check && active && S != MCCNN_SM_OCCLUSION;                            // :1062
+	if (o.lr_check) active = active && T != MCCNN_SM_MISMATCH;                               // :1065
+	st.subpixel = active && S != MCCNN_SM_SUBPIXEL;                                           // :1067
+	active = active && T != MCCNN_SM_SUBPIXEL;                                                // :1071
+	st.median = active && S != MCCNN_SM_MEDIAN;                                               // :1072
+	active = active && T != MCCNN_SM_MEDIAN;                                                  // :1076
+	st.bilateral = active && S != MCCNN_SM_BILATERAL;                                         // :1077
+	return st;
+}
+
+// direction +1 is consumed only by the outlier map of the interpolations (or a caller that wants the right volume)
+bool needs_right(const mccnn_params &o, const Stages &st, const float *volR)
+{
+	return (o.lr_check && (st.occlusion || st.mismatch)) || volR;
 }
 
 // gaussian(blur_sigma) (main.lua:1078 gaussian(opt.blur_sigma):cuda()) into p->gauss; the buffer grows only when the kernel
@@ -394,11 +438,13 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 	const int ld = (W + 3) & ~3;
 	const long HW = (long)H * W, V = (long)D * H * ld;
 	const mccnn_params &o = p->prm;
+	const Stages st = stages_of(o);
 	float *volsL = p->vols, *volsR = p->vols + V;
+	const int cbca_i1 = st.cbca1 ? o.cbca_i1 : 0, cbca_i2 = st.cbca2 ? o.cbca_i2 : 0, sgm_i = st.sgm ? o.sgm_i : 0;
 
 	// cross arms: identical for both directions (main.lua:993-996 recomputes them)
 	const int maxlen = pipe_maxlen(p);       // bound on the arm length cross() can produce
-	const int ncbca = o.cbca_i1 + o.cbca_i2;
+	const int ncbca = cbca_i1 + cbca_i2;
 	// fix_border copies column W-n-1 over the border columns: for D > W - n - 1 that column holds NaN at "valid"
 	// positions, which only the tap-by-tap generic kernel treats like the reference (NaN only where a tap is NaN)
 	const bool nan_in_valid = o.border > 0 && D > W - o.border - 1;
@@ -424,24 +470,27 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		return adc_cbca_packed(p->packed, p->x0c, p->x1c, in, out, D, H, W, ld, direction, nan_in_valid ? (1 << 20) : maxlen, ds);
 	};
 
-	float *dispR = p->maps, *dispL = p->maps + HW;
+	// every map is written straight into `disp` when no later step runs (an early -sm_terminate, or skipped tail steps)
+	const bool after_mis = st.subpixel || st.median || st.bilateral, after_occ = st.mismatch || after_mis;
+	float *m = p->maps;
+	float *dispR = m, *dispL = (st.occlusion || after_occ) ? m + HW : disp;
 	float *final_left = nullptr;
 	// One direction of main.lua:955-1051 on stream `ds`: cur/spare ping-pong, acc = SGM accumulator.
 	// k = 0: direction +1 (right volume), k = 1: direction -1 (left volume).
 	auto run_direction = [&](int k, cudaStream_t ds, float *cur, float *spare, float *acc, uint8_t *tab) -> int {
 		const int direction = k == 0 ? 1 : -1;                                                   // :955
-		for (int i = 0; i < o.cbca_i1; i++) {                                                    // :998-1001
+		for (int i = 0; i < cbca_i1; i++) {                                                      // :998-1001
 			STEP(cbca(cur, spare, direction, ds));
 			float *t = cur; cur = spare; spare = t; nl += 1;
 		}
 		if (k == 0 && p->overlap) STEP((int)cudaEventRecord(p->ev_stagger, ds));                 // the other direction may start
 		cudaStream_t ss = ds;                                                                    // stream of the SGM phase
-		if (p->overlap && o.sgm_i > 0) {
+		if (p->overlap && sgm_i > 0) {
 			ss = p->hi_stream[k];
 			STEP((int)cudaEventRecord(p->ev_hi_in[k], ds));
 			STEP((int)cudaStreamWaitEvent(ss, p->ev_hi_in[k], 0));
 		}
-		for (int it = 0; it < o.sgm_i; it++) {                                                   // :1008-1020
+		for (int it = 0; it < sgm_i; it++) {                                                     // :1008-1020
 			STEP(adc_transpose_dhw_pitched_to_hwd(cur, spare, D, H, W, ld, ss));                 // :1008
 			STEP(adc_sgm2(imgL, imgR, spare, acc, tab, H, W, D, o.pi1, o.pi2, o.tau_so, o.alpha1,
 				      o.sgm_q1, o.sgm_q2, direction, /*zero_out=*/true, ss));                    // :1014-1016
@@ -452,7 +501,7 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 			STEP((int)cudaEventRecord(p->ev_hi_out[k], ss));
 			STEP((int)cudaStreamWaitEvent(ds, p->ev_hi_out[k], 0));
 		}
-		for (int i = 0; i < o.cbca_i2; i++) {                                                    // :1035-1038
+		for (int i = 0; i < cbca_i2; i++) {                                                      // :1035-1038
 			STEP(cbca(cur, spare, direction, ds));
 			float *t = cur; cur = spare; spare = t; nl += 1;
 		}
@@ -464,8 +513,8 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		return 0;
 	};
 	// main.lua:954-955: without the LR check (mb) only direction -1 is consumed, unless the caller asks for the
-	// right volume (`-a predict` writes right.bin)
-	const bool need_right = o.lr_check || volR;
+	// right volume (`-a predict` writes right.bin); with it, only when an interpolation reads the outlier map
+	const bool need_right = needs_right(o, st, volR);
 	if (!need_right) {
 		STEP(run_direction(1, s, volsL, p->bufA, p->bufC, p->sgmtab));
 	} else if (!p->overlap) {
@@ -482,18 +531,34 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		STEP((int)cudaStreamWaitEvent(s, p->ev_join, 0));
 	}
 
-	float *m = p->maps;
 	const float *curd = dispL;                                                                   // disp[2]
-	if (o.lr_check) {                                                                            // :1054-1066
-		float *outlier = m + 2 * HW;
-		STEP(adcensus_outlier_detection(dispL, dispR, outlier, H, W, D, s));                     // :1056
-		STEP(adcensus_interpolate_occlusion(curd, outlier, m + 3 * HW, H, W, s));                // :1058
-		STEP(adcensus_interpolate_mismatch(m + 3 * HW, outlier, m + 4 * HW, H, W, s));           // :1063
-		curd = m + 4 * HW; nl += 3;
+	float *outlier = m + 2 * HW;
+	if (st.occlusion || st.mismatch) {                                                           // :1056 (unread otherwise)
+		STEP(adcensus_outlier_detection(dispL, dispR, outlier, H, W, D, s)); nl += 1;
 	}
-	STEP(adc_subpixel(curd, final_left, m + 5 * HW, H, W, ld, D, s));                            // :1068
-	STEP(adcensus_median2d(m + 5 * HW, m + 6 * HW, H, W, 5, s));                                 // :1073
-	STEP(adcensus_mean2d(m + 6 * HW, p->gauss, disp, H, W, p->ks, o.blur_t, s)); nl += 3;        // :1078
+	if (st.occlusion) {                                                                          // :1058
+		float *out = after_occ ? m + 3 * HW : disp;
+		STEP(adcensus_interpolate_occlusion(curd, outlier, out, H, W, s)); nl += 1;
+		curd = out;
+	}
+	if (st.mismatch) {                                                                           // :1063
+		float *out = after_mis ? m + 4 * HW : disp;
+		STEP(adcensus_interpolate_mismatch(curd, outlier, out, H, W, s)); nl += 1;
+		curd = out;
+	}
+	if (st.subpixel) {                                                                           // :1068
+		float *out = st.median || st.bilateral ? m + 5 * HW : disp;
+		STEP(adc_subpixel(curd, final_left, out, H, W, ld, D, s)); nl += 1;
+		curd = out;
+	}
+	if (st.median) {                                                                             // :1073
+		float *out = st.bilateral ? m + 6 * HW : disp;
+		STEP(adcensus_median2d(curd, out, H, W, 5, s)); nl += 1;
+		curd = out;
+	}
+	if (st.bilateral) {                                                                          // :1078
+		STEP(adcensus_mean2d(curd, p->gauss, disp, H, W, p->ks, o.blur_t, s)); nl += 1;
+	}
 	p->launches = nl;
 	return 0;
 }
@@ -522,7 +587,7 @@ extern "C" int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D
 	const long V = (long)D * H * ld;
 	const size_t row = (size_t)W * sizeof(float), pitch = (size_t)ld * sizeof(float);
 	ADC_CUDA(cudaMemcpy2DAsync(p->vols, pitch, volL, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
-	if (p->prm.lr_check || outR)                                           // only then is the right volume read
+	if (needs_right(p->prm, stages_of(p->prm), outR))                      // only then is the right volume read
 		ADC_CUDA(cudaMemcpy2DAsync(p->vols + V, pitch, volR, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
 	return run_chain(p, H, W, D, imgL, imgR, disp, outL, outR, 0, s);
 }

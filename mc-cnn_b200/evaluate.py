@@ -21,8 +21,13 @@ Deliberate deviations from main.lua:
 * ``submit`` refuses a non-empty output directory instead of running ``rm -rf out/*``;
 * n_te is ``len(x0) - len(dispnoc)`` instead of the constant 195 / 200 (preprocess_kitti.lua writes dispnoc for the
   training rows only, so on real data the two agree), and KITTI's H and W come from x0's shape;
-* ``-at 1`` (the combined 2012 + 2015 loader, used for training), ``-color rgb``, ``-debug``, ``-use_cache`` /
-  ``-make_cache`` and ``-sm_terminate`` / ``-sm_skip`` are refused (none changes the default result);
+* ``-at 1`` (the combined 2012 + 2015 loader, used for training), ``-color rgb``, ``-debug`` and ``-use_cache`` /
+  ``-make_cache`` are refused (none changes the default result);
+* ``-sm_terminate`` / ``-sm_skip`` (``Evaluator(..., sm_skip="sgm")``) accept only the step names main.lua tests
+  (:data:`pipeline.SM_TERMINATE`, :data:`pipeline.SM_SKIP`); main.lua ignores any other name and runs the full chain.
+  :func:`check_options` does not see the architecture and refuses both; :func:`check_stage_options`, which the command
+  line uses, also refuses a step that does no work in the stereo method at hand (``-sm_terminate cbca1`` for kitti
+  fast, which has no CBCA), whose result main.lua would print under the wrong variant's name;
 * a Middlebury set smaller than 30 images submits all of them.
 
 As in main.lua, the first example's runtime includes one-time initialisation; there is no hidden warm-up.
@@ -61,10 +66,34 @@ def check_options(dataset, at=0, color="gray", debug=False, use_cache=False, mak
                          "matters for training")
     if color != "gray":
         raise ValueError("-color %s is not supported: only grey Middlebury sets (-color gray) are" % color)
-    for name, v in (("-debug", debug), ("-use_cache", use_cache), ("-make_cache", make_cache),
-                    ("-sm_terminate", sm_terminate), ("-sm_skip", sm_skip)):
+    for name, v in (("-debug", debug), ("-use_cache", use_cache), ("-make_cache", make_cache)):
         if v:
             raise ValueError("%s is not supported" % name)
+    # which steps exist depends on the architecture and its parameters, which this check does not see
+    for name, v in (("-sm_terminate", sm_terminate), ("-sm_skip", sm_skip)):
+        if v:
+            raise ValueError("%s is checked with the stereo method it applies to: use check_stage_options(dataset, arch, "
+                             "...)" % name)
+
+
+def preset_name(dataset, arch):
+    """the census / ad presets of main.lua:146-204 are shared by kitti and kitti2015"""
+    return "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
+
+
+def check_stage_options(dataset, arch, sm_terminate="", sm_skip="", **overrides):
+    """Refuse a -sm_terminate / -sm_skip value that is not one of main.lua's step names, or that names a step doing no work
+    in the stereo method of (dataset, arch) with `overrides` (pipeline.idle_steps): main.lua would run it and print the
+    result of another variant under this one's name -- a wrong row in an ablation table."""
+    opt = pipeline.make_params(preset_name(dataset, arch), arch, sm_terminate=sm_terminate, sm_skip=sm_skip, **overrides)
+    idle = pipeline.idle_steps(opt)
+    for option, name in (("sm_terminate", sm_terminate), ("sm_skip", sm_skip)):
+        if name in idle:
+            raise ValueError("-%s %s: that step does no work in the %s %s stereo method (cbca_i1 %d, cbca_i2 %d, sgm_i %d, "
+                             "LR check %s), so the result would be another variant's"
+                             % (option, name, dataset, arch, opt.cbca_i1, opt.cbca_i2, opt.sgm_i,
+                                "on" if opt.lr_check else "off"))
+    return opt
 
 
 def _fromfile(path):
@@ -196,8 +225,7 @@ class Evaluator:
             self.net = frontend.load_net(net_fname, arch)
             overrides.setdefault("border", frontend.net_border(self.net))
         # the census / ad presets of main.lua:146-204 are shared by kitti and kitti2015
-        preset = "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
-        self.opt = pipeline.make_params(preset, arch, **overrides)
+        self.opt = pipeline.make_params(preset_name(dataset, arch), arch, **overrides)
         self.dev = torch.device("cuda", device)
         if self.net is not None:
             self.tower, self.head = frontend.make_stages(self.net, self.dev)

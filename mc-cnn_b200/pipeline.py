@@ -37,10 +37,72 @@ class Params(ctypes.Structure):
         ("blur_t", ctypes.c_float),
         ("border", ctypes.c_int),
         ("lr_check", ctypes.c_int),
+        ("sm_terminate", ctypes.c_int),   # a SM_TERMINATE code (main.lua's -sm_terminate), 0 = the full chain
+        ("sm_skip", ctypes.c_int),        # a SM_SKIP code (-sm_skip), 0 = none
     ]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+# main.lua's -sm_terminate / -sm_skip values (main.lua:953-1082) -> the MCCNN_SM_* codes of include/adcensus_b200.h.
+# "" means neither option.  main.lua accepts any string and ignores the ones it does not test; these tables refuse them, so
+# that a misspelt step cannot silently give the full chain.
+SM_TERMINATE = {"": 0, "cnn": 1, "cbca1": 2, "sgm": 3, "cbca2": 4, "occlusion": 5, "mismatch": 6,
+                "subpixel_enchancement": 7, "median": 8}
+SM_SKIP = {"": 0, "cbca": 10, "sgm": 3, "occlusion": 5, "subpixel_enchancement": 7, "median": 8, "bilateral": 9}
+
+
+def stage_code(option, name):
+    """the code of main.lua's ``-sm_terminate`` / ``-sm_skip`` value `name` (option "sm_terminate" or "sm_skip")"""
+    table = SM_TERMINATE if option == "sm_terminate" else SM_SKIP
+    if not isinstance(name, str) or name not in table:
+        raise ValueError("-%s %r is not a step (valid: %s)" % (option, name, " ".join(n for n in table if n)))
+    return table[name]
+
+
+def idle_steps(opt):
+    """The -sm_skip / -sm_terminate names whose step does no work under `opt`'s parameters: skipping or stopping after such a
+    step gives the result of another variant (skip cbca without CBCA iterations is the full chain, terminate cbca1 with
+    cbca_i1 = 0 is terminate cnn, ...).  The LR-check steps do no work without the LR check (mb)."""
+    idle = set()
+    if opt.cbca_i1 + opt.cbca_i2 == 0:
+        idle.add("cbca")
+    if opt.cbca_i1 == 0:
+        idle.add("cbca1")
+    if opt.cbca_i2 == 0:
+        idle.add("cbca2")
+    if opt.sgm_i == 0:
+        idle.add("sgm")
+    if not opt.lr_check:
+        idle |= {"occlusion", "mismatch"}
+    return idle
+
+
+def stages(opt):
+    """Which steps of main.lua:953-1082 run for the stage fields of `opt`: a dict step -> bool over cbca1 (the cross arms and
+    the first CBCA block), sgm, cbca2, occlusion, mismatch, subpixel, median, bilateral.  csrc/pipeline.cu's stages_of is the
+    same table."""
+    T, S = opt.sm_terminate, opt.sm_skip
+    lr = bool(opt.lr_check)
+    st = {}
+    active = T != SM_TERMINATE["cnn"]                                              # :988
+    st["cbca1"] = active and S != SM_SKIP["cbca"]                                  # :992
+    active = active and T != SM_TERMINATE["cbca1"]                                 # :1005
+    st["sgm"] = active and S != SM_SKIP["sgm"]                                     # :1007
+    active = active and T != SM_TERMINATE["sgm"]                                   # :1031
+    st["cbca2"] = active and S != SM_SKIP["cbca"]                                  # :1033
+    active = active and T != SM_TERMINATE["cbca2"]                                 # :1040
+    st["occlusion"] = lr and active and S != SM_SKIP["occlusion"]                  # :1057
+    active = active and not (lr and T == SM_TERMINATE["occlusion"])                # :1060
+    st["mismatch"] = lr and active and S != SM_SKIP["occlusion"]                   # :1062
+    active = active and not (lr and T == SM_TERMINATE["mismatch"])                 # :1065
+    st["subpixel"] = active and S != SM_SKIP["subpixel_enchancement"]             # :1067
+    active = active and T != SM_TERMINATE["subpixel_enchancement"]                 # :1071
+    st["median"] = active and S != SM_SKIP["median"]                               # :1072
+    active = active and T != SM_TERMINATE["median"]                                # :1076
+    st["bilateral"] = active and S != SM_SKIP["bilateral"]                         # :1077
+    return st
 
 
 # (dataset, arch) -> stereo-method options, main.lua:70-295.  `border` = (window-1)/2 of the
@@ -76,8 +138,12 @@ PRESETS = {
 
 
 def make_params(dataset="kitti", arch="fast", **overrides):
+    """The preset of (dataset, arch) with `overrides`; ``sm_terminate`` / ``sm_skip`` take main.lua's step names."""
     d = dict(PRESETS[(dataset, arch)])
     d.setdefault("sgm_i", 1)
+    for k in ("sm_terminate", "sm_skip"):
+        if k in overrides:
+            overrides[k] = stage_code(k, overrides[k])
     d.update(overrides)
     return Params(**d)
 
@@ -118,31 +184,35 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
     else:
         raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
 
+    st = stages(opt)                                                              # -sm_terminate / -sm_skip
     disp = {}
     out_vols = {}
     vol = None
     for direction in (1, -1):                                                     # :955
         vol = vols[0:1] if direction == -1 else vols[1:2]                         # :986
-        x0c = torch.empty((1, 4, H, W), device=dev, dtype=torch.float32)          # :993-996
-        x1c = torch.empty((1, 4, H, W), device=dev, dtype=torch.float32)
-        adcensus.cross(x_batch[0], x0c, opt.L1, opt.tau1)
-        adcensus.cross(x_batch[1], x1c, opt.L1, opt.tau1)
-        tmp_cbca = torch.empty_like(vol)
-        for _ in range(opt.cbca_i1):                                              # :998-1001
-            adcensus.cbca(x0c, x1c, vol, tmp_cbca, direction)
-            vol.copy_(tmp_cbca)
-        volt = adcensus.transpose_dhw_to_hwd(vol)                                 # :1008
-        out = torch.empty_like(volt)
-        tmp = torch.empty((W, disp_max), device=dev, dtype=torch.float32)         # :1012
-        for _ in range(opt.sgm_i):
-            out.zero_()                                                           # :1014
-            adcensus.sgm2(x_batch[0], x_batch[1], volt, out, tmp, opt.pi1, opt.pi2, opt.tau_so, opt.alpha1,
-                          opt.sgm_q1, opt.sgm_q2, direction)                      # :1015
-            volt.copy_(out).div_(4)                                               # :1017
-        vol.copy_(adcensus.transpose_hwd_to_dhw_div4(out))                        # :1019-1020
-        for _ in range(opt.cbca_i2):                                              # :1035-1038
-            adcensus.cbca(x0c, x1c, vol, tmp_cbca, direction)
-            vol.copy_(tmp_cbca)
+        if st["cbca1"]:                                                           # :992
+            x0c = torch.empty((1, 4, H, W), device=dev, dtype=torch.float32)      # :993-996
+            x1c = torch.empty((1, 4, H, W), device=dev, dtype=torch.float32)
+            adcensus.cross(x_batch[0], x0c, opt.L1, opt.tau1)
+            adcensus.cross(x_batch[1], x1c, opt.L1, opt.tau1)
+            tmp_cbca = torch.empty_like(vol)
+            for _ in range(opt.cbca_i1):                                          # :998-1001
+                adcensus.cbca(x0c, x1c, vol, tmp_cbca, direction)
+                vol.copy_(tmp_cbca)
+        if st["sgm"]:                                                             # :1007
+            volt = adcensus.transpose_dhw_to_hwd(vol)                             # :1008
+            out = torch.empty_like(volt)
+            tmp = torch.empty((W, disp_max), device=dev, dtype=torch.float32)     # :1012
+            for _ in range(opt.sgm_i):
+                out.zero_()                                                       # :1014
+                adcensus.sgm2(x_batch[0], x_batch[1], volt, out, tmp, opt.pi1, opt.pi2, opt.tau_so, opt.alpha1,
+                              opt.sgm_q1, opt.sgm_q2, direction)                  # :1015
+                volt.copy_(out).div_(4)                                           # :1017
+            vol.copy_(adcensus.transpose_hwd_to_dhw_div4(out))                    # :1019-1020
+        if st["cbca2"]:                                                           # :1033
+            for _ in range(opt.cbca_i2):                                          # :1035-1038
+                adcensus.cbca(x0c, x1c, vol, tmp_cbca, direction)
+                vol.copy_(tmp_cbca)
         if want_vols:
             out_vols[direction] = vol.clone()                                     # :1042-1047
         disp[1 if direction == 1 else 2] = adcensus.argmin(vol)                   # :1049-1050
@@ -151,11 +221,16 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
     if opt.lr_check:                                                              # :1054-1066
         outlier = torch.zeros_like(d)
         adcensus.outlier_detection(disp[2], disp[1], outlier, disp_max)
-        d = adcensus.interpolate_occlusion(d, outlier)
-        d = adcensus.interpolate_mismatch(d, outlier)
-    d = adcensus.subpixel_enchancement(d, vol, disp_max)                          # :1068 (left volume)
-    d = adcensus.median2d(d, 5)                                                   # :1073
-    d = adcensus.mean2d(d, adcensus.gaussian(opt.blur_sigma).to(dev), opt.blur_t)  # :1078
+        if st["occlusion"]:
+            d = adcensus.interpolate_occlusion(d, outlier)
+        if st["mismatch"]:
+            d = adcensus.interpolate_mismatch(d, outlier)
+    if st["subpixel"]:
+        d = adcensus.subpixel_enchancement(d, vol, disp_max)                      # :1068 (left volume)
+    if st["median"]:
+        d = adcensus.median2d(d, 5)                                               # :1073
+    if st["bilateral"]:
+        d = adcensus.mean2d(d, adcensus.gaussian(opt.blur_sigma).to(dev), opt.blur_t)  # :1078
     if want_vols:
         return d, out_vols[-1], out_vols[1]
     return d

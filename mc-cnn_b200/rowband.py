@@ -104,8 +104,13 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
 
     featL/featR (C,H,W) and imgL/imgR (H,W) are the FULL tensors on every rank (only this rank's
     rows of the features are read).  `chunks`: column chunks of the vertical SGM wavefront (default: 4 per rank, at
-    least 32 columns each).  Returns the full (H,W) disparity map on every rank.
+    least 32 columns each).  Returns the full (H,W) disparity map on every rank.  Only the full chain: parameters with
+    ``sm_terminate`` / ``sm_skip`` set are refused before any work (run them on one GPU through the fused pipeline).
     """
+    for k in ("sm_terminate", "sm_skip"):
+        if getattr(opt, k, 0):
+            raise ValueError("row-band stereo_predict runs the full chain only: -%s is not supported (use the "
+                             "single-GPU pipeline)" % k)
     comm = comm or Comm()
     H, W = imgL.shape
     N, r = comm.world, comm.rank

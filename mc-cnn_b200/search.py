@@ -20,6 +20,9 @@ The CBCA mode is the one :class:`evaluate.Evaluator` runs for the arch, so that 
 mode for 'fast' (``run_shape``), the exact mode for 'slow', 'ad' and 'census' (the operator chain, bit-identical to the
 reference).  Bad pixels are counted on the device (main.lua:1230-1236 in float32) with one host read per candidate.
 
+A candidate may also set main.lua's ``sm_skip`` / ``sm_terminate`` (``s.score({"sm_skip": "sgm"})``): the same cached volumes
+and the same pipeline then score a stereo-method ablation (:func:`ablation_variants`, tools/ablation.py).
+
 The log lines are hs.py's (``score dataset arch test_te -name value ... -use_cache`` / ``-net_fname N``), so hs.sh.* output
 and ours can be mixed.
 """
@@ -180,6 +183,23 @@ def propose(method, params, rng, results=None):
                 ns.append(x[i] + 1)
             x[i] = rng.choice(ns)
     return x
+
+
+def ablation_variants(opt):
+    """The stereo-method ablation for the parameters `opt` (a pipeline.Params) as [(label, overrides)]: the full chain, each
+    ``-sm_skip`` step, then each ``-sm_terminate`` step (main.lua:953-1082), in the order the chain runs them.  Steps that
+    do no work with these parameters (pipeline.idle_steps: the LR-check steps on mb, CBCA in the fast presets, ...) are
+    left out, since their variants repeat another one's result."""
+    idle = pipeline.idle_steps(opt)
+    out = [("full", {})]
+    for option, names in (("sm_skip", SKIP_STEPS), ("sm_terminate", TERMINATE_STEPS)):
+        out += [("-%s %s" % (option, n), {option: n}) for n in names if n not in idle]
+    return out
+
+
+# main.lua's step names in chain order (main.lua:988-1077); the same names as pipeline.SM_SKIP / SM_TERMINATE
+SKIP_STEPS = ("cbca", "sgm", "occlusion", "subpixel_enchancement", "median", "bilateral")
+TERMINATE_STEPS = ("cnn", "cbca1", "sgm", "cbca2", "occlusion", "mismatch", "subpixel_enchancement", "median")
 
 
 def preset_name(dataset, arch):

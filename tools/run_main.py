@@ -5,9 +5,11 @@
     python tools/run_main.py mb census -a test_te -rect imperfect -color gray
     python tools/run_main.py kitti fast -a time -net_fname N [-tiny]
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70
+    python tools/run_main.py kitti fast -a test_te -net_fname N -sm_skip sgm          # or -sm_terminate cbca1, ...
 
 Option names are main.lua's (-gpu is 1-based as there); -L1 ... -blur_t override the stereo method's preset
-(main.lua:70-295).  Datasets are read relative to -data_root (default: the working directory), as main.lua reads them
+(main.lua:70-295); -sm_terminate / -sm_skip stop after / leave out one step of it (main.lua:953-1082; unknown step
+names, and steps that do no work with these parameters, are refused).  Datasets are read relative to -data_root (default: the working directory), as main.lua reads them
 relative to its own.  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
 what each action computes and where it deliberately differs from main.lua.
 """
@@ -64,8 +66,12 @@ def parse_args(argv=None):
     if args.gpu < 1:
         raise SystemExit("run_main.py: -gpu is 1-based")
     evaluate.check_options(args.dataset, at=args.at, color=args.color, debug=args.debug, use_cache=args.use_cache,
-                           make_cache=args.make_cache, sm_terminate=args.sm_terminate, sm_skip=args.sm_skip)
+                           make_cache=args.make_cache)
     overrides = {k: getattr(args, k) for k in PRESET_OPTIONS if getattr(args, k) is not None}
+    stage = {k: getattr(args, k) for k in ("sm_terminate", "sm_skip") if getattr(args, k)}
+    if stage:                                              # main.lua's step names; make_params maps them to codes
+        evaluate.check_stage_options(args.dataset, args.arch, **dict(overrides, **stage))
+        overrides.update(stage)
     args.device = args.gpu - 1
     return args, overrides
 
