@@ -178,7 +178,11 @@ __global__ void median_kernel(const float *__restrict__ img, float *__restrict__
 }
 
 // k = 5 (the only size main.lua uses, :1073): the n/2-th smallest of <= 25 values is found by
-// counting, which keeps everything in registers; same order statistic as the sort.
+// counting, which keeps everything in registers; same order statistic as the sort.  Counting agrees
+// with the sort only where equal values are equal bits: a window that holds a NaN (never below nor
+// equal to anything, while the sort leaves it where its swaps put it) or a -0 (equal to +0, the sort
+// decides which of them lands in the median slot) takes the reference's sort instead, over the
+// in-image taps in its order (x outer, y inner).
 __global__ void median5_kernel(const float *__restrict__ img, float *__restrict__ out, int size, int H, int W)
 {
 	int id = blockIdx.x * blockDim.x + threadIdx.x;
@@ -186,12 +190,24 @@ __global__ void median5_kernel(const float *__restrict__ img, float *__restrict_
 	int x = id % W, y = id / W;
 	float v[25];
 	int n = 0;
+	bool unordered = false;
 #pragma unroll
 	for (int i = 0; i < 25; i++) {
 		int xx = x - 2 + i / 5, yy = y - 2 + i % 5;
 		bool ok = 0 <= xx && xx < W && 0 <= yy && yy < H;
 		v[i] = ok ? __ldg(img + yy * W + xx) : CUDART_INF_F;        // +inf never below the median slot
 		n += ok;
+		unordered |= v[i] != v[i] || __float_as_uint(v[i]) == 0x80000000u;
+	}
+	if (unordered) {
+		float xs[25];
+		int m = 0;
+		for (int xx = x - 2; xx <= x + 2; xx++)
+			for (int yy = y - 2; yy <= y + 2; yy++)
+				if (0 <= xx && xx < W && 0 <= yy && yy < H) xs[m++] = __ldg(img + yy * W + xx);
+		sel_sort(xs, m);
+		out[id] = xs[m / 2];                                        // :1592
+		return;
 	}
 	const int want = n / 2;                                         // rank (0-based) in ascending order
 	float res = 0.0f;
