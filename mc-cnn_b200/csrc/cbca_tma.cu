@@ -160,8 +160,10 @@ cbca_tma_kernel(const __grid_constant__ CUtensorMap tmap,
 		const bool valid_col = x < W && xs >= 0 && xs < W;
 		const int off = (x0 + sh) - a1x0;                 // window column of tile column 0
 		// does the tile hold entries of the invalid triangle (NaN)?  They never lie inside a run, but a
-		// prefix sum would carry them along the row: count them as 0.
-		const bool clean = direction < 0 ? (x0 - HX - d < 0) : (x0 + CT_TX + R + d >= W);
+		// prefix sum would carry them along the row: count them as 0.  The whole box counts, up to column
+		// x0 - HX + TWP - 1, not only the columns a run can reach: a lane's base (its inclusive total minus
+		// its own last value) is NaN when any of its EPL columns is, which spreads a NaN EPL - 1 columns left.
+		const bool clean = direction < 0 ? (x0 - HX - d < 0) : (x0 - HX + TWP + d > W);
 		mbar_wait(&bars[s], (dd >> 1) & 1);
 
 		// 1. inclusive prefix of every tile row, in place: a warp per row, a lane owns EPL consecutive columns (stride-5 word

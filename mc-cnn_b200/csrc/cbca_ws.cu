@@ -20,8 +20,8 @@
 //     value added back, one store.  No block-wide barrier in the steady state.
 // Compared with cbca_tma.cu (32-row tiles, 2 CTAs per SM, prefix and walk as barrier-separated phases): 64-row tiles
 // (less halo per output) and prefix and walk of different planes overlapped.  NOT bit-exact by construction (1e-4
-// contract; measured ~1e-7).  Arms up to 5 pixels (R <= 4, the KITTI presets); longer arms stay on cbca_tma.cu / the
-// exact kernels.
+// contract; the constant-work kernels measured up to 1.2e-5 on the volume kinds of DESIGN.md §5).  Arms up to 5 pixels
+// (R <= 4, the KITTI presets); longer arms stay on cbca_tma.cu / the exact kernels.
 #include "common.cuh"
 #include "tma.cuh"
 

@@ -251,3 +251,351 @@ def median_kernel(ksize):
 
 
 MEDIAN_K = (1, 3, 5, 7, 9, 11)
+
+
+# ----------------------------------------------------------------------------------------------------------------- CBCA
+# Exact kernels (cross_cbca.cu): tile (columns, rows) and disparities per CTA
+CBCA_EXACT_KERNELS = ("win1", "win4", "loop8", "loop13", "generic")
+# constant-work kernels (cbca_ws.cu, cbca_tma.cu): cbca_ws_kernel<1, 6>, <4, 4>, cbca_tma_kernel<8>, <13>
+CBCA_FAST_KERNELS = ("ws1", "ws4", "tma8", "tma13")
+CBCA_TILE = {"win1": (128, 32), "win4": (128, 32), "loop8": (64, 16), "loop13": (64, 16),
+             "ws1": (128, 64), "ws4": (128, 64), "tma8": (128, 32), "tma13": (128, 32)}
+CBCA_R = {"win1": 1, "win4": 4, "loop8": 8, "loop13": 13, "ws1": 1, "ws4": 4, "tma8": 8, "tma13": 13}
+
+
+def _by_halo(halo, names):
+    return names[0] if halo <= 1 else names[1] if halo <= 4 else names[2] if halo <= 8 else names[3] if halo <= 13 else names[4]
+
+
+def cbca_gate(maxlen):
+    """cross_cbca.cu adcensus_cbca: every candidate kernel is launched with a gate on the longest arm, held on the device
+    (win<1> 0-2, win<4> 3-5, loop<8> 6-9, loop<13> 10-14, generic >= 15)"""
+    return _by_halo(maxlen - 1, CBCA_EXACT_KERNELS)
+
+
+def cbca_packed_kernel(max_arm):
+    """cross_cbca.cu adc_cbca_packed (adcensus_cbca_ex, mccnn_cbca_packed, the pipeline's exact mode): the caller's bound,
+    halo = max_arm - 1: <= 1 win<1>, <= 4 win<4>, <= 8 loop<8>, <= 13 loop<13>, else generic"""
+    return _by_halo(max_arm - 1, CBCA_EXACT_KERNELS)
+
+
+def cbca_ex_clamp(max_arm):
+    """cross_cbca.cu adcensus_cbca_ex: the packed arm lengths are cut at max_arm when max_arm <= 14; beyond, the generic
+    kernel reads the float arms themselves (no cut).  0 = no cut."""
+    return max_arm if max_arm <= 14 else 0
+
+
+def pack_maxlen(x0c, x1c):
+    """cross_cbca.cu pack_arms_kernel: the longest arm length (x - left end, right end - x, y - upper end, lower end - y)
+    of either image; 1 << 20 (the generic kernel) when any length is negative, i.e. the arms are not cross() outputs"""
+    m = 0
+    for xc in (x0c, x1c):
+        H, W = xc.shape[1:]
+        ys, xs = np.mgrid[0:H, 0:W]
+        lens = np.stack([xs - xc[0], xc[1] - xs, ys - xc[2], xc[3] - ys]).astype(np.int64)
+        if lens.min() < 0:
+            return 1 << 20
+        m = max(m, int(lens.max()))
+    return m
+
+
+def clip_arms(xc, bound):
+    """the arms adcensus_cbca_ex aggregates over for a stated bound below the real arms: every length cut at `bound`"""
+    H, W = xc.shape[1:]
+    ys, xs = np.mgrid[0:H, 0:W]
+    return np.stack([np.maximum(xc[0], xs - bound), np.minimum(xc[1], xs + bound),
+                     np.maximum(xc[2], ys - bound), np.minimum(xc[3], ys + bound)]).astype(np.float32)
+
+
+def cbca_fast_kernel(max_arm):
+    """cbca_tma.cu adc_cbca_tma: halo = max_arm - 1: <= 1 cbca_ws<1>, <= 4 cbca_ws<4>, <= 8 cbca_tma<8>, <= 13
+    cbca_tma<13>, otherwise ADCENSUS_ELIMIT"""
+    return _by_halo(max_arm - 1, CBCA_FAST_KERNELS + ("ELIMIT",))
+
+
+def cbca_fast_refusal(W, ld, in_off, out_off, aliased, max_arm):
+    """cbca_tma.cu mccnn_cbca_fast_pitched / mccnn_cbca_fast_pitched_packed: EINVAL for vol_in == vol_out, ld < W,
+    ld % 4 != 0 or a base not 16-byte aligned; ELIMIT for a halo above 13.  None: the call runs."""
+    if aliased or ld < W or ld % 4 or (4 * in_off) % 16 or (4 * out_off) % 16 or max_arm < 1:
+        return "EINVAL"
+    return "ELIMIT" if max_arm - 1 > 13 else None
+
+
+def cbca_dchunk(kernel, D):
+    """disparities per CTA: launch_win 14, launch_tile 16, launch_tma 20, launch_ws equal chunks of at most 20
+    (12 x 19 at D = 228); the generic kernel has no chunks"""
+    if kernel in ("ws1", "ws4"):
+        return -(-D // -(-D // 20))
+    return {"win1": 14, "win4": 14, "loop8": 16, "loop13": 16, "tma8": 20, "tma13": 20}.get(kernel)
+
+
+def cbca_nproc(x0, d0, dn, W, direction, TX):
+    """the planes of a chunk that are aggregated (cbca_win_kernel, cbca_ws_kernel, cbca_tma_kernel: `nproc`; the loop and
+    generic kernels copy column by column): a tile whose columns all have x + d * direction
+    outside the image is a plain copy (adcensus.cu:353-354), and those planes form a suffix of the chunk"""
+    n = 0
+    while n < dn and not ((x0 + TX - 1 - (d0 + n) < 0) if direction < 0 else (x0 + d0 + n >= W)):
+        n += 1
+    return n
+
+
+def cbca_copy_paths(kernel, D, W, direction):
+    """{'whole', 'partial'}: some chunk of some tile column is copied entirely (nproc == 0; cbca_ws copies it before any
+    staging) / only after some aggregated planes (0 < nproc < dn)"""
+    TX = CBCA_TILE[kernel][0]
+    dch = cbca_dchunk(kernel, D)
+    out = set()
+    for x0 in range(0, W, TX):
+        for d0 in range(0, D, dch):
+            dn = min(dch, D - d0)
+            n = cbca_nproc(x0, d0, dn, W, direction, TX)
+            if n == 0:
+                out.add("whole")
+            elif n < dn:
+                out.add("partial")
+    return out
+
+
+def pipe_cbca_route(fast_mode, L1, border, D, W):
+    """pipeline.cu run_chain: 'fast' (adc_cbca_tma) when the mode is fast, max(L1, 2) - 1 <= 4 (pipe_fast_cbca_ok) and
+    not nan_in_valid; 'generic' (adc_cbca_packed with maxlen 1 << 20) when nan_in_valid = border > 0 and
+    D > W - border - 1, in both modes; else 'packed' (the exact kernel of max(L1, 2))"""
+    if border > 0 and D > W - border - 1:
+        return "generic"
+    return "fast" if fast_mode and max(L1, 2) - 1 <= 4 else "packed"
+
+
+def cbca_image(H, W, L, seed):
+    """a blocky quantised image whose cross() arms (tau1 = 0.5, L1 = L) are as long as L along the blocks' long side and
+    short across them: the longest arm is exactly L when max(H, W) > L"""
+    rng = np.random.default_rng(seed)
+    bh, bw = (3, 2 * L + 2) if W > L else (2 * L + 2, 3)
+    lv = rng.integers(0, 4, (H // bh + 2, W // bw + 2))
+    oy, ox = rng.integers(0, bh), rng.integers(0, bw)
+    img = np.kron(lv, np.ones((bh, bw)))[oy:oy + H, ox:ox + W]
+    noise = rng.random((H, W)) < 0.05                                     # a few pixels that cut the arms
+    img[noise] = rng.integers(0, 4, noise.sum())
+    return img.astype(np.float32)
+
+
+CBCA_TAU1 = 0.5
+
+# H, W, D, L (L1 = the longest arm), direction, entry ('gate' adcensus_cbca, 'ex' adcensus_cbca_ex, 'packed'
+# mccnn_pack_arms + mccnn_cbca_packed), max_arm (the stated bound; None for the gate), kernel, and `arms`: 'cross', 'clip'
+# (bound below the arms: the expected result aggregates clipped arms) or 'negative' (one arm of negative length)
+CbcaCase = namedtuple("CbcaCase", "H W D L direction entry max_arm kernel arms")
+
+# the longest arm on each side of each boundary of the exact tables, and a shape for it (W in {1, 127, 128, 129, 257},
+# H in {1, 31, 32, 33, 63, 64, 65}; D below 128 and above, where whole tiles lie in the invalid triangle)
+CBCA_EXACT_SHAPES = {
+    2: [(33, 129, 20), (1, 257, 150)],
+    3: [(31, 127, 15), (65, 1, 9)],
+    5: [(64, 128, 30), (32, 257, 150)],
+    6: [(63, 129, 17), (1, 127, 40)],
+    9: [(65, 128, 33), (33, 257, 131)],
+    10: [(32, 127, 16), (64, 1, 5)],
+    14: [(31, 129, 18), (1, 257, 135)],
+    15: [(33, 128, 14), (65, 33, 40)],
+}
+CBCA_BOUNDARIES = ((2, 3), (5, 6), (9, 10), (14, 15))
+
+
+def _cbca_exact_cases():
+    cases = []
+    for L, shapes in CBCA_EXACT_SHAPES.items():
+        for i, (H, W, D) in enumerate(shapes):
+            direction = -1 if i == 0 else 1
+            k = cbca_packed_kernel(L)
+            cases += [CbcaCase(H, W, D, L, direction, "gate", None, k, "cross"),
+                      CbcaCase(H, W, D, L, -direction, "gate", None, k, "cross"),
+                      CbcaCase(H, W, D, L, direction, "ex", L, k, "cross"),
+                      CbcaCase(H, W, D, L, -direction, "packed", L, k, "cross")]
+    # a stated bound above the real arms: a bigger kernel for short arms (both host-bound entries)
+    for L, bound, (H, W, D) in ((2, 9, (33, 129, 20)), (3, 14, (31, 127, 15)), (6, 20, (63, 129, 17)),
+                                (5, 13, (32, 257, 150))):
+        for e, direction in (("ex", -1), ("packed", 1)):
+            cases.append(CbcaCase(H, W, D, L, direction, e, bound, cbca_packed_kernel(bound), "cross"))
+    # a stated bound below the real arms (adcensus_cbca_ex only): the lengths are cut at the bound
+    for L, bound, (H, W, D) in ((6, 2, (63, 129, 17)), (9, 5, (65, 128, 33)), (15, 14, (33, 128, 14)),
+                                (10, 7, (32, 127, 16))):
+        for direction in (-1, 1):
+            cases.append(CbcaCase(H, W, D, L, direction, "ex", bound, cbca_packed_kernel(bound), "clip"))
+    # arms that are not cross() outputs: one negative length sends adcensus_cbca to the generic kernel
+    for direction in (-1, 1):
+        cases.append(CbcaCase(31, 129, 18, 5, direction, "gate", None, "generic", "negative"))
+    return cases
+
+
+CBCA_EXACT_CASES = _cbca_exact_cases()
+
+
+def cbca_id(c):
+    b = "" if c.max_arm is None else "_b%d" % c.max_arm
+    return "%s_H%dW%dD%d_L%d%s_%s_%+d" % (c.entry, c.H, c.W, c.D, c.L, b, c.arms, c.direction)
+
+
+def cbca_arms(c, seed=0):
+    """(x0c, x1c) the arms case `c` hands to the kernel, and (a0, a1) the arms its expected result aggregates over"""
+    from oracle import oracle as orc
+    s = seed + 7 * c.H + 3 * c.W + c.L
+    x0c = orc.cross(cbca_image(c.H, c.W, c.L, s), c.L, CBCA_TAU1)
+    x1c = orc.cross(cbca_image(c.H, c.W, c.L, s + 1), c.L, CBCA_TAU1)
+    if c.arms == "negative":
+        x0c[0, c.H // 2, c.W // 2] = c.W // 2 + 1                        # left end right of the pixel: length -1
+    a0, a1 = x0c, x1c
+    if c.arms == "clip":
+        a0, a1 = clip_arms(x0c, c.max_arm), clip_arms(x1c, c.max_arm)
+    return x0c, x1c, a0, a1
+
+
+# Constant-work cases: H, W, D, L, direction, max_arm, kernel, ld (row pitch), kind (the volume, see cbca_volume)
+FastCase = namedtuple("FastCase", "H W D L direction max_arm kernel ld kind")
+CBCA_KINDS = ("stereojoin", "census1", "census3", "ad", "post_sgm", "offset_gradient")
+
+
+def _cbca_fast_cases():
+    cases = []
+    # per kernel: the largest arm it serves, and shapes at the tile and chunk edges
+    shapes = {
+        "ws1": [(64, 128, 20), (65, 129, 21), (1, 257, 228), (33, 1, 40), (63, 127, 41)],
+        "ws4": [(64, 257, 228), (31, 128, 20), (65, 129, 40), (32, 127, 21), (1, 129, 41)],
+        "tma8": [(32, 129, 20), (33, 257, 150), (63, 128, 21), (1, 127, 40), (64, 1, 41)],
+        "tma13": [(33, 128, 20), (31, 257, 160), (65, 129, 41), (32, 127, 21), (1, 129, 40)],
+    }
+    arm = {"ws1": (2, 2), "ws4": (3, 5), "tma8": (6, 9), "tma13": (10, 14)}
+    i = 0
+    for k, sh in shapes.items():
+        for j, (H, W, D) in enumerate(sh):
+            L = arm[k][j % 2]
+            direction = -1 if j % 2 == 0 else 1
+            ld = (W + 3) // 4 * 4 + (4 if j % 2 else 8)                      # ld > W + 3
+            for n in range(2):                                               # two volume kinds per shape
+                kind = CBCA_KINDS[(i + n) % len(CBCA_KINDS)]
+                if kind == "post_sgm" and H > W:
+                    kind = "ad"
+                cases.append(FastCase(H, W, D, L, direction if n == 0 else -direction, L, k, ld, kind))
+            i += 2
+    return cases
+
+
+CBCA_FAST_CASES = _cbca_fast_cases()
+
+
+def fast_id(c):
+    return "%s_H%dW%dD%d_L%d_ld%d_%s_%+d" % (c.kernel, c.H, c.W, c.D, c.L, c.ld, c.kind, c.direction)
+
+
+def cbca_volume(kind, H, W, D, direction, seed=0):
+    """an (D, H, W) cost volume of `kind` with the NaN triangle (x < d for direction -1, x >= W - d for +1) and a finite
+    valid part: StereoJoin of unit features ([-1, 1]); census of quantised images with 1 or 3 channels (0 .. 81); AD of
+    the images; a post-SGM volume (sgm2 of a StereoJoin volume, / 4, as main.lua:1017 hands it to cbca_i2); and a large
+    common offset (3000) with a steep gradient along x (40 per column), which stresses cancellation in row prefixes"""
+    from oracle import oracle as orc
+    rng = np.random.default_rng(seed + 17 * H + 5 * W + D + (direction > 0))
+    d, xs = np.arange(D)[:, None, None], np.arange(W)[None, None, :]
+    tri = (xs < d) if direction < 0 else (xs >= W - d)
+    if kind in ("stereojoin", "post_sgm", "offset_gradient"):
+        f = rng.standard_normal((2, 8, H, W)).astype(np.float32)
+        f /= np.sqrt((f * f).sum(1, keepdims=True))
+        vL, vR = orc.stereo_join(f[0], f[1], D)
+        vol = vL if direction < 0 else vR
+        if kind == "post_sgm":
+            img = (rng.integers(0, 16, (2, H, W)) / 8.0).astype(np.float32)
+            hwd = orc.sgm2(img[0], img[1], orc.transpose_dhw_to_hwd(vol), 1.32, 24.25, 0.08, 2.0, 3.0, 2.0, direction)
+            vol = np.ascontiguousarray(hwd.transpose(2, 0, 1)) / np.float32(4)
+        elif kind == "offset_gradient":
+            vol = vol + np.float32(3000) + np.float32(40) * np.arange(W, dtype=np.float32)[None, None, :]
+    elif kind in ("census1", "census3"):
+        nch = 1 if kind == "census1" else 3
+        a = (rng.integers(0, 6, (2, nch, H, W)) / 5.0).astype(np.float32)
+        vol = orc.census(a[0], a[1], D, direction) if direction < 0 else orc.census(a[1], a[0], D, direction)
+    elif kind == "ad":
+        a = rng.standard_normal((2, H, W)).astype(np.float32)
+        vol = orc.ad(a[0], a[1], D, direction) if direction < 0 else orc.ad(a[1], a[0], D, direction)
+    else:
+        raise ValueError(kind)
+    vol = np.array(vol, np.float32)
+    vol[np.broadcast_to(tri, vol.shape)] = np.nan
+    return vol
+
+
+def cbca_f64(x0c, x1c, vol, direction):
+    """adcensus.cu:343-377 in float64: the tap sums over each output's cross support, as (row runs, then rows); the
+    order does not matter at this precision.  Entries with x + d * direction outside the image are copied."""
+    D, H, W = vol.shape
+    out = np.array(vol, np.float64)
+    ys, xs = np.mgrid[0:H, 0:W]
+    v = np.nan_to_num(np.asarray(vol, np.float64), nan=0.0)
+    m = int(max(pack_maxlen(x0c, x1c), 1))
+    for d in range(D):
+        sh = d * direction
+        xp = xs + sh
+        ok = (xp >= 0) & (xp < W)
+        xpc = np.clip(xp, 0, W - 1)
+        lft = np.minimum(xs - x0c[0], xpc - x1c[0][ys, xpc])           # run (x - L, x + R) of row yy, :362-363
+        rgt = np.minimum(x0c[1] - xs, x1c[1][ys, xpc] - xpc)
+        up = np.minimum(ys - x0c[2], ys - x1c[2][ys, xpc])              # rows (y - U, y + Dn), :359-360
+        dn = np.minimum(x0c[3] - ys, x1c[3][ys, xpc] - ys)
+        S = np.zeros((H, W))
+        C = np.zeros((H, W))
+        for dx in range(-m + 1, m):
+            inrun = (dx > -lft) & (dx < rgt)
+            S += np.where(inrun, np.roll(v[d], -dx, axis=1), 0.0)
+            C += inrun
+        T = np.zeros((H, W))
+        N = np.zeros((H, W))
+        for dy in range(-m + 1, m):
+            inside = (dy > -up) & (dy < dn)
+            T += np.where(inside, np.roll(S, -dy, axis=0), 0.0)
+            N += np.where(inside, np.roll(C, -dy, axis=0), 0.0)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            out[d] = np.where(ok, T / N, out[d])
+    return out
+
+
+# the fast entries' refusals: (W, ld, in_off, out_off, aliased, max_arm) -> expected return code
+CBCA_FAST_REFUSALS = [
+    (30, 28, 0, 0, False, 5, "EINVAL"),     # ld < W
+    (30, 30, 0, 0, False, 5, "EINVAL"),     # ld % 4
+    (30, 36, 1, 0, False, 5, "EINVAL"),     # vol_in 4 bytes off
+    (30, 36, 0, 2, False, 5, "EINVAL"),     # vol_out 8 bytes off
+    (30, 36, 0, 0, True, 5, "EINVAL"),      # vol_in == vol_out
+    (30, 36, 0, 0, False, 15, "ELIMIT"),    # halo 14
+    (30, 36, 0, 0, False, 14, None),        # halo 13: runs
+]
+
+
+# ------------------------------------------------------------------------------------------------------------ AD / census
+AD_TILE, AD_DCH = (128, 8), 8                      # adcensus_cost.cu ad_kernel: 128 x 8 outputs, 8 disparities per CTA
+CENSUS_TX, CENSUS_DCH = 128, 16                    # census_cost_kernel: 128 pixels of a row, 16 disparities per CTA
+
+
+def census_kernel(nch):
+    """adcensus_cost.cu adcensus_census: census_cost_kernel<1>, <3>, the runtime-nch <0> for 2 and 4, ELIMIT above 4"""
+    return "ELIMIT" if nch > 4 else {1: "nch1", 3: "nch3"}.get(nch, "nch_rt")
+
+
+# H, W, D, nch, nan (NaN pixels in the images)
+AdCensusCase = namedtuple("AdCensusCase", "H W D nch nan")
+AD_CENSUS_CASES = [
+    AdCensusCase(1, 129, 8, 1, False),        # one row; D = one AD chunk
+    AdCensusCase(1, 127, 9, 3, True),
+    AdCensusCase(17, 1, 16, 1, True),         # one column; D = one census chunk, D > W
+    AdCensusCase(9, 1, 17, 4, False),
+    AdCensusCase(10, 128, 16, 4, True),       # the runtime-nch kernel at its limit
+    AdCensusCase(9, 255, 17, 2, False),
+    AdCensusCase(12, 256, 7, 3, True),
+    AdCensusCase(7, 257, 33, 1, True),
+    AdCensusCase(8, 383, 24, 4, False),
+    AdCensusCase(11, 385, 9, 3, False),
+]
+
+
+def ad_census_images(c, seed=0):
+    """(a, b): two (nch, H, W) images on a grid of 1/3 (census ties), with a few NaN pixels when c.nan"""
+    rng = np.random.default_rng(seed + c.H * c.W + c.nch + c.D)
+    a, b = (np.round(rng.standard_normal((2, c.nch, c.H, c.W)) * 3) / 3).astype(np.float32)
+    if c.nan:
+        for x in (a, b):
+            x.reshape(-1)[rng.choice(x.size, max(1, x.size // 50), replace=False)] = np.nan
+    return a, b

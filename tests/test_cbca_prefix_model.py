@@ -1,5 +1,9 @@
 """CPU: design study for a tolerance-mode CBCA -- the prefix-sum formulation (constant work per pixel) must
-reproduce the reference's tap-by-tap sums within rounding, with the error bounded by the tile size."""
+reproduce the reference's tap-by-tap sums within rounding, with the error bounded by the tile size -- and an index-for-index
+emulation of the kernel the default mode runs, cbca_ws_kernel, with the mistakes the GPU tests can see."""
+import importlib.util
+import os
+
 import numpy as np
 import pytest
 
@@ -46,88 +50,52 @@ def test_error_grows_with_prefix_length(oracle):
     assert err[(24, 64)] <= err[(24, 600)] * 1.5 + 1e-9 and err[(24, 600)] < 1e-4
 
 
-def _pack_arms(xc):
-    """pack_arms_kernel (cross_cbca.cu): arm LENGTHS as bytes, L | R << 8 | U << 16 | D << 24"""
-    H, W = xc.shape[1:]
-    ys, xs = np.mgrid[0:H, 0:W]
-    l = np.clip(xs - xc[0], 0, 255).astype(np.uint32)
-    r = np.clip(xc[1] - xs, 0, 255).astype(np.uint32)
-    u = np.clip(ys - xc[2], 0, 255).astype(np.uint32)
-    d = np.clip(xc[3] - ys, 0, 255).astype(np.uint32)
-    return l | (r << 8) | (u << 16) | (d << 24)
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+_spec = importlib.util.spec_from_file_location("dispatch_cases", os.path.join(ROOT, "tests", "dispatch_cases.py"))
+dc = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(dc)
+
+# constant-work cases of tests/test_gpu_dispatch_edges.py that cbca_ws_kernel serves, small enough for the emulation
+WS_CASES = [c for c in dc.CBCA_FAST_CASES if c.kernel in ("ws1", "ws4") and c.H > 1 and c.W > 1 and c.D * c.H * c.W < 400000]
 
 
-def _emulate_o1_kernel(a0, a1, vol, direction, R, TX=128, TY=32):
-    """cbca_o1_kernel (cross_cbca.cu) restated index for index in numpy: same tile, halo, offsets and buffers"""
-    D, H, W = vol.shape
-    TH, TWP = TY + 2 * R + 1, TX + 2 * R + 1               # one extra row / column: the excluded end-points are indexed
-    out = np.full_like(vol, np.float32(-12345.0))
-    bmin = lambda p, q: np.minimum(p & 255, q & 255) | (np.minimum((p >> 8) & 255, (q >> 8) & 255) << 8) | \
-        (np.minimum((p >> 16) & 255, (q >> 16) & 255) << 16) | (np.minimum(p >> 24, q >> 24) << 24)
-    for d in range(D):
-        sh = d * direction
-        for y0 in range(0, H, TY):
-            for x0 in range(0, W, TX):
-                scomb = np.zeros((TH, TX), np.uint32)
-                sv = np.zeros((TH, TWP), np.float32)
-                for r in range(TH):
-                    yy = y0 - R - 1 + r
-                    if not (0 <= yy < H):
-                        continue
-                    for c in range(TX):
-                        xx, xr = x0 + c, x0 + c + sh
-                        a = a0[yy, xx] if xx < W else np.uint32(0)
-                        b = a1[yy, xr] if 0 <= xr < W else np.uint32(0)
-                        scomb[r, c] = bmin(np.uint32(a), np.uint32(b))
-                    for c in range(TWP):
-                        xx = x0 - R - 1 + c
-                        if 0 <= xx < W:
-                            v = vol[d, yy, xx]
-                            sv[r, c] = v if v == v else 0.0
-                I = np.cumsum(sv, axis=1, dtype=np.float32)                       # 1. row prefixes, in place
-                sS = np.zeros((TH, TX), np.float32)
-                sN = np.zeros((TH, TX), np.float32)
-                for r in range(TH):                                              # 2. run sums / lengths
-                    for cx in range(TX):
-                        c = int(scomb[r, cx])
-                        L, Rr = c & 255, (c >> 8) & 255
-                        if L > 0:
-                            sS[r, cx] = I[r, cx + R + 1 + Rr - 1] - I[r, cx + R + 1 - L]
-                            sN[r, cx] = L + Rr - 1
-                sS = np.cumsum(sS, axis=0, dtype=np.float32)                      # 3. column prefixes
-                sN = np.cumsum(sN, axis=0, dtype=np.float32)
-                for ty_ in range(TY):                                            # 4. outputs
-                    y = y0 + ty_
-                    if y >= H:
-                        continue
-                    for cx in range(TX):
-                        x = x0 + cx
-                        if x >= W:
-                            continue
-                        xs = x + sh
-                        if 0 <= xs < W:
-                            ty = ty_ + R + 1
-                            c = int(scomb[ty, cx])
-                            U, Dn = (c >> 16) & 255, c >> 24
-                            hi, lo = ty + Dn - 1, ty - U
-                            with np.errstate(invalid="ignore", divide="ignore"):
-                                out[d, y, x] = (sS[hi, cx] - sS[lo, cx]) / (sN[hi, cx] - sN[lo, cx])
-                        else:
-                            out[d, y, x] = vol[d, y, x]
-    return out
+def _ws_inputs(c):
+    x0c, x1c, _, _ = dc.cbca_arms(dc.CbcaCase(c.H, c.W, c.D, c.L, c.direction, "ex", c.max_arm, None, "cross"))
+    return x0c, x1c, dc.cbca_volume(c.kind, c.H, c.W, c.D, c.direction)
 
 
-@pytest.mark.parametrize("L1,tau1,direction,H,W,D", [(5, 0.13, -1, 37, 140, 7), (5, 0.13, 1, 37, 140, 7),
-                                                      (2, 0.5, -1, 20, 131, 5), (9, 5.0, 1, 34, 129, 4)])
-def test_o1_kernel_indexing_emulated(oracle, L1, tau1, direction, H, W, D):
-    """the experimental kernel's tile / halo / offset arithmetic, emulated index for index on the CPU (one and a
-    bit tiles in x and y, image edges, both directions), against the reference's tap sums"""
-    x0c, x1c, volL, volR = _case(oracle, H, W, D, L1, tau1, seed=H + L1)
-    vol = volL if direction == -1 else volR
-    want = oracle.cbca(x0c, x1c, vol, direction)
-    maxlen = max(L1, 2)
-    R = 1 if maxlen - 1 <= 1 else 4 if maxlen - 1 <= 4 else 8 if maxlen - 1 <= 8 else 13   # adc_cbca_packed's choice
-    got = _emulate_o1_kernel(_pack_arms(x0c), _pack_arms(x1c), vol, direction, R)
-    assert np.array_equal(np.isnan(got), np.isnan(want))
+def _err(got, want):
+    """(NaN pattern equal, max relative error over the finite entries of want)"""
     m = ~np.isnan(want)
-    assert (np.abs(got[m] - want[m]) / np.maximum(1.0, np.abs(want[m]))).max() < 1e-4 / 4
+    with np.errstate(invalid="ignore"):
+        e = np.abs(got[m] - want[m]) / np.maximum(1.0, np.abs(want[m]))
+    return np.array_equal(np.isnan(got), np.isnan(want)), float(np.nan_to_num(e, nan=np.inf).max()) if m.any() else 0.0
+
+
+@pytest.mark.parametrize("c", WS_CASES, ids=dc.fast_id)
+def test_ws_kernel_indexing_emulated(oracle, c):
+    """cbca_ws_kernel's tile, chunk, scan and ring arithmetic, emulated index for index, against the reference's tap
+    sums and the float64 tap sums: NaN pattern identical, inside the 1e-4 contract"""
+    x0c, x1c, vol = _ws_inputs(c)
+    got = model.emulate_ws(x0c, x1c, vol, c.direction, dc.CBCA_R[c.kernel])
+    for want in (oracle.cbca(x0c, x1c, vol, c.direction), dc.cbca_f64(x0c, x1c, vol, c.direction)):
+        nan_ok, err = _err(got, want)
+        assert nan_ok and err <= 1e-4, err
+
+
+MUTANT_CASES = [c for c in WS_CASES if c.kind in ("stereojoin", "census3", "offset_gradient")]
+
+
+@pytest.mark.parametrize("c", MUTANT_CASES, ids=dc.fast_id)
+def test_ws_kernel_mistakes_exceed_the_bar(c):
+    """on the GPU cases' inputs, a run end one column off, U and Dn swapped, or the scrub predicate dropped each move
+    the result past the 1e-4 bar (or change its NaN pattern), so the GPU test would see them.  Dropping the centring does
+    NOT: on these volumes, the large-offset one included, the uncentred prefixes stay inside the bar too, so the
+    centring is a margin the tests do not pin."""
+    x0c, x1c, vol = _ws_inputs(c)
+    want = dc.cbca_f64(x0c, x1c, vol, c.direction)
+    R = dc.CBCA_R[c.kernel]
+    for mutation in (dict(run_end=1), dict(swap_ud=True), dict(scrub_rule=False)):
+        nan_ok, err = _err(model.emulate_ws(x0c, x1c, vol, c.direction, R, **mutation), want)
+        assert not nan_ok or err > 1e-4, mutation
+    assert _err(model.emulate_ws(x0c, x1c, vol, c.direction, R, centre=False), want) [1] <= 1e-4

@@ -176,3 +176,161 @@ def test_nan_skipping_median_disagrees_with_the_reference(oracle):
     for kind in ("ties", "inf"):                                      # the counting is right without NaN and -0
         img = dc.median_image(kind, 9, 13)
         assert np.array_equal(median5_nan_skipping(img), oracle.median2d(img, 5), equal_nan=True)
+
+
+# ----------------------------------------------------------------------------------------------------------------- CBCA
+
+def test_cbca_tables():
+    assert [dc.cbca_gate(m) for m in (1, 2, 3, 5, 6, 9, 10, 14, 15, 1 << 20)] == \
+        ["win1", "win1", "win4", "win4", "loop8", "loop8", "loop13", "loop13", "generic", "generic"]
+    for m in range(1, 40):
+        assert dc.cbca_gate(m) == dc.cbca_packed_kernel(m)                     # the gate and the halo table agree
+    assert [dc.cbca_fast_kernel(m) for m in (1, 2, 3, 5, 6, 9, 10, 14, 15)] == \
+        ["ws1", "ws1", "ws4", "ws4", "tma8", "tma8", "tma13", "tma13", "ELIMIT"]
+    assert [dc.cbca_ex_clamp(m) for m in (1, 14, 15)] == [1, 14, 0]
+    assert [dc.cbca_dchunk("ws4", D) for D in (20, 21, 40, 41, 228)] == [20, 11, 20, 14, 19]
+    assert [dc.cbca_dchunk(k, 100) for k in ("win1", "loop13", "tma8")] == [14, 16, 20]
+    assert dc.pipe_cbca_route(True, 5, 4, 35, 40) == "fast" and dc.pipe_cbca_route(False, 5, 4, 35, 40) == "packed"
+    assert dc.pipe_cbca_route(True, 5, 4, 36, 40) == "generic" and dc.pipe_cbca_route(False, 5, 4, 36, 40) == "generic"
+    assert dc.pipe_cbca_route(True, 14, 5, 20, 100) == "packed" and dc.pipe_cbca_route(True, 5, 0, 200, 100) == "fast"
+    assert dc.pipe_cbca_route(True, 6, 4, 20, 100) == "packed"
+
+
+@pytest.mark.parametrize("c", dc.CBCA_EXACT_CASES, ids=dc.cbca_id)
+def test_cbca_exact_case_selects_its_kernel(oracle, c):
+    """the arms' longest length is the case's L exactly (large runs, L1 = L), and the entry selects the claimed kernel"""
+    x0c, x1c, a0, a1 = dc.cbca_arms(c)
+    m = dc.pack_maxlen(x0c, x1c)
+    if c.arms == "negative":
+        assert m == 1 << 20 and c.entry == "gate"
+    else:
+        assert m == c.L
+    k = dc.cbca_gate(m) if c.entry == "gate" else dc.cbca_packed_kernel(c.max_arm)
+    assert k == c.kernel
+    if c.arms == "clip":
+        assert c.entry == "ex" and c.max_arm < c.L and dc.cbca_ex_clamp(c.max_arm) == c.max_arm
+        assert dc.pack_maxlen(a0, a1) == c.max_arm
+    elif c.max_arm is not None:
+        assert c.max_arm >= c.L
+
+
+def test_cbca_exact_cases_reach_every_kernel_and_boundary():
+    pairs = {(c.entry, c.kernel) for c in dc.CBCA_EXACT_CASES if c.arms == "cross"}
+    assert pairs == {(e, k) for e in ("gate", "ex", "packed") for k in dc.CBCA_EXACT_KERNELS}
+    for lo, hi in dc.CBCA_BOUNDARIES:                                        # both sides of every boundary, every entry
+        for e in ("gate", "ex", "packed"):
+            Ls = {c.L for c in dc.CBCA_EXACT_CASES if c.entry == e and c.arms == "cross" and c.max_arm in (None, c.L)}
+            assert {lo, hi} <= Ls, (e, lo, hi)
+    over = {c.entry for c in dc.CBCA_EXACT_CASES if c.max_arm and c.max_arm > c.L}
+    assert over == {"ex", "packed"}
+    assert any(dc.cbca_packed_kernel(c.max_arm) != dc.cbca_gate(c.L) for c in dc.CBCA_EXACT_CASES if c.max_arm and c.max_arm > c.L)
+    assert {c.entry for c in dc.CBCA_EXACT_CASES if c.arms == "clip"} == {"ex"}
+    assert {c.kernel for c in dc.CBCA_EXACT_CASES if c.arms == "negative"} == {"generic"}
+    assert {1, 127, 128, 129, 257} <= {c.W for c in dc.CBCA_EXACT_CASES}
+    assert {1, 31, 32, 33, 63, 64, 65} <= {c.H for c in dc.CBCA_EXACT_CASES}
+    assert any(c.D > c.W for c in dc.CBCA_EXACT_CASES)
+    for k in ("win1", "win4"):                             # whole tiles in the invalid triangle (the loop kernels copy per column)
+        for direction in (-1, 1):
+            assert any("whole" in dc.cbca_copy_paths(k, c.D, c.W, direction) and "partial" in dc.cbca_copy_paths(k, c.D, c.W, direction)
+                       for c in dc.CBCA_EXACT_CASES if c.kernel == k and c.direction == direction and c.W > 1), (k, direction)
+
+
+@pytest.mark.parametrize("c", dc.CBCA_FAST_CASES, ids=dc.fast_id)
+def test_cbca_fast_case_selects_its_kernel(c):
+    assert dc.cbca_fast_kernel(c.max_arm) == c.kernel and c.max_arm == c.L
+    assert dc.cbca_fast_refusal(c.W, c.ld, 0, 0, False, c.max_arm) is None and c.ld > c.W + 3
+    assert c.kind in dc.CBCA_KINDS and (c.kind != "post_sgm" or c.H <= c.W)
+
+
+def test_cbca_fast_cases_reach_every_kernel_and_edge():
+    cases = dc.CBCA_FAST_CASES
+    assert {c.kernel for c in cases} == set(dc.CBCA_FAST_KERNELS)
+    assert {(c.kernel, c.direction) for c in cases} == {(k, d) for k in dc.CBCA_FAST_KERNELS for d in (-1, 1)}
+    for k in dc.CBCA_FAST_KERNELS:
+        mine = [c for c in cases if c.kernel == k]
+        assert {127, 128, 129, 257} <= {c.W for c in mine}, k
+        Ds = {c.D for c in mine}
+        assert {20, 21, 40, 41} <= Ds, k                                         # one, two and three chunks
+        for direction in (-1, 1):                                               # whole chunks copied, and partial ones
+            paths = set()
+            for c in mine:
+                if c.direction == direction:
+                    paths |= dc.cbca_copy_paths(k, c.D, c.W, direction)
+            assert paths == {"whole", "partial"}, (k, direction)
+    assert {c.kind for c in cases} == set(dc.CBCA_KINDS)
+    for kind in dc.CBCA_KINDS:                                                  # every kind through a ws and a tma kernel
+        ks = {c.kernel[:2] for c in cases if c.kind == kind}
+        assert ks == {"ws", "tm"}, kind
+    assert 228 in {c.D for c in cases if c.kernel.startswith("ws")} and dc.cbca_dchunk("ws4", 228) == 19
+    assert {1, 31, 32, 33, 63, 64, 65} <= {c.H for c in cases} and 1 in {c.W for c in cases}
+    assert {r[6] for r in dc.CBCA_FAST_REFUSALS} == {"EINVAL", "ELIMIT", None}
+    for W, ld, i, o, a, m, want in dc.CBCA_FAST_REFUSALS:
+        assert dc.cbca_fast_refusal(W, ld, i, o, a, m) == want
+
+
+def test_ad_census_cases_reach_every_edge():
+    cs = dc.AD_CENSUS_CASES
+    assert {dc.census_kernel(c.nch) for c in cs} == {"nch1", "nch3", "nch_rt"} and 4 in {c.nch for c in cs}
+    assert dc.census_kernel(5) == "ELIMIT"
+    assert any(c.H == 1 for c in cs) and any(c.W == 1 for c in cs) and any(c.nan for c in cs)
+    Ws = {c.W % 128 for c in cs if c.W > 1}
+    assert {0, 1, 127} <= Ws
+    Ds = {c.D for c in cs}
+    assert {8, 9, 16, 17} <= Ds and any(c.D > c.W for c in cs)
+
+
+# ---------------------------------------------------------------------------------------------------------------- teeth
+
+def _tap_sum(a0, a1, vol, direction, rows=1, cols=1):
+    """adcensus.cu:343-377 in float32 with one accumulator per output, rows and columns visited in the given order
+    (1 ascending, the reference's; -1 descending)"""
+    D, H, W = vol.shape
+    out = np.array(vol, np.float32)
+    ys, xs = np.mgrid[0:H, 0:W]
+    m = max(dc.pack_maxlen(a0, a1), 1)
+    for d in range(D):
+        sh = d * direction
+        xpc = np.clip(xs + sh, 0, W - 1)
+        ok = (xs + sh >= 0) & (xs + sh < W)
+        up = np.minimum(ys - a0[2], ys - a1[2][ys, xpc])
+        dn = np.minimum(a0[3] - ys, a1[3][ys, xpc] - ys)
+        acc = np.zeros((H, W), np.float32)
+        cnt = np.zeros((H, W), np.int64)
+        for dy in range(-m + 1, m)[::rows]:
+            yy = np.clip(ys + dy, 0, H - 1)
+            lft = np.minimum(xs - a0[0][yy, xs], xpc - a1[0][yy, xpc])
+            rgt = np.minimum(a0[1][yy, xs] - xs, a1[1][yy, xpc] - xpc)
+            rin = (dy > -up) & (dy < dn)
+            for dx in range(-m + 1, m)[::cols]:
+                tap = rin & (dx > -lft) & (dx < rgt)
+                v = vol[d][yy, np.clip(xs + dx, 0, W - 1)]
+                acc = np.where(tap, (acc + v).astype(np.float32), acc)
+                cnt += tap
+        with np.errstate(invalid="ignore", divide="ignore"):
+            out[d] = np.where(ok, acc / cnt.astype(np.float32), out[d])
+    return out
+
+
+TEETH_CASES = [c for c in dc.CBCA_EXACT_CASES if c.entry == "ex" and c.arms == "cross" and c.H > 1 and c.W > 1]
+
+
+@pytest.mark.parametrize("c", TEETH_CASES, ids=dc.cbca_id)
+def test_cbca_summation_order_changes_the_bits(oracle, c):
+    """the exact cases' volumes tell the reference's order (rows, then columns, ascending) from any other: a kernel that
+    summed a run or the rows the other way round would not be bit-identical"""
+    x0c, x1c, a0, a1 = dc.cbca_arms(c)
+    vol = dc.cbca_volume("stereojoin", c.H, c.W, min(c.D, 24), c.direction)
+    want = oracle.cbca(a0, a1, vol, c.direction)
+    assert np.array_equal(_tap_sum(a0, a1, vol, c.direction), want, equal_nan=True)     # the restatement is right
+    for rows, cols in ((1, -1), (-1, 1)):
+        assert not np.array_equal(_tap_sum(a0, a1, vol, c.direction, rows, cols), want, equal_nan=True), (rows, cols)
+
+
+@pytest.mark.parametrize("c", [c for c in dc.CBCA_EXACT_CASES if c.L == 3 and c.arms == "cross"], ids=dc.cbca_id)
+def test_cbca_gate_off_by_one_changes_the_result(oracle, c):
+    """arms of 3 aggregated by win<1> (a window of +-1 column and row: arms cut at 2), as a gate one off would do"""
+    x0c, x1c, a0, a1 = dc.cbca_arms(c)
+    vol = dc.cbca_volume("stereojoin", c.H, c.W, min(c.D, 24), c.direction)
+    want = oracle.cbca(a0, a1, vol, c.direction)
+    cut = oracle.cbca(dc.clip_arms(a0, 2), dc.clip_arms(a1, 2), vol, c.direction)
+    assert not np.array_equal(cut, want, equal_nan=True)

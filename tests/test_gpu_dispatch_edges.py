@@ -1,6 +1,7 @@
-"""GPU: every kernel variant of StereoJoin, SGM and the post-processing operators at the edges of its dispatch, bit for bit
-against the CPU oracle (NaN positions included), and -- where oracle/_ref/libadcensus_ref.so has been built -- median2d,
-mean2d and sgm2 against the reference's own kernels too.  The cases, and the variant each one selects, are in
+"""GPU: every kernel variant of StereoJoin, SGM, CBCA (exact and constant-work), AD / census and the post-processing operators
+at the edges of its dispatch, bit for bit against the CPU oracle (NaN positions included) -- the constant-work CBCA within
+its 1e-4 contract, against the oracle and a float64 tap-sum reference -- and, where oracle/_ref/libadcensus_ref.so has been
+built, median2d, mean2d, sgm2, cross and cbca against the reference's own kernels too.  The cases, and the variant each one selects, are in
 tests/dispatch_cases.py; tests/test_dispatch_cases.py checks on the CPU that they reach every variant and that their inputs
 tell a correct kernel from a subtly wrong one.  Every case is small (well under 1 GB of device memory)."""
 import ctypes
@@ -15,12 +16,16 @@ import torch
 pytestmark = pytest.mark.gpu
 
 import mccnn_b200  # noqa: E402,F401
-from mccnn_b200 import adcensus, rowband  # noqa: E402
+from mccnn_b200 import adcensus, pipeline, rowband, synth  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _spec = importlib.util.spec_from_file_location("dispatch_cases", os.path.join(ROOT, "tests", "dispatch_cases.py"))
 dc = importlib.util.module_from_spec(_spec)
 _spec.loader.exec_module(dc)
+_spec = importlib.util.spec_from_file_location("stage_chain", os.path.join(ROOT, "tests", "stage_chain.py"))
+sc = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(sc)
+EINVAL, ELIMIT = -1, -2
 
 
 def dev():
@@ -241,3 +246,202 @@ def test_transposes(oracle, c):
     src, dst = at_offset(hwd, c.off), at_offset(np.zeros((D, H, ld)), c.off)
     assert lib.mccnn_transpose_hwd_to_dhw_pitched_div4(vp(src), vp(dst), D, H, W, ld, s(src)) == 0
     same(dst.cpu().numpy()[:, :, :W], oracle.transpose_hwd_to_dhw_div4(hwd), "hwd -> pitched dhw / 4")
+
+
+# ----------------------------------------------------------------------------------------------------------------- CBCA
+
+def _exact_kind(i, c):
+    kind = dc.CBCA_KINDS[i % len(dc.CBCA_KINDS)]
+    return "stereojoin" if kind == "post_sgm" and c.H > c.W else kind
+
+
+@pytest.mark.parametrize("i,c", list(enumerate(dc.CBCA_EXACT_CASES)), ids=[dc.cbca_id(c) for c in dc.CBCA_EXACT_CASES])
+def test_cbca_exact(oracle, ref, i, c):
+    """adcensus_cbca (device gate), adcensus_cbca_ex and mccnn_pack_arms + mccnn_cbca_packed (host bound): bit-identical to
+    oracle.cbca on the arms the case aggregates (clipped at an understated bound), zero signs included; cross and cbca
+    against the reference's own kernels where built"""
+    x0c, x1c, a0, a1 = dc.cbca_arms(c)
+    vol = dc.cbca_volume(_exact_kind(i, c), c.H, c.W, c.D, c.direction)
+    want = oracle.cbca(a0, a1, vol, c.direction)
+    out = torch.full((1, c.D, c.H, c.W), 5.0, device=dev())
+    t0, t1, tv = cu(x0c)[None], cu(x1c)[None], cu(vol)[None]
+    if c.entry == "gate":
+        adcensus.cbca(t0, t1, tv, out, c.direction)
+    elif c.entry == "ex":
+        adcensus.cbca(t0, t1, tv, out, c.direction, max_arm=c.max_arm)
+    else:
+        packed = torch.zeros(2 * c.H * c.W + 1, dtype=torch.int32, device=dev())
+        lib, s = adcensus.lib(), adcensus._stream(tv)
+        assert lib.mccnn_pack_arms(vp(t0), vp(t1), vp(packed), c.H, c.W, s) == 0
+        assert lib.mccnn_cbca_packed(vp(packed), vp(t0), vp(t1), vp(tv), vp(out), c.D, c.H, c.W, c.direction, c.max_arm, s) == 0
+    same(out, want, "cbca %s" % c.entry)
+    if ref is not None:
+        img = dc.cbca_image(c.H, c.W, c.L, 7 * c.H + 3 * c.W + c.L)
+        rc = torch.empty((1, 4, c.H, c.W), device=dev())
+        ref.call("cross", cu(img)[None], rc, c.L, dc.CBCA_TAU1)
+        oc = torch.empty((1, 4, c.H, c.W), device=dev())
+        adcensus.cross(cu(img)[None], oc, c.L, dc.CBCA_TAU1)
+        same(oc, rc, "cross vs the live reference")
+        if c.arms != "clip":
+            ro = torch.empty((1, c.D, c.H, c.W), device=dev())
+            ref.call("cbca", t0, t1, tv, ro, c.direction)
+            same(out, ro, "cbca %s vs the live reference" % c.entry)
+
+
+def _run_fast(entry, x0c, x1c, vol, c):
+    """one aggregation through mccnn_cbca_fast_pitched or mccnn_pack_arms_hv + mccnn_cbca_fast_pitched_packed on (D, H, ld)
+    volumes whose padding holds 123 (input) / -7 (output): returns the (D, H, W) result; the padding must stay -7"""
+    D, H, W = vol.shape
+    vin = torch.full((D, H, c.ld), 123.0, device=dev())
+    vin[:, :, :W] = cu(vol)
+    vout = torch.full((D, H, c.ld), -7.0, device=dev())
+    a0, a1 = cu(x0c), cu(x1c)
+    lib, s = adcensus.lib(), adcensus._stream(vin)
+    if entry == "pitched":
+        rc = lib.mccnn_cbca_fast_pitched(vp(a0), vp(a1), vp(vin), vp(vout), D, H, W, c.ld, c.direction, c.max_arm, s)
+    else:
+        hv = torch.zeros(4 * H * W, dtype=torch.int32, device=dev())
+        assert lib.mccnn_pack_arms_hv(vp(a0), vp(a1), vp(hv), H, W, s) == 0
+        rc = lib.mccnn_cbca_fast_pitched_packed(vp(hv), vp(vin), vp(vout), D, H, W, c.ld, c.direction, c.max_arm, s)
+    assert rc == 0, rc
+    o = vout.cpu().numpy()
+    assert (o[:, :, W:] == -7.0).all(), "%s: padding columns were written" % entry
+    return o[:, :, :W]
+
+
+def _rel_err(got, want):
+    m = ~np.isnan(want)
+    return float((np.abs(got[m] - want[m]) / np.maximum(1.0, np.abs(want[m]))).max()) if m.any() else 0.0
+
+
+@pytest.mark.parametrize("c", dc.CBCA_FAST_CASES, ids=dc.fast_id)
+def test_cbca_fast(oracle, record_property, c):
+    """every constant-work kernel through both fast entries, on every volume kind: relative error <= 1e-4 max(1, |want|)
+    against oracle.cbca and the float64 tap sums, NaN pattern identical, padding columns untouched"""
+    x0c, x1c, _, _ = dc.cbca_arms(dc.CbcaCase(c.H, c.W, c.D, c.L, c.direction, "ex", c.max_arm, None, "cross"))
+    vol = dc.cbca_volume(c.kind, c.H, c.W, c.D, c.direction)
+    want, want64 = oracle.cbca(x0c, x1c, vol, c.direction), dc.cbca_f64(x0c, x1c, vol, c.direction)
+    for entry in ("pitched", "packed"):
+        got = _run_fast(entry, x0c, x1c, vol, c)
+        assert np.array_equal(np.isnan(got), np.isnan(want)), "%s: NaN pattern differs" % entry
+        e32, e64 = _rel_err(got, want), _rel_err(got, want64)
+        record_property("max_rel_err_f64_%s_%s" % (c.kind, entry), e64)
+        assert e32 <= 1e-4 and e64 <= 1e-4, "%s: max relative error %.3g (oracle), %.3g (float64)" % (entry, e32, e64)
+
+
+def test_cbca_fast_four_iterations_on_census(oracle):
+    """mb census's eight iterations of arms of 5 on a census volume: the error does not build up past the bar"""
+    c = dc.FastCase(70, 257, 40, 5, -1, 5, "ws4", 264, "census3")
+    x0c, x1c, _, _ = dc.cbca_arms(dc.CbcaCase(c.H, c.W, c.D, c.L, c.direction, "ex", 5, None, "cross"))
+    want = got = dc.cbca_volume(c.kind, c.H, c.W, c.D, c.direction)
+    for _ in range(8):
+        want = oracle.cbca(x0c, x1c, want, c.direction)
+        got = _run_fast("packed", x0c, x1c, got, c)
+    assert np.array_equal(np.isnan(got), np.isnan(want))
+    assert _rel_err(got, want) <= 1e-4
+
+
+@pytest.mark.parametrize("r", dc.CBCA_FAST_REFUSALS, ids=lambda r: "W%d_ld%d_off%d.%d_alias%d_arm%d" % r[:6])
+def test_cbca_fast_refusals(r):
+    """ld < W, ld % 4, a base off 16 bytes and vol_in == vol_out are EINVAL, a halo above 13 ELIMIT, for both entries"""
+    W, ld, in_off, out_off, aliased, max_arm, want = r
+    assert dc.cbca_fast_refusal(W, ld, in_off, out_off, aliased, max_arm) == want
+    D, H = 4, 8
+    code = {"EINVAL": EINVAL, "ELIMIT": ELIMIT, None: 0}[want]
+    vin = at_offset(np.zeros((D, H, ld)), in_off)
+    vout = vin if aliased else at_offset(np.zeros((D, H, ld)), out_off)
+    arms = cu(dc.clip_arms(np.zeros((4, H, W), np.float32), 1))
+    hv = torch.zeros(4 * H * W, dtype=torch.int32, device=dev())
+    lib, s = adcensus.lib(), adcensus._stream(vin)
+    assert lib.mccnn_pack_arms_hv(vp(arms), vp(arms), vp(hv), H, W, s) == 0
+    assert lib.mccnn_cbca_fast_pitched(vp(arms), vp(arms), vp(vin), vp(vout), D, H, W, ld, -1, max_arm, s) == code
+    assert lib.mccnn_cbca_fast_pitched_packed(vp(hv), vp(vin), vp(vout), D, H, W, ld, -1, max_arm, s) == code
+    torch.cuda.synchronize()
+
+
+# the pipeline: mb census (arms of 5, 8 + 8 iterations) in the default mode against the exact mode
+MB_H, MB_W, MB_D = 70, 257, 40
+
+
+@pytest.fixture(scope="module")
+def mb_census_pair(oracle):
+    p = synth.make_pair(MB_H, MB_W, 1, MB_D, seed=21)
+    volL = oracle.census(p["imgL"], p["imgR"], MB_D, -1)
+    volR = oracle.census(p["imgR"], p["imgL"], MB_D, 1)
+    return p, volL, volR
+
+
+@pytest.mark.parametrize("terminate", ["cbca1", ""])
+def test_pipeline_mb_census_fast_vs_exact(oracle, mb_census_pair, terminate):
+    """run_volumes on census volumes: after cbca1's 8 iterations (and after the full chain) the default mode's left volume
+    is within 1e-4 of the exact mode's, NaN pattern identical, and the map differs on < 5e-3 of the pixels; the exact mode
+    after cbca1 is bit-identical to the oracle chain"""
+    p, volL, volR = mb_census_pair
+    opt = pipeline.make_params("mb", "census", sm_terminate=terminate)
+    iL, iR = cu(p["imgL"]), cu(p["imgR"])
+    out = {}
+    for m in ("exact", "fast"):
+        sp = pipeline.StereoPipeline(1, MB_D, MB_H, MB_W, opt, cbca_mode=m)
+        vl = torch.empty((MB_D, MB_H, MB_W), device=dev())
+        d = sp.run_volumes(cu(volL), cu(volR), iL, iR, outL=vl)
+        torch.cuda.synchronize()
+        out[m] = (d.cpu().numpy(), vl.cpu().numpy())
+        sp.close()
+    (de, ve), (df, vf) = out["exact"], out["fast"]
+    assert np.array_equal(np.isnan(ve), np.isnan(vf)), "NaN pattern differs"
+    assert _rel_err(vf, ve) <= 1e-4
+    frac = float((np.abs(df - de) > 1e-4 * np.maximum(1.0, np.abs(de))).mean())
+    assert frac < 5e-3, "%.4f of the map changed" % frac
+    if terminate == "cbca1":
+        want, wL, _ = sc.oracle_chain(oracle, p["imgL"], p["imgR"], MB_D, opt, "cbca1", "", arch="volumes", volL=volL,
+                                      volR=volR, want_vols=True)
+        same(ve, wL, "exact mode after cbca1 vs the oracle chain")
+        same(de, want, "exact mode map after cbca1 vs the oracle chain")
+
+
+def test_pipeline_nan_in_valid_route(oracle):
+    """border > 0 and D > W - border - 1: fix_border leaves NaN at valid positions, and both modes run the generic kernel:
+    the left volume after cbca1 bit-identical to the oracle chain, and the default mode equal to the exact mode"""
+    H, W, C, D = 21, 40, 8, 40
+    opt = pipeline.make_params("kitti", "accurate_cbca4", sm_terminate="cbca1")
+    assert dc.pipe_cbca_route(True, opt.L1, opt.border, D, W) == "generic"
+    p = synth.make_pair(H, W, C, D, seed=5)
+    want, wL, _ = sc.oracle_chain(oracle, p["imgL"], p["imgR"], D, opt, "cbca1", "", featL=p["featL"], featR=p["featR"],
+                                  want_vols=True)
+    assert np.isnan(wL).any() and not np.isnan(wL).all()
+    got = {}
+    for m in ("exact", "fast"):
+        sp = pipeline.StereoPipeline(C, D, H, W, opt, cbca_mode=m)
+        vl = torch.empty((D, H, W), device=dev())
+        d = sp.run(cu(p["featL"]), cu(p["featR"]), cu(p["imgL"]), cu(p["imgR"]), volL=vl)
+        torch.cuda.synchronize()
+        got[m] = (d.clone(), vl.clone())
+        sp.close()
+        same(vl, wL, "%s mode: left volume after cbca1" % m)
+        same(d, want, "%s mode: map after cbca1" % m)
+    same(got["fast"][1], got["exact"][1], "fast == exact")
+
+
+# ------------------------------------------------------------------------------------------------------------ AD / census
+
+@pytest.mark.parametrize("c", dc.AD_CENSUS_CASES, ids=lambda c: "H%dW%dD%d_nch%d%s" % (c.H, c.W, c.D, c.nch, "_nan" * c.nan))
+def test_ad_census(oracle, c):
+    """census (nch 1, 3 and the runtime-nch kernel at 2 and 4) and AD bit for bit: NaN pixels, one row, one column,
+    W = 128k +- 1, D at the chunk edges (8 for AD, 16 for census) and D > W"""
+    a, b = dc.ad_census_images(c)
+    for direction in (-1, 1):
+        o = torch.full((1, c.D, c.H, c.W), 3.0, device=dev())
+        adcensus.census(cu(a)[None], cu(b)[None], o, direction)
+        same(o, oracle.census(a, b, c.D, direction), "census nch %d (%s)" % (c.nch, dc.census_kernel(c.nch)))
+        o = torch.full((1, c.D, c.H, c.W), 3.0, device=dev())
+        adcensus.ad(cu(a[:1])[None], cu(b[:1])[None], o, direction)
+        same(o, oracle.ad(a[0], b[0], c.D, direction), "ad")
+
+
+def test_census_refuses_five_channels():
+    a = torch.zeros((5, 6, 20), device=dev())
+    o = torch.full((4, 6, 20), 3.0, device=dev())
+    assert dc.census_kernel(5) == "ELIMIT"
+    assert adcensus.lib().adcensus_census(vp(a), vp(a), vp(o), 4, 5, 6, 20, -1, adcensus._stream(a)) == ELIMIT
+    torch.cuda.synchronize()
+    assert bool((o == 3.0).all())
