@@ -15,22 +15,51 @@ it: raw THCudaTensor_data + sizes, strides never read).
 """
 import ctypes
 import os
+import re
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libadcensus_b200.so")
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "adcensus_b200.h")
 _lib = None
 
-_c_float_p = ctypes.c_void_p
+# the C types include/adcensus_b200.h uses; every pointer (and adcensus_stream_t) is c_void_p
+_C_TYPES = {"int": ctypes.c_int, "float": ctypes.c_float, "double": ctypes.c_double, "long long": ctypes.c_longlong,
+            "size_t": ctypes.c_size_t, "adcensus_stream_t": ctypes.c_void_p, "void": None}
 
 
 class AdcensusError(RuntimeError):
     """What luaL_error raises in the reference (adcensus.cu:31-36)."""
 
 
+def _ctype(t, fn):
+    """the ctypes type of C type `t`: a return type, or a parameter with its name (a pointer parameter may keep it)"""
+    t = " ".join(t.replace("*", " * ").split())
+    if t == "const char *":                       # adcensus_version's string
+        return ctypes.c_char_p
+    if "*" in t:
+        return ctypes.c_void_p
+    if t not in _C_TYPES:
+        raise AdcensusError("%s: unsupported C type '%s' in %s" % (fn, t, os.path.basename(HEADER_PATH)))
+    return _C_TYPES[t]
+
+
+def prototypes(src):
+    """{name: (restype, argtypes)} of every adcensus_* / mccnn_* function declared in the C header text `src`"""
+    out = {}
+    for decl in re.sub(r"/\*.*?\*/|^\s*#[^\n]*", " ", src, flags=re.S | re.M).split(";"):
+        m = re.fullmatch(r"(.*?)\b((?:adcensus|mccnn)_\w+)\s*\((.*)\)", decl.strip(), re.S)
+        if m:
+            ret, fn, params = m.groups()
+            params = [] if params.strip() == "void" else params.split(",")
+            out[fn] = (_ctype(ret, fn), [_ctype(p if "*" in p else p.rsplit(None, 1)[0], fn) for p in params])
+    return out
+
+
 def lib():
-    """Load libadcensus_b200.so (fails loudly if it has not been built)."""
+    """Load libadcensus_b200.so (fails loudly if it has not been built) and type every function include/adcensus_b200.h
+    declares, so that each call converts its arguments as the C prototype says."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
@@ -38,9 +67,14 @@ def lib():
                 "libadcensus_b200.so not built (run `python -c 'import __graft_entry__ as g; g.build()'`); "
                 "there is no fallback path"
             )
-        _lib = ctypes.CDLL(LIB_PATH)
-        _lib.adcensus_version.restype = ctypes.c_char_p
-        _lib.mccnn_pipeline_device_bytes.restype = ctypes.c_size_t
+        if not os.path.exists(HEADER_PATH):
+            raise AdcensusError("%s not found: the library's prototypes are read from it" % HEADER_PATH)
+        with open(HEADER_PATH) as f:
+            protos = prototypes(f.read())
+        l = ctypes.CDLL(LIB_PATH)
+        for fn, (restype, argtypes) in protos.items():
+            getattr(l, fn).restype, getattr(l, fn).argtypes = restype, argtypes
+        _lib = l
     return _lib
 
 
@@ -56,21 +90,19 @@ def _check(rc, what):
     raise AdcensusError("%s: %s" % (what, {-1: "invalid argument", -2: "size limit exceeded"}.get(rc, "error %d" % rc)))
 
 
-def _t(x, narg, name):
-    # luaT_checkudata(L, narg, "torch.CudaTensor")
+def _t(x, narg, name, optional=False):
+    # luaT_checkudata(L, narg, "torch.CudaTensor"); optional: None passes as NULL
+    if optional and x is None:
+        return None
     if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.float32:
         raise AdcensusError("bad argument #%d to '%s' (torch.CudaTensor expected)" % (narg, name))
     if not x.is_contiguous():
         raise AdcensusError("bad argument #%d to '%s' (contiguous tensor expected)" % (narg, name))
-    return ctypes.c_void_p(x.data_ptr())
+    return x.data_ptr()
 
 
 def _stream(x):
-    return ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-
-
-def _f(v):
-    return ctypes.c_float(float(v))
+    return torch.cuda.current_stream(x.device).cuda_stream
 
 
 def StereoJoin(input_L, input_R, output_L, output_R):
@@ -89,7 +121,7 @@ def cross(x0, out, L1, tau1):
     p0, po = _t(x0, 1, n), _t(out, 2, n)
     H, W = out.size(2), out.size(3)
     with torch.cuda.device(out.device):
-        _check(lib().adcensus_cross(p0, po, H, W, int(L1), _f(tau1), _stream(out)), n)
+        _check(lib().adcensus_cross(p0, po, H, W, int(L1), tau1, _stream(out)), n)
 
 
 def cbca(x0c, x1c, vol_in, vol_out, direction, max_arm=None):
@@ -111,11 +143,11 @@ def sgm2(x0, x1, input, output, tmp, pi1, pi2, tau_so, alpha1, sgm_q1, sgm_q2, d
     """adcensus.sgm2(...)  adcensus.cu:620-697; input/output are (1,H,W,D)"""
     n = "sgm2"
     p0, p1, pi, po = _t(x0, 1, n), _t(x1, 2, n), _t(input, 3, n), _t(output, 4, n)
-    pt = _t(tmp, 5, n) if tmp is not None else ctypes.c_void_p(0)
+    pt = _t(tmp, 5, n, optional=True)
     H, W, D = input.size(1), input.size(2), input.size(3)
     with torch.cuda.device(input.device):
-        _check(lib().adcensus_sgm2(p0, p1, pi, po, pt, H, W, D, _f(pi1), _f(pi2), _f(tau_so), _f(alpha1),
-                                   _f(sgm_q1), _f(sgm_q2), int(direction), _stream(input)), n)
+        _check(lib().adcensus_sgm2(p0, p1, pi, po, pt, H, W, D, pi1, pi2, tau_so, alpha1,
+                                   sgm_q1, sgm_q2, int(direction), _stream(input)), n)
 
 
 def outlier_detection(d0, d1, outlier, disp_max):
@@ -174,7 +206,7 @@ def mean2d(img, kernel, alpha2):
     a, k = _t(img, 1, n), _t(kernel, 2, n)
     out = torch.empty_like(img)
     with torch.cuda.device(img.device):
-        _check(lib().adcensus_mean2d(a, k, _t(out, 0, n), img.size(-2), img.size(-1), kernel.size(0), _f(alpha2),
+        _check(lib().adcensus_mean2d(a, k, _t(out, 0, n), img.size(-2), img.size(-1), kernel.size(0), alpha2,
                                      _stream(img)), n)
     return out
 
@@ -261,7 +293,7 @@ def remove_white(x, y):
 def fill_nan(t):
     """vols:fill(0/0)  main.lua:946"""
     with torch.cuda.device(t.device):
-        _check(lib().mccnn_fill_nan(_t(t, 1, "fill_nan"), ctypes.c_size_t(t.numel()), _stream(t)), "fill_nan")
+        _check(lib().mccnn_fill_nan(_t(t, 1, "fill_nan"), t.numel(), _stream(t)), "fill_nan")
 
 
 def fix_border(vol, n, direction):
@@ -303,7 +335,7 @@ def argmin(vol):
 def gaussian(sigma):
     """gaussian(sigma)  main.lua:528-540 (host tensor, float32)"""
     l = lib()
-    ks = l.mccnn_gaussian(ctypes.c_double(sigma), None)
+    ks = l.mccnn_gaussian(sigma, None)
     out = torch.empty((ks, ks), dtype=torch.float32)
-    l.mccnn_gaussian(ctypes.c_double(sigma), ctypes.c_void_p(out.data_ptr()))
+    l.mccnn_gaussian(sigma, out.data_ptr())
     return out

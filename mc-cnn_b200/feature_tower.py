@@ -28,7 +28,7 @@ class FeatureTower:
         wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         self._h = ctypes.c_void_p()
-        stream = ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
         adcensus._check(adcensus.lib().mccnn_feature_tower_create(ctypes.byref(self._h), self.n_in, self.fm, self.l1, relu_last,
                                                                   normalize, wp, bp, self.device.index, stream),
                         "mccnn_feature_tower_create")
@@ -54,7 +54,7 @@ class FeatureTower:
         N, _, H, W = x_batch.shape
         out = torch.empty((N, self.fm, H, W), device=x_batch.device, dtype=torch.float32)
         with torch.cuda.device(x_batch.device):
-            rc = adcensus.lib().mccnn_feature_tower_forward(self._h, px, ctypes.c_void_p(out.data_ptr()), N, H, W, nterms,
+            rc = adcensus.lib().mccnn_feature_tower_forward(self._h, px, out.data_ptr(), N, H, W, nterms,
                                                             adcensus._stream(x_batch))
         adcensus._check(rc, n)
         return out

@@ -85,8 +85,6 @@ def make_batch_cuda(left, right, device=0):
     views as :func:`load_bytes` returns them, (H, W) or (H, W, 3) uint8 numpy arrays or torch tensors (host or device), both
     grey or both colour.  Only the bytes are copied to `device` (a torch.device or index); returns x_batch (2,1,H,W) CUDA
     float32.  Waits for the two views' statistics and refuses a constant view, as :func:`standardise` does."""
-    import ctypes
-
     import torch
 
     from .adcensus import _check, _stream, lib
@@ -105,9 +103,8 @@ def make_batch_cuda(left, right, device=0):
         views = [v.to(dev).contiguous() for v in views]
         x_batch = torch.empty((2, 1, H, W), dtype=torch.float32, device=dev)
         stats = torch.empty((2, 3), dtype=torch.float64, device=dev)
-        p = lambda t: ctypes.c_void_p(t.data_ptr())
-        _check(lib().mccnn_frontend_batch(p(views[0]), p(views[1]), nch, H, W, p(x_batch), p(stats), _stream(x_batch)),
-               "mccnn_frontend_batch")
+        _check(lib().mccnn_frontend_batch(views[0].data_ptr(), views[1].data_ptr(), nch, H, W, x_batch.data_ptr(),
+                                          stats.data_ptr(), _stream(x_batch)), "mccnn_frontend_batch")
         var = stats[:, 2].cpu()
     for name, v in zip(("left", "right"), var.tolist()):
         if not v > 0:

@@ -299,12 +299,11 @@ class StereoPipeline:
         n = "mccnn_pipeline_run"
         if disp is None:
             disp = torch.empty((self.H, self.W), device=featL.device, dtype=torch.float32)
-        vp = lambda t: adcensus._t(t, 0, n) if t is not None else ctypes.c_void_p(0)
         with torch.cuda.device(featL.device):
             rc = adcensus.lib().mccnn_pipeline_run(self._h, adcensus._t(featL, 1, n), adcensus._t(featR, 2, n),
                                                    adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
-                                                   adcensus._t(disp, 5, n), vp(volL), vp(volR),
-                                                   adcensus._stream(featL))
+                                                   adcensus._t(disp, 5, n), adcensus._t(volL, 0, n, optional=True),
+                                                   adcensus._t(volR, 0, n, optional=True), adcensus._stream(featL))
         adcensus._check(rc, n)
         return disp
 
@@ -325,12 +324,11 @@ class StereoPipeline:
         for name, t, shape in want:
             if t is not None and tuple(t.shape) != shape:
                 raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
-        vp = lambda t, i: adcensus._t(t, i, n) if t is not None else ctypes.c_void_p(0)
         with torch.cuda.device(imgL.device):
             rc = adcensus.lib().mccnn_pipeline_run_shape(self._h, H, W, D, adcensus._t(featL, 1, n), adcensus._t(featR, 2, n),
                                                          adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
-                                                         adcensus._t(disp, 5, n), vp(volL, 6), vp(volR, 7),
-                                                         adcensus._stream(imgL))
+                                                         adcensus._t(disp, 5, n), adcensus._t(volL, 6, n, optional=True),
+                                                         adcensus._t(volR, 7, n, optional=True), adcensus._stream(imgL))
         adcensus._check(rc, n)
         return disp
 
@@ -355,9 +353,9 @@ class StereoPipeline:
                 raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
         if volR is None and (self.params.lr_check or outR is not None):
             raise adcensus.AdcensusError("%s: volR is needed (LR check or outR)" % n)
-        vp = lambda t, i: adcensus._t(t, i, n) if t is not None else ctypes.c_void_p(0)
-        ptrs = (adcensus._t(volL, 1, n), vp(volR, 2), adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
-                adcensus._t(disp, 5, n), vp(outL, 6), vp(outR, 7))
+        ptrs = (adcensus._t(volL, 1, n), adcensus._t(volR, 2, n, optional=True), adcensus._t(imgL, 3, n),
+                adcensus._t(imgR, 4, n), adcensus._t(disp, 5, n), adcensus._t(outL, 6, n, optional=True),
+                adcensus._t(outR, 7, n, optional=True))
         with torch.cuda.device(imgL.device):
             rc = adcensus.lib().mccnn_pipeline_run_volumes(self._h, H, W, D, *ptrs, adcensus._stream(imgL))
         adcensus._check(rc, n)
@@ -371,7 +369,7 @@ class StereoPipeline:
         k = len(pairs)
         if disps is None:
             disps = [torch.empty((self.H, self.W), device=pairs[0][0].device, dtype=torch.float32) for _ in range(k)]
-        arr = lambda ts, i: (ctypes.c_void_p * k)(*[adcensus._t(t, i, n).value for t in ts])
+        arr = lambda ts, i: (ctypes.c_void_p * k)(*[adcensus._t(t, i, n) for t in ts])
         with torch.cuda.device(pairs[0][0].device):
             rc = adcensus.lib().mccnn_pipeline_run_batch(
                 self._h, k, arr([p[0] for p in pairs], 1), arr([p[1] for p in pairs], 2), arr([p[2] for p in pairs], 3),
@@ -388,8 +386,8 @@ class StereoPipeline:
                 raise adcensus.AdcensusError("%s: contiguous host float tensors expected" % n)
         if disp is None:
             disp = torch.empty((self.H, self.W), dtype=torch.float32)
-        p = lambda t: ctypes.c_void_p(t.data_ptr())
-        rc = adcensus.lib().mccnn_pipeline_run_host(self._h, p(featL), p(featR), p(imgL), p(imgR), p(disp))
+        rc = adcensus.lib().mccnn_pipeline_run_host(self._h, featL.data_ptr(), featR.data_ptr(), imgL.data_ptr(),
+                                                    imgR.data_ptr(), disp.data_ptr())
         adcensus._check(rc, n)
         return disp
 

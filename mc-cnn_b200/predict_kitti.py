@@ -110,8 +110,6 @@ class Prefetch:
 def error_counts(disp, gt16, err_at=ERR_AT):
     """(bad, valid) pixel counts of one device map against its PNG16 ground truth (mccnn_kitti_error_count): disp (H, W) CUDA
     float32, gt16 (H, W) uint16 values (numpy, or an int16 / uint16 torch tensor).  Returns a (2,) int64 CUDA tensor."""
-    import ctypes
-
     import torch
 
     from .adcensus import _check, _stream, _t, lib
@@ -129,8 +127,7 @@ def error_counts(disp, gt16, err_at=ERR_AT):
     with torch.cuda.device(disp.device):
         g = gt16.to(disp.device).contiguous()
         counts = torch.empty(2, dtype=torch.int64, device=disp.device)
-        _check(lib().mccnn_kitti_error_count(p, ctypes.c_void_p(g.data_ptr()), H, W, ctypes.c_float(err_at),
-                                             ctypes.c_void_p(counts.data_ptr()), _stream(disp)), name)
+        _check(lib().mccnn_kitti_error_count(p, g.data_ptr(), H, W, err_at, counts.data_ptr(), _stream(disp)), name)
     return counts
 
 

@@ -201,8 +201,6 @@ def load_host(data_root, dataset, height=HEIGHT, width=WIDTH, log=None):
 def kitti_nnz(disp, x0, is_te):
     """preprocess_kitti.lua:93-116 on the GPU: disp (n, 1, H, W) and x0 (>= n, 1, H, W) CUDA float32 on one device, is_te
     (n) booleans -> (nnz_tr, nnz_te), (rows, 4) CUDA float32 tensors.  disp is not modified."""
-    import ctypes
-
     import torch
 
     from .adcensus import AdcensusError, _check, _stream, _t, lib
@@ -222,14 +220,12 @@ def kitti_nnz(disp, x0, is_te):
         flags = torch.as_tensor(np.asarray(is_te, dtype=np.int32)).to(dev)
         counts = torch.zeros(2, dtype=torch.int64, device=dev)
         l, s = lib(), _stream(disp)
-        pf = ctypes.c_void_p(flags.data_ptr())
-        _check(l.mccnn_kitti_nnz_count(pd, px, pf, n, H, W, ctypes.c_void_p(counts.data_ptr()), s), name)
+        _check(l.mccnn_kitti_nnz_count(pd, px, flags.data_ptr(), n, H, W, counts.data_ptr(), s), name)
         n_tr_rows, n_te_rows = (int(v) for v in counts.cpu())
         nnz_tr = torch.empty((n_tr_rows, 4), dtype=torch.float32, device=dev)
         nnz_te = torch.empty((n_te_rows, 4), dtype=torch.float32, device=dev)
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr() if t.numel() else None)
-        _check(l.mccnn_kitti_nnz_fill(pd, px, pf, n, H, W, ptr(nnz_tr), ctypes.c_longlong(n_tr_rows), ptr(nnz_te),
-                                      ctypes.c_longlong(n_te_rows), s), name)
+        _check(l.mccnn_kitti_nnz_fill(pd, px, flags.data_ptr(), n, H, W, nnz_tr.data_ptr(), n_tr_rows, nnz_te.data_ptr(),
+                                      n_te_rows, s), name)
     return nnz_tr, nnz_te
 
 
@@ -453,15 +449,13 @@ def mb_scenes(data_root, rect):
 
 
 def _u8(x, narg, name):
-    import ctypes
-
     import torch
 
     from .adcensus import AdcensusError
 
     if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.uint8 or not x.is_contiguous():
         raise AdcensusError("bad argument #%d to '%s' (contiguous CUDA uint8 tensor expected)" % (narg, name))
-    return ctypes.c_void_p(x.data_ptr())
+    return x.data_ptr()
 
 
 def _rgb_stack(x, name):
@@ -483,7 +477,7 @@ def mb_views(rgb, nchannel):
     n, H, W = _rgb_stack(rgb, name)
     with torch.cuda.device(rgb.device):
         out = torch.empty((n, nchannel, H, W), dtype=torch.float32, device=rgb.device)
-        _check(lib().mccnn_mb_views(p, _ptr(out), n, H, W, nchannel, _stream(rgb)), name)
+        _check(lib().mccnn_mb_views(p, out.data_ptr(), n, H, W, nchannel, _stream(rgb)), name)
     return out
 
 
@@ -498,7 +492,7 @@ def mb_half_image(rgb):
     n, H, W = _rgb_stack(rgb, name)
     with torch.cuda.device(rgb.device):
         out = torch.empty((n, H // 2, W // 2, 3), dtype=torch.uint8, device=rgb.device)
-        _check(lib().mccnn_mb_half_image(p, _ptr(out), n, H, W, _stream(rgb)), name)
+        _check(lib().mccnn_mb_half_image(p, out.data_ptr(), n, H, W, _stream(rgb)), name)
     return out
 
 
@@ -515,7 +509,7 @@ def mb_half_disp(d):
     n, H, W = d.shape
     with torch.cuda.device(d.device):
         out = torch.empty((n, H // 2, W // 2), dtype=torch.float32, device=d.device)
-        _check(lib().mccnn_mb_half_disp(p, _ptr(out), n, H, W, _stream(d)), name)
+        _check(lib().mccnn_mb_half_disp(p, out.data_ptr(), n, H, W, _stream(d)), name)
     return out
 
 
@@ -534,15 +528,13 @@ def mb_mask(d0, d1, d0y=None):
     H, W = d0.shape
     with torch.cuda.device(d0.device):
         out = torch.empty((H, W), dtype=torch.uint8, device=d0.device)
-        _check(lib().mccnn_mb_mask(ps[0], ps[2] if d0y is not None else None, ps[1], H, W, _ptr(out), _stream(d0)), name)
+        _check(lib().mccnn_mb_mask(ps[0], ps[2] if d0y is not None else None, ps[1], H, W, out.data_ptr(), _stream(d0)), name)
     return out
 
 
 def mb_nnz(d0, mask, image):
     """dispnoc and the training rows of one map on the GPU: d0 (H, W) CUDA float32, mask (H, W) CUDA uint8, image 1-based
     -> (dispnoc (H, W), rows (n, 4) float32 (image, y, x, d0) for mask == 255 in row-major order)"""
-    import ctypes
-
     import torch
 
     from .adcensus import AdcensusError, _check, _stream, _t, lib
@@ -557,18 +549,12 @@ def mb_nnz(d0, mask, image):
     with torch.cuda.device(dev):
         count = torch.zeros(1, dtype=torch.int64, device=dev)
         s = _stream(d0)
-        _check(lib().mccnn_mb_nnz_count(pm, H, W, _ptr(count), s), name)
+        _check(lib().mccnn_mb_nnz_count(pm, H, W, count.data_ptr(), s), name)
         n = int(count.item())
         dispnoc = torch.empty((H, W), dtype=torch.float32, device=dev)
         rows = torch.empty((n, 4), dtype=torch.float32, device=dev)
-        _check(lib().mccnn_mb_nnz_fill(pd, pm, H, W, int(image), _ptr(dispnoc), _ptr(rows), ctypes.c_longlong(n), s), name)
+        _check(lib().mccnn_mb_nnz_fill(pd, pm, H, W, int(image), dispnoc.data_ptr(), rows.data_ptr(), n, s), name)
     return dispnoc, rows
-
-
-def _ptr(t):
-    import ctypes
-
-    return ctypes.c_void_p(t.data_ptr() if t.numel() else None)
 
 
 def check_mb_outputs_absent(d):

@@ -275,34 +275,28 @@ class CudaOps:
         return torch.empty_like(t)
 
     def sgm_band(self, imgL, imgR, cost, acc, Ht, Wt, yoff, xoff, opt, direction, pass_mask, zero_out):
-        import ctypes
-
         from . import adcensus
 
         H, W, D = cost.shape
-        f = ctypes.c_float
-        p = lambda t: adcensus._t(t, 0, "mccnn_sgm2_band")
+        n = "mccnn_sgm2_band"
         with torch.cuda.device(cost.device):
-            rc = adcensus.lib().mccnn_sgm2_band(p(imgL), p(imgR), p(cost), p(acc), H, W, D, Ht, Wt, yoff, xoff,
-                                                f(opt.pi1), f(opt.pi2), f(opt.tau_so), f(opt.alpha1), f(opt.sgm_q1),
-                                                f(opt.sgm_q2), int(direction), int(pass_mask), int(bool(zero_out)),
-                                                adcensus._stream(cost))
+            rc = adcensus.lib().mccnn_sgm2_band(adcensus._t(imgL, 0, n), adcensus._t(imgR, 0, n), adcensus._t(cost, 0, n),
+                                                adcensus._t(acc, 0, n), H, W, D, Ht, Wt, yoff, xoff, opt.pi1, opt.pi2,
+                                                opt.tau_so, opt.alpha1, opt.sgm_q1, opt.sgm_q2, int(direction),
+                                                int(pass_mask), int(bool(zero_out)), adcensus._stream(cost))
         adcensus._check(rc, "mccnn_sgm2_band")
 
     def sgm_tables(self, imgL, imgR, D, opt, direction):
         """penalty-class tables + selector words of the full image pair for one `direction` (mccnn_sgm_tables_build)"""
-        import ctypes
-
         from . import adcensus
 
         lib = adcensus.lib()
-        lib.mccnn_sgm_tables_bytes.restype = ctypes.c_size_t
         Ht, Wt = imgL.shape
         tab = torch.empty(lib.mccnn_sgm_tables_bytes(Ht, Wt, D), dtype=torch.uint8, device=imgL.device)
-        p = lambda t: adcensus._t(t, 0, "mccnn_sgm_tables_build")
+        n = "mccnn_sgm_tables_build"
         with torch.cuda.device(imgL.device):
-            rc = lib.mccnn_sgm_tables_build(p(imgL.contiguous()), p(imgR.contiguous()), ctypes.c_void_p(tab.data_ptr()), Ht, Wt, D,
-                                            ctypes.c_float(opt.tau_so), int(direction), adcensus._stream(imgL))
+            rc = lib.mccnn_sgm_tables_build(adcensus._t(imgL.contiguous(), 0, n), adcensus._t(imgR.contiguous(), 0, n),
+                                            tab.data_ptr(), Ht, Wt, D, opt.tau_so, int(direction), adcensus._stream(imgL))
         adcensus._check(rc, "mccnn_sgm_tables_build")
         return tab
 
@@ -312,18 +306,16 @@ class CudaOps:
         return torch.empty((W, adcensus.lib().mccnn_sgm_state_pitch(D)), device=like.device, dtype=torch.float32)
 
     def sgm_rows(self, tab, cost, acc, Ht, yoff, opt, direction, pass_mask, zero_out, xa, xb, state_in, state_out):
-        import ctypes
-
         from . import adcensus
 
         H, W, D = cost.shape
-        f = ctypes.c_float
-        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+        n = "mccnn_sgm2_rows"
         with torch.cuda.device(cost.device):
-            rc = adcensus.lib().mccnn_sgm2_rows(p(tab), p(cost), p(acc), H, W, D, int(Ht), int(yoff), f(opt.pi1), f(opt.pi2),
-                                                f(opt.tau_so), f(opt.alpha1), f(opt.sgm_q1), f(opt.sgm_q2), int(direction),
-                                                int(pass_mask), int(bool(zero_out)), int(xa), int(xb), p(state_in), p(state_out),
-                                                adcensus._stream(cost))
+            rc = adcensus.lib().mccnn_sgm2_rows(tab.data_ptr(), cost.data_ptr(), acc.data_ptr(), H, W, D, int(Ht), int(yoff),
+                                                opt.pi1, opt.pi2, opt.tau_so, opt.alpha1, opt.sgm_q1, opt.sgm_q2,
+                                                int(direction), int(pass_mask), int(bool(zero_out)), int(xa), int(xb),
+                                                adcensus._t(state_in, 0, n, optional=True),
+                                                adcensus._t(state_out, 0, n, optional=True), adcensus._stream(cost))
         adcensus._check(rc, "mccnn_sgm2_rows")
 
     def argmin(self, vol):

@@ -32,7 +32,7 @@ class ScorerHead:
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         self._h = ctypes.c_void_p()
         lib = adcensus.lib()
-        stream = ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
         adcensus._check(lib.mccnn_scorer_head_create(ctypes.byref(self._h), self.fm, self.nh2, self.l2, wp, bp,
                                                      self.device.index, stream), "mccnn_scorer_head_create")
 
@@ -61,9 +61,9 @@ class ScorerHead:
         vols = []
         for want in (want_left, want_right):
             vols.append(torch.full((1, D, H, W), float("nan"), device=featL.device) if want else None)   # main.lua:962
-        vp = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
         with torch.cuda.device(featL.device):
-            rc = adcensus.lib().mccnn_scorer_head_forward(self._h, pL, pR, vp(vols[0]), vp(vols[1]), H, W, D, nterms,
+            rc = adcensus.lib().mccnn_scorer_head_forward(self._h, pL, pR, adcensus._t(vols[0], 0, n, optional=True),
+                                                          adcensus._t(vols[1], 0, n, optional=True), H, W, D, nterms,
                                                           adcensus._stream(featL))
         adcensus._check(rc, n)
         return vols[0], vols[1]

@@ -194,8 +194,8 @@ def randperm(stream, n):
     for i0 in range(0, max(n - 1, 0), step):
         k = min(step, n - 1 - i0)
         d = np.ascontiguousarray(stream.raw(k))
-        _check(lib().mccnn_randperm_swaps(perm.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(n), ctypes.c_longlong(i0),
-                                          d.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(k)), "randperm")
+        _check(lib().mccnn_randperm_swaps(perm.ctypes.data_as(ctypes.c_void_p), n, i0, d.ctypes.data_as(ctypes.c_void_p), k),
+               "randperm")
     return perm + 1
 
 
@@ -286,9 +286,8 @@ def mb_sample_starts(raw, base, d_exp, cap):
     raw = np.ascontiguousarray(raw, np.uint32)
     starts = np.zeros(cap, np.int64)
     count, used = ctypes.c_longlong(), ctypes.c_longlong()
-    _check(lib().mccnn_mb_sample_starts(raw.ctypes.data_as(ctypes.c_void_p), ctypes.c_longlong(len(raw)), base,
-                                        ctypes.c_double(d_exp), starts.ctypes.data_as(ctypes.c_void_p),
-                                        ctypes.c_longlong(cap), ctypes.byref(count), ctypes.byref(used)),
+    _check(lib().mccnn_mb_sample_starts(raw.ctypes.data_as(ctypes.c_void_p), len(raw), base, d_exp,
+                                        starts.ctypes.data_as(ctypes.c_void_p), cap, ctypes.byref(count), ctypes.byref(used)),
            "mccnn_mb_sample_starts")
     return starts[:count.value], used.value
 
@@ -377,8 +376,8 @@ def sample_patches(X0, X1, warps, ws):
     w = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(X0.device)
     out = torch.empty((len(warps), ws, ws), dtype=torch.float32, device=X0.device)
     with torch.cuda.device(X0.device):
-        _check(lib().mccnn_train_sample(p0, p1, n_img, H, W, ctypes.c_void_p(w.data_ptr()), len(warps), ws,
-                                        ctypes.c_void_p(out.data_ptr()), _stream(out)), name)
+        _check(lib().mccnn_train_sample(p0, p1, n_img, H, W, w.data_ptr(), len(warps), ws, out.data_ptr(), _stream(out)),
+               name)
     return out
 
 
@@ -407,9 +406,8 @@ def sample_patches_pairs(planes, warps, ws):
     w = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(dev)
     out = torch.empty((len(warps), ws, ws), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        _check(lib().mccnn_train_sample_pairs(ctypes.c_void_p(table.data_ptr()), len(planes), ctypes.c_void_p(w.data_ptr()),
-                                              len(warps), ws, ctypes.c_void_p(out.data_ptr()), _stream(out)),
-               "sample_patches_pairs")
+        _check(lib().mccnn_train_sample_pairs(table.data_ptr(), len(planes), w.data_ptr(), len(warps), ws, out.data_ptr(),
+                                              _stream(out)), "sample_patches_pairs")
     return out
 
 
@@ -440,26 +438,24 @@ class Trainer:
                 tp = t.ctypes.data_as(ctypes.c_void_p)
                 if self.arch == "slow":
                     _check(lib().mccnn_trainer_create_slow_pairs(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2,
-                                                                 self.bs, ctypes.c_float(o["mom"]), tp, len(t), chunk,
-                                                                 loss_cap, self.dev.index, _stream(src)),
+                                                                 self.bs, o["mom"], tp, len(t), chunk, loss_cap, self.dev.index,
+                                                                 _stream(src)),
                            "mccnn_trainer_create_slow_pairs")
                 else:
-                    _check(lib().mccnn_trainer_create_pairs(ctypes.byref(self._h), self.l1, self.fm, self.bs,
-                                                            ctypes.c_float(o["m"]), o["pow"], ctypes.c_float(o["mom"]), tp,
-                                                            len(t), chunk, loss_cap, self.dev.index, _stream(src)),
+                    _check(lib().mccnn_trainer_create_pairs(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"], o["pow"],
+                                                            o["mom"], tp, len(t), chunk, loss_cap, self.dev.index,
+                                                            _stream(src)),
                            "mccnn_trainer_create_pairs")
             elif self.arch == "slow":
                 n_img, _, H, W = X0.shape
                 _check(lib().mccnn_trainer_create_slow(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2, self.bs,
-                                                       ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
-                                                       _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
-                                                       _stream(X0)), "mccnn_trainer_create_slow")
+                                                       o["mom"], _t(X0, 1, "Trainer"), _t(X1, 2, "Trainer"), n_img, H, W,
+                                                       chunk, loss_cap, self.dev.index, _stream(X0)), "mccnn_trainer_create_slow")
             else:
                 n_img, _, H, W = X0.shape
-                _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, ctypes.c_float(o["m"]),
-                                                  o["pow"], ctypes.c_float(o["mom"]), _t(X0, 1, "Trainer"),
-                                                  _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap, self.dev.index,
-                                                  _stream(X0)), "mccnn_trainer_create")
+                _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"], o["pow"], o["mom"],
+                                                  _t(X0, 1, "Trainer"), _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap,
+                                                  self.dev.index, _stream(X0)), "mccnn_trainer_create")
         self.launches_per_step = lib().mccnn_trainer_launches_per_step(self._h)
 
     def close(self):
@@ -475,14 +471,10 @@ class Trainer:
         except Exception:
             pass
 
-    def _s(self):
-        return ctypes.c_void_p(self.stream.cuda_stream)
-
     def size(self, what):
         from .adcensus import lib
 
-        lib().mccnn_trainer_size.restype = ctypes.c_longlong
-        return int(lib().mccnn_trainer_size(self._h, what))
+        return lib().mccnn_trainer_size(self._h, what)
 
     def get(self, what):
         """a copy of one of the trainer's buffers (TRAIN_*) as a CUDA float32 tensor"""
@@ -491,7 +483,7 @@ class Trainer:
         from .adcensus import _check, lib
 
         out = torch.empty(self.size(what), dtype=torch.float32, device=self.dev)
-        _check(lib().mccnn_trainer_get(self._h, what, ctypes.c_void_p(out.data_ptr()), self._s()), "mccnn_trainer_get")
+        _check(lib().mccnn_trainer_get(self._h, what, out.data_ptr(), self.stream.cuda_stream), "mccnn_trainer_get")
         return out
 
     def set(self, what, src):
@@ -502,7 +494,7 @@ class Trainer:
         t = torch.as_tensor(src, dtype=torch.float32).reshape(-1).to(self.dev).contiguous()
         if t.numel() != self.size(what):
             raise ValueError("Trainer.set: %d values for a buffer of %d" % (t.numel(), self.size(what)))
-        _check(lib().mccnn_trainer_set(self._h, what, ctypes.c_void_p(t.data_ptr()), self._s()), "mccnn_trainer_set")
+        _check(lib().mccnn_trainer_set(self._h, what, t.data_ptr(), self.stream.cuda_stream), "mccnn_trainer_set")
         self.stream.synchronize()
 
     def set_layers(self, layers, head=None):
@@ -527,8 +519,7 @@ class Trainer:
         if isinstance(warps, np.ndarray):
             warps = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(self.dev)
         nsteps = warps.numel() // (WARP_DTYPE.itemsize * self.N)
-        _check(lib().mccnn_trainer_run(self._h, ctypes.c_void_p(warps.data_ptr()), nsteps, ctypes.c_double(lr), self._s()),
-               "mccnn_trainer_run")
+        _check(lib().mccnn_trainer_run(self._h, warps.data_ptr(), nsteps, lr, self.stream.cuda_stream), "mccnn_trainer_run")
         return warps
 
     def step_patches(self, patches, lr):
@@ -539,14 +530,14 @@ class Trainer:
         t = torch.as_tensor(patches, dtype=torch.float32).to(self.dev).contiguous()
         if t.numel() != self.N * self.ws * self.ws:
             raise ValueError("step_patches: (%d, 1, %d, %d) patches expected" % (self.N, self.ws, self.ws))
-        _check(lib().mccnn_trainer_step_patches(self._h, ctypes.c_void_p(t.data_ptr()), ctypes.c_double(lr), self._s()),
+        _check(lib().mccnn_trainer_step_patches(self._h, t.data_ptr(), lr, self.stream.cuda_stream),
                "mccnn_trainer_step_patches")
         self._last = t
 
     def reset_losses(self):
         from .adcensus import _check, lib
 
-        _check(lib().mccnn_trainer_reset_losses(self._h, self._s()), "mccnn_trainer_reset_losses")
+        _check(lib().mccnn_trainer_reset_losses(self._h, self.stream.cuda_stream), "mccnn_trainer_reset_losses")
 
 
 def flatten(layers):

@@ -32,6 +32,48 @@ def test_header_symbols_exported(lib):
         assert hasattr(lib, n), "libadcensus_b200.so does not export %s" % n
 
 
+C_TYPES = {"int": ctypes.c_int, "float": ctypes.c_float, "double": ctypes.c_double, "long long": ctypes.c_longlong,
+           "size_t": ctypes.c_size_t, "adcensus_stream_t": ctypes.c_void_p, "void": None, "const char *": ctypes.c_char_p}
+
+
+def test_loader_types_every_declared_function(lib):
+    """the loader types exactly the functions the header declares, each as the header's prototype reads"""
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "adcensus_b200.h")).read(), flags=re.S)
+    names = declared_functions()
+    assert sorted(adcensus.prototypes(src)) == names
+    for n in names:
+        ret, params = re.search(r"([\w ]+?\s*\**)\s*\b%s\s*\(([^)]*)\)" % n, src).groups()
+        want = [ctypes.c_void_p if "*" in q else C_TYPES[q.rsplit(None, 1)[0].strip()]
+                for q in params.split(",") if q.strip() != "void"]
+        fn = getattr(lib, n)
+        assert fn.restype is C_TYPES[ret.strip()], n
+        assert fn.argtypes == want, n
+
+
+def test_loader_prototypes_pinned(lib):
+    """a few prototypes written out, so that a parser bug cannot pass by agreeing with itself"""
+    f, i, p = ctypes.c_float, ctypes.c_int, ctypes.c_void_p
+    assert lib.adcensus_sgm2.argtypes == [p] * 5 + [i] * 3 + [f] * 6 + [i, p]
+    assert lib.adcensus_sgm2.restype is i
+    assert lib.mccnn_trainer_run.argtypes == [p, p, i, ctypes.c_double, p]
+    assert lib.mccnn_trainer_size.restype is ctypes.c_longlong
+    assert lib.mccnn_packed_hv_bytes.restype is ctypes.c_size_t
+    assert lib.mccnn_sgm_tables_bytes.restype is ctypes.c_size_t
+    assert lib.mccnn_fill_nan.argtypes == [p, ctypes.c_size_t, p]
+    assert lib.mccnn_pipeline_destroy.restype is None
+    assert lib.adcensus_version.restype is ctypes.c_char_p and lib.adcensus_version.argtypes == []
+    assert lib.mccnn_mb_sample_starts.argtypes == [p, ctypes.c_longlong, i, ctypes.c_double, p, ctypes.c_longlong, p, p]
+
+
+def test_loader_refuses_unsupported_types():
+    with pytest.raises(adcensus.AdcensusError, match="mccnn_x: unsupported C type 'short'"):
+        adcensus.prototypes("/* int mccnn_y(int a); */\nint mccnn_x(int a,\n            short b);\n")
+    with pytest.raises(adcensus.AdcensusError, match="adcensus_u: unsupported C type 'unsigned'"):
+        adcensus.prototypes("unsigned adcensus_u(void);")
+    got = adcensus.prototypes("/* int mccnn_y(float a); */\n#define X(a) a\nvoid mccnn_z(const float *const *a,\n  long long n);")
+    assert got == {"mccnn_z": (None, [ctypes.c_void_p, ctypes.c_longlong])}
+
+
 def test_version(lib):
     assert "sm_90a" in adcensus.version()
 
@@ -64,7 +106,6 @@ def test_round2_entry_points_reject_bad_arguments_without_a_gpu(lib):
     kernels are not built for -- all decided before the first CUDA call"""
     h = ctypes.c_void_p()
     arr = (ctypes.c_void_p * 5)(*[16] * 5)
-    lib.mccnn_scorer_head_create.restype = lib.mccnn_feature_tower_create.restype = ctypes.c_int
     sh = lambda fm, nh2, l2, W=arr, b=arr: lib.mccnn_scorer_head_create(ctypes.byref(h), fm, nh2, l2, W, b, 0, None)
     assert sh(112, 384, 3, None) == -1 and sh(112, 384, 3, arr, None) == -1
     assert lib.mccnn_scorer_head_create(None, 112, 384, 3, arr, arr, 0, None) == -1

@@ -1,7 +1,6 @@
 """Time one CBCA iteration at the bench size on pitched volumes (L2 flushed between launches):
 constant-work TMA kernel vs the exact kernel.  Prints ms and GB/s of the algorithmic 2V + 32HW bytes."""
 import argparse
-import ctypes
 import os
 import sys
 
@@ -35,7 +34,6 @@ ds = torch.arange(D, device=dev)[:, None, None]
 vin[(xs < ds).expand(D, H, ld)] = float("nan")
 vout = torch.empty_like(vin)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-vp = lambda t: ctypes.c_void_p(t.data_ptr())
 s = adcensus._stream(vin)
 
 
@@ -56,10 +54,12 @@ def timeit(fn):
 
 
 bytes_alg = 2 * 4 * D * H * W + 32 * H * W
-med, mn = timeit(lambda: lib.mccnn_cbca_fast_pitched(vp(x0c), vp(x1c), vp(vin), vp(vout), D, H, W, ld, -1, max(a.L1, 2), s))
+med, mn = timeit(lambda: lib.mccnn_cbca_fast_pitched(x0c.data_ptr(), x1c.data_ptr(), vin.data_ptr(), vout.data_ptr(), D, H, W, ld,
+                                                     -1, max(a.L1, 2), s))
 print("cbca_tma   L1=%d: median %.4f ms  min %.4f ms  %.0f GB/s (algorithmic)" % (a.L1, med, mn, bytes_alg / med / 1e6))
 if ld == W or True:
     vc = vin[:, :, :W].contiguous()[None]
     oc = torch.empty_like(vc)
-    med, mn = timeit(lambda: lib.adcensus_cbca_ex(vp(x0c), vp(x1c), vp(vc), vp(oc), D, H, W, -1, max(a.L1, 2), s))
+    med, mn = timeit(lambda: lib.adcensus_cbca_ex(x0c.data_ptr(), x1c.data_ptr(), vc.data_ptr(), oc.data_ptr(), D, H, W, -1,
+                                                  max(a.L1, 2), s))
     print("cbca exact L1=%d: median %.4f ms  min %.4f ms  %.0f GB/s (algorithmic)" % (a.L1, med, mn, bytes_alg / med / 1e6))

@@ -1,7 +1,6 @@
 """Time StereoJoin at the bench size (L2 flushed between launches): the pitched form the fused pipeline runs vs the operator
 on contiguous tensors."""
 import argparse
-import ctypes
 import os
 import sys
 
@@ -30,7 +29,6 @@ oR = torch.empty((D, H, ld), device=dev)
 cL = torch.empty((1, D, H, W), device=dev)
 cR = torch.empty((1, D, H, W), device=dev)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-vp = lambda t: ctypes.c_void_p(t.data_ptr())
 s = adcensus._stream(fL)
 
 
@@ -52,7 +50,8 @@ def timeit(fn):
 
 valid = 4 * H * (D * W - D * (D - 1) // 2)
 bytes_alg = 2 * 4 * C * H * W + 2 * valid
-med, mn = timeit(lambda: lib.mccnn_stereo_join_pitched(vp(fL), vp(fR), vp(oL), vp(oR), C, D, H, W, ld, s))
+med, mn = timeit(lambda: lib.mccnn_stereo_join_pitched(fL.data_ptr(), fR.data_ptr(), oL.data_ptr(), oR.data_ptr(), C, D, H, W,
+                                                       ld, s))
 print("StereoJoin pitched : median %.4f ms  min %.4f ms  %.0f GB/s (algorithmic 2F + 2 valid)" % (med, mn, bytes_alg / med / 1e6))
-med, mn = timeit(lambda: lib.adcensus_StereoJoin(vp(fL), vp(fR), vp(cL), vp(cR), C, D, H, W, s))
+med, mn = timeit(lambda: lib.adcensus_StereoJoin(fL.data_ptr(), fR.data_ptr(), cL.data_ptr(), cR.data_ptr(), C, D, H, W, s))
 print("StereoJoin operator: median %.4f ms  min %.4f ms  %.0f GB/s (algorithmic 2F + 2 valid)" % (med, mn, bytes_alg / med / 1e6))
