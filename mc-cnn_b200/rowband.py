@@ -24,9 +24,17 @@ from BASELINE.json's wording:
 
 The operators are injected (``ops``), so the same driver runs on the CUDA library (CudaOps) and,
 in the CPU tests, on any object with the same methods over CPU tensors.
+
+Where a band's cost volumes come from (:func:`band_source`): :func:`stereo_predict_rowband` takes the replicated
+'fast' features; :func:`band_predict` / :func:`predict_pair` start from the two standardised images, replicated, and run
+the feature tower (and the 'slow' scorer head) or census / AD on the band's rows only.  The 'fast', 'ad' and 'census'
+volumes are cheap, so they cover the extended band of the first CBCA block as above.  The 'slow' head dominates the
+pair's time, so each pixel is scored on exactly one rank and the first block exchanges its halo rows like the second.
 """
 import math
+import os
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -98,6 +106,17 @@ class Comm:
         self.exchange(sends, recvs)
         return top, bot
 
+    def barrier(self):
+        if self.on:
+            dist.barrier()
+
+
+def _refuse_stage_options(opt):
+    for k in ("sm_terminate", "sm_skip"):
+        if getattr(opt, k, 0):
+            raise ValueError("row-band stereo_predict runs the full chain only: -%s is not supported (use the "
+                             "single-GPU pipeline)" % k)
+
 
 def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chunks=None):
     """main.lua:929-1082 (arch 'fast') with the rows of one pair split over the ranks of `comm`.
@@ -107,17 +126,109 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
     least 32 columns each).  Returns the full (H,W) disparity map on every rank.  Only the full chain: parameters with
     ``sm_terminate`` / ``sm_skip`` set are refused before any work (run them on one GPU through the fused pipeline).
     """
-    for k in ("sm_terminate", "sm_skip"):
-        if getattr(opt, k, 0):
-            raise ValueError("row-band stereo_predict runs the full chain only: -%s is not supported (use the "
-                             "single-GPU pipeline)" % k)
+    _refuse_stage_options(opt)
+
+    def join(a, b, dirs):
+        volL, volR = ops.stereo_join(featL[:, a:b].contiguous(), featR[:, a:b].contiguous(), D)   # :946-947
+        ops.fix_border(volL, opt.border, -1)                                                     # :948
+        ops.fix_border(volR, opt.border, 1)                                                      # :949
+        return volL, volR
+
+    return band_chain(ops, join, True, imgL, imgR, D, opt, comm, chunks)
+
+
+def band_source(ops, x_batch, D, opt, arch, tower=None, head=None):
+    """The cost volumes of image rows [a, b) of one pair, as main.lua:929-981 holds them at :986 (NaN fill, fix_border
+    applied), without computing the volumes of any other row.
+
+    x_batch (2,1,H,W): the two standardised images (left, right), whole.  arch 'fast' / 'slow' take `tower` (an object
+    with ``forward((2,1,h,W)) -> (2,fm,h,W)`` and ``l1`` 3x3 layers: :class:`feature_tower.FeatureTower`) and for 'slow'
+    `head` (``volumes(fL, fR, D, want_left=, want_right=)``: :class:`scorer_head.ScorerHead`).  The tower runs on the rows
+    [a - l1, b + l1) and keeps [a, b): every pixel it keeps is then as far from the crop's zero padding as the tower
+    reaches; census / AD (9 x 9 windows) likewise run on [a - 4, b + 4).
+
+    Returns (volumes, extends): volumes(a, b, dirs) -> (volL, volR), each (D, b - a, W) or None when its direction
+    (-1 left, 1 right) is not in `dirs` and skipping it saves work; `extends` says whether the volumes of a row are cheap
+    enough to compute again on the neighbouring bands ('fast', 'ad', 'census': the first CBCA block then runs on the
+    extended band) or not ('slow': every row is scored by exactly one rank, the first block exchanges halo rows)."""
+    H = x_batch.shape[2]
+
+    def rows(a, b, m):
+        """image rows [a - m, b + m) clipped to the image, and where row a lies in them"""
+        a0, b0 = max(0, a - m), min(H, b + m)
+        return x_batch[:, :, a0:b0].contiguous(), a - a0
+
+    if arch in ("ad", "census"):
+        cost = ops.census if arch == "census" else ops.ad
+
+        def volumes(a, b, dirs):
+            x, o = rows(a, b, 4)
+            vl = cost(x[0], x[1], D, -1)[:, o:o + b - a].contiguous() if -1 in dirs else None   # :934 / :940
+            vr = cost(x[1], x[0], D, 1)[:, o:o + b - a].contiguous() if 1 in dirs else None     # :935 / :941
+            return vl, vr
+
+        return volumes, True
+    if arch not in ("fast", "slow"):
+        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
+    if tower is None or (arch == "slow" and head is None):
+        raise ValueError("arch '%s' needs the feature tower%s" % (arch, " and the scorer head" if arch == "slow" else ""))
+
+    def volumes(a, b, dirs):
+        x, o = rows(a, b, int(tower.l1))
+        f = tower.forward(x)                                                                  # :944 / :957
+        fL, fR = f[0, :, o:o + b - a].contiguous(), f[1, :, o:o + b - a].contiguous()
+        del f
+        if arch == "fast":
+            vl, vr = ops.stereo_join(fL, fR, D)                                               # :946-947
+        else:
+            vl, vr = head.volumes(fL, fR, D, want_left=-1 in dirs, want_right=1 in dirs)      # :962-979
+            vl, vr = (v[0] if v is not None else None for v in (vl, vr))
+        if vl is not None:
+            ops.fix_border(vl, opt.border, -1)                                                # :948 / :981
+        if vr is not None:
+            ops.fix_border(vr, opt.border, 1)
+        return vl, vr
+
+    return volumes, arch == "fast"
+
+
+def band_predict(ops, x_batch, D, opt, arch, tower=None, head=None, comm=None, chunks=None, want_vols=False):
+    """main.lua:929-1082 for any architecture, from the standardised images (2,1,H,W) (whole, on every rank) with the rows
+    split over the ranks of `comm`: each rank computes the cost volumes of its own band only (:func:`band_source`).
+
+    Returns the full (H,W) disparity map on every rank; with `want_vols` also this rank's rows [y0, y1) = split(H, N, r) of
+    the left and right volumes after the chain (D, y1 - y0, W), both directions computed even without the LR check, as
+    main.lua's -a predict writes both (main.lua:1042-1047)."""
+    _refuse_stage_options(opt)
+    volumes, extends = band_source(ops, x_batch, D, opt, arch, tower, head)
+    return band_chain(ops, volumes, extends, x_batch[0, 0], x_batch[1, 0], D, opt, comm, chunks, want_vols)
+
+
+def cbca_halo(opt):
+    """(max_arm, halo): the longest cross arm max(L1, 2), and the rows one CBCA iteration reaches into a neighbouring band
+    (0 without CBCA)"""
+    max_arm = max(int(opt.L1), 2)
+    return max_arm, (max_arm - 1 if (opt.cbca_i1 + opt.cbca_i2) > 0 else 0)
+
+
+def source_rows(H, world, rank, opt, extends):
+    """[ya, yb): the rows whose cost volumes rank `rank` of `world` computes -- its band split(H, world, rank), extended by
+    cbca_i1 * halo rows on either side (clipped to the image) when the volume source `extends`"""
+    y0, y1 = split(H, world, rank)
+    e1 = cbca_halo(opt)[1] * int(opt.cbca_i1) if extends else 0
+    return max(0, y0 - e1), min(H, y1 + e1)
+
+
+def band_chain(ops, volumes, extends, imgL, imgR, D, opt, comm=None, chunks=None, want_vols=False):
+    """The chain of main.lua:986-1082 on this rank's band from `volumes(a, b, dirs)` (see :func:`band_source`).  With
+    `extends` the first CBCA block runs on the band extended by cbca_i1 * halo rows, whose volumes are computed here too;
+    otherwise on the band itself, with the halo rows exchanged with the neighbours."""
     comm = comm or Comm()
     H, W = imgL.shape
     N, r = comm.world, comm.rank
     y0, y1 = split(H, N, r)
     Hb = y1 - y0
-    max_arm = max(int(opt.L1), 2)
-    halo = max_arm - 1 if (opt.cbca_i1 + opt.cbca_i2) > 0 else 0
+    max_arm, halo = cbca_halo(opt)
     band_min = min(split(H, N, p)[1] - split(H, N, p)[0] for p in range(N))
     if N > 1:
         assert band_min >= max(halo, 1), "bands thinner than the CBCA halo"
@@ -126,12 +237,12 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
     # costs (N - 1 + K) chunk times: K = N is the measured sweet spot (K = 4 N made 39 hops of 94 columns at Middlebury size)
     K = chunks if chunks else max(1, min(N, W // 32)) if N > 1 else 1
 
-    # first CBCA block on the band extended by cbca_i1 * halo rows: StereoJoin covers the extension (features are replicated)
-    e1 = halo * int(opt.cbca_i1)
-    ya, yb = max(0, y0 - e1), min(H, y1 + e1)
-    volL, volR = ops.stereo_join(featL[:, ya:yb].contiguous(), featR[:, ya:yb].contiguous(), D)     # :946-947
-    ops.fix_border(volL, opt.border, -1)                                                             # :948
-    ops.fix_border(volR, opt.border, 1)                                                              # :949
+    # first CBCA block on the band extended by cbca_i1 * halo rows when the volume source covers the extension (features or
+    # images are replicated), else on the band with an exchange
+    ya, yb = source_rows(H, N, r, opt, extends)
+    # main.lua:954-955: without the LR check (mb) only direction -1 is consumed, unless the volumes are asked for
+    dirs = (1, -1) if (opt.lr_check or want_vols) else (-1,)
+    src = dict(zip((-1, 1), volumes(ya, yb, dirs)))                                                  # :929-981
     x0c = ops.cross(imgL, opt.L1, opt.tau1)                                                          # :995 (full image)
     x1c = ops.cross(imgR, opt.L1, opt.tau1)                                                          # :996
 
@@ -183,12 +294,15 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
                 comm.send(st_out[xa:xb], nxt)
 
     disp = {}
-    vol_left = None
-    # main.lua:954-955: without the LR check (mb) only direction -1 is consumed
-    for direction in ((1, -1) if opt.lr_check else (-1,)):                                           # :955
-        ext = volL if direction == -1 else volR                                                      # :986
-        ext = cbca_block(ext, ya, yb, int(opt.cbca_i1), direction)                                   # :998-1001
-        vol = ext[:, y0 - ya: y0 - ya + Hb].contiguous() if (ya != y0 or yb != y1) else ext
+    band_vols = {}
+    for direction in dirs:                                                                           # :955
+        ext = src.pop(direction)                                                                     # :986
+        if extends:
+            ext = cbca_block(ext, ya, yb, int(opt.cbca_i1), direction)                               # :998-1001
+            vol = ext[:, y0 - ya: y0 - ya + Hb].contiguous() if (ya != y0 or yb != y1) else ext
+        else:
+            vol = cbca_exchanging(ext, int(opt.cbca_i1), direction)
+        del ext
         for _ in range(opt.sgm_i):                                                                   # :1008-1020
             tab = ops.sgm_tables(imgL, imgR, D, opt, direction)
             cost = ops.to_hwd(vol)                                                                   # (Hb, W, D)
@@ -199,8 +313,9 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
             vol = ops.from_hwd_div4(acc)                                                             # :1017-1020
         vol = cbca_exchanging(vol, int(opt.cbca_i2), direction)                                      # :1035-1038
         disp[direction] = comm.all_gather_rows(ops.argmin(vol), H)                                   # :1049-1050
-        if direction == -1:
-            vol_left = vol
+        if want_vols or direction == -1:
+            band_vols[direction] = vol
+    vol_left = band_vols[-1]
 
     d = disp[-1]
     if opt.lr_check:                                                                                 # :1054-1066
@@ -219,7 +334,8 @@ def stereo_predict_rowband(ops, featL, featR, imgL, imgR, D, opt, comm=None, chu
 
     d = band_filter(lambda t: ops.median2d(t, 5), d, 2)                                              # :1073
     kr = int(math.ceil(float(opt.blur_sigma) * 3))                                                   # main.lua:529: kernel radius
-    return band_filter(lambda t: ops.mean2d(t, opt.blur_sigma, opt.blur_t), d, kr)                   # :1078
+    d = band_filter(lambda t: ops.mean2d(t, opt.blur_sigma, opt.blur_t), d, kr)                      # :1078
+    return (d, band_vols[-1], band_vols[1]) if want_vols else d
 
 
 class CudaOps:
@@ -241,6 +357,25 @@ class CudaOps:
         from . import adcensus
 
         adcensus.fix_border(vol[None], n, direction)
+
+    def _image_cost(self, fn, x0, x1, D, direction):
+        """x0, x1 (nch, h, W) -> the (D, h, W) volume of adcensus.ad / census on a NaN-filled tensor (main.lua:933-941)"""
+        from . import adcensus
+
+        out = torch.empty((1, D) + tuple(x0.shape[1:]), device=x0.device, dtype=torch.float32)
+        adcensus.fill_nan(out)
+        fn(x0[None].contiguous(), x1[None].contiguous(), out, direction)
+        return out[0]
+
+    def ad(self, x0, x1, D, direction):
+        from . import adcensus
+
+        return self._image_cost(adcensus.ad, x0, x1, D, direction)
+
+    def census(self, x0, x1, D, direction):
+        from . import adcensus
+
+        return self._image_cost(adcensus.census, x0, x1, D, direction)
 
     def cross(self, img, L1, tau1):
         from . import adcensus
@@ -354,3 +489,90 @@ class CudaOps:
         from . import adcensus
 
         return adcensus.mean2d(d[None, None].contiguous(), adcensus.gaussian(sigma).to(d.device), t)[0, 0]
+
+
+def write_outputs(out_dir, disp, volL, volR, comm=None):
+    """right.bin and left.bin ((1, D, H, W) raw little-endian fp32, main.lua:1042-1047) and disp.bin ((1, 1, H, W), :1103)
+    from what each rank holds: `disp` (H, W), the same on every rank, and this rank's rows [y0, y1) of the two volumes
+    (D, y1 - y0, W).  Rank 0 creates the files at their full size; then every rank writes its rows of each disparity plane
+    at their offsets (D writes of (y1 - y0) x W floats per volume).  No volume crosses a GPU: each rank copies its own band
+    to the host and nothing else.  The ranks must share `out_dir` (one node, or a shared file system)."""
+    comm = comm or Comm()
+    H, W = disp.shape
+    D = volL.shape[0]
+    y0, y1 = split(H, comm.world, comm.rank)
+    files = (("right.bin", volR), ("left.bin", volL))                  # direction 1 comes first
+    if comm.rank == 0:
+        os.makedirs(out_dir, exist_ok=True)
+        for name, _ in files:
+            with open(os.path.join(out_dir, name), "wb") as f:
+                f.truncate(D * H * W * 4)
+    comm.barrier()
+    for name, v in files:
+        a = np.ascontiguousarray(v.cpu().numpy() if isinstance(v, torch.Tensor) else v, dtype="<f4")
+        assert a.shape == (D, y1 - y0, W), "volume rows %s, expected %s" % (a.shape, (D, y1 - y0, W))
+        fd = os.open(os.path.join(out_dir, name), os.O_WRONLY)
+        try:
+            for d in range(D):
+                os.pwrite(fd, a[d].tobytes(), (d * H + y0) * W * 4)
+        finally:
+            os.close(fd)
+    if comm.rank == 0:
+        d = np.ascontiguousarray(disp.cpu().numpy() if isinstance(disp, torch.Tensor) else disp, dtype="<f4")
+        d.tofile(os.path.join(out_dir, "disp.bin"))
+    comm.barrier()
+
+
+def predict_pair(left=None, right=None, dataset="kitti", arch="census", disp_max=70, x_batch=None, net_fname=None,
+                 tower=None, head=None, comm=None, device=None, out_dir=None, want_vols=False, chunks=None, **overrides):
+    """``main.lua <dataset> <arch> -a predict`` (:func:`frontend.predict`) with the rows of the pair split over the ranks of
+    `comm`, one GPU per rank (`device`: a torch.device or index, default the current device).
+
+    The pair: the image files (or arrays) `left` / `right`, standardised on every rank as :func:`frontend.make_batch` does,
+    or the standardised batch `x_batch` (2,1,H,W).  arch 'fast' / 'slow' take the network from `net_fname` (the reference's
+    ascii .t7), or the stages `tower` (and for 'slow' `head`) built on this rank's device; 'ad' / 'census' need neither.
+    `overrides` are the stereo method's options (pipeline.make_params); -sm_terminate / -sm_skip are refused.
+
+    With `out_dir`, writes right.bin, left.bin and disp.bin there (:func:`write_outputs`): the bytes frontend.predict writes
+    for the same images, dataset, arch, network, disp_max and overrides.  Returns the disparity map (H, W) float32 numpy on
+    every rank; with `want_vols` also this rank's rows of the left and right volumes, (D, y1 - y0, W) device tensors.
+    Every check on the arguments and the network file is made before any GPU work."""
+    from . import frontend, pipeline
+
+    if arch not in ("fast", "slow", "ad", "census"):
+        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
+    opt = pipeline.make_params(dataset, arch, **overrides)
+    _refuse_stage_options(opt)
+    net = None
+    if arch in ("fast", "slow") and tower is None:
+        if net_fname is None:
+            raise ValueError("arch '%s' needs -net_fname (or the stage objects `tower` / `head`)" % arch)
+        net = frontend.load_net(net_fname, arch)                                     # main.lua:893-901
+    elif arch == "slow" and head is None:
+        raise ValueError("arch 'slow' needs the scorer head with the feature tower")
+    if x_batch is None:
+        x_batch = frontend.make_batch(left, right)                                   # main.lua:1085-1100
+    D = int(disp_max)
+    dev = device if isinstance(device, torch.device) else \
+        torch.device("cuda", torch.cuda.current_device() if device is None else device)
+    comm = comm or Comm()
+    with torch.cuda.device(dev):
+        xb = torch.as_tensor(x_batch, dtype=torch.float32).to(dev).contiguous()
+        if xb.dim() != 4 or xb.shape[:2] != (2, 1):
+            raise ValueError("x_batch: (2, 1, H, W) expected, got %s" % (tuple(xb.shape),))
+        own = net is not None
+        if own:
+            tower, head = frontend.make_stages(net, dev)
+        try:
+            vols = want_vols or out_dir is not None
+            out = band_predict(CudaOps(dev), xb, D, opt, arch, tower, head, comm, chunks, want_vols=vols)
+            disp, volL, volR = out if vols else (out, None, None)
+        finally:
+            if own:
+                tower.close()
+                if head is not None:
+                    head.close()
+        disp_h = disp.cpu().numpy()
+        if out_dir is not None:
+            write_outputs(out_dir, disp_h, volL, volR, comm)
+    return (disp_h, volL, volR) if want_vols else disp_h
