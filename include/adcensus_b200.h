@@ -557,6 +557,38 @@ int mccnn_randperm_swaps(long long *perm, long long n, long long i0, const unsig
 int mccnn_mb_sample_starts(const unsigned *raw, long long n_raw, int base, double d_exp, long long *starts, long long cap,
 			   long long *count, long long *used);
 
+/* ---- images of the results: samples/bin2png.lua and main.lua -debug (csrc/render.cu, render.py) ----------------------
+ * Every output is 8-bit, quantised as Torch7's image.save writes a float image: clamp to [0, 1] (NaN -> 0, as x86's
+ * conversion gives), times 255 in double, truncated.  Grey images are (H, W) bytes, colour images (H, W, 3) R, G, B
+ * bytes, both in the PNG's pixel order.  Input maps are DEVICE float32 (H, W). */
+
+#define ADCENSUS_ERANGE (-3)   /* mccnn_render_jet: an input whose colour-map value is NaN or outside [-0.1, 4.1] */
+#define ADCENSUS_EIO (-4)      /* mccnn_render_volume_file: the file cannot be opened or is shorter than D * H * W floats */
+
+/* bin2png.lua:17-24 for a (D, H, W) float32 little-endian volume FILE (left.bin / right.bin): NaN -> 1e38 (fromfile),
+ * the 1-based arg-min over D keeping the first index on ties (TH's CPU min), divided by D in fp32, quantised into grey
+ * (H, W) DEVICE bytes.  The volume is read in row chunks of at most 64 MiB through two pinned host buffers, each chunk's
+ * copy overlapping the previous chunk's kernel; neither the host nor the device ever holds it whole.  Returns once the
+ * file has been read; grey is complete in `stream`'s order.  D, H, W >= 1 and H * W < 2^31 (else ADCENSUS_EINVAL). */
+int mccnn_render_volume_file(const char *path, int D, int H, int W, unsigned char *grey, adcensus_stream_t stream);
+
+/* bin2png.lua:27-28: grey = quantise(f32(x) / d) with NaN -> 1e38 first (fromfile), for a map x (H, W). */
+int mccnn_render_map(const float *x, int H, int W, int d, unsigned char *grey, adcensus_stream_t stream);
+
+/* adcensus.grey2jet (adcensus.cu:2001-2053) of the map as main.lua:1242 / 1260 give it: v = ((double)x + 1) / disp_max * 4
+ * in double, the five bands with the reference's comparisons, rgb (H, W, 3) = the quantised colours.  mask_blue != 0
+ * multiplies the blue channel by (x != 0) before quantising (main.lua:1261, the ground-truth image).  The reference asserts
+ * on a value outside the bands; here the kernel raises a device flag, the call waits for `stream` and returns
+ * ADCENSUS_ERANGE (rgb is then written, with black at the refused pixels).  disp_max >= 1. */
+int mccnn_render_jet(const float *x, int H, int W, int disp_max, int mask_blue, unsigned char *rgb, adcensus_stream_t stream);
+
+/* main.lua:1243-1252 in fp32 as the cutorch ops compute it: grey = x0 * 50 + 150, then div(255), which cutorch performs as a
+ * multiplication by f32(1 / 255); mask = gt != 0, bad = (|gt - pred| > err_at) * mask, good = (|gt - pred| <= err_at) * mask;
+ * R = grey + 0.5 bad - 0.5 good, G = grey - 0.5 bad + 0.5 good, B = grey - 0.5 bad - 0.5 good (each term added in that
+ * order), quantised into rgb (H, W, 3).  x0, pred and gt are (H, W). */
+int mccnn_render_error(const float *x0, const float *pred, const float *gt, int H, int W, float err_at, unsigned char *rgb,
+		       adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,7 +87,8 @@ def _check(rc, what):
         return
     if rc > 0:
         raise AdcensusError("%s: CUDA error %d" % (what, rc))
-    raise AdcensusError("%s: %s" % (what, {-1: "invalid argument", -2: "size limit exceeded"}.get(rc, "error %d" % rc)))
+    raise AdcensusError("%s: %s" % (what, {-1: "invalid argument", -2: "size limit exceeded", -3: "value out of range",
+                                           -4: "file cannot be read"}.get(rc, "error %d" % rc)))
 
 
 def _t(x, narg, name, optional=False):

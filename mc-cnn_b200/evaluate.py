@@ -22,7 +22,8 @@ Deliberate deviations from main.lua:
 * n_te is ``len(x0) - len(dispnoc)`` instead of the constant 195 / 200 (preprocess_kitti.lua writes dispnoc for the
   training rows only, so on real data the two agree), and KITTI's H and W come from x0's shape;
 * ``-at 1`` (the combined 2012 + 2015 loader, used for training), ``-color rgb``, ``-debug`` and ``-use_cache`` /
-  ``-make_cache`` are refused (none changes the default result);
+  ``-make_cache`` are refused (none changes the default result); -debug's images come from ``test(..., debug_dir=...)``
+  (tools/debug_images.py) instead;
 * ``-sm_terminate`` / ``-sm_skip`` (``Evaluator(..., sm_skip="sgm")``) accept only the step names main.lua tests
   (:data:`pipeline.SM_TERMINATE`, :data:`pipeline.SM_SKIP`); main.lua ignores any other name and runs the full chain.
   :func:`check_options` does not see the architecture and refuses both; :func:`check_stage_options`, which the command
@@ -66,7 +67,10 @@ def check_options(dataset, at=0, color="gray", debug=False, use_cache=False, mak
                          "matters for training")
     if color != "gray":
         raise ValueError("-color %s is not supported: only grey Middlebury sets (-color gray) are" % color)
-    for name, v in (("-debug", debug), ("-use_cache", use_cache), ("-make_cache", make_cache)):
+    if debug:
+        raise ValueError("-debug is not supported: write its images with tools/debug_images.py (Evaluator.test(debug_dir=...)); "
+                         "its other effect, saving the net after every training epoch (main.lua:877), is not implemented")
+    for name, v in (("-use_cache", use_cache), ("-make_cache", make_cache)):
         if v:
             raise ValueError("%s is not supported" % name)
     # which steps exist depends on the architecture and its parameters, which this check does not see
@@ -275,8 +279,10 @@ class Evaluator:
             pred, runtime = self.timed(x_batch, disp_max)
             yield ex, id_, runtime, pred.cpu().numpy(), img_height, img_width
 
-    def test(self, action="test_te", data_root=".", data=None, rect="imperfect", color="gray", verbose=True):
-        """``-a test_te`` / ``-a test_all``: per example ``runtime\\terr`` and the mean bad-pixel rate (main.lua:1224-1238, 1292)"""
+    def test(self, action="test_te", data_root=".", data=None, rect="imperfect", color="gray", verbose=True, debug_dir=None):
+        """``-a test_te`` / ``-a test_all``: per example ``runtime\\terr`` and the mean bad-pixel rate (main.lua:1224-1238, 1292).
+        With `debug_dir`, each example's images of main.lua -debug are written there after its timed region
+        (main.lua:1240-1265, :func:`render.write_debug_images`)."""
         if action not in ("test_te", "test_all"):
             raise ValueError("test() runs test_te or test_all, not %r" % (action,))
         data = data or load_data(self.dataset, data_root, rect, color)
@@ -285,10 +291,17 @@ class Evaluator:
         for ex, id_, runtime, pred, _, img_width in self._loop(data, data.examples(action)):
             if np.isnan(pred).any():                                                            # main.lua:1224
                 raise ValueError("example %s: the prediction contains NaN" % (id_,))
-            err = dataio.bad_pixel_rate(pred, data.ground_truth(ex, img_width), err_at)
+            gt = data.ground_truth(ex, img_width)
+            err = dataio.bad_pixel_rate(pred, gt, err_at)
             out.append((ex, id_, runtime, err))
             if verbose:
                 print("%s\t%s" % (lua_num(runtime), lua_num(err)), flush=True)
+            if debug_dir is not None:
+                from . import render
+
+                x, disp_max = data.example(ex)[:2]
+                render.write_debug_images(debug_dir, self.dataset, self.arch, id_, x[0, 0], pred, gt, disp_max, err_at,
+                                          device=self.dev)
         mean = sum(e[3] for e in out) / len(out) if out else float("nan")
         if verbose:
             print(lua_num(mean), flush=True)
