@@ -589,6 +589,39 @@ int mccnn_render_jet(const float *x, int H, int W, int disp_max, int mask_blue, 
 int mccnn_render_error(const float *x0, const float *pred, const float *gt, int H, int W, float err_at, unsigned char *rgb,
 		       adcensus_stream_t stream);
 
+/* ---- the KITTI 2012 / 2015 devkits' stereo metrics (csrc/kitti_eval.cu, kitti_eval.py) ---------------------------------
+ * One estimate against its two PNG16 ground truths (disp_noc* and disp_occ*, uint16 disparity * 256, 0 = none) and, for
+ * KITTI 2015, its obj_map (8-bit, 0 = background, else foreground), restated from the devkits' description (DESIGN.md §17;
+ * parity with the devkit binaries is not pinned).
+ *
+ * The estimate is either a float map `disp` (quantised as dataio.write_png16 writes it: v = d < 1e-5 ? 0 : d * 256 in fp32,
+ * truncated, clamped to [0, 65535], NaN -> 0) or the stored values `disp16`; exactly one of them is non-NULL.  v == 0 is
+ * invalid (-1), else d = v / 256.  Then interpolateBackground: each row's interior runs of invalid pixels take the smaller
+ * of their two valid neighbours, the pixels before the row's first valid pixel its value, those after its last valid pixel
+ * its value; then the rows above the first row with a valid pixel take that row, those below the last such row that row;
+ * whatever is left stays -1.  `ipol` (H, W) receives that map when non-NULL.
+ *
+ * Over the pixels with ground truth, e = |gt / 256 - ipol| in fp32; per region r (0 = noc, 1 = all, i.e. occ) the int64
+ * counts[r * MCCNN_KITTI_NCOUNT + k] below, and sums[r] = sum of e in float64, reduced in a fixed order (the same bits on
+ * every run).  D1 bad: e > 3 and e / (gt / 256) > 0.05f (fp32 divide).  obj_map NULL: every pixel is background.  DEVICE
+ * pointers; counts and sums are overwritten.  H, W >= 1, H * W < 2^31 (else ADCENSUS_EINVAL / ADCENSUS_ELIMIT). */
+enum {
+	MCCNN_KITTI_GT,          /* pixels with ground truth */
+	MCCNN_KITTI_DENSE,       /* ... whose estimate was valid before the interpolation (density's numerator) */
+	MCCNN_KITTI_OUT2,        /* ... with e > 2 */
+	MCCNN_KITTI_OUT3,        /* e > 3 */
+	MCCNN_KITTI_OUT4,        /* e > 4 */
+	MCCNN_KITTI_OUT5,        /* e > 5 */
+	MCCNN_KITTI_D1_BG,       /* D1-bad background pixels */
+	MCCNN_KITTI_D1_FG,       /* D1-bad foreground pixels */
+	MCCNN_KITTI_GT_BG,       /* background pixels with ground truth */
+	MCCNN_KITTI_GT_FG,       /* foreground pixels with ground truth */
+	MCCNN_KITTI_NCOUNT
+};
+int mccnn_kitti_devkit_counts(const float *disp, const unsigned short *disp16, const unsigned short *gt_noc,
+			      const unsigned short *gt_occ, const unsigned char *obj_map, int H, int W, float *ipol,
+			      long long *counts, double *sums, adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -165,6 +165,42 @@ def write_kitti_raw(root, dataset="kitti", n_tr=41, n_te=2, H=375, widths=(1242,
     return unzip
 
 
+def write_kitti_eval_maps(unzip, dataset="kitti", seed=0):
+    """The ground truth the devkits' metrics read besides disp_noc, next to a write_kitti_raw tree (`unzip` is what it
+    returned): ``training/disp_occ/`` (``disp_occ_0/`` for 'kitti2015') is disp_noc with its invalid pixels filled in
+    vertical bands (every third band of 37 columns, with disparities in [1, 64) quantised to 1/256), and for 'kitti2015'
+    ``training/obj_map/``, 8-bit, 0 (background) except a few random rectangles numbered 1, 2, ...  Returns the number of
+    pairs written."""
+    import os
+
+    from PIL import Image
+
+    from . import dataio
+
+    rgb = dataset == "kitti2015"
+    sub = os.path.join(unzip, "training")
+    noc_dir = os.path.join(sub, "disp_noc_0" if rgb else "disp_noc")
+    occ_dir = os.path.join(sub, "disp_occ_0" if rgb else "disp_occ")
+    os.makedirs(occ_dir, exist_ok=True)
+    if rgb:
+        os.makedirs(os.path.join(sub, "obj_map"), exist_ok=True)
+    rng = np.random.default_rng(seed)
+    names = sorted(os.listdir(noc_dir))
+    for name in names:
+        noc = dataio.read_png16_raw(os.path.join(noc_dir, name))
+        H, W = noc.shape
+        band = ((np.arange(W) // 37) % 3 == 0)[None, :] & (noc == 0)
+        occ = np.where(band, rng.integers(256, 64 * 256, (H, W)), noc).astype(np.uint16)
+        Image.fromarray(occ).save(os.path.join(occ_dir, name), format="PNG")
+        if rgb:
+            obj = np.zeros((H, W), np.uint8)
+            for k in range(1, 5):
+                y, x = int(rng.integers(0, H)), int(rng.integers(0, W))
+                obj[y:y + int(rng.integers(10, 120)), x:x + int(rng.integers(20, 300))] = k
+            Image.fromarray(obj, "L").save(os.path.join(sub, "obj_map", name), format="PNG")
+    return len(names)
+
+
 def write_mb_set(root, n=6, shapes=((40, 96, 24), (48, 130, 32)), seed=0, rect="imperfect", color="gray"):
     """A small seeded Middlebury set in preprocess_mb.py's layout under ``root/data.mb.<rect>_<color>``: per image k = 1..n
     x_<k>_1.bin (views, 1, H, W) (4 views for image 5, else 2) and dispnoc<k>.bin (H, W), meta.bin (n, 3) int32 (H, W,
