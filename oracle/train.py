@@ -176,19 +176,22 @@ def init_weights(g, l1, fm, n_in=1, ks=3):
     return out
 
 
-def step64(patches, layers, margin, pow_):
+def step64(patches, layers, margin, pow_, inter=False, device=None):
     """One forward / backward of net_tr + Margin2 in float64 autograd: patches (2 bs, 1, ws, ws); layers [(W, b)] ->
-    (loss, [(gW, gb)]) as float64 numpy"""
+    (loss, [(gW, gb)]) as float64 numpy.  With `inter`, a third item: a dict of float64 numpy arrays, "z" and "dz" (each
+    layer's convolution output, before its ReLU, and dLoss/dz), "norm" (N,), "normalized" (N, fm), "join" (bs,), "hinge"
+    (bs / 2,): the per-sample terms before the mean.  `device` is where torch computes (default the CPU)."""
     import torch
 
-    x = torch.as_tensor(np.asarray(patches), dtype=torch.float64)
+    x = torch.as_tensor(np.asarray(patches), dtype=torch.float64, device=device)
     ps = []
     for w, b in layers:
-        ps.append(torch.tensor(np.asarray(w, np.float64), requires_grad=True))
-        ps.append(torch.tensor(np.asarray(b, np.float64), requires_grad=True))
-    h = x
+        ps.append(torch.tensor(np.asarray(w, np.float64), requires_grad=True, device=device))
+        ps.append(torch.tensor(np.asarray(b, np.float64), requires_grad=True, device=device))
+    h, zs = x, []
     for i in range(len(layers)):
         h = torch.nn.functional.conv2d(h, ps[2 * i], ps[2 * i + 1])
+        zs.append(h)
         if i < len(layers) - 1:
             h = torch.relu(h)
     norm = (h * h).sum(1, keepdim=True) + 1e-5                  # Normalize2: x / sqrt(sum x^2 + 1e-5)
@@ -196,10 +199,16 @@ def step64(patches, layers, margin, pow_):
     s = (h[0::2] * h[1::2]).sum(1).reshape(-1)                 # StereoJoin1: (bs,)
     f = s[1::2] - s[0::2] + margin                             # Margin2: neg - pos + m
     f = torch.clamp(f, min=0)
-    loss = (f if pow_ == 1 else 0.5 * f * f).mean()
-    grads = torch.autograd.grad(loss, ps)
-    g = [t.numpy() for t in grads]
-    return float(loss.detach()), [(g[2 * i], g[2 * i + 1]) for i in range(len(layers))]
+    terms = f if pow_ == 1 else 0.5 * f * f
+    loss = terms.mean()
+    grads = torch.autograd.grad(loss, ps + (zs if inter else []))
+    g = [t.cpu().numpy() for t in grads]
+    out = float(loss.detach()), [(g[2 * i], g[2 * i + 1]) for i in range(len(layers))]
+    if not inter:
+        return out
+    np64 = lambda t: t.detach().cpu().numpy()
+    return out + (dict(z=[np64(t) for t in zs], dz=g[len(ps):], norm=np64(norm).reshape(-1),
+                       normalized=np64(h).reshape(len(h), -1), join=np64(s), hinge=np64(terms)),)
 
 
 def update32(p, v, g, mom, lr):
