@@ -622,6 +622,37 @@ int mccnn_kitti_devkit_counts(const float *disp, const unsigned short *disp16, c
 			      const unsigned short *gt_occ, const unsigned char *obj_map, int H, int W, float *ipol,
 			      long long *counts, double *sums, adcensus_stream_t stream);
 
+/* ---- the MiddEval3 SDK's evaldisp metrics (csrc/mb_eval.cu, mb_eval.py) -------------------------------------------------
+ * One map `disp` (h, w) against its ground truth `gt` (Hg, Wg), top-down rows, +inf = unknown, restated from the SDK's
+ * evaldisp (DESIGN.md §18; parity with the SDK binary and the website is not pinned).  scale = Wg / w must be 1, 2 or 4
+ * with Wg == scale w and Hg == scale h (else ADCENSUS_EINVAL); Hg * Wg < 2^31 (else ADCENSUS_ELIMIT).
+ *
+ * Per gt pixel (x, y) with gt != +inf, in fp32: d = (float)scale * disp[y / scale][x / scale]; valid when d != +inf; a
+ * valid d becomes max(0, min(maxd, d)) with maxd = (float)(scale * maxdisp), both as (a < b) ? a : b / (a > b) ? a : b (NaN
+ * stays NaN, -inf becomes 0); err = fabsf(d - gt).  Region 0 (nonocc) takes the pixels whose `mask` (Hg, Wg) byte is 255,
+ * every pixel when mask is NULL (evaldisp without a mask); region 1 (all) takes every pixel.
+ *
+ * Outputs, DEVICE pointers, overwritten: counts[r * MCCNN_MB_NCOUNT + k] int64; sums[2 r] = sum of err and sums[2 r + 1] =
+ * sum of (double)err^2 over the valid pixels, float64 in a fixed order (the same bits on every run); quantiles[4 r + j] the
+ * k-th smallest err over the valid pixels, k = ceil(q nvalid) for q = 0.50, 0.90, 0.95, 0.99 (exact, by radix select on
+ * the fp32 bits; NaN errs last), NaN when there is none.  `scratch` is a DEVICE buffer of MCCNN_MB_EVAL_SCRATCH_BYTES bytes,
+ * 8-byte aligned, that no other call uses until this one has run; nothing is allocated and nothing is read back.
+ * maxdisp >= 1. */
+#define MCCNN_MB_EVAL_SCRATCH_BYTES 49152
+enum {
+	MCCNN_MB_N,          /* pixels of the region with known ground truth */
+	MCCNN_MB_VALID,      /* ... whose d is not +inf */
+	MCCNN_MB_BAD05,      /* valid with err > 0.5 */
+	MCCNN_MB_BAD1,       /* err > 1 */
+	MCCNN_MB_BAD2,       /* err > 2 */
+	MCCNN_MB_BAD4,       /* err > 4 */
+	MCCNN_MB_INVALID,    /* ... whose d is +inf */
+	MCCNN_MB_NCOUNT
+};
+int mccnn_mb_evaldisp(const float *disp, int h, int w, const float *gt, int Hg, int Wg, const unsigned char *mask,
+		      int maxdisp, long long *counts, double *sums, float *quantiles, void *scratch,
+		      adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

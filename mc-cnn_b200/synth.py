@@ -377,3 +377,45 @@ def write_mb_raw(root, n2014=11, full=(80, 192), half_size=(40, 96), D=48, seed=
             save(rgb(views[0]), base, "im0.png")
             save(rgb(views[1]), base, "im1.png")
     return unzip
+
+
+def write_mb_eval_gt(unzip, seed=0):
+    """The MiddEval3 training ground truth as the SDK's MiddEval3-GT0-H.zip / -GT0-F.zip unpack it, next to a write_mb_raw
+    tree (`unzip` is what it returned): per ``MiddEval3/trainingH/<scene>`` of h x w views, ``disp0GT.pfm`` (rows
+    bottom-up; disparities in [0, ndisp) with inf holes) and ``mask0nocc.png`` (8-bit 0 where unknown, else 255 or, on
+    about a fifth of the pixels, 128), and the same at exactly 2h x 2w under ``MiddEval3/trainingF/<scene>`` (twice the
+    disparities of each half-size pixel's block, jittered by less than a pixel, with holes and masks of their own).
+    Returns the number of scenes written."""
+    import os
+    import re
+
+    from PIL import Image
+
+    from . import dataio
+
+    rng = np.random.default_rng(seed)
+    eval3 = os.path.join(unzip, "MiddEval3")
+    scenes = sorted(os.listdir(os.path.join(eval3, "trainingH")))
+
+    def write(sub, s, gt, mask):
+        base = os.path.join(eval3, sub, s)
+        os.makedirs(base, exist_ok=True)
+        dataio.write_pfm(np.flipud(gt.astype(np.float32)), os.path.join(base, "disp0GT.pfm"))
+        Image.fromarray(mask, "L").save(os.path.join(base, "mask0nocc.png"))
+
+    def holes_and_mask(gt, p_hole):
+        gt = np.where(rng.random(gt.shape) < p_hole, np.inf, gt).astype(np.float32)
+        mask = np.where(rng.random(gt.shape) < 0.2, 128, 255).astype(np.uint8)
+        return gt, np.where(np.isinf(gt), 0, mask).astype(np.uint8)
+
+    for s in scenes:
+        base = os.path.join(eval3, "trainingH", s)
+        with Image.open(os.path.join(base, "im0.png")) as im:
+            w, h = im.size
+        with open(os.path.join(base, "calib.txt")) as f:
+            ndisp = int(re.search("ndisp=(.*)", f.read()).group(1))
+        gt = rng.uniform(0, ndisp, (h, w)).astype(np.float32)
+        write("trainingH", s, *holes_and_mask(gt, 0.05))
+        full = np.kron(gt, np.ones((2, 2), np.float32)) * 2 + rng.uniform(-0.9, 0.9, (2 * h, 2 * w)).astype(np.float32)
+        write("trainingF", s, *holes_and_mask(np.maximum(full, 0), 0.08))
+    return len(scenes)
