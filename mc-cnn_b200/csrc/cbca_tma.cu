@@ -10,7 +10,7 @@
 // per iteration).  NOT bit-exact by construction: it serves the north star's 1e-4 bar for float aggregation
 // (measured ~1e-6 relative; prefixes are local to a 32 x 128 tile + halo, which bounds the cancellation).
 // The bit-exact kernels stay in cross_cbca.cu and remain selectable.
-// This first-generation kernel serves arms of 6 to 14 pixels (R = 8, 13); shorter arms go to cbca_ws.cu.
+// This first-generation kernel serves the longer arms, the second-generation cbca_ws_kernel below the shorter ones.
 //
 // Per CTA: a 32 x 128 pixel tile, a chunk of `dch` disparities.
 //   * the plane tile (+halo, zero-filled outside the image; its first column 16-byte aligned, which the TMA
@@ -316,18 +316,448 @@ int launch_tma(const CUtensorMap &tm, const uint32_t *hv, const float *vol, floa
 	       cudaStream_t s)
 {
 	using C = CTCfg<R>;
-	static bool attr_done[64] = {false};
-	int dev = 0;
-	cudaGetDevice(&dev);
-	if (!attr_done[dev & 63]) {
-		ADC_CUDA(cudaFuncSetAttribute(cbca_tma_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-		attr_done[dev & 63] = true;
-	}
+	if (int rc = adc_smem_optin(cbca_tma_kernel<R>, C::SMEM)) return rc;
 	const long HW = (long)H * W;
 	dim3 grid(adc_div_up(W, CT_TX), adc_div_up(H, CT_TY), adc_div_up(D, CT_DCH));
 	cbca_tma_kernel<R><<<grid, CT_NT, C::SMEM, s>>>(tm, hv, hv + 2 * HW, hv + HW, hv + 3 * HW, vol, out, D, H, W, ld, direction, CT_DCH);
 	ADC_CHECK_LAUNCH();
 	return 0;
+}
+
+// ------------------------------------------------------------------ second generation
+// Warp-specialised, three-stage TMA pipeline, running vertical sums in a per-thread ring.
+//
+// Same decomposition as cbca_tma_kernel -- the run of a support row depends on (d, row, column) only, so with I the
+// inclusive prefix of a tile row
+//     S(r, x) = I(r, x + R_ - 1) - I(r, x - L)          sum of the run (x - L, x + R_) of row r        (:362-369)
+//     out(y, x) = sum_{r = y-U+1}^{y+Dn-1} S(r, x) / sum of the run lengths                            (:361, :373)
+// -- but the work is split by ROLE instead of by phase:
+//   * one PRODUCER thread keeps three plane tiles in flight (cp.async.bulk.tensor.3d, one box of 144 x (64 + 2R + 1)
+//     floats per disparity, zero-filled outside the image) behind full / ready / empty mbarriers;
+//   * four PREFIX warps turn each landed tile into row prefixes in place: two tile rows per warp instruction
+//     (16 lanes x 9 consecutive columns each, bank-conflict free at the 144-float pitch), two such pairs interleaved
+//     (the scan is a chain of dependent adds and shuffles), a 4-step shuffle scan, centred on one value per tile (its
+//     mid pixel) so that |I| stays a random walk instead of growing with the mean (less cancellation in the differences);
+//   * eight WALKER warps: thread = (column, half of the 64 output rows).  A thread walks 32 + 2R tile rows once;
+//     per row one LDS of the right image's arms, one packed 16-bit minimum against its own column's arms (registers
+//     for the whole disparity chunk), two prefix look-ups -> (S, run length) as a packed float pair added to the
+//     running sums (T, N) down the column, which go into a per-thread shared-memory ring of 16 rows.  An output is the
+//     difference of two ring entries (rows y + Dn - 1 and y - U), a reciprocal with one Newton step, the tile's centre
+//     value added back, one store.  No block-wide barrier in the steady state.
+// Compared with cbca_tma_kernel (32-row tiles, 2 CTAs per SM, prefix and walk as barrier-separated phases): 64-row tiles
+// (less halo per output) and prefix and walk of different planes overlapped.  NOT bit-exact by construction (1e-4
+// contract; the constant-work kernels measured up to 1.2e-5 on the volume kinds of DESIGN.md §5).  Serves the short
+// arms (the KITTI presets); longer arms stay on cbca_tma_kernel / the exact kernels.
+
+constexpr int WS_TX = 128, WS_TY = 64;
+constexpr int WS_HO = 32;                   // output rows per walker thread
+constexpr int WS_NWT = WS_TX * (WS_TY / WS_HO);   // walker threads: column x row group
+constexpr int WS_NPW = 4;                   // prefix warps
+constexpr int WS_NT = WS_NWT + 32 * WS_NPW + 32;  // walkers + prefix warps + one producer warp
+constexpr int WS_NST = 3;                   // tile stages
+constexpr int WS_DCH = 20;                  // max disparities per CTA
+constexpr int WS_WW = WS_TX + WS_DCH;       // pitch of the right-image arm windows
+constexpr int WS_TWP = 144;                 // tile pitch = TMA box width: 16 lanes x 9 columns, = 16 (mod 32)
+constexpr int WS_RING = 16;                 // rows of (T, N) per walker thread: a power of two >= 2R + 2
+
+template <int R>
+struct WSCfg {
+	static constexpr int HALO = R + 1;                 // the prefix differences index the first EXCLUDED pixel
+	static constexpr int HX = (HALO + 3) & ~3;         // left halo in columns (TMA: 16-byte aligned start along x)
+	static constexpr int TH = WS_TY + 2 * R + 1;       // image rows y0 - HALO .. y0 + TY + R - 1
+	static constexpr int NWALK = 2 * R + WS_HO;        // rows a thread walks for its HO outputs
+	static constexpr int TILE_BYTES = TH * WS_TWP * 4; // bytes one TMA box delivers
+	static constexpr int STAGE_BYTES = (TILE_BYTES + 127) & ~127;
+	static constexpr int OFF_WINH = WS_NST * STAGE_BYTES;
+	static constexpr int OFF_WINV = OFF_WINH + ((TH * WS_WW * 4 + 15) & ~15);
+	static constexpr int OFF_MU = OFF_WINV + ((WS_TY * WS_WW * 2 + 15) & ~15);
+	static constexpr int OFF_BAR = OFF_MU + 16;
+	static constexpr int OFF_RING = OFF_BAR + ((3 * WS_NST * 8 + 15) & ~15);   // [WS_RING][WS_NWT] (T, N) per thread
+	static constexpr int SMEM = OFF_RING + WS_RING * WS_NWT * 8;
+	static_assert(SMEM <= 232448, "shared memory budget");
+	static_assert(WS_RING >= 2 * R + 2, "ring too small");
+	static_assert(HX + WS_TX + R <= WS_TWP, "tile pitch too small");
+	static_assert(TH <= 256, "TMA box limit");
+};
+
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
+{
+	asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tma_smem_addr(bar)) : "memory");
+}
+__device__ __forceinline__ unsigned long long ws_pack2(float lo, float hi)
+{
+	unsigned long long r;
+	asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
+	return r;
+}
+__device__ __forceinline__ void ws_unpack2(unsigned long long v, float &lo, float &hi)
+{
+	asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+}
+// packed pair: two independent round-to-nearest adds (sm_90 has no packed fp32 add: two scalar ops, same bits)
+__device__ __forceinline__ unsigned long long ws_add2(unsigned long long a, unsigned long long b)
+{
+	float a0, a1, b0, b1;
+	ws_unpack2(a, a0, a1);
+	ws_unpack2(b, b0, b1);
+	return ws_pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+
+// planes [da, db) of the tile (x0, y0): out = vol (the entries with x + d * direction outside the image, :353-354), as aligned
+// float4 copies with 8 independent loads in flight per thread (rows start 16-byte aligned: x0 % 128 == 0, ld % 4 == 0)
+__device__ __forceinline__ void ws_copy_planes(const float *__restrict__ vol, float *__restrict__ out, int da, int db, int x0, int y0,
+					       int H, int W, int ld, int tid, int nthreads)
+{
+	constexpr int Q = WS_TX / 4;                             // float4 per tile row
+	const int total = (db - da) * WS_TY * Q;
+#pragma unroll 8
+	for (int i = tid; i < total; i += nthreads) {
+		const int q = i % Q, r = (i / Q) % WS_TY, d = da + i / (Q * WS_TY);
+		const int y = y0 + r, x = x0 + 4 * q;
+		if (y >= H || x >= W) continue;
+		const long idx = ((long)d * H + y) * ld + x;
+		if (x + 3 < W) {
+			*reinterpret_cast<float4 *>(out + idx) = __ldg(reinterpret_cast<const float4 *>(vol + idx));
+		} else {
+			for (int e = 0; x + e < W; e++) out[idx + e] = __ldg(vol + idx + e);
+		}
+	}
+}
+
+// The prefix warps subtract one value per tile (the tile's mid pixel, 0 when that is not finite) before the row prefix, so
+// the running sums (T, N) down a walker's column carry deviations from it; the walker adds it back to each output.
+template <int R, int WB>
+__global__ void __launch_bounds__(WS_NT, 1)
+cbca_ws_kernel(const __grid_constant__ CUtensorMap tmap,
+	       const uint32_t *__restrict__ a0h, const uint32_t *__restrict__ a0v,
+	       const uint32_t *__restrict__ a1h, const uint32_t *__restrict__ a1v,
+	       const float *__restrict__ vol, float *__restrict__ out,
+	       int D, int H, int W, int ld, int direction, int dch)
+{
+	using C = WSCfg<R>;
+	constexpr int HALO = C::HALO, HX = C::HX, TH = C::TH, NWALK = C::NWALK, TWP = WS_TWP;
+	extern __shared__ __align__(128) unsigned char ws_smem[];
+	uint32_t *winH = reinterpret_cast<uint32_t *>(ws_smem + C::OFF_WINH);   // [TH][WS_WW] right-image H words
+	uint16_t *winV = reinterpret_cast<uint16_t *>(ws_smem + C::OFF_WINV);   // [WS_TY][WS_WW] right-image U | D << 8
+	float *mus = reinterpret_cast<float *>(ws_smem + C::OFF_MU);            // [WS_NST] centre value of the stage's tile
+	uint64_t *bar_full = reinterpret_cast<uint64_t *>(ws_smem + C::OFF_BAR);   // TMA landed
+	uint64_t *bar_ready = bar_full + WS_NST;                                   // prefixes done
+	uint64_t *bar_empty = bar_ready + WS_NST;                                  // walkers done
+
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int x0 = blockIdx.x * WS_TX, y0 = blockIdx.y * WS_TY, d0 = blockIdx.z * dch;
+	const int dn = min(dch, D - d0);
+	const int a1x0 = direction > 0 ? x0 + d0 : x0 - (d0 + dch - 1);   // image column of window column 0
+
+	// disparities whose tile is not entirely inside the invalid triangle form a prefix of the chunk (:353-354)
+	int nproc = 0;
+	while (nproc < dn && !(direction < 0 ? (x0 + WS_TX - 1 - (d0 + nproc) < 0) : (x0 + d0 + nproc >= W))) nproc++;
+
+	if (nproc == 0) {                                      // the whole chunk lies in the invalid triangle: a plain copy, no staging
+		ws_copy_planes(vol, out, d0, d0 + dn, x0, y0, H, W, ld, tid, WS_NT);
+		return;
+	}
+	if (tid == 0) {
+#pragma unroll
+		for (int s = 0; s < WS_NST; s++) {
+			mbar_init(&bar_full[s], 1);
+			mbar_init(&bar_ready[s], WS_NPW);
+			mbar_init(&bar_empty[s], WS_NWT / 32);
+		}
+		mbar_fence_init();
+		tma_prefetch_desc(&tmap);
+	}
+	__syncthreads();
+
+	constexpr int W_PROD = WS_NWT / 32 + WS_NPW;       // the producer warp (after the walkers and the prefix warps)
+	if (warp == W_PROD && lane == 0) {                 // the first tiles fly while the arm windows are staged
+#pragma unroll
+		for (int s = 0; s < WS_NST; s++)
+			if (s < nproc) {
+				mbar_arrive_expect_tx(&bar_full[s], C::TILE_BYTES);
+				tma_load_3d(ws_smem + s * C::STAGE_BYTES, &tmap, x0 - HX, y0 - HALO, d0 + s, &bar_full[s]);
+			}
+	}
+
+	// right-image arm windows (once per CTA), 0 outside the image: a warp per window row, lanes along x.  Only the walkers
+	// need them: they stage them among themselves (named barrier) while the prefix warps already work on the first tile
+	if (warp < WS_NWT / 32) {
+		constexpr int NW = WS_NWT / 32, NCH = (WS_WW + 31) / 32;
+		for (int r = warp; r < TH; r += NW) {
+			const int yy = y0 - HALO + r;
+			const bool rowok = yy >= 0 && yy < H;
+			const uint32_t *grow = a1h + (long)(rowok ? yy : 0) * W;
+#pragma unroll
+			for (int m = 0; m < NCH; m++) {
+				const int j = lane + 32 * m, xx = a1x0 + j;
+				if (j < WS_WW) {
+					const bool ok = rowok && xx >= 0 && xx < W;
+					const unsigned dst = (unsigned)__cvta_generic_to_shared(winH + r * WS_WW + j);
+					const int nbytes = ok ? 4 : 0;
+					asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(grow + (ok ? xx : 0)), "r"(nbytes));
+				}
+			}
+		}
+		asm volatile("cp.async.commit_group;");
+		for (int r = warp; r < WS_TY; r += NW) {
+			const int yy = y0 + r;
+			const uint32_t *grow = a1v + (long)(yy < H ? yy : 0) * W;
+			uint32_t v[NCH];
+#pragma unroll
+			for (int m = 0; m < NCH; m++) {
+				const int xx = a1x0 + lane + 32 * m;
+				v[m] = (yy < H && xx >= 0 && xx < W) ? __ldg(grow + xx) : 0u;
+			}
+#pragma unroll
+			for (int m = 0; m < NCH; m++) {
+				const int j = lane + 32 * m;
+				if (j < WS_WW) winV[r * WS_WW + j] = (uint16_t)(((v[m] >> 8) & 255u) | ((v[m] >> 16) & 0xff00u));   // U | D << 8
+			}
+		}
+		asm volatile("cp.async.wait_group 0;");
+		asm volatile("bar.sync 2, %0;" ::"n"(WS_NWT) : "memory");   // windows visible to the walkers
+	}
+
+	if (warp == W_PROD) {
+		// ---------------------------------------------------------------- producer
+		if (lane == 0) {
+			for (int dd = WS_NST; dd < nproc; dd++) {
+				const int s = dd % WS_NST, k = dd / WS_NST;
+				mbar_wait(&bar_empty[s], (k - 1) & 1);          // the walkers are done with plane dd - NST
+				mbar_arrive_expect_tx(&bar_full[s], C::TILE_BYTES);
+				tma_load_3d(ws_smem + s * C::STAGE_BYTES, &tmap, x0 - HX, y0 - HALO, d0 + dd, &bar_full[s]);
+			}
+		}
+		return;
+	}
+
+	if (warp >= WS_NWT / 32) {
+		// ---------------------------------------------------------------- prefix warps
+		constexpr int EPL = 9;
+		static_assert(EPL * 16 == TWP, "two rows per warp: 16 lanes x 9 columns");
+		const int pw = warp - WS_NWT / 32;
+		const int half = lane >> 4, li = lane & 15;
+		for (int dd = 0; dd < nproc; dd++) {
+			const int s = dd % WS_NST, d = d0 + dd;
+			float *P = reinterpret_cast<float *>(ws_smem + s * C::STAGE_BYTES);
+			// does the tile hold entries of the invalid triangle (NaN)?  They never lie inside a run, but a prefix
+			// sum would carry them along the row: count them as 0.
+			const bool scrub = direction < 0 ? (x0 - HX - d < 0) : (x0 - HX + TWP + d > W);
+			mbar_wait(&bar_full[s], (dd / WS_NST) & 1);
+			const float m = P[(HALO + WS_TY / 2) * TWP + HX + WS_TX / 2];
+			const float mu = (fabsf(m) <= 3.0e38f) ? m : 0.0f;   // finite (NaN and inf fail the compare)
+			if (pw == 0 && lane == 0) mus[s] = mu;
+			asm volatile("bar.sync 1, %0;" ::"n"(32 * WS_NPW) : "memory");   // every prefix warp has read it before any row is rewritten
+			// two independent row pairs per iteration (the scan of one is a chain of dependent adds and shuffles: a single
+			// pair per iteration left the prefix warps latency-bound and the walkers waiting for them)
+			constexpr int UP = 2;
+			for (int pr0 = pw; pr0 < (TH + 1) / 2; pr0 += UP * WS_NPW) {
+				float v[UP][EPL];
+				float *row[UP];
+				bool act[UP];
+#pragma unroll
+				for (int u = 0; u < UP; u++) {
+					const int r = 2 * (pr0 + u * WS_NPW) + half;
+					act[u] = r < TH;
+					row[u] = P + (act[u] ? r : 0) * TWP + li * EPL;
+#pragma unroll
+					for (int i = 0; i < EPL; i++) v[u][i] = row[u][i];
+				}
+#pragma unroll
+				for (int u = 0; u < UP; u++) {
+#pragma unroll
+					for (int i = 0; i < EPL; i++) v[u][i] -= mu;
+					if (scrub) {
+#pragma unroll
+						for (int i = 0; i < EPL; i++) v[u][i] = v[u][i] == v[u][i] ? v[u][i] : 0.0f;
+					}
+				}
+#pragma unroll
+				for (int i = 1; i < EPL; i++)
+#pragma unroll
+					for (int u = 0; u < UP; u++) v[u][i] += v[u][i - 1];
+				float incl[UP];
+#pragma unroll
+				for (int u = 0; u < UP; u++) incl[u] = v[u][EPL - 1];
+#pragma unroll
+				for (int o = 1; o < 16; o <<= 1) {
+					float up[UP];
+#pragma unroll
+					for (int u = 0; u < UP; u++) up[u] = __shfl_up_sync(0xffffffffu, incl[u], o, 16);
+					if (li >= o) {
+#pragma unroll
+						for (int u = 0; u < UP; u++) incl[u] += up[u];
+					}
+				}
+#pragma unroll
+				for (int u = 0; u < UP; u++) {
+					const float base = incl[u] - v[u][EPL - 1];
+					if (act[u]) {
+#pragma unroll
+						for (int i = 0; i < EPL; i++) row[u][i] = v[u][i] + base;
+					}
+				}
+			}
+			fence_proxy_async_smem();                      // generic writes of this stage before its next TMA refill
+			__syncwarp();
+			if (lane == 0) mbar_arrive(&bar_ready[s]);
+		}
+		return;
+	}
+
+	// -------------------------------------------------------------------- walkers
+	const int c = tid & (WS_TX - 1), h = tid >> 7;      // column, row group (output rows HO h .. HO h + HO - 1)
+	const int x = x0 + c;
+	const int yb = y0 + WS_HO * h;                       // first output row of this thread
+	const int nv = x < W ? max(0, min(WS_HO, H - yb)) : 0;   // output rows of this thread inside the image
+	// this thread's own column of the left image's arms: registers for the whole chunk
+	uint32_t ah[NWALK], av[WS_HO];
+#pragma unroll
+	for (int w = 0; w < NWALK; w++) {
+		const int yy = yb - HALO + 1 + w;
+		ah[w] = (x < W && yy >= 0 && yy < H) ? __ldg(a0h + (long)yy * W + x) : 0u;
+	}
+#pragma unroll
+	for (int k = 0; k < WS_HO; k++) {
+		const int yy = yb + k;
+		av[k] = (x < W && yy < H) ? __ldg(a0v + (long)yy * W + x) : 0u;
+	}
+
+	for (int dd = 0; dd < nproc; dd++) {
+		const int d = d0 + dd, s = dd % WS_NST;
+		const float *P = reinterpret_cast<const float *>(ws_smem + s * C::STAGE_BYTES);
+		const int sh = d * direction;
+		const int xs = x + sh;
+		const bool valid_col = x < W && xs >= 0 && xs < W;
+		const int off = (x0 + sh) - a1x0;                 // window column of tile column 0
+		mbar_wait(&bar_ready[s], (dd / WS_NST) & 1);
+		const float mu = mus[s];
+
+		// column walk: relative row rr <-> tile row 32h + rr <-> image row yb - HALO + rr
+		const char *Pc = reinterpret_cast<const char *>(P + (WS_HO * h) * TWP + c + HX);   // own pixel's prefix entry, relative row 0
+		const uint32_t *wh = winH + (WS_HO * h) * WS_WW + c + off;
+		const uint16_t *wv = winV + (WS_HO * h) * WS_WW + c + off;
+		char *po = reinterpret_cast<char *>(out + ((long)d * H + yb) * ld + x);
+		const long ldb = (long)ld * 4;
+		const int nst = valid_col ? nv : 0;                          // rows this thread stores from the walk
+		constexpr int RROW = WS_NWT * 8;                             // ring row pitch in bytes
+		char *rgb = reinterpret_cast<char *>(ws_smem + C::OFF_RING) + tid * 8;
+		unsigned long long run = ws_pack2(0.0f, 0.0f);
+		*reinterpret_cast<unsigned long long *>(rgb) = run;          // relative row 0: the excluded row of output 0
+		// rows in batches of WB: all the shared-memory reads of a batch are issued before its arithmetic
+#pragma unroll
+		for (int b0 = 1; b0 <= NWALK; b0 += WB) {
+			uint32_t hw[WB], vw[WB];
+			float ph[WB], pl[WB];
+#pragma unroll
+			for (int i = 0; i < WB; i++) {
+				const int rr = b0 + i;
+				if (rr <= NWALK) {
+					hw[i] = __vminu2(ah[rr - 1], wh[rr * WS_WW]);   // min of lengths = (max of left ends, min of right ends), :362-363
+					if (rr >= 2 * R + 1) {
+						const int k = rr - 2 * R - 1;
+						vw[i] = __vminu2(av[k], __byte_perm((uint32_t)wv[k * WS_WW], 0u, 0x1404));   // :359-360
+					}
+				}
+			}
+#pragma unroll
+			for (int i = 0; i < WB; i++) {
+				const int rr = b0 + i;
+				if (rr <= NWALK) {
+					const int L4 = hw[i] & 0xffffu, R4 = hw[i] >> 16;
+					const char *pr = Pc + rr * (TWP * 4);
+					ph[i] = *reinterpret_cast<const float *>(pr + R4);
+					pl[i] = *reinterpret_cast<const float *>(pr - L4);
+				}
+			}
+#pragma unroll
+			for (int i = 0; i < WB; i++) {
+				const int rr = b0 + i;
+				if (rr > NWALK) continue;
+				const int L4 = hw[i] & 0xffffu, R4 = hw[i] >> 16;
+				// run length L + R_ - 1 = (L4 + R4) / 4 as a float without a conversion: (2^23 + m) / 4 - 2^21, all exact
+				const float nf = fmaf(__int_as_float(0x4B000000 + L4 + R4), 0.25f, -2097152.0f);   // :368
+				const float S = ph[i] - pl[i];                         // sum of the run (x - L, x + R_), :364-367
+				run = ws_add2(run, ws_pack2(S, nf));
+				*reinterpret_cast<unsigned long long *>(rgb + (rr % WS_RING) * RROW) = run;
+				if (rr >= 2 * R + 1) {
+					const int k = rr - 2 * R - 1;                    // output row yb + k = relative row HALO + k = k + R + 1
+					const unsigned U8 = vw[i] & 0xffffu, D8 = vw[i] >> 16;   // U << 8, Dn << 8
+					constexpr int RB = WS_RING * RROW;
+					constexpr int SC = RROW / 256;                 // U8 = U << 8: U8 * SC = U * RROW
+					const int rk = HALO + k;
+					// rows y - U + 1 .. y + Dn - 1 (:361): run(rk + Dn - 1) - run(rk - U); the ring index wraps only
+					// where the (compile-time) row position says it can
+					const int sb = (rk - 1) % WS_RING, sb2 = rk % WS_RING;
+					int oh = D8 * SC + sb * RROW;
+					if (sb + R + 1 >= WS_RING) oh &= RB - 1;
+					int ol = sb2 * RROW - U8 * SC;
+					if (sb2 - R - 1 < 0) ol = (ol + RB) & (RB - 1);
+					const float2 a = *reinterpret_cast<const float2 *>(rgb + oh), b = *reinterpret_cast<const float2 *>(rgb + ol);
+					const float T = a.x - b.x, N = a.y - b.y;
+					float rc;
+					asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(N));   // count >= 1
+					float q = T * rc;
+					q = fmaf(fmaf(-q, N, T), rc, q);                     // one Newton step: T / N to the last bit or so (:373)
+					q += mu;
+					asm volatile("{\n\t.reg .pred p;\n\tsetp.lt.s32 p, %2, %3;\n\t@p st.global.f32 [%0], %1;\n\t}" ::"l"(po), "f"(q), "r"(k), "r"(nst)
+						     : "memory");
+					po += ldb;
+				}
+			}
+		}
+		if (!valid_col && nv > 0) {                        // x + d*direction outside the image: plain copy, keeps NaN (:353-354)
+			const long idx0 = ((long)d * H + yb) * ld + x;
+#pragma unroll 8
+			for (int k = 0; k < nv; k++) out[idx0 + (long)k * ld] = __ldg(vol + idx0 + (long)k * ld);
+		}
+		// the walkers only READ the stage: the mbarrier release / acquire orders those reads before the refill (the
+		// proxy fence is needed after generic WRITES, i.e. in the prefix warps; here it would also wait for the
+		// thread's global stores to drain, once per plane)
+		__syncwarp();
+		if (lane == 0) mbar_arrive(&bar_empty[s]);
+	}
+	if (nproc < dn) {                                      // planes entirely inside the invalid triangle: plain copy
+		ws_copy_planes(vol, out, d0 + nproc, d0 + dn, x0, y0, H, W, ld, tid, WS_NWT);
+	}
+}
+
+template <int R, int WB>
+int launch_ws(const CUtensorMap &tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
+	      cudaStream_t s)
+{
+	using C = WSCfg<R>;
+	if (int rc = adc_smem_optin(cbca_ws_kernel<R, WB>, C::SMEM)) return rc;
+	const int dch = adc_div_up(D, adc_div_up(D, WS_DCH));   // equal chunks (19 x 12 at D = 228)
+	const long HW = (long)H * W;
+	dim3 grid(adc_div_up(W, WS_TX), adc_div_up(H, WS_TY), adc_div_up(D, dch));
+	cbca_ws_kernel<R, WB><<<grid, WS_NT, C::SMEM, s>>>(tm, hv, hv + 2 * HW, hv + HW, hv + 3 * HW, vol, out, D, H, W, ld, direction, dch);
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
+// The constant-work kernels, shortest arms first.  A row serves a support radius (halo = longest arm - 1) up to its
+// `halo`; the tensor map of its input volume has a box of box_w x box_h floats.
+struct FastKernel {
+	int halo, box_w, box_h;
+	int (*launch)(const CUtensorMap &tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
+		      cudaStream_t s);
+};
+template <int R, int WB> constexpr FastKernel ws_row() { return {R, WS_TWP, WSCfg<R>::TH, launch_ws<R, WB>}; }
+template <int R> constexpr FastKernel tma_row() { return {R, CTCfg<R>::TWP, CTCfg<R>::TH, launch_tma<R>}; }
+constexpr FastKernel FAST_KERNELS[] = {ws_row<1, 6>(), ws_row<4, 4>(), tma_row<8>(), tma_row<13>()};
+
+// The fused pipeline aggregates with the constant-work kernels only up to the last cbca_ws_kernel row (the KITTI presets):
+// with the Middlebury presets' arms of up to 14 pixels cbca_tma_kernel's float prefixes over 27 x 27 windows reach 1.03e-4
+// after six iterations (measured, mb slow at 300 x 700 x 128) -- outside the 1e-4 contract -- so those presets run the
+// exact tile kernels in every mode.
+constexpr int FAST_PIPELINE_MAX_HALO = FAST_KERNELS[1].halo;
+
+const FastKernel *fast_kernel(int halo)
+{
+	for (const FastKernel &k : FAST_KERNELS)
+		if (halo <= k.halo) return &k;
+	return nullptr;
 }
 
 }  // namespace
@@ -344,55 +774,57 @@ int adc_pack_arms_hv(const float *xc, uint32_t *hv, int which, int H, int W, cud
 	return 0;
 }
 
-// second-generation kernel for short arms (cbca_ws.cu)
-int adc_cbca_ws_max_halo();
-void adc_cbca_ws_box(int halo, int *box_w, int *box_h);
-int adc_cbca_ws(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
-		int halo, cudaStream_t s);
+int adc_cbca_fast_pipeline_max_halo() { return FAST_PIPELINE_MAX_HALO; }
 
-// largest support radius (longest arm - 1) the constant-work kernel is instantiated for
-int adc_cbca_tma_max_halo() { return 13; }
-
-// box of the tensor map a volume needs for support radius `halo` (= longest arm - 1)
-void adc_cbca_tma_box(int halo, int *box_w, int *box_h)
+// box of the tensor map a volume needs for support radius `halo` (= longest arm - 1); ADCENSUS_ELIMIT beyond the last row
+int adc_cbca_fast_box(int halo, int *box_w, int *box_h)
 {
-	if (halo <= adc_cbca_ws_max_halo()) adc_cbca_ws_box(halo, box_w, box_h);
-	else if (halo <= 8) { *box_w = CTCfg<8>::TWP; *box_h = CTCfg<8>::TH; }
-	else { *box_w = CTCfg<13>::TWP; *box_h = CTCfg<13>::TH; }
+	const FastKernel *k = fast_kernel(halo);
+	if (!k) return ADCENSUS_ELIMIT;
+	*box_w = k->box_w;
+	*box_h = k->box_h;
+	return 0;
 }
 
 // vol/out: (D, H, ld) with ld % 4 == 0 and 16-byte aligned bases; tm: tensor map of `vol` with the box of `halo`
-int adc_cbca_tma(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
-		 int halo, cudaStream_t s)
+int adc_cbca_fast(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
+		  int halo, cudaStream_t s)
 {
-	if (halo <= adc_cbca_ws_max_halo()) return adc_cbca_ws(tm, hv, vol, out, D, H, W, ld, direction, halo, s);
-	if (halo <= 8) return launch_tma<8>(*tm, hv, vol, out, D, H, W, ld, direction, s);
-	if (halo <= 13) return launch_tma<13>(*tm, hv, vol, out, D, H, W, ld, direction, s);
-	return ADCENSUS_ELIMIT;
+	const FastKernel *k = fast_kernel(halo);
+	return k ? k->launch(*tm, hv, vol, out, D, H, W, ld, direction, s) : ADCENSUS_ELIMIT;
 }
 
 // ---- public: one aggregation pass on pitched volumes ---------------------------------------------
+// the argument checks of both entry points below, and the tensor map of vol_in for arms of at most max_arm pixels
+static int fast_check_and_encode(CUtensorMap *tm, const float *vol_in, const float *vol_out, int D, int H, int W, int ld, int direction,
+				 int max_arm)
+{
+	if (!vol_in || !vol_out || vol_in == vol_out) return ADCENSUS_EINVAL;
+	if (D < 1 || H < 1 || W < 1 || ld < W || (ld & 3) || (direction != 1 && direction != -1) || max_arm < 1) return ADCENSUS_EINVAL;
+	if ((((uintptr_t)vol_in) | ((uintptr_t)vol_out)) & 15) return ADCENSUS_EINVAL;
+	int bw, bh;
+	int rc = adc_cbca_fast_box(max_arm - 1, &bw, &bh);
+	if (!rc) rc = adc_tma_encode_volume(tm, vol_in, D, H, W, ld, bw, bh);
+	return rc;
+}
+
 // Constant-work aggregation (1e-4 contract, not bit-exact).  vol_in / vol_out are (D, H, ld) with ld >= W,
-// ld % 4 == 0, 16-byte aligned; x0c / x1c are cross() outputs (4,H,W) with arms of at most max_arm <= 14 pixels.
+// ld % 4 == 0, 16-byte aligned; x0c / x1c are cross() outputs (4,H,W) with arms of at most max_arm pixels, a length
+// the last row of FAST_KERNELS serves (ADCENSUS_ELIMIT otherwise).
 extern "C" int mccnn_cbca_fast_pitched(const float *x0c, const float *x1c, const float *vol_in, float *vol_out,
 				       int D, int H, int W, int ld, int direction, int max_arm, adcensus_stream_t stream)
 {
-	if (!x0c || !x1c || !vol_in || !vol_out || vol_in == vol_out) return ADCENSUS_EINVAL;
-	if (D < 1 || H < 1 || W < 1 || ld < W || (ld & 3) || (direction != 1 && direction != -1) || max_arm < 1) return ADCENSUS_EINVAL;
-	if ((((uintptr_t)vol_in) | ((uintptr_t)vol_out)) & 15) return ADCENSUS_EINVAL;
-	if (max_arm - 1 > adc_cbca_tma_max_halo()) return ADCENSUS_ELIMIT;
+	if (!x0c || !x1c) return ADCENSUS_EINVAL;
 	cudaStream_t s = adc_stream(stream);
 	CUtensorMap tm;
-	int bw, bh;
-	adc_cbca_tma_box(max_arm - 1, &bw, &bh);
-	int rc = adc_tma_encode_volume(&tm, vol_in, D, H, W, ld, bw, bh);
+	int rc = fast_check_and_encode(&tm, vol_in, vol_out, D, H, W, ld, direction, max_arm);
 	if (rc) return rc;
 	uint32_t *hv = nullptr;
 	rc = adc_scratch_alloc((void **)&hv, adc_packed_hv_words(H, W) * sizeof(uint32_t), s);
 	if (rc) return rc;
 	rc = adc_pack_arms_hv(x0c, hv, 0, H, W, s);
 	if (!rc) rc = adc_pack_arms_hv(x1c, hv, 1, H, W, s);
-	if (!rc) rc = adc_cbca_tma(&tm, hv, vol_in, vol_out, D, H, W, ld, direction, max_arm - 1, s);
+	if (!rc) rc = adc_cbca_fast(&tm, hv, vol_in, vol_out, D, H, W, ld, direction, max_arm - 1, s);
 	int rc2 = adc_scratch_free(hv, s);
 	return rc ? rc : rc2;
 }
@@ -412,14 +844,9 @@ extern "C" int mccnn_pack_arms_hv(const float *x0c, const float *x1c, void *hv, 
 extern "C" int mccnn_cbca_fast_pitched_packed(const void *hv, const float *vol_in, float *vol_out,
 					      int D, int H, int W, int ld, int direction, int max_arm, adcensus_stream_t stream)
 {
-	if (!hv || !vol_in || !vol_out || vol_in == vol_out) return ADCENSUS_EINVAL;
-	if (D < 1 || H < 1 || W < 1 || ld < W || (ld & 3) || (direction != 1 && direction != -1) || max_arm < 1) return ADCENSUS_EINVAL;
-	if ((((uintptr_t)vol_in) | ((uintptr_t)vol_out)) & 15) return ADCENSUS_EINVAL;
-	if (max_arm - 1 > adc_cbca_tma_max_halo()) return ADCENSUS_ELIMIT;
+	if (!hv) return ADCENSUS_EINVAL;
 	CUtensorMap tm;
-	int bw, bh;
-	adc_cbca_tma_box(max_arm - 1, &bw, &bh);
-	int rc = adc_tma_encode_volume(&tm, vol_in, D, H, W, ld, bw, bh);
+	int rc = fast_check_and_encode(&tm, vol_in, vol_out, D, H, W, ld, direction, max_arm);
 	if (rc) return rc;
-	return adc_cbca_tma(&tm, (const uint32_t *)hv, vol_in, vol_out, D, H, W, ld, direction, max_arm - 1, adc_stream(stream));
+	return adc_cbca_fast(&tm, (const uint32_t *)hv, vol_in, vol_out, D, H, W, ld, direction, max_arm - 1, adc_stream(stream));
 }

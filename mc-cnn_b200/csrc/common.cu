@@ -1,4 +1,8 @@
-// common.cu -- device properties cache, stream-ordered scratch, version string
+// common.cu -- device properties cache, stream-ordered scratch, shared-memory opt-in, version string
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "common.cuh"
 
 int adc_num_sms()
@@ -37,6 +41,31 @@ int adc_scratch_alloc(void **p, size_t bytes, cudaStream_t s)
 int adc_scratch_free(void *p, cudaStream_t s)
 {
 	return p ? (int)cudaFreeAsync(p, s) : 0;
+}
+
+// The attribute only ever grows: a launch that needs less than an earlier one must not lower it under a launch of
+// another host thread.  `granted` is the record per (device, kernel), written under the lock; each host thread keeps a
+// copy of what it has read there, so a launch whose amount is already granted takes no lock.
+int adc_smem_optin(const void *kernel, size_t bytes)
+{
+	if (bytes <= 48 * 1024) return 0;
+	if (bytes > 232448) return ADCENSUS_ELIMIT;
+	int dev = 0;
+	ADC_CUDA(cudaGetDevice(&dev));
+	const std::pair<int, const void *> key(dev, kernel);
+	thread_local std::map<std::pair<int, const void *>, size_t> seen;
+	const auto it = seen.find(key);
+	if (it != seen.end() && it->second >= bytes) return 0;
+	static std::mutex mu;
+	static std::map<std::pair<int, const void *>, size_t> granted;
+	std::lock_guard<std::mutex> lock(mu);
+	size_t &g = granted[key];
+	if (g < bytes) {
+		ADC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+		g = bytes;
+	}
+	seen[key] = g;
+	return 0;
 }
 
 // give the stream-ordered scratch kept by the operator-level calls back to the driver (after the work using it has completed)

@@ -30,6 +30,16 @@ int adc_num_sms();
 int adc_scratch_alloc(void **p, size_t bytes, cudaStream_t s);
 int adc_scratch_free(void *p, cudaStream_t s);
 
+// Lets `kernel` launch on the current device with `bytes` of dynamic shared memory: nothing to do up to 48 KB,
+// ADCENSUS_ELIMIT above the 227 KB per-block limit of sm_90.  Safe to call from several host threads and cheap on
+// every launch once the amount has been granted.
+int adc_smem_optin(const void *kernel, size_t bytes);
+template <typename Kernel>
+int adc_smem_optin(Kernel *kernel, size_t bytes)
+{
+	return adc_smem_optin((const void *)kernel, bytes);
+}
+
 __device__ __forceinline__ float adc_nan() { return __int_as_float(0x7fffffff); }
 
 // streaming (evict-first) global accesses for data touched exactly once

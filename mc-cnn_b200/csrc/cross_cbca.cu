@@ -409,17 +409,11 @@ __global__ void cbca_generic_kernel(const float *__restrict__ x0c, const float *
 
 template <int R>
 int launch_win(const uint32_t *a0, const uint32_t *a1, const float *vol, float *out, int D, int H, int W, int ld, int direction, cudaStream_t s,
-	       const int *gate = nullptr, int gate_lo = 0, int gate_hi = 0)
+	       const int *gate, int gate_lo, int gate_hi)
 {
 	using Cfg = CWCfg<R>;
 	constexpr int SMEM = Cfg::SMEM;
-	static bool attr_done[64] = {false};
-	int dev = 0;
-	cudaGetDevice(&dev);
-	if (!attr_done[dev & 63]) {
-		ADC_CUDA(cudaFuncSetAttribute(cbca_win_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-		attr_done[dev & 63] = true;
-	}
+	if (int rc = adc_smem_optin(cbca_win_kernel<R>, SMEM)) return rc;
 	// disparities per CTA.  The kernel is issue-bound and balances dynamically, so the chunk size hardly matters; timed on an
 	// H100 through the exact-mode pipeline at 370x1226x228 (ms per pair, two rounds): 8 -> 17.29 / 17.43, 10 -> 17.24 / 17.39,
 	// 14 -> 17.18 / 17.16, 20 -> 17.15 / 17.23.
@@ -431,12 +425,26 @@ int launch_win(const uint32_t *a0, const uint32_t *a1, const float *vol, float *
 }
 
 template <int R>
-void launch_tile(const uint32_t *a0, const uint32_t *a1, const float *vol, float *out, int D, int H, int W, int ld, int direction, cudaStream_t s,
-		 const int *gate = nullptr, int gate_lo = 0, int gate_hi = 0)
+int launch_tile(const uint32_t *a0, const uint32_t *a1, const float *vol, float *out, int D, int H, int W, int ld, int direction, cudaStream_t s,
+		const int *gate, int gate_lo, int gate_hi)
 {
 	dim3 grid(adc_div_up(W, CB_TX), adc_div_up(H, CB_TY), adc_div_up(D, CB_DCH));
 	cbca_loop_kernel<R><<<grid, CB_NT, 0, s>>>(a0, a1, vol, out, D, H, W, ld, direction, gate, gate_lo, gate_hi);
+	return 0;
 }
+
+// The exact kernels, shortest arms first.  A row serves a support radius (halo = longest arm - 1) up to its `halo`;
+// beyond the last row, and for arms that are not cross() outputs, cbca_generic_kernel reads the float arms itself.
+// gate: the launch returns at once unless gate_lo <= *gate <= gate_hi (the longest arm, known on the device only).
+struct ExactKernel {
+	int halo;
+	int (*launch)(const uint32_t *a0, const uint32_t *a1, const float *vol, float *out, int D, int H, int W, int ld, int direction,
+		      cudaStream_t s, const int *gate, int gate_lo, int gate_hi);
+};
+template <int R> constexpr ExactKernel win_row() { return {R, launch_win<R>}; }
+template <int R> constexpr ExactKernel tile_row() { return {R, launch_tile<R>}; }
+constexpr ExactKernel EXACT_KERNELS[] = {win_row<1>(), win_row<4>(), tile_row<8>(), tile_row<13>()};
+constexpr int EXACT_MAX_HALO = EXACT_KERNELS[sizeof(EXACT_KERNELS) / sizeof(EXACT_KERNELS[0]) - 1].halo;
 
 }  // namespace
 
@@ -457,27 +465,36 @@ int adc_pack_arms(const float *xc, uint32_t *pk, int which, int H, int W, int *m
 	return pack_arms(xc, pk, which, H, W, maxlen_dev, 0, s);
 }
 
+// Packs the arms of both images into *pk (mccnn_packed_arms_bytes(H, W) bytes; scratch-allocated first when *pk is null,
+// the caller frees it), the longest arm into the word after the packed words; clamp as in pack_arms_kernel.
+static int pack_both(const float *x0c, const float *x1c, uint32_t **pk, int H, int W, int clamp, cudaStream_t s)
+{
+	if (!*pk) {
+		int rc = adc_scratch_alloc((void **)pk, mccnn_packed_arms_bytes(H, W), s);
+		if (rc) return rc;
+	}
+	int *maxlen_dev = (int *)(*pk + adc_packed_words(H, W));
+	int rc = (int)cudaMemsetAsync(maxlen_dev, 0, sizeof(int), s);
+	if (!rc) rc = pack_arms(x0c, *pk, 0, H, W, maxlen_dev, clamp, s);
+	if (!rc) rc = pack_arms(x1c, *pk, 1, H, W, maxlen_dev, clamp, s);
+	return rc;
+}
+
 // Exact (bit-identical) aggregation.  maxlen = longest arm (distance to the exclusive end-point) of either
 // image; vol / out are (D, H, ld) with ld >= W (ld == W: the API-facing contiguous tensors).
 int adc_cbca_packed(const uint32_t *pk, const float *x0c, const float *x1c,
 		    const float *vol, float *out, int D, int H, int W, int ld, int direction, int maxlen, cudaStream_t s)
 {
 	const long HW = (long)H * W;
-	const uint32_t *a0 = pk, *a1 = pk + HW;
-	int halo = maxlen - 1;
-	if (halo <= 1) {
-		int rc = launch_win<1>(a0, a1, vol, out, D, H, W, ld, direction, s);
-		if (rc) return rc;
-	} else if (halo <= 4) {
-		int rc = launch_win<4>(a0, a1, vol, out, D, H, W, ld, direction, s);
-		if (rc) return rc;
-	}
-	else if (halo <= 8) launch_tile<8>(a0, a1, vol, out, D, H, W, ld, direction, s);
-	else if (halo <= 13) launch_tile<13>(a0, a1, vol, out, D, H, W, ld, direction, s);
-	else {
-		long size = (long)D * H * W;
-		cbca_generic_kernel<<<adc_div_up(size, 256), 256, 0, s>>>(x0c, x1c, vol, out, size, H, W, ld, direction, nullptr, 0, 0);
-	}
+	for (const ExactKernel &k : EXACT_KERNELS)
+		if (maxlen - 1 <= k.halo) {
+			int rc = k.launch(pk, pk + HW, vol, out, D, H, W, ld, direction, s, nullptr, 0, 0);
+			if (rc) return rc;
+			ADC_CHECK_LAUNCH();
+			return 0;
+		}
+	long size = (long)D * H * W;
+	cbca_generic_kernel<<<adc_div_up(size, 256), 256, 0, s>>>(x0c, x1c, vol, out, size, H, W, ld, direction, nullptr, 0, 0);
 	ADC_CHECK_LAUNCH();
 	return 0;
 }
@@ -487,14 +504,8 @@ int adc_cbca_packed(const uint32_t *pk, const float *x0c, const float *x1c,
 extern "C" int mccnn_pack_arms(const float *x0c, const float *x1c, void *packed, int H, int W, adcensus_stream_t stream)
 {
 	if (!x0c || !x1c || !packed || H < 1 || W < 1) return ADCENSUS_EINVAL;
-	cudaStream_t s = adc_stream(stream);
 	uint32_t *pk = (uint32_t *)packed;
-	const long HW = (long)H * W;
-	int *maxlen_dev = (int *)(pk + adc_packed_words(H, W));
-	int rc = (int)cudaMemsetAsync(maxlen_dev, 0, sizeof(int), s);
-	if (!rc) rc = adc_pack_arms(x0c, pk, 0, H, W, maxlen_dev, s);
-	if (!rc) rc = adc_pack_arms(x1c, pk, 1, H, W, maxlen_dev, s);
-	return rc;
+	return pack_both(x0c, x1c, &pk, H, W, 0, adc_stream(stream));
 }
 
 extern "C" size_t mccnn_packed_arms_bytes(int H, int W) { return (adc_packed_words(H, W) + 1) * sizeof(uint32_t); }
@@ -523,15 +534,10 @@ extern "C" int adcensus_cbca_ex(const float *x0c, const float *x1c, const float 
 	if (!x0c || !x1c || !vol_in || !vol_out || vol_in == vol_out) return ADCENSUS_EINVAL;
 	if (D < 1 || H < 1 || W < 1 || (direction != 1 && direction != -1) || max_arm < 1) return ADCENSUS_EINVAL;
 	cudaStream_t s = adc_stream(stream);
-	long HW = (long)H * W;
 	uint32_t *packed = nullptr;
-	int rc = adc_scratch_alloc((void **)&packed, (adc_packed_words(H, W) + 1) * sizeof(uint32_t), s);
-	if (rc) return rc;
-	int *maxlen_dev = (int *)(packed + adc_packed_words(H, W));
-	rc = (int)cudaMemsetAsync(maxlen_dev, 0, sizeof(int), s);
-	const int clamp = max_arm <= 14 ? max_arm : 0;            // beyond 14 the generic kernel reads the float arms themselves
-	if (!rc) rc = pack_arms(x0c, packed, 0, H, W, maxlen_dev, clamp, s);
-	if (!rc) rc = pack_arms(x1c, packed, 1, H, W, maxlen_dev, clamp, s);
+	// beyond the tiled kernels' arms the generic kernel reads the float arms themselves
+	const int clamp = max_arm - 1 <= EXACT_MAX_HALO ? max_arm : 0;
+	int rc = pack_both(x0c, x1c, &packed, H, W, clamp, s);
 	if (!rc) rc = adc_cbca_packed(packed, x0c, x1c, vol_in, vol_out, D, H, W, W, direction, max_arm, s);
 	int rc2 = adc_scratch_free(packed, s);
 	return rc ? rc : rc2;
@@ -545,23 +551,20 @@ extern "C" int adcensus_cbca(const float *x0c, const float *x1c, const float *vo
 	cudaStream_t s = adc_stream(stream);
 	const long HW = (long)H * W;
 	uint32_t *packed = nullptr;
-	int rc = adc_scratch_alloc((void **)&packed, (adc_packed_words(H, W) + 1) * sizeof(uint32_t), s);
-	if (rc) return rc;
-	int *maxlen_dev = (int *)(packed + adc_packed_words(H, W));
-	rc = (int)cudaMemsetAsync(maxlen_dev, 0, sizeof(int), s);
-	if (!rc) rc = adc_pack_arms(x0c, packed, 0, H, W, maxlen_dev, s);
-	if (!rc) rc = adc_pack_arms(x1c, packed, 1, H, W, maxlen_dev, s);
+	int rc = pack_both(x0c, x1c, &packed, H, W, 0, s);
 	if (!rc) {
 		// The longest arm is only known on the device.  Instead of reading it back (a host synchronisation per call),
 		// every candidate kernel is launched with a gate on that device value; the ones out of range return at once.
-		const uint32_t *a0 = packed, *a1 = packed + HW;
-		rc = launch_win<1>(a0, a1, vol_in, vol_out, D, H, W, W, direction, s, maxlen_dev, 0, 2);
-		if (!rc) rc = launch_win<4>(a0, a1, vol_in, vol_out, D, H, W, W, direction, s, maxlen_dev, 3, 5);
+		// A row runs for the longest arms its halo serves and the previous row's does not.
+		const int *maxlen_dev = (const int *)(packed + adc_packed_words(H, W));
+		int lo = 0;
+		for (const ExactKernel &k : EXACT_KERNELS) {
+			if (!rc) rc = k.launch(packed, packed + HW, vol_in, vol_out, D, H, W, W, direction, s, maxlen_dev, lo, k.halo + 1);
+			lo = k.halo + 2;
+		}
 		if (!rc) {
-			launch_tile<8>(a0, a1, vol_in, vol_out, D, H, W, W, direction, s, maxlen_dev, 6, 9);
-			launch_tile<13>(a0, a1, vol_in, vol_out, D, H, W, W, direction, s, maxlen_dev, 10, 14);
 			const long size = (long)D * H * W;
-			cbca_generic_kernel<<<adc_div_up(size, 256), 256, 0, s>>>(x0c, x1c, vol_in, vol_out, size, H, W, W, direction, maxlen_dev, 15, 1 << 30);
+			cbca_generic_kernel<<<adc_div_up(size, 256), 256, 0, s>>>(x0c, x1c, vol_in, vol_out, size, H, W, W, direction, maxlen_dev, lo, 1 << 30);
 			rc = (int)cudaPeekAtLastError();
 		}
 	}

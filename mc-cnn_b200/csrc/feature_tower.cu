@@ -466,9 +466,6 @@ extern "C" int mccnn_feature_tower_forward(const mccnn_feature_tower *h, const f
 		conv3x3_first_kernel<<<grid, 128, sm, s>>>(img, h->w0, h->b0, dst, h->n_in, h->fm, H, W, relu);
 		rc = (int)cudaPeekAtLastError();
 	}
-	static bool attr3[64] = {false}, attr1[64] = {false};
-	int dev = 0;
-	cudaGetDevice(&dev);
 	for (int l = 1; l < h->l1 && !rc; l++) {
 		const bool last = l + 1 == h->l1;
 		FTParams p;
@@ -483,38 +480,25 @@ extern "C" int mccnn_feature_tower_forward(const mccnn_feature_tower *h, const f
 		if (p.taps_per_pass > 9) p.taps_per_pass = 9;
 		const dim3 grid(adc_div_up(W, SH_M), H, nimg);
 		if (h->fm == 64) {                          // weights resident, persistent CTAs (the fast architecture)
-			static bool attr_r3[64] = {false}, attr_r1[64] = {false};
 			const int ntile = nimg * H * adc_div_up(W, SH_M);
 			const int nb = ntile < adc_num_sms() ? ntile : adc_num_sms();
 			if (nterms == 3) {
-				if (!attr_r3[dev & 63]) {
-					rc = (int)cudaFuncSetAttribute(conv3x3_resident_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_SMEM);
-					attr_r3[dev & 63] = !rc;
-				}
+				rc = adc_smem_optin(conv3x3_resident_kernel<3>, F2_SMEM);
 				if (!rc) conv3x3_resident_kernel<3><<<nb, F2_NT, F2_SMEM, s>>>(p, nimg);
 			} else {
-				if (!attr_r1[dev & 63]) {
-					rc = (int)cudaFuncSetAttribute(conv3x3_resident_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_SMEM);
-					attr_r1[dev & 63] = !rc;
-				}
+				rc = adc_smem_optin(conv3x3_resident_kernel<1>, F2_SMEM);
 				if (!rc) conv3x3_resident_kernel<1><<<nb, F2_NT, F2_SMEM, s>>>(p, nimg);
 			}
 			if (!rc) rc = (int)cudaPeekAtLastError();
 			continue;
 		}
 		if (nterms == 3) {
-			if (!attr3[dev & 63]) {
-				rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<3, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				if (!rc) rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<3, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				attr3[dev & 63] = !rc;
-			}
+			rc = adc_smem_optin(conv3x3_wgmma_kernel<3, 128>, FT_SMEM);
+			if (!rc) rc = adc_smem_optin(conv3x3_wgmma_kernel<3, 64>, FT_SMEM);
 			if (!rc) ft_launch<3>(p, grid, s);
 		} else {
-			if (!attr1[dev & 63]) {
-				rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				if (!rc) rc = (int)cudaFuncSetAttribute(conv3x3_wgmma_kernel<1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM);
-				attr1[dev & 63] = !rc;
-			}
+			rc = adc_smem_optin(conv3x3_wgmma_kernel<1, 128>, FT_SMEM);
+			if (!rc) rc = adc_smem_optin(conv3x3_wgmma_kernel<1, 64>, FT_SMEM);
 			if (!rc) ft_launch<1>(p, grid, s);
 		}
 		if (!rc) rc = (int)cudaPeekAtLastError();

@@ -27,10 +27,10 @@ int adc_cbca_packed(const uint32_t *pk, const float *x0c, const float *x1c,
 		    const float *vol, float *out, int D, int H, int W, int ld, int direction, int maxlen, cudaStream_t s);
 size_t adc_packed_hv_words(int H, int W);
 int adc_pack_arms_hv(const float *xc, uint32_t *hv, int which, int H, int W, cudaStream_t s);
-int adc_cbca_ws_max_halo();
-void adc_cbca_tma_box(int halo, int *box_w, int *box_h);
-int adc_cbca_tma(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
-		 int halo, cudaStream_t s);
+int adc_cbca_fast_pipeline_max_halo();
+int adc_cbca_fast_box(int halo, int *box_w, int *box_h);
+int adc_cbca_fast(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
+		  int halo, cudaStream_t s);
 size_t adc_sgm_table_bytes(int H, int W, int D);
 int adc_sgm2(const float *x0, const float *x1, const float *in, float *out, uint8_t *tab, int H, int W, int D,
 	     float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction,
@@ -108,10 +108,8 @@ int dev_alloc(void **p, size_t bytes, size_t *acc)
 // longest arm cross() can produce for this preset, and the CBCA support radius
 int pipe_maxlen(const mccnn_pipeline *p) { return p->prm.L1 > 2 ? p->prm.L1 : 2; }
 
-// Constant-work aggregation only for arms <= 5 (the KITTI presets, cbca_ws.cu): with the Middlebury presets' arms of up to
-// 14 pixels the first-generation kernel's float prefixes over 27 x 27 windows reach 1.03e-4 after six iterations (measured,
-// mb slow at 300 x 700 x 128) -- outside the 1e-4 contract -- so those presets run the exact tile kernels in every mode.
-bool pipe_fast_cbca_ok(const mccnn_pipeline *p) { return pipe_maxlen(p) - 1 <= adc_cbca_ws_max_halo(); }
+// constant-work aggregation only for the arms the 1e-4 contract allows (cbca_tma.cu FAST_PIPELINE_MAX_HALO)
+bool pipe_fast_cbca_ok(const mccnn_pipeline *p) { return pipe_maxlen(p) - 1 <= adc_cbca_fast_pipeline_max_halo(); }
 
 // a map of `buf` as a (tm_D, tm_H, tm_W) volume with rows of tm_W rounded up to 4 floats
 int add_tensor_map(mccnn_pipeline *p, const float *buf)
@@ -121,8 +119,8 @@ int add_tensor_map(mccnn_pipeline *p, const float *buf)
 	if (!p->tm_D) return 0;                            // no valid shape: the next run encodes every map
 	if (p->ntm >= 6) return ADCENSUS_EINVAL;
 	int bw, bh;
-	adc_cbca_tma_box(halo, &bw, &bh);
-	int rc = adc_tma_encode_volume(&p->tm[p->ntm], buf, p->tm_D, p->tm_H, p->tm_W, (p->tm_W + 3) & ~3, bw, bh);
+	int rc = adc_cbca_fast_box(halo, &bw, &bh);
+	if (!rc) rc = adc_tma_encode_volume(&p->tm[p->ntm], buf, p->tm_D, p->tm_H, p->tm_W, (p->tm_W + 3) & ~3, bw, bh);
 	if (rc) return rc;
 	p->tm_ptr[p->ntm++] = buf;
 	return 0;
@@ -465,7 +463,7 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		if (tma) {
 			const CUtensorMap *tm = find_tensor_map(p, in);
 			if (!tm) return ADCENSUS_EINVAL;
-			return adc_cbca_tma(tm, hv, in, out, D, H, W, ld, direction, maxlen - 1, ds);
+			return adc_cbca_fast(tm, hv, in, out, D, H, W, ld, direction, maxlen - 1, ds);
 		}
 		return adc_cbca_packed(p->packed, p->x0c, p->x1c, in, out, D, H, W, ld, direction, nan_in_valid ? (1 << 20) : maxlen, ds);
 	};

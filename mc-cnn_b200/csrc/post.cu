@@ -622,9 +622,7 @@ int adcensus_mean2d(const float *img, const float *kernel, float *out, int H, in
 	const int r = ksize / 2;
 	const size_t smem = ((size_t)(M2_TY + 2 * r) * (M2_TX + 2 * r) + (size_t)ksize * ksize) * sizeof(float);
 	if (smem <= 200 * 1024) {
-		if (smem > 48 * 1024) {
-			ADC_CUDA(cudaFuncSetAttribute(mean2d_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-		}
+		if (int rc = adc_smem_optin(mean2d_tile_kernel, smem)) return rc;
 		dim3 grid(adc_div_up(W, M2_TX), adc_div_up(H, M2_TY)), block(M2_TX, M2_TY);
 		mean2d_tile_kernel<<<grid, block, smem, adc_stream(stream)>>>(img, kernel, out, r, H, W, alpha2);
 		ADC_CHECK_LAUNCH();

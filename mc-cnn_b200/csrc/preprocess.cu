@@ -193,7 +193,7 @@ int launch_rows(int mode, float *y, const float *disp, const float *x0, const in
 	const void *fn = mode == ROW_OCCLUDED ? (const void *)rows_kernel<ROW_OCCLUDED>
 			 : mode == ROW_COUNT  ? (const void *)rows_kernel<ROW_COUNT>
 					      : (const void *)rows_kernel<ROW_FILL>;
-	if (smem > 48 * 1024) ADC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	if (int rc = adc_smem_optin(fn, smem)) return rc;
 	if (mode == ROW_OCCLUDED)
 		rows_kernel<ROW_OCCLUDED><<<(unsigned)rows, PP_THREADS, smem, s>>>(y, disp, x0, is_te, H, W, count, off_tr, off_te, nnz_tr,
 									 cap_tr, nnz_te, cap_te);

@@ -325,21 +325,12 @@ extern "C" void mccnn_scorer_head_destroy(mccnn_scorer_head *h)
 template <int NH>
 static int sh_launch(const SHParams &p, dim3 grid, int nterms, cudaStream_t s)
 {
-	static bool attr3[64] = {false}, attr1[64] = {false};
-	int dev = 0;
-	cudaGetDevice(&dev);
 	int rc = 0;
 	if (nterms == 3) {
-		if (!attr3[dev & 63]) {
-			rc = (int)cudaFuncSetAttribute(scorer_head_kernel<3, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize, SHCfg<3>::SMEM);
-			attr3[dev & 63] = !rc;
-		}
+		rc = adc_smem_optin(scorer_head_kernel<3, NH>, SHCfg<3>::SMEM);
 		if (!rc) scorer_head_kernel<3, NH><<<grid, SH_NT, SHCfg<3>::SMEM, s>>>(p);
 	} else {
-		if (!attr1[dev & 63]) {
-			rc = (int)cudaFuncSetAttribute(scorer_head_kernel<1, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize, SHCfg<1>::SMEM);
-			attr1[dev & 63] = !rc;
-		}
+		rc = adc_smem_optin(scorer_head_kernel<1, NH>, SHCfg<1>::SMEM);
 		if (!rc) scorer_head_kernel<1, NH><<<grid, SH_NT, SHCfg<1>::SMEM, s>>>(p);
 	}
 	return rc;

@@ -520,18 +520,12 @@ sgm_hpair_kernel(const uint8_t *__restrict__ tab, const float *__restrict__ in, 
 
 constexpr int SGM_SMEM_MAX = 160 * 1024;
 
-// done: one flag array per kernel instantiation (the caller's static)
+// every scan kernel is granted SGM_SMEM_MAX at once, whatever the first launch needs
 template <typename Kern>
-int sgm_allow_smem(Kern kern, int smem, bool *done)
+int sgm_allow_smem(Kern kern, int smem)
 {
 	if (smem > SGM_SMEM_MAX) return ADCENSUS_ELIMIT;
-	int dev = 0;
-	cudaGetDevice(&dev);
-	if (!done[dev & 63]) {
-		ADC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SGM_SMEM_MAX));
-		done[dev & 63] = true;
-	}
-	return 0;
+	return adc_smem_optin(kern, SGM_SMEM_MAX);
 }
 
 template <int K, bool VEC, int SD, bool ZERO>
@@ -544,8 +538,7 @@ int launch_pass(const uint8_t *tab, const float *in, float *out, int H, int W, i
 	using Scan = SgmScan<K, VEC, SD, PF>;
 	const int smem = WPB * (PF * 2 * Scan::VSZ * 4 + Scan::CRING_WORDS * 4 + (SD < 2 ? 2 * sgm_row_bytes(prm.Wt, pad) : 0));
 	auto kern = sgm_pass_kernel<K, VEC, SD, ZERO, PF, WPB>;
-	static bool done[64] = {false};
-	int rc = sgm_allow_smem(kern, smem, done);
+	int rc = sgm_allow_smem(kern, smem);
 	if (rc) return rc;
 	const int nlines = prm.line1 - prm.line0;
 	if (nlines <= 0) return 0;
@@ -561,8 +554,7 @@ int launch_hpair(const uint8_t *tab, const float *in, float *out, int H, int W, 
 	constexpr int PF = K >= 16 ? 6 : 8;
 	const int smem = 2 * PF * 2 * 32 * K * 4 + 2 * sgm_row_bytes(prm.Wt, pad);
 	auto kern = sgm_hpair_kernel<K, VEC, PF>;
-	static bool done[64] = {false};
-	int rc = sgm_allow_smem(kern, smem, done);
+	int rc = sgm_allow_smem(kern, smem);
 	if (rc) return rc;
 	kern<<<H, 64, smem, s>>>(tab, in, out, H, W, D, pad, prm);
 	ADC_CHECK_LAUNCH();

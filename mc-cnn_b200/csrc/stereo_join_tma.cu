@@ -239,13 +239,7 @@ template <int NS>
 int launch_tma(const CUtensorMap &tmL, const CUtensorMap &tmR, float *outL, float *outR, int C, int D, int H, int W, int ldo, cudaStream_t s)
 {
 	using Cfg = STCfg<NS>;
-	static bool attr_done[64] = {false};
-	int dev = 0;
-	cudaGetDevice(&dev);
-	if (!attr_done[dev & 63]) {
-		ADC_CUDA(cudaFuncSetAttribute(stereo_join_tma_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
-		attr_done[dev & 63] = true;
-	}
+	if (int rc = adc_smem_optin(stereo_join_tma_kernel<NS>, Cfg::SMEM)) return rc;
 	dim3 grid(adc_div_up(W + 3, ST_TX), H, adc_div_up(D, Cfg::DC));
 	stereo_join_tma_kernel<NS><<<grid, Cfg::NT, Cfg::SMEM, s>>>(tmL, tmR, outL, outR, C, D, H, W, ldo);
 	ADC_CHECK_LAUNCH();

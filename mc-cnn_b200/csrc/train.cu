@@ -809,12 +809,9 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	int prev = 0;
 	cudaGetDevice(&prev);
 	int rc = (int)cudaSetDevice(device);
-	int optin = 0;
-	if (!rc) rc = (int)cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
 	if (!slow) {
-		if (!rc && h->smem > optin) rc = ADCENSUS_ELIMIT;
-		if (!rc) rc = (int)cudaFuncSetAttribute(tower_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
-		if (!rc) rc = (int)cudaFuncSetAttribute(tower_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem);
+		if (!rc) rc = adc_smem_optin(tower_fwd_kernel, h->smem);
+		if (!rc) rc = adc_smem_optin(tower_bwd_kernel, h->smem);
 	}
 	for (int what = 0; what < TRAIN_NALL && !rc; what++) {
 		long n;

@@ -14,7 +14,7 @@ aggregation; index outputs stay bit-exact only as far as no arg-min is decided b
 `tile` limits the length of every prefix (a kernel works on tiles with a halo), which bounds the
 cancellation error; `dtype` is the precision the prefixes are held in.
 
-`emulate_ws` restates the kernel that ships in the default mode, cbca_ws_kernel (csrc/cbca_ws.cu), index for index in
+`emulate_ws` restates the kernel that ships in the default mode, cbca_ws_kernel (csrc/cbca_tma.cu), index for index in
 float32 numpy, with switches for the mistakes the GPU tests must be able to see.
 """
 import numpy as np
@@ -73,7 +73,7 @@ def cbca_prefix(x0c, x1c, vol, direction, dtype=np.float32, tile=(32, 128)):
     return out
 
 
-# cbca_ws.cu's constants
+# cbca_ws_kernel's constants (cbca_tma.cu)
 WS_TX, WS_TY, WS_HO, WS_TWP, WS_RING, WS_DCH, EPL = 128, 64, 32, 144, 16, 20, 9
 f32 = np.float32
 
@@ -108,7 +108,7 @@ def _row_prefix(row):
 
 
 def emulate_ws(x0c, x1c, vol, direction, R, centre=True, scrub_rule=True, run_end=0, swap_ud=False):
-    """cbca_ws_kernel<R> (cbca_ws.cu) restated index for index in numpy float32: equal D chunks of <= 20 and the nproc
+    """cbca_ws_kernel<R> (cbca_tma.cu) restated index for index in numpy float32: equal D chunks of <= 20 and the nproc
     copy of planes whose tile lies in the invalid triangle; per plane the TMA box from (x0 - HX, y0 - HALO) at the 144-float
     pitch, zero outside the image; the tile's mid pixel subtracted (centring) and NaN counted as 0 where the box reaches
     the invalid triangle (scrub); row prefixes as the prefix warps scan them (9 columns per lane, 16 lanes); each walker

@@ -256,7 +256,7 @@ MEDIAN_K = (1, 3, 5, 7, 9, 11)
 # ----------------------------------------------------------------------------------------------------------------- CBCA
 # Exact kernels (cross_cbca.cu): tile (columns, rows) and disparities per CTA
 CBCA_EXACT_KERNELS = ("win1", "win4", "loop8", "loop13", "generic")
-# constant-work kernels (cbca_ws.cu, cbca_tma.cu): cbca_ws_kernel<1, 6>, <4, 4>, cbca_tma_kernel<8>, <13>
+# constant-work kernels (cbca_tma.cu): cbca_ws_kernel<1, 6>, <4, 4>, cbca_tma_kernel<8>, <13>
 CBCA_FAST_KERNELS = ("ws1", "ws4", "tma8", "tma13")
 CBCA_TILE = {"win1": (128, 32), "win4": (128, 32), "loop8": (64, 16), "loop13": (64, 16),
              "ws1": (128, 64), "ws4": (128, 64), "tma8": (128, 32), "tma13": (128, 32)}
@@ -308,7 +308,7 @@ def clip_arms(xc, bound):
 
 
 def cbca_fast_kernel(max_arm):
-    """cbca_tma.cu adc_cbca_tma: halo = max_arm - 1: <= 1 cbca_ws<1>, <= 4 cbca_ws<4>, <= 8 cbca_tma<8>, <= 13
+    """cbca_tma.cu adc_cbca_fast: halo = max_arm - 1: <= 1 cbca_ws<1>, <= 4 cbca_ws<4>, <= 8 cbca_tma<8>, <= 13
     cbca_tma<13>, otherwise ADCENSUS_ELIMIT"""
     return _by_halo(max_arm - 1, CBCA_FAST_KERNELS + ("ELIMIT",))
 
@@ -357,7 +357,7 @@ def cbca_copy_paths(kernel, D, W, direction):
 
 
 def pipe_cbca_route(fast_mode, L1, border, D, W):
-    """pipeline.cu run_chain: 'fast' (adc_cbca_tma) when the mode is fast, max(L1, 2) - 1 <= 4 (pipe_fast_cbca_ok) and
+    """pipeline.cu run_chain: 'fast' (adc_cbca_fast) when the mode is fast, max(L1, 2) - 1 <= 4 (pipe_fast_cbca_ok) and
     not nan_in_valid; 'generic' (adc_cbca_packed with maxlen 1 << 20) when nan_in_valid = border > 0 and
     D > W - border - 1, in both modes; else 'packed' (the exact kernel of max(L1, 2))"""
     if border > 0 and D > W - border - 1:
