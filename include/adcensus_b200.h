@@ -125,6 +125,15 @@ int mccnn_sgm2_band(const float *x0, const float *x1, const float *input, float 
 		    float pi1, float pi2, float tau_so, float alpha1, float sgm_q1, float sgm_q2,
 		    int direction, int pass_mask, int zero_out, adcensus_stream_t stream);
 
+/* The fused pipeline's sgm2: all four directions of the whole image into `output` as if it were zero on entry (it is
+ * written, never read), bit-identical to mccnn_sgm2_band with pass_mask 15 and zero_out.  Forward scans store their line
+ * states in `scratch` (16-byte aligned) and the backward scans recompute from them, 7 volume passes instead of 11.
+ * mccnn_sgm2_ckpt_bytes gives the scratch it needs (0: not at this shape); with less, it runs the 11-pass kernels. */
+size_t mccnn_sgm2_ckpt_bytes(int H, int W, int D);
+int mccnn_sgm2_ckpt(const float *x0, const float *x1, const float *input, float *output, void *scratch,
+		    size_t scratch_bytes, int H, int W, int D, float pi1, float pi2, float tau_so, float alpha1,
+		    float sgm_q1, float sgm_q2, int direction, adcensus_stream_t stream);
+
 /* Wavefront split of sgm2 over ROW bands (the multi-GPU single-volume path, rowband.py).  Build the penalty-class tables
  * of the image pair once (mccnn_sgm_tables_bytes bytes; classes + the selector words of one `direction`), then run the
  * passes band by band on (H,W,D) band volumes at image row offset yoff: horizontal passes (bits 0-1) are band-local; a

@@ -32,9 +32,8 @@ int adc_cbca_fast_box(int halo, int *box_w, int *box_h);
 int adc_cbca_fast(const CUtensorMap *tm, const uint32_t *hv, const float *vol, float *out, int D, int H, int W, int ld, int direction,
 		  int halo, cudaStream_t s);
 size_t adc_sgm_table_bytes(int H, int W, int D);
-int adc_sgm2(const float *x0, const float *x1, const float *in, float *out, uint8_t *tab, int H, int W, int D,
-	     float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction,
-	     bool zero_out, cudaStream_t s);
+int adc_sgm2_ckpt(const float *x0, const float *x1, const float *in, float *out, uint8_t *tab, void *scratch, size_t scratch_bytes,
+		  int H, int W, int D, float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction, cudaStream_t s);
 int adc_transpose_dhw_pitched_to_hwd(const float *in, float *out, int D, int H, int W, int ld, cudaStream_t s);
 int adc_transpose_hwd_to_dhw_pitched_div4(const float *in, float *out, int D, int H, int W, int ld, cudaStream_t s);
 int adc_stereo_join(const float *input_L, const float *input_R, float *output_L, float *output_R,
@@ -490,8 +489,9 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 		}
 		for (int it = 0; it < sgm_i; it++) {                                                     // :1008-1020
 			STEP(adc_transpose_dhw_pitched_to_hwd(cur, spare, D, H, W, ld, ss));                 // :1008
-			STEP(adc_sgm2(imgL, imgR, spare, acc, tab, H, W, D, o.pi1, o.pi2, o.tau_so, o.alpha1,
-				      o.sgm_q1, o.sgm_q2, direction, /*zero_out=*/true, ss));                    // :1014-1016
+			// cur is dead between the two transposes: it holds SGM's line-state checkpoints
+			STEP(adc_sgm2_ckpt(imgL, imgR, spare, acc, tab, cur, (size_t)V * sizeof(float), H, W, D, o.pi1, o.pi2,
+					   o.tau_so, o.alpha1, o.sgm_q1, o.sgm_q2, direction, ss));                // :1014-1016
 			STEP(adc_transpose_hwd_to_dhw_pitched_div4(acc, cur, D, H, W, ld, ss));              // :1017-1020
 			nl += 7;
 		}

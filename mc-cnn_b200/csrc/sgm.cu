@@ -33,7 +33,13 @@
 // Layout: input/output (H,W,D) like the reference (INDEX, adcensus.cu:531-533).
 // Algorithmic traffic per call: 4 passes x (read input + read-modify-write
 // output) = 12V bytes (V = 4*D*H*W); 11V when the caller guarantees a zeroed
-// output (pipeline), because the first pass then skips the read.
+// output, because the first pass then skips the read.  The fused pipeline
+// (adc_sgm2_ckpt) has a dead volume to spare for line-state checkpoints and
+// moves 7V plus the checkpoints instead: forward scans that write only
+// checkpoints (2V), the leftward scan writing (0 + right) + left (2V), the
+// upward scan writing (out + down) + up (3V), the forward values recomputed
+// from the checkpoints.  The operator and the band entry points keep the 11V /
+// 12V kernels: they have no scratch and the band paths carry line states.
 #include "common.cuh"
 
 namespace {
@@ -179,6 +185,18 @@ __device__ __forceinline__ void read_slot(float (&r)[K], const float *slot)
 	}
 }
 
+template <int K>
+__device__ __forceinline__ void write_slot(float *slot, const float (&r)[K])
+{
+	if constexpr (K % 4 == 0) {
+#pragma unroll
+		for (int k = 0; k < K; k += 4) *reinterpret_cast<float4 *>(slot + k) = make_float4(r[k], r[k + 1], r[k + 2], r[k + 3]);
+	} else {
+#pragma unroll
+		for (int k = 0; k < K; k++) slot[k] = r[k];
+	}
+}
+
 template <int K, bool VEC>
 __device__ __forceinline__ void store_vec(const float (&r)[K], float *p, int dbase, int D)
 {
@@ -258,7 +276,7 @@ struct SgmScan {
 	// image column 0 of the band.  cring_: (vertical) this warp's class ring.
 	__device__ __forceinline__ void init(const uint8_t *tab, const float *in_, float *out_, float *ring_, unsigned *cring_,
 					      const uint8_t *srow1, const uint8_t *srow2, int H, int W_, int D_,
-					      int pad, const SgmParams &prm, int line)
+					      int pad, const SgmParams &prm, int line, int start = 0)
 	{
 		in = in_; out = out_; ring = ring_;
 		lane = threadIdx.x & 31;
@@ -271,8 +289,8 @@ struct SgmScan {
 		P1s = prm.pi1 / (prm.q1 * prm.q2); P2s = prm.pi2 / (prm.q1 * prm.q2);
 		P1m = prm.pi1 / prm.q1; P2m = prm.pi2 / prm.q1;
 		P1f_a = P1f / prm.alpha1; P1s_a = P1s / prm.alpha1; P1m_a = P1m / prm.alpha1;
-		x = SD == 0 ? 0 : (SD == 1 ? W - 1 : line);
-		y = SD == 2 ? 0 : (SD == 3 ? H - 1 : line);
+		x = SD == 0 ? start : (SD == 1 ? W - 1 - start : line);
+		y = SD == 2 ? start : (SD == 3 ? H - 1 - start : line);
 		pix_step = (long)(dy * W + dx) * D;
 		base = ((long)y * W + x) * D + dbase;
 		// NaN in the padding slots of the ring (never overwritten)
@@ -283,8 +301,9 @@ struct SgmScan {
 		// The stored difference at (y, j) pairs pixel j with its left / upper neighbour, so scans
 		// that look right / down (dx = -1, dy = -1) read the entry one further (tshift).
 		if constexpr (HORIZ) {
-			// step 0 uses no penalties; prepare step 1 = pixel x + dx
-			const int xs = clampx(x + dx);
+			// step 0 uses no penalties, so a scan from the line's start prepares step 1 = pixel x + dx; one
+			// that starts further in prepares its first step
+			const int xs = clampx(start ? x : x + dx);
 			p1 = srow1 + tshift_x;
 			const uint8_t *r2 = srow2 + tshift_x;
 			up = dx * ddir < 0;                        // slot k of the next step = slot k-1 of this one
@@ -301,7 +320,7 @@ struct SgmScan {
 			cring = cring_;
 			cstep = (long)dy * W * 32;
 			selp = reinterpret_cast<const unsigned *>(tab + sgm_sel_offset(prm.Ht, Wp)) +
-			       ((long)(y + prm.yoff + tshift_y) * W + x) * 32 + lane;       // step 0 (never fetched)
+			       ((long)(y + prm.yoff + tshift_y) * W + x) * 32 + lane;       // step `start` (never fetched when 0)
 		}
 	}
 
@@ -336,11 +355,13 @@ struct SgmScan {
 		}
 	}
 
-	// steps [s_begin, s_end) of the scan; use_out: read-modify-write the accumulator (else it is
-	// known to hold zeros).  Streams the cost (and accumulator) vectors of the next PF pixels into
-	// the shared-memory ring with cp.async; every lane fetches exactly the elements it consumes.
-	// carried: the scan continues a line whose state is already in `prev` (vertical wavefront): step 0 is an ordinary step
-	__device__ __forceinline__ void run(int s_begin, int s_end, bool use_out, bool carried = false)
+	// steps [s_begin, s_end) of the scan; use_out: stream the accumulator too (`cout`, else unset).
+	// Streams the cost (and accumulator) vectors of the next PF pixels into the shared-memory ring
+	// with cp.async; every lane fetches exactly the elements it consumes.  step(s, val, cout) takes
+	// this lane's K values of step s before they become the line state.  A step s > 0 continues
+	// from `prev`; carried: step 0 does too (the line state of a row band above, vertical wavefront).
+	template <typename Step>
+	__device__ __forceinline__ void scan(int s_begin, int s_end, bool use_out, bool carried, Step &&step)
 	{
 #pragma unroll
 		for (int u = 0; u < PF; u++) {
@@ -403,13 +424,9 @@ struct SgmScan {
 					val[k] = cin[k] + cost - m;                                        // :615
 				}
 			}
-			float o[K];
+			step(s, val, cout);
 #pragma unroll
-			for (int k = 0; k < K; k++) {
-				o[k] = (use_out ? cout[k] : 0.0f) + val[k];                            // :569 / :616
-				prev[k] = val[k];                                                      // :570 / :617
-			}
-			store_vec<K, VEC>(o, out + base, dbase, D);
+			for (int k = 0; k < K; k++) prev[k] = val[k];                                  // :570 / :617
 			// refill this ring slot with step s + PF (its values are in registers by now)
 			if (s + PF < s_end) {
 				issue_vec<K, VEC>(rs, in + base + PF * pix_step, dbase, D);
@@ -425,6 +442,17 @@ struct SgmScan {
 			}
 		}
 		asm volatile("cp.async.wait_group 0;");
+	}
+
+	// steps [s_begin, s_end) accumulated into `out`: read-modify-write when use_out, else it is known to hold zeros
+	__device__ __forceinline__ void run(int s_begin, int s_end, bool use_out, bool carried = false)
+	{
+		scan(s_begin, s_end, use_out, carried, [&](int, const float (&val)[K], const float (&cout)[K]) {
+			float o[K];
+#pragma unroll
+			for (int k = 0; k < K; k++) o[k] = (use_out ? cout[k] : 0.0f) + val[k];       // :569 / :616
+			store_vec<K, VEC>(o, out + base, dbase, D);
+		});
 	}
 };
 
@@ -585,6 +613,166 @@ int launch_all(const uint8_t *tab, const float *in, float *out, int H, int W, in
 	return rc;
 }
 
+// ---------------------------------------------------------------- checkpoint schedule (fused pipeline)
+// The four scans of a zero accumulator in 7V instead of 11V.  A forward launch runs the rightward and the downward
+// scans and writes only their line states, after every CK_H-th / CK_V-th step (checkpoint b = the state entering step
+// b * CK, at [line][b][32K] floats with ceil(L / CK) slots per line of L steps; slot 0 is unused).  The two backward launches run the leftward and the upward scans and
+// recompute the forward values block by block from those checkpoints: a block restarts from its checkpoint with the
+// same expressions, so it reproduces the forward values bit for bit.  out = (0 + right) + left, then
+// (out + down) + up: the reference's order.  CK_V = 8 keeps the upward launch's per-warp block buffer small enough
+// for one wave of column warps at D <= 256 (10 warps per SM); rows are few, so CK_H = 16 halves their checkpoints.
+constexpr int SGM_CK_H = 16, SGM_CK_V = 8, SGM_CK_PF = 6;
+
+// One launch, two kinds of CTA (one warp each): blocks [0, H) scan rows rightward, blocks [H, H + W) scan columns
+// downward (the long row scans first).  Reads `in` once; writes checkpoints only.
+template <int K, bool VEC, int PF>
+__global__ void __launch_bounds__(32)
+sgm_fwd_kernel(const uint8_t *__restrict__ tab, const float *__restrict__ in, float *__restrict__ ckh, float *__restrict__ ckv,
+	       int H, int W, int D, int pad, SgmParams prm)
+{
+	extern __shared__ __align__(16) float sgm_smem[];
+	constexpr int VSZ = 32 * K;
+	const int lane = threadIdx.x;
+	float *ring = sgm_smem + lane * K;
+	unsigned *extra = reinterpret_cast<unsigned *>(sgm_smem + PF * 2 * VSZ);
+	if ((int)blockIdx.x < H) {
+		const int line = blockIdx.x, nb = (W + SGM_CK_H - 1) / SGM_CK_H;
+		const int Wp = prm.Wt + 2 * pad, RB = sgm_row_bytes(prm.Wt, pad);
+		const long plane = (long)prm.Ht * Wp;
+		const uint8_t *s1 = sgm_stage_row(extra, tab + (long)line * Wp, Wp, lane, 32) + pad;
+		const uint8_t *s2 = sgm_stage_row(extra + RB / 4, tab + 2 * plane + (long)line * Wp, Wp, lane, 32) + pad;
+		__syncwarp();
+		SgmScan<K, VEC, 0, PF> sc;
+		sc.init(tab, in, nullptr, ring, nullptr, s1, s2, H, W, D, pad, prm, line);
+		float *ck = ckh + (size_t)line * nb * VSZ + lane * K;
+		sc.scan(0, W, false, false, [&](int s, const float (&val)[K], const float (&)[K]) {
+			if ((s + 1) % SGM_CK_H == 0 && s + 1 < W) write_slot<K>(ck + (size_t)(s + 1) / SGM_CK_H * VSZ, val);
+		});
+	} else {
+		const int line = blockIdx.x - H, nb = (H + SGM_CK_V - 1) / SGM_CK_V;
+		SgmScan<K, VEC, 2, PF> sc;
+		sc.init(tab, in, nullptr, ring, extra + lane, nullptr, nullptr, H, W, D, pad, prm, line);
+		float *ck = ckv + (size_t)line * nb * VSZ + lane * K;
+		sc.scan(0, H, false, false, [&](int s, const float (&val)[K], const float (&)[K]) {
+			if ((s + 1) % SGM_CK_V == 0 && s + 1 < H) write_slot<K>(ck + (size_t)(s + 1) / SGM_CK_V * VSZ, val);
+		});
+	}
+}
+
+// One CTA per row: warp 1 scans leftward and writes out = (0 + right) + left; warp 0 recomputes the rightward values
+// one block of CK_H columns ahead of it (blocks from the right end), into a double-buffered shared-memory block.
+template <int K, bool VEC, int PF>
+__global__ void __launch_bounds__(64)
+sgm_bwd_h_kernel(const uint8_t *__restrict__ tab, const float *__restrict__ in, float *__restrict__ out, const float *__restrict__ ckh,
+		 int H, int W, int D, int pad, SgmParams prm)
+{
+	extern __shared__ __align__(16) float sgm_smem[];
+	constexpr int VSZ = 32 * K, BLK = SGM_CK_H * VSZ;
+	const int line = blockIdx.x, wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	const int nb = (W + SGM_CK_H - 1) / SGM_CK_H;
+	float *ring = sgm_smem + (size_t)wib * PF * 2 * VSZ + lane * K;
+	float *blk = sgm_smem + 2 * PF * 2 * VSZ + lane * K;                  // [2][CK_H][32K]: block b in half b & 1
+	const int Wp = prm.Wt + 2 * pad, RB = sgm_row_bytes(prm.Wt, pad);
+	const long plane = (long)prm.Ht * Wp;
+	unsigned *rows = reinterpret_cast<unsigned *>(sgm_smem + 2 * PF * 2 * VSZ + 2 * BLK);
+	const uint8_t *s1 = sgm_stage_row(rows, tab + (long)line * Wp, Wp, threadIdx.x, 64) + pad;
+	const uint8_t *s2 = sgm_stage_row(rows + RB / 4, tab + 2 * plane + (long)line * Wp, Wp, threadIdx.x, 64) + pad;
+	__syncthreads();
+	// one barrier per block: after warp 0 has filled block b and warp 1 has finished block b + 1 (the other half)
+	if (wib == 0) {
+		SgmScan<K, VEC, 0, PF> sc;
+		for (int b = nb - 1; b >= 0; b--) {
+			const int x0 = b * SGM_CK_H;
+			sc.init(tab, in, nullptr, ring, nullptr, s1, s2, H, W, D, pad, prm, line, x0);
+			if (b > 0) read_slot<K>(sc.prev, ckh + ((size_t)line * nb + b) * VSZ + lane * K);
+			float *dst = blk + (b & 1) * BLK;
+			sc.scan(x0, min(W, x0 + SGM_CK_H), false, false,
+				[&](int s, const float (&val)[K], const float (&)[K]) { write_slot<K>(dst + (s - x0) * VSZ, val); });
+			__syncthreads();
+		}
+	} else {
+		SgmScan<K, VEC, 1, PF> sc;
+		sc.init(tab, in, out, ring, nullptr, s1, s2, H, W, D, pad, prm, line);
+		sc.scan(0, W, false, false, [&](int s, const float (&val)[K], const float (&)[K]) {
+			const int x = W - 1 - s;
+			if (s == 0 || (x + 1) % SGM_CK_H == 0) __syncthreads();       // first column of a block
+			float r[K], o[K];
+			read_slot<K>(r, blk + (x / SGM_CK_H & 1) * BLK + (x % SGM_CK_H) * VSZ);
+#pragma unroll
+			for (int k = 0; k < K; k++) o[k] = (0.0f + r[k]) + val[k];               // :569 / :616
+			store_vec<K, VEC>(o, out + sc.base, sc.dbase, D);
+		});
+	}
+}
+
+// One warp per column: the upward scan, block by block of CK_V rows from the bottom; before each block the warp
+// recomputes the downward values of its rows from their checkpoint into a shared-memory block, then writes
+// out = (out + down) + up.
+template <int K, bool VEC, int PF>
+__global__ void __launch_bounds__(32, 8)
+sgm_bwd_v_kernel(const uint8_t *__restrict__ tab, const float *__restrict__ in, float *__restrict__ out, const float *__restrict__ ckv,
+		 int H, int W, int D, int pad, SgmParams prm)
+{
+	extern __shared__ __align__(16) float sgm_smem[];
+	constexpr int VSZ = 32 * K;
+	const int line = blockIdx.x, lane = threadIdx.x;
+	const int nb = (H + SGM_CK_V - 1) / SGM_CK_V;
+	float *ring = sgm_smem + lane * K;                                     // shared by the two scans, which alternate
+	float *blk = sgm_smem + PF * 2 * VSZ + lane * K;                       // [CK_V][32K]
+	unsigned *cring = reinterpret_cast<unsigned *>(sgm_smem + PF * 2 * VSZ + SGM_CK_V * VSZ) + lane;
+	SgmScan<K, VEC, 3, PF> up;
+	up.init(tab, in, out, ring, cring, nullptr, nullptr, H, W, D, pad, prm, line);
+	for (int b = nb - 1; b >= 0; b--) {
+		const int y0 = b * SGM_CK_V, y1 = min(H, y0 + SGM_CK_V);
+		{
+			SgmScan<K, VEC, 2, PF> dn;
+			dn.init(tab, in, nullptr, ring, cring, nullptr, nullptr, H, W, D, pad, prm, line, y0);
+			if (b > 0) read_slot<K>(dn.prev, ckv + ((size_t)line * nb + b) * VSZ + lane * K);
+			dn.scan(y0, y1, false, false,
+				[&](int s, const float (&val)[K], const float (&)[K]) { write_slot<K>(blk + (s - y0) * VSZ, val); });
+		}
+		up.scan(H - y1, H - y0, true, false, [&](int s, const float (&val)[K], const float (&cout)[K]) {
+			float dv[K], o[K];
+			read_slot<K>(dv, blk + (H - 1 - s - y0) * VSZ);
+#pragma unroll
+			for (int k = 0; k < K; k++) o[k] = (cout[k] + dv[k]) + val[k];           // :616, down then up
+			store_vec<K, VEC>(o, out + up.base, up.dbase, D);
+		});
+	}
+}
+
+// shared-memory bytes of the three launches
+template <int K>
+void ckpt_smem(int W, int pad, int *f, int *h, int *v)
+{
+	constexpr int PF = SGM_CK_PF, VSZ = 32 * K;
+	const int RB = sgm_row_bytes(W, pad);
+	*f = PF * 2 * VSZ * 4 + (2 * RB > PF * 32 * 4 ? 2 * RB : PF * 32 * 4);
+	*h = 2 * PF * 2 * VSZ * 4 + 2 * SGM_CK_H * VSZ * 4 + 2 * RB;
+	*v = PF * 2 * VSZ * 4 + SGM_CK_V * VSZ * 4 + PF * 32 * 4;
+}
+
+template <int K, bool VEC>
+int launch_ckpt(const uint8_t *tab, const float *in, float *out, float *ck, int H, int W, int D, int pad, const SgmParams &prm,
+		cudaStream_t s)
+{
+	constexpr int PF = SGM_CK_PF;
+	int sf, sh, sv, rc;
+	ckpt_smem<K>(W, pad, &sf, &sh, &sv);
+	auto kf = sgm_fwd_kernel<K, VEC, PF>;
+	auto kh = sgm_bwd_h_kernel<K, VEC, PF>;
+	auto kv = sgm_bwd_v_kernel<K, VEC, PF>;
+	if ((rc = sgm_allow_smem(kf, sf)) || (rc = sgm_allow_smem(kh, sh)) || (rc = sgm_allow_smem(kv, sv))) return rc;
+	float *ckh = ck, *ckv = ck + (size_t)H * adc_div_up(W, SGM_CK_H) * 32 * K;
+	kf<<<H + W, 32, sf, s>>>(tab, in, ckh, ckv, H, W, D, pad, prm);
+	ADC_CHECK_LAUNCH();
+	kh<<<H, 64, sh, s>>>(tab, in, out, ckh, H, W, D, pad, prm);
+	ADC_CHECK_LAUNCH();
+	kv<<<W, 32, sv, s>>>(tab, in, out, ckv, H, W, D, pad, prm);
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
 }  // namespace
 
 // lanes carry 32*K disparity slots (K from D); the class tables are padded by that many columns so
@@ -664,6 +852,73 @@ int adc_sgm2(const float *x0, const float *x1, const float *in, float *out, uint
 	int rc = adc_sgm_classes(x0, x1, tab, H, W, D, tau_so, s);
 	if (rc) return rc;
 	return adc_sgm2_band(in, out, tab, H, W, D, H, W, 0, 0, pi1, pi2, tau_so, alpha1, q1, q2, direction, zero_out, 15, s);
+}
+
+// ---- the fused pipeline's sgm2 on the checkpoint schedule ---------------------------------------------------------
+// Bytes of line-state checkpoints adc_sgm2_ckpt needs at this shape; 0 when the shape cannot use the schedule (its
+// shared memory exceeds SGM_SMEM_MAX).
+size_t adc_sgm2_ckpt_bytes(int H, int W, int D)
+{
+	const int pad = sgm_slots(D);
+	int f, h, v;
+	switch (pad / 32) {
+	case 1: ckpt_smem<1>(W, pad, &f, &h, &v); break;
+	case 2: ckpt_smem<2>(W, pad, &f, &h, &v); break;
+	case 4: ckpt_smem<4>(W, pad, &f, &h, &v); break;
+	case 8: ckpt_smem<8>(W, pad, &f, &h, &v); break;
+	default: ckpt_smem<16>(W, pad, &f, &h, &v); break;
+	}
+	if (f > SGM_SMEM_MAX || h > SGM_SMEM_MAX || v > SGM_SMEM_MAX) return 0;
+	return ((size_t)H * adc_div_up(W, SGM_CK_H) + (size_t)W * adc_div_up(H, SGM_CK_V)) * pad * sizeof(float);
+}
+
+// adc_sgm2 of a zero accumulator (all four directions, whole image) in five launches like it, moving 7V instead of
+// 11V.  `scratch` (scratch_bytes, 16-byte aligned) holds the checkpoints; when it is too small, adc_sgm2 runs instead
+// (same bits).  tab: scratch of adc_sgm_table_bytes(H, W, D) bytes.  `out` is written, never read.
+int adc_sgm2_ckpt(const float *x0, const float *x1, const float *in, float *out, uint8_t *tab, void *scratch, size_t scratch_bytes,
+		  int H, int W, int D, float pi1, float pi2, float tau_so, float alpha1, float q1, float q2, int direction, cudaStream_t s)
+{
+	const size_t need = adc_sgm2_ckpt_bytes(H, W, D);
+	if (!need || need > scratch_bytes || (uintptr_t)scratch % 16)
+		return adc_sgm2(x0, x1, in, out, tab, H, W, D, pi1, pi2, tau_so, alpha1, q1, q2, direction, true, s);
+	int rc = adc_sgm_classes(x0, x1, tab, H, W, D, tau_so, s);
+	if (!rc) rc = adc_sgm_selectors(tab, W, D, H, W, 0, direction, s);
+	if (rc) return rc;
+	SgmParams prm{pi1, pi2, tau_so, alpha1, q1, q2, direction, H, W, 0, 0, nullptr, nullptr, 0, W};
+	const int pad = sgm_slots(D);
+	const bool vec = (D % 4 == 0) && (((uintptr_t)in | (uintptr_t)out) % 16 == 0);
+	float *ck = static_cast<float *>(scratch);
+	if (D <= 32) return launch_ckpt<1, false>(tab, in, out, ck, H, W, D, pad, prm, s);
+	if (D <= 64) return launch_ckpt<2, false>(tab, in, out, ck, H, W, D, pad, prm, s);
+	if (D <= 128) return vec ? launch_ckpt<4, true>(tab, in, out, ck, H, W, D, pad, prm, s)
+				 : launch_ckpt<4, false>(tab, in, out, ck, H, W, D, pad, prm, s);
+	if (D <= 256) return vec ? launch_ckpt<8, true>(tab, in, out, ck, H, W, D, pad, prm, s)
+				 : launch_ckpt<8, false>(tab, in, out, ck, H, W, D, pad, prm, s);
+	return vec ? launch_ckpt<16, true>(tab, in, out, ck, H, W, D, pad, prm, s)
+		   : launch_ckpt<16, false>(tab, in, out, ck, H, W, D, pad, prm, s);
+}
+
+extern "C" size_t mccnn_sgm2_ckpt_bytes(int H, int W, int D)
+{
+	if (H < 1 || W < 1 || D < 1 || D > ADCENSUS_MAX_DISP) return 0;
+	return adc_sgm2_ckpt_bytes(H, W, D);
+}
+
+extern "C" int mccnn_sgm2_ckpt(const float *x0, const float *x1, const float *input, float *output, void *scratch,
+			       size_t scratch_bytes, int H, int W, int D, float pi1, float pi2, float tau_so, float alpha1,
+			       float sgm_q1, float sgm_q2, int direction, adcensus_stream_t stream)
+{
+	if (!x0 || !x1 || !input || !output || input == output) return ADCENSUS_EINVAL;
+	if (H < 1 || W < 1 || D < 1 || (direction != 1 && direction != -1)) return ADCENSUS_EINVAL;
+	if (D > ADCENSUS_MAX_DISP) return ADCENSUS_ELIMIT;
+	cudaStream_t s = adc_stream(stream);
+	uint8_t *tab = nullptr;
+	int rc = adc_scratch_alloc((void **)&tab, adc_sgm_table_bytes(H, W, D), s);
+	if (rc) return rc;
+	rc = adc_sgm2_ckpt(x0, x1, input, output, tab, scratch, scratch ? scratch_bytes : 0, H, W, D, pi1, pi2, tau_so, alpha1,
+			   sgm_q1, sgm_q2, direction, s);
+	int rc2 = adc_scratch_free(tab, s);
+	return rc ? rc : rc2;
 }
 
 // ---- band-wise entry point for the row-band / column-band multi-GPU split (rowband.py) ----------
