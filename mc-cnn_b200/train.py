@@ -184,6 +184,15 @@ class Stream:
     def uniform(self, n, a, b):
         return self.raw(n) * TWO32 * (b - a) + a
 
+    def state(self):
+        """-> (MT19937 key (624,) uint32, pos, carry): everything the next raw() depends on"""
+        s = self.bg.state["state"]
+        return np.asarray(s["key"], np.uint32).copy(), int(s["pos"]), self.carry.copy()
+
+    def restore(self, key, pos, carry):
+        self.bg.state = {"bit_generator": "MT19937", "state": {"key": np.asarray(key, np.uint32), "pos": int(pos)}}
+        self.carry = np.asarray(carry, np.uint32).copy()
+
 
 def randperm(stream, n):
     """``torch.randperm(n)`` as 1-based int64 (THTensor_(randperm): n - 1 swaps, one draw each)"""
@@ -539,6 +548,37 @@ class Trainer:
 
         _check(lib().mccnn_trainer_reset_losses(self._h, self.stream.cuda_stream), "mccnn_trainer_reset_losses")
 
+    def run_chunk(self, warps, lr):
+        """run() from a WARP_DTYPE numpy array through two pinned host buffers, alternating; the host waits only before
+        it refills a buffer, for the chunk that last read it"""
+        import torch
+
+        if not hasattr(self, "_pinned"):
+            rec = WARP_DTYPE.itemsize * self.N
+            self._pinned = [torch.empty(self.chunk * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+            self._events, self._next = [None, None], 0
+        b, nbytes = self._next, warps.nbytes
+        if self._events[b] is not None:
+            self._events[b].synchronize()
+        self._pinned[b][:nbytes].numpy()[:] = warps.view(np.uint8)
+        self.run(self._pinned[b][:nbytes], lr)
+        self._events[b] = torch.cuda.Event()
+        self._events[b].record(self.stream)
+        self._next = 1 - b
+
+    def losses(self, n):
+        """the first n per-step losses since reset_losses(), float32"""
+        return self.get(TRAIN_LOSS)[:n].cpu().numpy()
+
+    def state(self):
+        """-> (parameters, momenta) float32, read after the stream has drained"""
+        self.stream.synchronize()
+        return tuple(self.get(w).cpu().numpy() for w in (TRAIN_PARAMS, TRAIN_MOMENTA))
+
+    def load_state(self, params, momenta):
+        self.set(TRAIN_PARAMS, params)
+        self.set(TRAIN_MOMENTA, momenta)
+
 
 def flatten(layers):
     return np.concatenate([np.concatenate([np.asarray(w, np.float32).reshape(-1), np.asarray(b, np.float32).reshape(-1)])
@@ -686,11 +726,185 @@ def net_path(data_root, dataset, args, arch="fast"):
     return os.path.join(data_root, "net", "net_%s.t7" % cmd_str(dataset, args, arch))
 
 
+# Checkpoints (-checkpoint_steps / -stop_after / -resume): <net file without .t7>.state.npz holds the position, the
+# parameters and momenta, the epoch's losses so far and the random stream, with a fingerprint of the run it belongs to.
+CHECKPOINT_FORMAT = 1
+EX_TEMPFAIL = 75                     # the exit status of a run stopped by -stop_after: "try again"
+
+
+class CheckpointError(ValueError):
+    """a checkpoint that cannot be resumed, or checkpoint options that cannot be honoured"""
+
+
+class Stopped(Exception):
+    """-stop_after ran out: the state is in `path`, to continue at (`epoch`, `step`)"""
+
+    def __init__(self, path, epoch, step):
+        super().__init__("stopped: checkpoint %s at epoch %d, step %d" % (path, epoch, step))
+        self.path, self.epoch, self.step = path, epoch, step
+
+
+def checkpoint_path(data_root, dataset, args, arch="fast"):
+    return net_path(data_root, dataset, args, arch)[:-len(".t7")] + ".state.npz"
+
+
+def check_checkpoint_options(checkpoint_steps=None, stop_after=None):
+    if checkpoint_steps is not None and (checkpoint_steps < 1 or checkpoint_steps % CHUNK):
+        raise CheckpointError("-checkpoint_steps %s: must be a positive multiple of the chunk size %d (checkpoints are "
+                              "taken at chunk boundaries)" % (checkpoint_steps, CHUNK))
+    if stop_after is not None and not stop_after > 0:
+        raise CheckpointError("-stop_after %s: must be a positive number of seconds" % (stop_after,))
+
+
+def fingerprint(dataset, action, o, seed, cmd, nnz, shapes, rect=None):
+    """what a checkpoint must match to be resumed: the run's options and the training set's nnz rows (a SHA-256 of their
+    bytes) and file shapes `shapes` [(name, shape)].  The pixels are not hashed."""
+    import hashlib
+
+    nnz = np.ascontiguousarray(nnz, np.float32)
+    return dict(dataset=dataset, arch=arch_of(o), action=action, o=dict(o), seed=int(seed), rect=rect, cmd_str=cmd,
+                nnz_rows=len(nnz), nnz_sha256=hashlib.sha256(nnz.tobytes()).hexdigest(),
+                shapes=[[name, [int(v) for v in shape]] for name, shape in shapes])
+
+
+def _library_version():
+    from . import adcensus
+
+    return adcensus.version()
+
+
+def save_checkpoint(path, fp, epoch, step, lr, elapsed, params, momenta, losses, stream):
+    """write the state to a temporary name, fsync it, then replace `path`: a stop during the write keeps the old file"""
+    import json
+
+    key, pos, carry = stream.state()
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        np.savez(f, format=np.int64(CHECKPOINT_FORMAT), version=np.array(_library_version()),
+                 fingerprint=np.array(json.dumps(fp, sort_keys=True)), epoch=np.int64(epoch), step=np.int64(step),
+                 lr=np.float64(lr), elapsed=np.float64(elapsed), params=np.asarray(params, np.float32),
+                 momenta=np.asarray(momenta, np.float32), losses=np.asarray(losses, np.float32), mt_key=key,
+                 mt_pos=np.int64(pos), carry=carry)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+    try:                                                                         # make the rename itself durable
+        dfd = os.open(os.path.dirname(os.path.abspath(path)), os.O_RDONLY)
+        try:
+            os.fsync(dfd)
+        finally:
+            os.close(dfd)
+    except OSError:
+        pass
+
+
+def load_checkpoint(path, fp):
+    """-> dict of the saved state; refuses a file that is truncated, of another format or of another run (naming the
+    field of the fingerprint that differs)"""
+    import json
+
+    try:
+        with np.load(path, allow_pickle=False) as z:
+            st = {k: z[k] for k in z.files}
+    except Exception as e:  # noqa: BLE001 -- a truncated zip fails in several ways
+        raise CheckpointError("%s: not a readable checkpoint (truncated?): %s" % (path, e))
+    want = ("format", "version", "fingerprint", "epoch", "step", "lr", "elapsed", "params", "momenta", "losses",
+            "mt_key", "mt_pos", "carry")
+    if "format" not in st or int(st["format"]) != CHECKPOINT_FORMAT:
+        raise CheckpointError("%s: checkpoint format %s, this library reads format %d"
+                              % (path, st["format"] if "format" in st else "missing", CHECKPOINT_FORMAT))
+    missing = [k for k in want if k not in st]
+    if missing:
+        raise CheckpointError("%s: checkpoint lacks %s (truncated?)" % (path, ", ".join(missing)))
+    got, fp = json.loads(str(st["fingerprint"])), json.loads(json.dumps(fp, sort_keys=True))
+    for k in sorted(set(got) | set(fp)):
+        if k == "o":
+            for name in sorted(set(got.get(k, {})) | set(fp[k])):
+                if got.get(k, {}).get(name) != fp[k].get(name):
+                    raise CheckpointError("%s: belongs to another run: option -%s is %s there, %s here"
+                                          % (path, name, got.get(k, {}).get(name), fp[k].get(name)))
+        elif got.get(k) != fp.get(k):
+            raise CheckpointError("%s: belongs to another run: %s is %s there, %s here" % (path, k, got.get(k), fp.get(k)))
+    out = {k: st[k] for k in ("params", "momenta", "losses", "mt_key", "carry")}
+    out.update(epoch=int(st["epoch"]), step=int(st["step"]), lr=float(st["lr"]), elapsed=float(st["elapsed"]),
+               mt_pos=int(st["mt_pos"]), version=str(st["version"]))
+    return out
+
+
+class Checkpoints:
+    """Where and when :func:`fit` writes the state: `steps` (within an epoch, a multiple of CHUNK, or None) and at every
+    epoch's end if `steps` is set; `stop_after` seconds of this process's training (or None), after which it writes the
+    state and raises :class:`Stopped` at the next chunk boundary.  `clock` is the clock of `stop_after`."""
+
+    def __init__(self, path, fp, steps=None, stop_after=None, clock=time.monotonic):
+        check_checkpoint_options(steps, stop_after)
+        self.path, self.fp, self.steps, self.stop_after, self.clock = path, fp, steps, stop_after, clock
+        self.t_begin = None
+
+    def start(self):
+        self.t_begin = self.clock()
+
+    def stop_due(self):
+        return self.stop_after is not None and self.clock() - self.t_begin >= self.stop_after
+
+    def due(self, step):
+        return self.steps is not None and step % self.steps == 0
+
+    def save(self, tr, stream, epoch, step, lr, elapsed, losses):
+        params, momenta = tr.state()
+        save_checkpoint(self.path, self.fp, epoch, step, lr, elapsed, params, momenta, losses, stream)
+
+
+def fit(tr, nnz, perm, build, o, stream, epochs=EPOCHS, log=print, ckpt=None, start=None):
+    """main.lua:779-881: the epochs of chunks from (start["epoch"], start["step"]) (or from the beginning), driving `tr`
+    (a :class:`Trainer`) with the records `build`(n steps, nnz rows) makes from `stream`; `log` receives the epoch lines.
+    With `ckpt` (:class:`Checkpoints`) the state is written at chunk boundaries and at the end of each epoch."""
+    h = o["bs"] // 2
+    nsteps = steps_per_epoch(len(nnz), o["bs"])
+    epoch0, step0 = (start["epoch"], start["step"]) if start else (1, 0)
+    t0 = time.time() - (start["elapsed"] if start else 0.0)
+    if ckpt:
+        ckpt.start()
+    for epoch in range(epoch0, epochs + 1):
+        lr = lr_at(o["lr"], epoch)
+        tr.reset_losses()
+        first = step0 if epoch == epoch0 else 0
+        done = np.asarray(start["losses"], np.float32) if start and epoch == epoch0 else np.zeros(0, np.float32)
+        for s0 in range(first, nsteps, CHUNK):
+            n = min(CHUNK, nsteps - s0)
+            rows = nnz[perm[s0 * h:(s0 + n) * h] - 1]                          # perm[t + i - 1], :820
+            tr.run_chunk(build(n, rows), lr)
+            s1 = s0 + n
+            if ckpt and s1 < nsteps:
+                stop = ckpt.stop_due()
+                if stop or ckpt.due(s1):
+                    ckpt.save(tr, stream, epoch, s1, lr, time.time() - t0, np.concatenate([done, tr.losses(s1 - first)]))
+                if stop:
+                    raise Stopped(ckpt.path, epoch, s1)
+        losses = np.concatenate([done, tr.losses(nsteps - first)]).astype(np.float64)
+        ok = (losses >= 0) & (losses < 100)                                      # :861-866
+        for v in losses[~ok]:
+            log("WARNING! err=%f" % v)
+        err = np.cumsum(losses[ok])[-1] / ok.sum() if ok.any() else float("nan")
+        log(epoch_line(epoch, err, lr, time.time() - t0))
+        if ckpt:
+            stop = epoch < epochs and ckpt.stop_due()
+            if stop or ckpt.steps is not None:
+                ckpt.save(tr, stream, epoch + 1, 0, lr_at(o["lr"], epoch + 1), time.time() - t0, np.zeros(0, np.float32))
+            if stop:
+                raise Stopped(ckpt.path, epoch + 1, 0)
+
+
 def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS,
-          rect="imperfect"):
+          rect="imperfect", checkpoint_steps=None, stop_after=None, resume=False):
     """main.lua:602-890 for arch 'fast' or 'slow' (as `o` was made): returns the saved net's file name.  `args` are main.lua's arguments after
     dataset and arch (for the file name), `stereo` the stereo method's overrides for the evaluation that follows;
-    `log` receives the printed lines.  For dataset mb the set is data.mb.<rect>_gray (see :class:`MbTrainSet`)."""
+    `log` receives the printed lines.  For dataset mb the set is data.mb.<rect>_gray (see :class:`MbTrainSet`).
+
+    Checkpoints (:func:`checkpoint_path`, next to the net): `checkpoint_steps` K writes the state every K steps of an
+    epoch and at each epoch's end; `stop_after` S writes it at the first chunk boundary after S seconds and raises
+    :class:`Stopped`; `resume` continues from the checkpoint if there is one.  A resumed run gives the bits of an
+    uninterrupted one; the checkpoint is deleted once the net file is written."""
     import torch
 
     from . import t7
@@ -698,6 +912,7 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     if action not in ("train_tr", "train_all"):
         raise ValueError("action must be train_tr or train_all, got %r" % (action,))
     check(o)
+    check_checkpoint_options(checkpoint_steps, stop_after)
     arch = arch_of(o)
     fname = net_path(data_root, dataset, args, arch)
     if os.path.exists(fname):
@@ -707,10 +922,21 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     data = evaluate.load_data(dataset, data_root, rect)
     mb = MbTrainSet(data_root, rect, action) if dataset == "mb" else None
     nnz = mb.nnz if mb else load_nnz(data, action, data_root)
+    ckpt = start = None
+    if checkpoint_steps is not None or stop_after is not None or resume:
+        shapes = [(os.path.basename(p), dims) for _, _, p, dims in mb.groups] if mb else \
+            [("x0.bin", data.X0.shape), ("x1.bin", data.X1.shape)]
+        fp = fingerprint(dataset, action, o, seed, cmd_str(dataset, args, arch), nnz, shapes, rect if mb else None)
+        ckpt = Checkpoints(checkpoint_path(data_root, dataset, args, arch), fp, checkpoint_steps, stop_after)
+        if resume and os.path.exists(ckpt.path):
+            start = load_checkpoint(ckpt.path, fp)
+        os.makedirs(os.path.dirname(ckpt.path), exist_ok=True)
     planes = mb.upload(device) if mb else None
     stream = Stream(seed)                                                        # main.lua:340
     perm = randperm(stream, len(nnz))                                            # :657
     tower, head = init_net(stream, o)                                            # :663-736
+    if start:                                                                    # the initial weights are replaced
+        stream.restore(start["mt_key"], start["mt_pos"], start["carry"])
     for line in net_lines(o):
         log(line)
     h = o["bs"] // 2
@@ -726,33 +952,11 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
             tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
             build = lambda n, rows: make_warps(draw_params(stream, o, n * h), rows, tr.ws)
         try:
-            tr.set_layers(tower, head)
-            rec = WARP_DTYPE.itemsize * tr.N
-            pinned = [torch.empty(CHUNK * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
-            events = [None, None]
-            t0 = time.time()
-            lr = o["lr"]
-            for epoch in range(1, epochs + 1):
-                if epoch == LR_DROP_EPOCH:
-                    lr = lr / 10
-                tr.reset_losses()
-                for k, s0 in enumerate(range(0, nsteps, CHUNK)):
-                    n = min(CHUNK, nsteps - s0)
-                    rows = nnz[perm[s0 * h:(s0 + n) * h] - 1]                  # perm[t + i - 1], :820
-                    warps = build(n, rows)
-                    b = k % 2
-                    if events[b] is not None:
-                        events[b].synchronize()
-                    pinned[b][:n * rec].numpy()[:] = warps.view(np.uint8)
-                    tr.run(pinned[b][:n * rec], lr)
-                    events[b] = torch.cuda.Event()
-                    events[b].record(tr.stream)
-                losses = tr.get(TRAIN_LOSS)[:nsteps].cpu().numpy().astype(np.float64)
-                ok = (losses >= 0) & (losses < 100)                              # :861-866
-                for v in losses[~ok]:
-                    log("WARNING! err=%f" % v)
-                err = np.cumsum(losses[ok])[-1] / ok.sum() if ok.any() else float("nan")
-                log(epoch_line(epoch, err, lr, time.time() - t0))
+            if start:
+                tr.load_state(start["params"], start["momenta"])
+            else:
+                tr.set_layers(tower, head)
+            fit(tr, nnz, perm, build, o, stream, epochs=epochs, log=log, ckpt=ckpt, start=start)
             tower, head = tr.net()
         finally:
             tr.close()
@@ -762,6 +966,8 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     os.makedirs(os.path.dirname(fname), exist_ok=True)
     extra = dict(rect=rect, color="gray") if mb else {}
     t7.save_net(fname, tower, head, opt=dict(o, a=action, seed=seed, gpu=device + 1, **extra))   # :883, save_net(0)
+    if ckpt and os.path.exists(ckpt.path):                                       # the net file holds the result now
+        os.remove(ckpt.path)
     ev = evaluate.Evaluator(dataset, arch, net_fname=fname, device=device, **(stereo or {}))
     try:
         if action == "train_tr":                                                 # :884-888

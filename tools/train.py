@@ -9,6 +9,18 @@ run_main.py (-L1 ... -blur_t) for the evaluation that follows.  The net goes to 
 main.lua's arguments.  Everything the trainer does not implement is refused before any GPU work; see mc-cnn_b200/train.py.
 The slow architecture is trained by tools/train_slow.py, and both architectures on Middlebury by tools/train_mb.py; both
 share this parser.
+
+Checkpoints (none of these three is part of the net's name):
+
+    -checkpoint_steps K   write the training state every K steps of an epoch (K a positive multiple of 256, the chunk
+                          size) and at the end of every epoch, to <data_root>/net/net_<cmd_str>.state.npz
+    -stop_after S         at the first chunk boundary after S seconds of training, write the state and exit with 75
+    -resume               continue from this command line's checkpoint if there is one, otherwise start fresh
+
+    while python tools/train.py kitti fast -a train_tr -data_root /data -resume -stop_after 3000; [ $? -eq 75 ]; do :; done
+
+A resumed run prints the remaining epoch lines and writes the net an uninterrupted run would, bit for bit; the checkpoint is
+deleted once the net file is written.  A checkpoint of other options or another training set is refused.
 """
 import argparse
 import os
@@ -18,7 +30,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from run_main import PRESET_OPTIONS, _flag  # noqa: E402
 
-TOOL_ONLY = ("-data_root", "-out")
+TOOL_ONLY = ("-data_root", "-out", "-checkpoint_steps", "-stop_after")     # options with a value
+TOOL_FLAGS = ("-resume",)
 
 
 def _names(mb):
@@ -39,6 +52,9 @@ def parser(prog="train.py", description=__doc__.splitlines()[0], mb=False):
     ap.add_argument("-out", default="out")
     ap.add_argument("-subset", type=float, default=1)
     ap.add_argument("-debug", nargs="?", const=True, default=False, type=_flag)
+    ap.add_argument("-checkpoint_steps", type=int, default=None)
+    ap.add_argument("-stop_after", type=float, default=None)
+    ap.add_argument("-resume", action="store_true")
     if mb:
         ap.add_argument("-rect", choices=("perfect", "imperfect"), default="imperfect")
         ap.add_argument("-color", default="gray")
@@ -57,7 +73,7 @@ def main_args(argv):
             skip = False
         elif a in TOOL_ONLY:
             skip = True
-        elif not a.startswith(TOOL_ONLY):
+        elif a not in TOOL_FLAGS and not a.startswith(TOOL_ONLY):
             out.append(a)
     return out
 
@@ -100,6 +116,10 @@ def parse_args(argv=None, arch="fast"):
         raise SystemExit("%s: -subset %s is not supported (the whole training set is used)" % (prog, args.subset))
     if args.debug:
         raise SystemExit("%s: -debug (a net file per epoch) is not supported" % prog)
+    try:
+        train.check_checkpoint_options(args.checkpoint_steps, args.stop_after)
+    except ValueError as e:
+        raise SystemExit("%s: %s" % (prog, e))
     given = {k: getattr(args, k) for k in _names(mb) if getattr(args, k) is not None}
     try:
         o = train.options(args.dataset, args.arch, **given)
@@ -127,11 +147,15 @@ def main(argv=None, arch="fast"):
         except (OSError, ValueError) as e:
             raise SystemExit("%s: %s" % (prog, e))
     print(" ".join(args.argv) + " ", flush=True)                                  # main.lua:6-9
+    ckpt = dict(checkpoint_steps=args.checkpoint_steps, stop_after=args.stop_after, resume=args.resume)
     try:
         train.train(args.dataset, args.a, o, args=main_args(args.argv), data_root=args.data_root, seed=args.seed,
-                    device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True), **rect)
-    except MemoryError as e:                                                      # the mb planes do not fit
+                    device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True), **rect, **ckpt)
+    except (MemoryError, train.CheckpointError) as e:                            # the mb planes do not fit, a bad checkpoint
         raise SystemExit("%s: %s" % (prog, e))
+    except train.Stopped as e:
+        print("%s: %s" % (prog, e), file=sys.stderr, flush=True)
+        return train.EX_TEMPFAIL
     return 0
 
 
