@@ -531,6 +531,49 @@ int mccnn_trainer_create_slow_pairs(mccnn_trainer **h, int l1, int fm, int l2, i
 				    const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
 				    adcensus_stream_t stream);
 
+/* Data-parallel training: the trainer of rank `rank` of `world` ranks (a power of two, at most 256 and at most 2 bs, else
+ * ADCENSUS_ELIMIT), each on its own device with the same pair table, parameters and momenta.  A step is three segments,
+ * each a captured graph, with two all-gathers the caller runs on `stream` between them: after segment 0 of
+ * SHARD_TOWER_OUT, after segment 1 of SHARD_WGRAD_PART, every rank's slots (mccnn_trainer_shard_slot) from that rank.
+ * The parameters, momenta and losses are then those of the one-GPU trainer of the same arch, bit for bit, on every rank.
+ *
+ * 'fast' (mccnn_trainer_create_shard): rank r holds the batch's patches n = r, r + world, ... as its patches 0, 1, ...;
+ * mccnn_trainer_size's PATCHES, TOWER and DZ are that share.
+ *   segment 0: the sampler and the tower on the rank's patches; its last layer -> its slot of SHARD_TOWER_OUT;
+ *   segment 1: Normalize2 / StereoJoin1 / Margin2 on the whole batch (every rank the same), the tower's backward pass on
+ *              the rank's patches and its partial weight gradient (levels 128 .. world of wgrad's tree) -> its slot of
+ *              SHARD_WGRAD_PART;
+ *   segment 2: the tree's levels world / 2 .. 1 over the ranks' partials, then the update.
+ * 'slow' (mccnn_trainer_create_slow_shard): the buffers are the whole batch's.  Rank r owns the patches [N r / world,
+ * N (r + 1) / world) and in each tower layer the weight-gradient splits that start in them (mccnn_trainer_slow_shard_plan);
+ * it runs the tower on its patches and on those its splits read past them.
+ *   segment 0: the sampler and the tower forward; SHARD_TOWER_OUT is the last layer (ROWS), the rank's slot its rows;
+ *   segment 1: the Linear layers, BCE and their gradients on the whole batch, the tower backward, the rank's splits of
+ *              each layer's weight gradient; SHARD_WGRAD_PART is the split workspace, one slot per layer (piece);
+ *   segment 2: the splits added in split order, then the update.
+ * mccnn_trainer_run and _step_patches refuse a shard; get / set / size / reset_losses work as for the others, and
+ * launches_per_step counts the kernels of the three segments. */
+int mccnn_trainer_create_shard(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom,
+			       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
+			       int world, adcensus_stream_t stream);
+int mccnn_trainer_create_slow_shard(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom,
+				    const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
+				    int world, adcensus_stream_t stream);
+/* the next nsteps <= chunk steps' records of the patches the rank samples, (nsteps, its share) mccnn_warp ('fast': the
+ * patches rank, rank + world, ...; 'slow': the patches plan[0] .. plan[2] - 1), and the lr; then call the segments 0,
+ * 1, 2 once per step, in order */
+int mccnn_trainer_shard_begin(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr, adcensus_stream_t stream);
+int mccnn_trainer_shard_segment(mccnn_trainer *h, int segment, adcensus_stream_t stream);
+/* a gathered buffer (trainer-owned device memory, *count floats), its number of pieces, and the slot of piece `piece`
+ * that rank `rank` owns (offset and count in floats; a count may be 0) */
+enum { MCCNN_SHARD_TOWER_OUT, MCCNN_SHARD_WGRAD_PART };
+int mccnn_trainer_shard_buffer(mccnn_trainer *h, int what, float **ptr, long long *count);
+int mccnn_trainer_shard_pieces(mccnn_trainer *h, int what);
+int mccnn_trainer_shard_slot(mccnn_trainer *h, int what, int piece, int rank, long long *offset, long long *count);
+/* HOST helper: a slow shard's share for (l1, fm, bs) -> plan (3 + 3 l1): the patches it owns [plan[0], plan[1]), the end
+ * plan[2] of the patches it runs, then per layer k the splits it owns [plan[3 + 3k], plan[4 + 3k]) of plan[5 + 3k] */
+int mccnn_trainer_slow_shard_plan(int l1, int fm, int bs, int rank, int world, long long *plan);
+
 /* The trainer's buffers, for get / set (set: PARAMS and MOMENTA only) and the tests.  Sizes in floats from
  * mccnn_trainer_size.  TOWER: every layer's output, layer k (N, fm, s_k, s_k) after the previous layers, s_k = ws - 2k, post
  * ReLU except the last ('fast') or post ReLU ('slow'); DZ: the gradient of the loss wrt each layer's pre-activation output,

@@ -266,17 +266,20 @@ __global__ void tower_bwd_kernel(Layout L, const float *__restrict__ P, const fl
 	}
 }
 
-// layer k's gradient: block (ci, co) writes G's 9 weights of (co, ci) and, for ci == 0, the bias of co
-__global__ void __launch_bounds__(WG_NT) wgrad_kernel(Layout L, int k, const float *__restrict__ X, const float *__restrict__ act,
-						      const float *__restrict__ dz, float *__restrict__ G)
+// layer k's gradient over the L.N patches of X / act / dz with NT threads: thread t sums patches t, t + NT, ... in order,
+// then a shared-memory tree with strides NT / 2 .. 1; block (ci, co) writes G's 9 weights of (co, ci) and, for ci == 0, the
+// bias of co
+template <int NT>
+__device__ __forceinline__ void wgrad_block(const Layout &L, int k, const float *__restrict__ X, const float *__restrict__ act,
+					    const float *__restrict__ dz, float *__restrict__ G)
 {
-	__shared__ float red[10][WG_NT];
+	__shared__ float red[10][NT];
 	const int ci = blockIdx.x, co = blockIdx.y, fm = L.fm, cin = k ? fm : 1;
 	const int so = side(L, k), si = so + 2;
 	float acc[10];
 #pragma unroll
 	for (int j = 0; j < 10; j++) acc[j] = 0.f;
-	for (int n = threadIdx.x; n < L.N; n += WG_NT) {
+	for (int n = threadIdx.x; n < L.N; n += NT) {
 		const float *gz = dz + L.aoff[k] + ((long)n * fm + co) * so * so;
 		const float *a = k ? act + L.aoff[k - 1] + ((long)n * fm + ci) * si * si : X + (long)n * si * si;
 		for (int y = 0; y < so; y++)
@@ -292,14 +295,50 @@ __global__ void __launch_bounds__(WG_NT) wgrad_kernel(Layout L, int k, const flo
 #pragma unroll
 	for (int j = 0; j < 10; j++) red[j][threadIdx.x] = acc[j];
 	__syncthreads();
-	for (int s = WG_NT / 2; s > 0; s >>= 1) {
+	for (int s = NT / 2; s > 0; s >>= 1) {
 		if (threadIdx.x < s)
 #pragma unroll
 			for (int j = 0; j < 10; j++) red[j][threadIdx.x] += red[j][threadIdx.x + s];
 		__syncthreads();
 	}
-	if (threadIdx.x < 9) G[L.woff[k] + ((long)co * cin + ci) * 9 + threadIdx.x] = red[threadIdx.x][0];
-	if (threadIdx.x == 9 && ci == 0) G[L.boff[k] + co] = red[9][0];
+	if constexpr (NT >= 10) {
+		if (threadIdx.x < 9) G[L.woff[k] + ((long)co * cin + ci) * 9 + threadIdx.x] = red[threadIdx.x][0];
+		if (threadIdx.x == 9 && ci == 0) G[L.boff[k] + co] = red[9][0];
+	} else {
+		for (int j = threadIdx.x; j < 10; j += NT) {
+			if (j < 9) G[L.woff[k] + ((long)co * cin + ci) * 9 + j] = red[j][0];
+			else if (ci == 0) G[L.boff[k] + co] = red[9][0];
+		}
+	}
+}
+
+__global__ void __launch_bounds__(WG_NT) wgrad_kernel(Layout L, int k, const float *__restrict__ X, const float *__restrict__ act,
+						      const float *__restrict__ dz, float *__restrict__ G)
+{
+	wgrad_block<WG_NT>(L, k, X, act, dz, G);
+}
+
+// Data parallel over R = WG_NT / NT ranks, rank r holding the patches n = r, r + R, ... as its local patches 0, 1, ...:
+// wgrad_kernel's thread t = r + R u sums exactly the patches r + R u, r + R u + 256, ..., which are this rank's local
+// patches u, u + NT, ...; the tree levels 128 .. R of wgrad_kernel only ever add a thread of residue r to another of
+// residue r, and in local numbering they are levels NT / 2 .. 1.  So this kernel on the rank's patches writes to G the
+// value wgrad_kernel's red[][r] holds after level R, bit for bit; wgrad_ranks_kernel runs the levels R / 2 .. 1.
+template <int NT>
+__global__ void __launch_bounds__(NT) wgrad_residue_kernel(Layout L, int k, const float *__restrict__ X,
+							   const float *__restrict__ act, const float *__restrict__ dz,
+							   float *__restrict__ G)
+{
+	wgrad_block<NT>(L, k, X, act, dz, G);
+}
+
+// wgrad_kernel's tree levels R / 2 .. 1 over the ranks' partial sums part (R, n), rank-major, in place; G = the root
+__global__ void wgrad_ranks_kernel(float *__restrict__ part, int R, long n, float *__restrict__ G)
+{
+	const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	for (int s = R / 2; s > 0; s >>= 1)
+		for (int t = 0; t < s; t++) part[t * n + i] = __fadd_rn(part[t * n + i], part[(t + s) * n + i]);
+	G[i] = part[i];
 }
 
 __global__ void update_kernel(float *__restrict__ P, float *__restrict__ V, const float *__restrict__ G, long n, float mom,
@@ -432,6 +471,18 @@ struct ConvWgrad {
 	__device__ void store(int m, int c, float acc, int z) const { part[((long)z * M + m) * N + c] = acc; }
 };
 
+// ConvWgrad's splits z0 .. z1 - 1 alone, launched as splits 0 .. z1 - z0 - 1: k is shifted by kbase = z0 kchunk and
+// op.part points at split z0, K ends where split z1 - 1 ends.  Each split is the same fmaf chain over the same k-range
+// as in the whole launch, so it writes the same bits.
+struct ConvWgradRange {
+	int M, N, K, kchunk;
+	ConvWgrad op;
+	int kbase;
+	__device__ float a(int m, int k) const { return op.a(m, k + kbase); }
+	__device__ float b(int k, int c) const { return op.b(k + kbase, c); }
+	__device__ void store(int m, int c, float acc, int z) const { op.store(m, c, acc, z); }
+};
+
 // Linear + ReLU: Y (bs, out) = ReLU(X (bs, in) W^T + b)
 struct FcFwd {
 	int M, N, K, kchunk;
@@ -549,6 +600,43 @@ void launch_gemm(const Op &op, int nsplit, cudaStream_t s)
 	gemm_kernel<Op><<<dim3(adc_div_up(op.N, BN), adc_div_up(op.M, BM), nsplit), GT, 0, s>>>(op);
 }
 
+// split each tower layer's weight-gradient GEMM (K = N s_k^2) so that it has about 256 blocks of at least 256 k each; the
+// split depends on the shapes only, so the summation order (and the bits) do not depend on the device
+void split_k(const Layout &L, SlowLayout &S)
+{
+	long poff = 0;
+	for (int k = 0; k < L.l1; k++) {
+		const int cin = k ? L.fm : 1, s = L.ws - 2 * (k + 1), K = L.N * s * s;
+		const int tiles = adc_div_up(L.fm, BM) * adc_div_up(cin * 9 + 1, BN);
+		const int want = std::max(1, std::min(adc_div_up(256, tiles), adc_div_up(K, 256)));
+		S.kchunk[k] = adc_div_up(adc_div_up(K, want), BK) * BK;
+		S.nsplit[k] = adc_div_up(K, S.kchunk[k]);
+		S.poff[k] = poff; poff += (long)S.nsplit[k] * L.fm * (cin * 9 + 1);
+	}
+}
+
+// A slow shard's share of the batch: rank r of R owns the patches [b0, b1) = [N r / R, N (r + 1) / R) and, in each tower
+// layer k, the weight-gradient splits whose first k-index falls in them, [z0[k], z1[k]) (each split has one owner).  It
+// runs the tower forward and backward on [b0, e): e >= b1 is the end of the last patch its splits read.
+struct SlowPlan {
+	int b0, b1, e, z0[LMAX], z1[LMAX];
+};
+
+SlowPlan slow_plan(const Layout &L, const SlowLayout &S, int rank, int world)
+{
+	SlowPlan p;
+	p.b0 = (int)((long)L.N * rank / world);
+	p.b1 = (int)((long)L.N * (rank + 1) / world);
+	p.e = p.b1;
+	for (int k = 0; k < L.l1; k++) {
+		const long P = (long)(L.ws - 2 * (k + 1)) * (L.ws - 2 * (k + 1)), K = L.N * P, kc = S.kchunk[k];
+		p.z0[k] = (int)((p.b0 * P + kc - 1) / kc);
+		p.z1[k] = (int)std::min<long>(S.nsplit[k], (p.b1 * P + kc - 1) / kc);
+		if (p.z1[k] > p.z0[k]) p.e = std::max(p.e, (int)((std::min(K, p.z1[k] * kc) + P - 1) / P));
+	}
+	return p;
+}
+
 }  // namespace
 
 struct mccnn_trainer {
@@ -568,56 +656,94 @@ struct mccnn_trainer {
 	int slow;
 	SlowLayout S;
 	float *rows, *fc, *sig, *bce_grad, *rows_grad, *fc_dz, *term, *dzo, *part, *bce_loss;
+	// a shard (rank of world > 0 ranks).  'fast': L covers the rank's patches n = rank + world j as local patches j, Lh the
+	// whole batch's last layer for head_kernel; nh the head's patches (L.N on one GPU).  'slow': L is the whole batch's,
+	// `plan` the rank's patches and splits.  nw: the warp records of one step.
+	int nh, rank, world, nmax, nw;
+	int shard_launches;                      // the kernel nodes of the three segments' graphs
+	SlowPlan plan;
+	long ntower;
+	Layout Lh;
+	float *hact, *hdz, *gact, *gpart;        // the batch's last layer and its head dz; the two gathered buffers
+	cudaGraphExec_t seg[3];
 };
 
-static int enqueue_slow(mccnn_trainer *h, cudaStream_t s)
+// The slow step on patches [n0, n1) and, per tower layer k, the weight-gradient splits [z0[k], z1[k]): the whole batch
+// and every split on one GPU; a shard's range and splits (slow_plan) otherwise.  Stage 0 is the tower forward, stage 1
+// the Linear layers, BCE and the backward passes, stage 2 the reduction of the splits and the update.  A patch's tower,
+// forward and backward, reads no other patch, and each output of ConvFwd / ConvBwdData is one thread's fmaf chain over
+// k, so a patch gets the same bits in any column range.
+static int enqueue_slow_stage(mccnn_trainer *h, cudaStream_t s, int stage, int n0, int n1, const int *z0, const int *z1)
 {
 	const Layout &L = h->L;
 	const SlowLayout &S = h->S;
-	const int bs = L.N / 2, fm = L.fm, nh2 = S.nh2, l2 = S.l2;
-	for (int k = 0; k < L.l1; k++) {                                         // tower forward
-		const int cin = k ? fm : 1, si = L.ws - 2 * k, so = si - 2;
-		const ConvFwd op{fm, L.N * so * so, cin * 9, cin * 9, cin, si, so, k ? h->act + L.aoff[k - 1] : h->X,
-				 h->P + L.woff[k], h->P + L.boff[k], h->act + L.aoff[k]};
-		launch_gemm(op, 1, s);
+	const int bs = L.N / 2, fm = L.fm, nh2 = S.nh2, l2 = S.l2, n = n1 - n0;
+	if (stage == 0) {
+		for (int k = 0; k < L.l1; k++) {                                 // tower forward
+			const int cin = k ? fm : 1, si = L.ws - 2 * k, so = si - 2;
+			const ConvFwd op{fm, n * so * so, cin * 9, cin * 9, cin, si, so,
+					 (k ? h->act + L.aoff[k - 1] : h->X) + (long)n0 * cin * si * si, h->P + L.woff[k],
+					 h->P + L.boff[k], h->act + L.aoff[k] + (long)n0 * fm * so * so};
+			launch_gemm(op, 1, s);
+		}
+	} else if (stage == 1) {
+		const float *x = h->rows;
+		for (int j = 0; j < l2; j++) {                                   // Linear + ReLU
+			const int in = j ? nh2 : 2 * fm;
+			const FcFwd op{bs, nh2, in, in, x, h->P + S.fwoff[j], h->P + S.fboff[j], h->fc + (long)j * bs * nh2};
+			launch_gemm(op, 1, s);
+			x = op.y;
+		}
+		slow_head_kernel<<<1, 512, 0, s>>>(bs, nh2, x, h->P + S.fwoff[l2], h->P + S.fboff[l2],
+						  h->fc + (long)l2 * bs * nh2, h->sig, h->bce_grad, h->term, h->dzo,
+						  h->fc_dz + (long)(l2 - 1) * bs * nh2, h->G + S.fwoff[l2], h->G + S.fboff[l2],
+						  h->bce_loss);
+		for (int j = l2 - 1; j >= 0; j--) {                              // Linear backward
+			const int in = j ? nh2 : 2 * fm;
+			const float *dz = h->fc_dz + (long)j * bs * nh2, *xj = j ? h->fc + (long)(j - 1) * bs * nh2 : h->rows;
+			const FcBwdData op{bs, in, nh2, nh2, dz, h->P + S.fwoff[j], xj,
+					   j ? h->fc_dz + (long)(j - 1) * bs * nh2 : h->dz + L.aoff[L.l1 - 1],
+					   j ? nullptr : h->rows_grad};
+			launch_gemm(op, 1, s);
+			const FcWgrad og{nh2, in + 1, bs, bs, dz, xj, h->G + S.fwoff[j], h->G + S.fboff[j]};
+			launch_gemm(og, 1, s);
+		}
+		for (int k = L.l1 - 1; k >= 1; k--) {                            // tower backward
+			const int so = L.ws - 2 * (k + 1), si = so + 2;
+			const long o = (long)n0 * fm * si * si;
+			const ConvBwdData op{fm, n * si * si, fm * 9, fm * 9, fm, si, so, h->P + L.woff[k],
+					     h->dz + L.aoff[k] + (long)n0 * fm * so * so, h->act + L.aoff[k - 1] + o,
+					     h->dz + L.aoff[k - 1] + o};
+			launch_gemm(op, 1, s);
+		}
+		for (int k = 0; k < L.l1; k++) {                                 // tower weight gradients, split over k
+			const int cin = k ? fm : 1, so = L.ws - 2 * (k + 1);
+			const ConvWgrad op{fm, cin * 9 + 1, L.N * so * so, S.kchunk[k], cin, so + 2, so, h->dz + L.aoff[k],
+					   k ? h->act + L.aoff[k - 1] : h->X, h->part + S.poff[k]};
+			if (z0[k] == 0 && z1[k] == S.nsplit[k]) {
+				launch_gemm(op, S.nsplit[k], s);
+			} else if (z1[k] > z0[k]) {
+				const int kbase = z0[k] * S.kchunk[k];
+				ConvWgradRange r{op.M, op.N, std::min(op.K, z1[k] * S.kchunk[k]) - kbase, op.kchunk, op, kbase};
+				r.op.part += (long)z0[k] * op.M * op.N;
+				launch_gemm(r, z1[k] - z0[k], s);
+			}
+		}
+	} else {
+		const long ntower = L.boff[L.l1 - 1] + fm;
+		wgrad_reduce_kernel<<<adc_div_up(ntower, 256), 256, 0, s>>>(L, S, h->part, h->G);
+		update_kernel<<<adc_div_up(h->nparam, 256), 256, 0, s>>>(h->P, h->V, h->G, h->nparam, h->mom, h->neg_lr,
+									 h->bce_loss, 1, h->loss, h->loss_cap, h->ctr);
 	}
-	const float *x = h->rows;
-	for (int j = 0; j < l2; j++) {                                           // Linear + ReLU
-		const int in = j ? nh2 : 2 * fm;
-		const FcFwd op{bs, nh2, in, in, x, h->P + S.fwoff[j], h->P + S.fboff[j], h->fc + (long)j * bs * nh2};
-		launch_gemm(op, 1, s);
-		x = op.y;
-	}
-	slow_head_kernel<<<1, 512, 0, s>>>(bs, nh2, x, h->P + S.fwoff[l2], h->P + S.fboff[l2], h->fc + (long)l2 * bs * nh2,
-					  h->sig, h->bce_grad, h->term, h->dzo, h->fc_dz + (long)(l2 - 1) * bs * nh2,
-					  h->G + S.fwoff[l2], h->G + S.fboff[l2], h->bce_loss);
-	for (int j = l2 - 1; j >= 0; j--) {                                      // Linear backward
-		const int in = j ? nh2 : 2 * fm;
-		const float *dz = h->fc_dz + (long)j * bs * nh2, *xj = j ? h->fc + (long)(j - 1) * bs * nh2 : h->rows;
-		const FcBwdData op{bs, in, nh2, nh2, dz, h->P + S.fwoff[j], xj,
-				   j ? h->fc_dz + (long)(j - 1) * bs * nh2 : h->dz + L.aoff[L.l1 - 1], j ? nullptr : h->rows_grad};
-		launch_gemm(op, 1, s);
-		const FcWgrad og{nh2, in + 1, bs, bs, dz, xj, h->G + S.fwoff[j], h->G + S.fboff[j]};
-		launch_gemm(og, 1, s);
-	}
-	for (int k = L.l1 - 1; k >= 1; k--) {                                    // tower backward
-		const int so = L.ws - 2 * (k + 1), si = so + 2;
-		const ConvBwdData op{fm, L.N * si * si, fm * 9, fm * 9, fm, si, so, h->P + L.woff[k], h->dz + L.aoff[k],
-				     h->act + L.aoff[k - 1], h->dz + L.aoff[k - 1]};
-		launch_gemm(op, 1, s);
-	}
-	for (int k = 0; k < L.l1; k++) {                                         // tower weight gradients, split over k
-		const int cin = k ? fm : 1, so = L.ws - 2 * (k + 1);
-		const ConvWgrad op{fm, cin * 9 + 1, L.N * so * so, S.kchunk[k], cin, so + 2, so, h->dz + L.aoff[k],
-				   k ? h->act + L.aoff[k - 1] : h->X, h->part + S.poff[k]};
-		launch_gemm(op, S.nsplit[k], s);
-	}
-	const long ntower = L.boff[L.l1 - 1] + fm;
-	wgrad_reduce_kernel<<<adc_div_up(ntower, 256), 256, 0, s>>>(L, S, h->part, h->G);
-	update_kernel<<<adc_div_up(h->nparam, 256), 256, 0, s>>>(h->P, h->V, h->G, h->nparam, h->mom, h->neg_lr, h->bce_loss, 1,
-								 h->loss, h->loss_cap, h->ctr);
 	ADC_CHECK_LAUNCH();
 	return 0;
+}
+
+static int enqueue_slow(mccnn_trainer *h, cudaStream_t s)
+{
+	int z0[LMAX] = {}, rc = 0;
+	for (int stage = 0; stage < 3 && !rc; stage++) rc = enqueue_slow_stage(h, s, stage, 0, h->L.N, z0, h->S.nsplit);
+	return rc;
 }
 
 static int enqueue_step(mccnn_trainer *h, cudaStream_t s, bool sample)
@@ -641,17 +767,91 @@ static int enqueue_step(mccnn_trainer *h, cudaStream_t s, bool sample)
 	return 0;
 }
 
-static int capture(mccnn_trainer *h, bool sample, cudaGraphExec_t *exec)
+// the patches n = q, q + R, ... of N: rank q's share
+static int shard_count(int N, int R, int q) { return (N - q + R - 1) / R; }
+
+// wgrad_residue_kernel<WG_NT / R>, by log2(R)
+using WgradFn = void (*)(Layout, int, const float *, const float *, const float *, float *);
+static const WgradFn RESIDUE_KERNELS[] = {wgrad_residue_kernel<256>, wgrad_residue_kernel<128>, wgrad_residue_kernel<64>,
+					  wgrad_residue_kernel<32>,  wgrad_residue_kernel<16>,  wgrad_residue_kernel<8>,
+					  wgrad_residue_kernel<4>,   wgrad_residue_kernel<2>,   wgrad_residue_kernel<1>};
+static_assert(WG_NT == 256, "one residue kernel per power of two up to WG_NT");
+
+// One step of a shard, segment `seg` of three.  'slow': enqueue_slow_stage on the plan's patches and splits, the sampler
+// first; the caller all-gathers the last layer's rows after segment 0 and the split partials after segment 1.  'fast':
+// the caller all-gathers gact after segment 0 and gpart after segment 1 (every rank's slot from its owner):
+//   0  the sampler and the tower on the rank's patches; its last layer -> gact slot `rank`
+//   1  the batch's last layer from gact in batch order -> head_kernel on the whole batch (as on one GPU) -> the rank's
+//      rows of its dz -> tower_bwd and wgrad_residue_kernel on the rank's patches -> gpart slot `rank`
+//   2  wgrad_ranks_kernel: the gradient; update_kernel
+static int enqueue_shard(mccnn_trainer *h, cudaStream_t s, int seg)
+{
+	const Layout &L = h->L;
+	if (h->slow) {                          // the all-gathers: the tower's last layer (ROWS), then the split partials
+		const SlowPlan &p = h->plan;
+		if (seg == 0)
+			train_sample_kernel<<<adc_div_up((long)h->nw * L.ws * L.ws, 128), 128, 0, s>>>(
+				h->pairs, h->n_pairs, h->warps, h->ctr, h->nw, L.ws, h->X + (long)p.b0 * L.ws * L.ws);
+		return enqueue_slow_stage(h, s, seg, p.b0, p.e, p.z0, p.z1);
+	}
+	const int fm = L.fm, R = h->world, r = h->rank, last = L.l1 - 1;
+	const size_t row = (size_t)fm * sizeof(float);
+	if (seg == 0) {
+		const long tot = (long)L.N * L.ws * L.ws;
+		train_sample_kernel<<<adc_div_up(tot, 128), 128, 0, s>>>(h->pairs, h->n_pairs, h->warps, h->ctr, L.N, L.ws, h->X);
+		tower_fwd_kernel<<<L.N, 256, h->smem, s>>>(L, h->X, h->P, h->act, h->bufsz);
+		ADC_CUDA(cudaMemcpyAsync(h->gact + (long)r * h->nmax * fm, h->act + L.aoff[last], L.N * row,
+					 cudaMemcpyDeviceToDevice, s));
+	} else if (seg == 1) {
+		for (int q = 0; q < R; q++)                                      // rank q's patch j is patch q + R j
+			ADC_CUDA(cudaMemcpy2DAsync(h->hact + (long)q * fm, R * row, h->gact + (long)q * h->nmax * fm, row, row,
+						   shard_count(h->nh, R, q), cudaMemcpyDeviceToDevice, s));
+		head_kernel<<<h->nh / 4, 4 * fm, 0, s>>>(h->Lh, h->hact, h->margin, h->pow2, h->norm, h->nout, h->join, h->gjoin,
+							 h->hinge, h->gout, h->hdz);
+		ADC_CUDA(cudaMemcpy2DAsync(h->dz + L.aoff[last], row, h->hdz + (long)r * fm, R * row, row, L.N,
+					   cudaMemcpyDeviceToDevice, s));
+		tower_bwd_kernel<<<L.N, 256, h->smem, s>>>(L, h->P, h->act, h->dz, h->bufsz);
+		int lg = 0;
+		while ((1 << lg) < R) lg++;
+		for (int k = 0; k < L.l1; k++)
+			RESIDUE_KERNELS[lg]<<<dim3(k ? fm : 1, fm), WG_NT / R, 0, s>>>(L, k, h->X, h->act, h->dz,
+											 h->gpart + (long)r * h->ntower);
+	} else {
+		wgrad_ranks_kernel<<<adc_div_up(h->ntower, 256), 256, 0, s>>>(h->gpart, R, h->ntower, h->G);
+		update_kernel<<<adc_div_up(h->nparam, 256), 256, 0, s>>>(h->P, h->V, h->G, h->nparam, h->mom, h->neg_lr, h->hinge,
+									 h->nh / 4, h->loss, h->loss_cap, h->ctr);
+	}
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
+template <class Enqueue>
+static int capture_with(mccnn_trainer *h, Enqueue enqueue, cudaGraphExec_t *exec, int *kernels = nullptr)
 {
 	cudaGraph_t g = nullptr;
 	ADC_CUDA(cudaStreamBeginCapture(h->cap, cudaStreamCaptureModeThreadLocal));
-	const int rc = enqueue_step(h, h->cap, sample);
+	const int rc = enqueue(h->cap);
 	const cudaError_t e = cudaStreamEndCapture(h->cap, &g);
 	if (rc) { if (g) cudaGraphDestroy(g); return rc; }
 	ADC_CUDA(e);
+	if (kernels) {                                                           // add the graph's kernel launches
+		size_t n = 0;
+		cudaGraphGetNodes(g, nullptr, &n);
+		std::vector<cudaGraphNode_t> nodes(n);
+		cudaGraphGetNodes(g, nodes.data(), &n);
+		for (cudaGraphNode_t v : nodes) {
+			cudaGraphNodeType t;
+			if (cudaGraphNodeGetType(v, &t) == cudaSuccess && t == cudaGraphNodeTypeKernel) ++*kernels;
+		}
+	}
 	const cudaError_t ei = cudaGraphInstantiate(exec, g, 0);
 	cudaGraphDestroy(g);
 	return (int)ei;
+}
+
+static int capture(mccnn_trainer *h, bool sample, cudaGraphExec_t *exec)
+{
+	return capture_with(h, [&](cudaStream_t s) { return enqueue_step(h, s, sample); }, exec);
 }
 
 // the trainer's buffers by id: the public MCCNN_TRAIN_* ids, then the slow step's internal ones (id >= MCCNN_TRAIN_NBUF).
@@ -662,12 +862,12 @@ static float **train_buffer(mccnn_trainer *h, int what, long *count)
 {
 	const Layout &L = h->L;
 	const SlowLayout &S = h->S;
-	const long N = L.N, fm = L.fm, bs = N / 2, nh2 = S.nh2;
+	const long N = L.N, fm = L.fm, bs = N / 2, nh2 = S.nh2, Nh = h->nh;
 	const int F = !h->slow, Sl = h->slow;
 	struct { float **p; long n; int ok; } t[] = {
 		{&h->P, h->nparam, 1}, {&h->V, h->nparam, 1}, {&h->G, h->nparam, 1}, {&h->X, N * L.ws * L.ws, 1},
-		{&h->act, L.aoff[L.l1 - 1] + N * fm, 1}, {&h->norm, N, F}, {&h->nout, N * fm, F}, {&h->join, N / 2, F},
-		{&h->gjoin, N / 2, F}, {&h->hinge, N / 4, F}, {&h->gout, N * fm, F}, {&h->dz, L.aoff[L.l1 - 1] + N * fm, 1},
+		{&h->act, L.aoff[L.l1 - 1] + N * fm, 1}, {&h->norm, Nh, F}, {&h->nout, Nh * fm, F}, {&h->join, Nh / 2, F},
+		{&h->gjoin, Nh / 2, F}, {&h->hinge, Nh / 4, F}, {&h->gout, Nh * fm, F}, {&h->dz, L.aoff[L.l1 - 1] + N * fm, 1},
 		{&h->loss, h->loss_cap, 1},
 		{&h->rows, bs * 2 * fm, Sl}, {&h->fc, S.l2 * bs * nh2 + bs, Sl}, {&h->sig, bs, Sl}, {&h->bce_grad, bs, Sl},
 		{&h->rows_grad, bs * 2 * fm, Sl},
@@ -747,6 +947,8 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	cudaSetDevice(h->device);
 	if (h->full) cudaGraphExecDestroy(h->full);
 	if (h->body) cudaGraphExecDestroy(h->body);
+	for (cudaGraphExec_t g : h->seg)
+		if (g) cudaGraphExecDestroy(g);
 	if (h->cap) cudaStreamDestroy(h->cap);
 	long n;
 	for (int what = 0; what < TRAIN_NALL; what++) {
@@ -757,20 +959,23 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	cudaFree(h->ctr);
 	cudaFree(h->warps);
 	cudaFree(h->pairs);
+	for (float *p : {h->hact, h->hdz, h->gact, h->gpart}) cudaFree(p);
 	cudaSetDevice(prev);
 	free(h);
 	return 0;
 }
 
 static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2, int bs, float margin, int pow, float mom,
-		  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, adcensus_stream_t stream)
+		  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, adcensus_stream_t stream,
+		  int rank = 0, int world = 0)
 {
 	*out = nullptr;
 	mccnn_trainer *h = (mccnn_trainer *)calloc(1, sizeof(mccnn_trainer));
 	if (!h) return ADCENSUS_EINVAL;
 	h->slow = slow;
 	Layout &L = h->L;
-	L.l1 = l1; L.fm = fm; L.ws = 1 + 2 * l1; L.N = 2 * bs;
+	L.l1 = l1; L.fm = fm; L.ws = 1 + 2 * l1; L.N = world && !slow ? shard_count(2 * bs, world, rank) : 2 * bs;
+	h->nh = 2 * bs; h->rank = rank; h->world = world;
 	long off = 0, aoff = 0;
 	for (int k = 0; k < l1; k++) {
 		const int cin = k ? fm : 1, s = L.ws - 2 * (k + 1);
@@ -786,17 +991,8 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 			S.fwoff[j] = off; off += (long)o * in;
 			S.fboff[j] = off; off += o;
 		}
-		// split k so that each weight-gradient GEMM has about 256 blocks of at least 256 k each; the split depends on the
-		// shapes only, so the summation order (and the bits) do not depend on the device
-		long poff = 0;
-		for (int k = 0; k < l1; k++) {
-			const int cin = k ? fm : 1, s = L.ws - 2 * (k + 1), K = L.N * s * s;
-			const int tiles = adc_div_up(fm, BM) * adc_div_up(cin * 9 + 1, BN);
-			const int want = std::max(1, std::min(adc_div_up(256, tiles), adc_div_up(K, 256)));
-			S.kchunk[k] = adc_div_up(adc_div_up(K, want), BK) * BK;
-			S.nsplit[k] = adc_div_up(K, S.kchunk[k]);
-			S.poff[k] = poff; poff += (long)S.nsplit[k] * fm * (cin * 9 + 1);
-		}
+		split_k(L, S);
+		if (world) h->plan = slow_plan(L, S, rank, world);
 	}
 	h->nparam = off;
 	h->bufsz = L.ws * L.ws;
@@ -825,13 +1021,33 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	if (!rc) rc = (int)cudaMemsetAsync(h->neg_lr, 0, sizeof(float), adc_stream(stream));
 	if (!rc) rc = (int)cudaMalloc((void **)&h->ctr, 2 * sizeof(int));
 	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, 2 * sizeof(int), adc_stream(stream));
-	if (!rc) rc = (int)cudaMalloc((void **)&h->warps, (size_t)chunk * L.N * sizeof(mccnn_warp));
-	if (!rc) rc = (int)cudaMemsetAsync(h->warps, 0, (size_t)chunk * L.N * sizeof(mccnn_warp), adc_stream(stream));
+	h->nw = slow && world ? h->plan.e - h->plan.b0 : L.N;
+	if (!rc) rc = (int)cudaMalloc((void **)&h->warps, (size_t)chunk * h->nw * sizeof(mccnn_warp));
+	if (!rc) rc = (int)cudaMemsetAsync(h->warps, 0, (size_t)chunk * h->nw * sizeof(mccnn_warp), adc_stream(stream));
 	if (!rc) rc = (int)cudaMalloc((void **)&h->pairs, (size_t)n_pairs * sizeof(mccnn_train_pair));
 	if (!rc) rc = (int)cudaMemcpy(h->pairs, pairs, (size_t)n_pairs * sizeof(mccnn_train_pair), cudaMemcpyHostToDevice);
+	if (world && !slow) {
+		h->Lh = L;
+		h->Lh.N = h->nh;
+		h->Lh.aoff[l1 - 1] = 0;
+		h->nmax = shard_count(h->nh, world, 0);
+		h->ntower = L.boff[l1 - 1] + fm;
+		const long n[4] = {(long)h->nh * fm, (long)h->nh * fm, (long)world * h->nmax * fm, world * h->ntower};
+		float **p[4] = {&h->hact, &h->hdz, &h->gact, &h->gpart};
+		for (int i = 0; i < 4 && !rc; i++) {
+			rc = (int)cudaMalloc((void **)p[i], (size_t)n[i] * sizeof(float));
+			if (!rc) rc = (int)cudaMemsetAsync(*p[i], 0, (size_t)n[i] * sizeof(float), adc_stream(stream));
+		}
+	}
 	if (!rc) rc = (int)cudaStreamCreateWithFlags(&h->cap, cudaStreamNonBlocking);
-	if (!rc) rc = capture(h, true, &h->full);
-	if (!rc) rc = capture(h, false, &h->body);
+	if (world) {
+		for (int seg = 0; seg < 3 && !rc; seg++)
+			rc = capture_with(h, [&](cudaStream_t s) { return enqueue_shard(h, s, seg); }, &h->seg[seg],
+					  &h->shard_launches);
+	} else {
+		if (!rc) rc = capture(h, true, &h->full);
+		if (!rc) rc = capture(h, false, &h->body);
+	}
 	if (!rc) rc = (int)cudaStreamSynchronize(adc_stream(stream));
 	cudaSetDevice(prev);
 	if (rc) {
@@ -892,6 +1108,34 @@ extern "C" int mccnn_trainer_create_slow_pairs(mccnn_trainer **out, int l1, int 
 	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, pairs, n_pairs, chunk, loss_cap, device, stream);
 }
 
+extern "C" int mccnn_trainer_create_shard(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
+					  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
+					  int world, adcensus_stream_t stream)
+{
+	if (!out || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || chunk < 1 || loss_cap < 1 || world < 1 ||
+	    (world & (world - 1)) || rank < 0 || rank >= world)
+		return ADCENSUS_EINVAL;
+	const int rc = check_pairs(pairs, n_pairs);
+	if (rc) return rc;
+	if (l1 > LMAX || fm > 128 || world > WG_NT || world > 2 * bs) return ADCENSUS_ELIMIT;
+	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, pairs, n_pairs, chunk, loss_cap, device, stream, rank, world);
+}
+
+extern "C" int mccnn_trainer_create_slow_shard(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
+					       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
+					       int rank, int world, adcensus_stream_t stream)
+{
+	if (!out || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || chunk < 1 || loss_cap < 1 || world < 1 ||
+	    (world & (world - 1)) || rank < 0 || rank >= world)
+		return ADCENSUS_EINVAL;
+	const int rc = check_pairs(pairs, n_pairs);
+	if (rc) return rc;
+	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) ||
+	    (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31) || world > WG_NT || world > 2 * bs)
+		return ADCENSUS_ELIMIT;
+	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, pairs, n_pairs, chunk, loss_cap, device, stream, rank, world);
+}
+
 static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
 {
 	const float v = (float)(-lr);                                           // add(-opt.lr, grads[i]): the scalar as float
@@ -903,7 +1147,7 @@ static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
 
 extern "C" int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr, adcensus_stream_t stream)
 {
-	if (!h || !warps || nsteps < 0) return ADCENSUS_EINVAL;
+	if (!h || h->world || !warps || nsteps < 0) return ADCENSUS_EINVAL;
 	if (nsteps > h->chunk) return ADCENSUS_ELIMIT;
 	if (!nsteps) return 0;
 	cudaStream_t s = adc_stream(stream);
@@ -918,9 +1162,104 @@ extern "C" int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int 
 	return rc;
 }
 
+extern "C" int mccnn_trainer_shard_begin(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr,
+					 adcensus_stream_t stream)
+{
+	if (!h || !h->world || !warps || nsteps < 0) return ADCENSUS_EINVAL;
+	if (nsteps > h->chunk) return ADCENSUS_ELIMIT;
+	if (!nsteps) return 0;
+	cudaStream_t s = adc_stream(stream);
+	int prev = 0;
+	cudaGetDevice(&prev);
+	cudaSetDevice(h->device);
+	int rc = set_lr(h, lr, s);
+	if (!rc) rc = (int)cudaMemcpyAsync(h->warps, warps, (size_t)nsteps * h->nw * sizeof(mccnn_warp), cudaMemcpyDefault, s);
+	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, sizeof(int), s);
+	cudaSetDevice(prev);
+	return rc;
+}
+
+extern "C" int mccnn_trainer_shard_segment(mccnn_trainer *h, int segment, adcensus_stream_t stream)
+{
+	if (!h || !h->world || segment < 0 || segment > 2) return ADCENSUS_EINVAL;
+	int prev = 0;
+	cudaGetDevice(&prev);
+	cudaSetDevice(h->device);
+	const int rc = (int)cudaGraphLaunch(h->seg[segment], adc_stream(stream));
+	cudaSetDevice(prev);
+	return rc;
+}
+
+extern "C" int mccnn_trainer_shard_buffer(mccnn_trainer *h, int what, float **ptr, long long *count)
+{
+	if (!h || !h->world || !ptr || !count || (what != MCCNN_SHARD_TOWER_OUT && what != MCCNN_SHARD_WGRAD_PART))
+		return ADCENSUS_EINVAL;
+	const Layout &L = h->L;
+	const bool tower = what == MCCNN_SHARD_TOWER_OUT;
+	long n = 0;
+	if (h->slow) {
+		*ptr = tower ? h->act + L.aoff[L.l1 - 1] : h->part;
+		train_buffer(h, tower ? MCCNN_TRAIN_ROWS : TRAIN_PART, &n);
+	} else {
+		*ptr = tower ? h->gact : h->gpart;
+		n = h->world * (tower ? (long)h->nmax * L.fm : h->ntower);
+	}
+	*count = n;
+	return 0;
+}
+
+extern "C" int mccnn_trainer_shard_pieces(mccnn_trainer *h, int what)
+{
+	if (!h || !h->world || (what != MCCNN_SHARD_TOWER_OUT && what != MCCNN_SHARD_WGRAD_PART)) return ADCENSUS_EINVAL;
+	return h->slow && what == MCCNN_SHARD_WGRAD_PART ? h->L.l1 : 1;
+}
+
+extern "C" int mccnn_trainer_shard_slot(mccnn_trainer *h, int what, int piece, int rank, long long *offset,
+					long long *count)
+{
+	if (!h || !h->world || !offset || !count || rank < 0 || rank >= h->world || piece < 0 ||
+	    piece >= mccnn_trainer_shard_pieces(h, what))
+		return ADCENSUS_EINVAL;
+	const Layout &L = h->L;
+	if (h->slow) {
+		const SlowPlan p = slow_plan(L, h->S, rank, h->world);
+		if (what == MCCNN_SHARD_TOWER_OUT) {
+			*offset = (long long)p.b0 * L.fm;
+			*count = (long long)(p.b1 - p.b0) * L.fm;
+		} else {
+			const long per = (long)L.fm * ((piece ? L.fm : 1) * 9 + 1);        // one split's partial sums
+			*offset = h->S.poff[piece] + p.z0[piece] * per;
+			*count = std::max(0, p.z1[piece] - p.z0[piece]) * per;
+		}
+	} else {
+		const long slot = what == MCCNN_SHARD_TOWER_OUT ? (long)h->nmax * L.fm : h->ntower;
+		*offset = rank * slot;
+		*count = slot;
+	}
+	return 0;
+}
+
+extern "C" int mccnn_trainer_slow_shard_plan(int l1, int fm, int bs, int rank, int world, long long *plan)
+{
+	if (l1 < 1 || l1 > LMAX || fm < 1 || bs < 1 || world < 1 || world > 2 * bs || rank < 0 || rank >= world || !plan)
+		return ADCENSUS_EINVAL;
+	Layout L{};
+	L.l1 = l1; L.fm = fm; L.ws = 1 + 2 * l1; L.N = 2 * bs;
+	SlowLayout S{};
+	split_k(L, S);
+	const SlowPlan p = slow_plan(L, S, rank, world);
+	plan[0] = p.b0; plan[1] = p.b1; plan[2] = p.e;
+	for (int k = 0; k < l1; k++) {
+		plan[3 + 3 * k] = p.z0[k];
+		plan[4 + 3 * k] = p.z1[k];
+		plan[5 + 3 * k] = S.nsplit[k];
+	}
+	return 0;
+}
+
 extern "C" int mccnn_trainer_step_patches(mccnn_trainer *h, const float *patches, double lr, adcensus_stream_t stream)
 {
-	if (!h || !patches) return ADCENSUS_EINVAL;
+	if (!h || h->world || !patches) return ADCENSUS_EINVAL;
 	cudaStream_t s = adc_stream(stream);
 	int prev = 0;
 	cudaGetDevice(&prev);
@@ -965,6 +1304,7 @@ extern "C" int mccnn_trainer_reset_losses(mccnn_trainer *h, adcensus_stream_t st
 extern "C" int mccnn_trainer_launches_per_step(mccnn_trainer *h)
 {
 	if (!h) return -1;
+	if (h->world) return h->shard_launches;
 	return h->slow ? 3 + 3 * h->L.l1 + 3 * h->S.l2 : 5 + h->L.l1;
 }
 

@@ -79,6 +79,53 @@ PAIR_DTYPE = np.dtype([("x0", "<u8"), ("x1", "<u8"), ("H", "<i4"), ("W", "<i4")]
 TRAIN_PARAMS, TRAIN_MOMENTA, TRAIN_GRADS, TRAIN_PATCHES, TRAIN_TOWER, TRAIN_NORM, TRAIN_NORMALIZED, TRAIN_JOIN, \
     TRAIN_JOIN_GRAD, TRAIN_HINGE, TRAIN_NORM_GRAD_OUT, TRAIN_DZ, TRAIN_LOSS = range(13)
 TRAIN_ROWS, TRAIN_FC, TRAIN_SIGMOID, TRAIN_BCE_GRAD, TRAIN_ROWS_GRAD = range(13, 18)      # arch 'slow' only
+SHARD_TOWER_OUT, SHARD_WGRAD_PART = range(2)                                               # a shard's gathered buffers
+WGRAD_THREADS = 256                          # csrc/train.cu's WG_NT: thread t of wgrad_kernel sums patches t, t + 256, ...
+
+
+def check_world(world, o):
+    """refuse a data-parallel run of `world` ranks that cannot give the one-GPU bits, before any GPU work"""
+    if world == 1:
+        return
+    if world < 1 or world & (world - 1):
+        raise ValueError("%s ranks: data-parallel training needs a power of two ranks, so that each rank's patches are "
+                         "whole residue classes of the %d-thread weight-gradient tree" % (world, WGRAD_THREADS))
+    if world > min(WGRAD_THREADS, 2 * o["bs"]):
+        raise ValueError("%d ranks: more ranks than the %d patches of a batch of -bs %d (at most %d ranks)"
+                         % (world, 2 * o["bs"], o["bs"], min(WGRAD_THREADS, 2 * o["bs"])))
+
+
+def shard_size(N, rank, world):
+    """the patches n = rank, rank + world, ... of a batch of N: an arch 'fast' rank's share"""
+    return (N - rank + world - 1) // world
+
+
+def slow_shard_plan(o, rank, world):
+    """an arch 'slow' rank's share (mccnn_trainer_slow_shard_plan) -> (b0, b1, e, [(z0, z1, nsplit)] per tower layer): it
+    owns the patches [b0, b1) and the weight-gradient splits [z0, z1) of each layer, and runs the tower on [b0, e)"""
+    from .adcensus import _check, lib
+
+    plan = np.zeros(3 + 3 * o["l1"], np.int64)
+    _check(lib().mccnn_trainer_slow_shard_plan(o["l1"], o["fm"], o["bs"], rank, world,
+                                               plan.ctypes.data_as(ctypes.c_void_p)), "mccnn_trainer_slow_shard_plan")
+    return int(plan[0]), int(plan[1]), int(plan[2]), [tuple(int(v) for v in plan[3 + 3 * k:6 + 3 * k])
+                                                      for k in range(o["l1"])]
+
+
+def shard_patches(o, rank, world):
+    """the patches of each batch a rank samples, as (first, stride, count): 'fast' rank, world, shard_size; 'slow' the
+    patches [b0, e) of its plan"""
+    if arch_of(o) == "slow":
+        b0, _, e, _ = slow_shard_plan(o, rank, world)
+        return b0, 1, e - b0
+    return rank, world, shard_size(2 * o["bs"], rank, world)
+
+
+def shard_warps(warps, o, rank, world):
+    """rank's records of a chunk of whole-batch records (nsteps N,) -> (nsteps count,) of :func:`shard_patches`"""
+    first, stride, count = shard_patches(o, rank, world)
+    w = np.asarray(warps).reshape(-1, 2 * o["bs"])
+    return np.ascontiguousarray(w[:, first:first + stride * (count - 1) + 1:stride]).reshape(-1)
 
 
 def options(dataset, arch="fast", **overrides):
@@ -423,13 +470,23 @@ def sample_patches_pairs(planes, warps, ws):
 class Trainer:
     """csrc/train.cu's trainer: net_tr + Margin2 ('fast') or + BCECriterion2 ('slow', when `o` has l2) and the momentum
     update on `device`, sampling from X0 / X1 (CUDA), or with `planes` = [(x0, x1)] CUDA (H, W) planes from that table of
-    stereo pairs (a warp's image is then a pair index)."""
+    stereo pairs (a warp's image is then a pair index).
 
-    def __init__(self, o, X0=None, X1=None, chunk=CHUNK, loss_cap=1, device=None, planes=None):
+    With `world` > 1, rank `rank` of a data-parallel run whose ranks exchange through `comm` (a rowband.Comm: send / recv
+    / exchange / barrier): every rank is given the same records, runs the tower on its share of each batch
+    (:func:`shard_warps`) and ends each step with the parameters, momenta and loss of the one-GPU trainer, bit for bit
+    (csrc/train.cu's mccnn_trainer_create_shard / _create_slow_shard)."""
+
+    def __init__(self, o, X0=None, X1=None, chunk=CHUNK, loss_cap=1, device=None, planes=None, rank=0, world=1,
+                 comm=None):
         import torch
 
         from .adcensus import _check, _stream, _t, lib
 
+        check_world(world, o)
+        if world > 1 and (comm is None or not 0 <= rank < world):
+            raise ValueError("Trainer: rank %s of %d ranks needs a communicator" % (rank, world))
+        self.rank, self.world, self.comm = rank, world, comm
         self.o, self.chunk = o, chunk
         src = X0 if planes is None else planes[0][0]
         self.dev = src.device if device is None else torch.device("cuda", device)
@@ -442,7 +499,24 @@ class Trainer:
         self._h = ctypes.c_void_p()
         with torch.cuda.device(self.dev):
             self.stream = torch.cuda.current_stream(self.dev)
-            if planes is not None:
+            if world > 1:
+                if planes is None:                                       # mccnn_trainer_create's table of X0 / X1
+                    planes = [(X0[i, 0], X1[i, 0]) for i in range(len(X0))]
+                t = pair_table(planes)
+                tp = t.ctypes.data_as(ctypes.c_void_p)
+                if self.arch == "slow":
+                    _check(lib().mccnn_trainer_create_slow_shard(ctypes.byref(self._h), self.l1, self.fm, self.l2,
+                                                                 self.nh2, self.bs, o["mom"], tp, len(t), chunk, loss_cap,
+                                                                 self.dev.index, rank, world, _stream(src)),
+                           "mccnn_trainer_create_slow_shard")
+                else:
+                    _check(lib().mccnn_trainer_create_shard(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"],
+                                                            o["pow"], o["mom"], tp, len(t), chunk, loss_cap,
+                                                            self.dev.index, rank, world, _stream(src)),
+                           "mccnn_trainer_create_shard")
+                self.n_warps = shard_patches(o, rank, world)[2]
+                self._gathered = [self._shard_slots(w) for w in (SHARD_TOWER_OUT, SHARD_WGRAD_PART)]
+            elif planes is not None:
                 t = pair_table(planes)
                 tp = t.ctypes.data_as(ctypes.c_void_p)
                 if self.arch == "slow":
@@ -466,6 +540,40 @@ class Trainer:
                                                   _t(X0, 1, "Trainer"), _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap,
                                                   self.dev.index, _stream(X0)), "mccnn_trainer_create")
         self.launches_per_step = lib().mccnn_trainer_launches_per_step(self._h)
+
+    def _shard_slots(self, what):
+        """a shard's gathered buffer as views of the trainer's memory: [piece][rank] -> CUDA tensor (that rank's slot)"""
+        import torch
+
+        from .adcensus import _check, lib
+
+        ptr, count = ctypes.c_void_p(), ctypes.c_longlong()
+        _check(lib().mccnn_trainer_shard_buffer(self._h, what, ctypes.byref(ptr), ctypes.byref(count)),
+               "mccnn_trainer_shard_buffer")
+        view = type("DeviceArray", (), {"__cuda_array_interface__": dict(shape=(count.value,), typestr="<f4",
+                                                                          data=(ptr.value, False), version=2)})()
+        buf = torch.as_tensor(view, device=self.dev)
+        out = []
+        for piece in range(lib().mccnn_trainer_shard_pieces(self._h, what)):
+            slots = []
+            for r in range(self.world):
+                off, n = ctypes.c_longlong(), ctypes.c_longlong()
+                _check(lib().mccnn_trainer_shard_slot(self._h, what, piece, r, ctypes.byref(off), ctypes.byref(n)),
+                       "mccnn_trainer_shard_slot")
+                slots.append(buf[off.value:off.value + n.value])
+            out.append(slots)
+        return out
+
+    def _all_gather(self, pieces):
+        """every rank's slot of each piece from that rank, on the trainer's stream (empty slots are not sent)"""
+        import torch
+
+        with torch.cuda.stream(self.stream):
+            for slots in pieces:
+                mine = slots[self.rank]
+                others = [p for p in range(self.world) if p != self.rank]
+                self.comm.exchange({p: mine for p in others if mine.numel()},
+                                   {p: slots[p] for p in others if slots[p].numel()})
 
     def close(self):
         from .adcensus import lib
@@ -520,15 +628,30 @@ class Trainer:
         return tower, (unflatten_head(v, self.l1, self.fm, self.l2, self.nh2) if self.arch == "slow" else None)
 
     def run(self, warps, lr):
-        """len(warps) / N steps (<= chunk) from a WARP_DTYPE array (pinned host or CUDA uint8 tensor, or numpy)"""
+        """len(warps) / N steps (<= chunk) from a WARP_DTYPE array (pinned host or CUDA uint8 tensor, or numpy).  A shard
+        takes the whole batch's records as numpy, or its own share (:func:`shard_warps`) as a tensor."""
         import torch
 
         from .adcensus import _check, lib
 
         if isinstance(warps, np.ndarray):
+            if self.world > 1:
+                warps = shard_warps(warps, self.o, self.rank, self.world)
             warps = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(self.dev)
-        nsteps = warps.numel() // (WARP_DTYPE.itemsize * self.N)
-        _check(lib().mccnn_trainer_run(self._h, warps.data_ptr(), nsteps, lr, self.stream.cuda_stream), "mccnn_trainer_run")
+        if self.world == 1:
+            nsteps = warps.numel() // (WARP_DTYPE.itemsize * self.N)
+            _check(lib().mccnn_trainer_run(self._h, warps.data_ptr(), nsteps, lr, self.stream.cuda_stream),
+                   "mccnn_trainer_run")
+            return warps
+        nsteps = warps.numel() // (WARP_DTYPE.itemsize * self.n_warps)
+        _check(lib().mccnn_trainer_shard_begin(self._h, warps.data_ptr(), nsteps, lr, self.stream.cuda_stream),
+               "mccnn_trainer_shard_begin")
+        for _ in range(nsteps):
+            for seg in range(3):
+                _check(lib().mccnn_trainer_shard_segment(self._h, seg, self.stream.cuda_stream),
+                       "mccnn_trainer_shard_segment")
+                if seg < 2:
+                    self._all_gather(self._gathered[seg])
         return warps
 
     def step_patches(self, patches, lr):
@@ -553,8 +676,10 @@ class Trainer:
         it refills a buffer, for the chunk that last read it"""
         import torch
 
+        if self.world > 1:
+            warps = shard_warps(warps, self.o, self.rank, self.world)
         if not hasattr(self, "_pinned"):
-            rec = WARP_DTYPE.itemsize * self.N
+            rec = WARP_DTYPE.itemsize * (self.N if self.world == 1 else self.n_warps)
             self._pinned = [torch.empty(self.chunk * rec, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
             self._events, self._next = [None, None], 0
         b, nbytes = self._next, warps.nbytes
@@ -855,10 +980,27 @@ class Checkpoints:
         save_checkpoint(self.path, self.fp, epoch, step, lr, elapsed, params, momenta, losses, stream)
 
 
-def fit(tr, nnz, perm, build, o, stream, epochs=EPOCHS, log=print, ckpt=None, start=None):
+def _agree(comm, flag, device):
+    """rank 0's `flag` on every rank of `comm` (a stop is decided by rank 0's clock alone)"""
+    import torch
+
+    if comm is None or comm.world == 1:
+        return flag
+    t = torch.tensor([int(flag)], dtype=torch.int32, device=device)
+    comm.exchange({p: t for p in range(1, comm.world)} if comm.rank == 0 else {}, {} if comm.rank == 0 else {0: t})
+    return bool(t.item())
+
+
+def fit(tr, nnz, perm, build, o, stream, epochs=EPOCHS, log=print, ckpt=None, start=None, comm=None):
     """main.lua:779-881: the epochs of chunks from (start["epoch"], start["step"]) (or from the beginning), driving `tr`
     (a :class:`Trainer`) with the records `build`(n steps, nnz rows) makes from `stream`; `log` receives the epoch lines.
-    With `ckpt` (:class:`Checkpoints`) the state is written at chunk boundaries and at the end of each epoch."""
+    With `ckpt` (:class:`Checkpoints`) the state is written at chunk boundaries and at the end of each epoch.  With `comm`
+    (a data-parallel run: every rank calls fit with the same arguments) only rank 0 logs and writes the state, and rank 0's
+    clock decides a stop for every rank."""
+    if comm is not None and comm.rank != 0:
+        log = lambda line: None                                                 # noqa: E731
+    writer = comm is None or comm.rank == 0
+    agree = (lambda flag: flag) if comm is None else (lambda flag: _agree(comm, flag, tr.dev))
     h = o["bs"] // 2
     nsteps = steps_per_epoch(len(nnz), o["bs"])
     epoch0, step0 = (start["epoch"], start["step"]) if start else (1, 0)
@@ -876,8 +1018,8 @@ def fit(tr, nnz, perm, build, o, stream, epochs=EPOCHS, log=print, ckpt=None, st
             tr.run_chunk(build(n, rows), lr)
             s1 = s0 + n
             if ckpt and s1 < nsteps:
-                stop = ckpt.stop_due()
-                if stop or ckpt.due(s1):
+                stop = agree(ckpt.stop_due())
+                if (stop or ckpt.due(s1)) and writer:
                     ckpt.save(tr, stream, epoch, s1, lr, time.time() - t0, np.concatenate([done, tr.losses(s1 - first)]))
                 if stop:
                     raise Stopped(ckpt.path, epoch, s1)
@@ -888,15 +1030,15 @@ def fit(tr, nnz, perm, build, o, stream, epochs=EPOCHS, log=print, ckpt=None, st
         err = np.cumsum(losses[ok])[-1] / ok.sum() if ok.any() else float("nan")
         log(epoch_line(epoch, err, lr, time.time() - t0))
         if ckpt:
-            stop = epoch < epochs and ckpt.stop_due()
-            if stop or ckpt.steps is not None:
+            stop = epoch < epochs and agree(ckpt.stop_due())
+            if (stop or ckpt.steps is not None) and writer:
                 ckpt.save(tr, stream, epoch + 1, 0, lr_at(o["lr"], epoch + 1), time.time() - t0, np.zeros(0, np.float32))
             if stop:
                 raise Stopped(ckpt.path, epoch + 1, 0)
 
 
 def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="out", stereo=None, log=print, epochs=EPOCHS,
-          rect="imperfect", checkpoint_steps=None, stop_after=None, resume=False):
+          rect="imperfect", checkpoint_steps=None, stop_after=None, resume=False, comm=None):
     """main.lua:602-890 for arch 'fast' or 'slow' (as `o` was made): returns the saved net's file name.  `args` are main.lua's arguments after
     dataset and arch (for the file name), `stereo` the stereo method's overrides for the evaluation that follows;
     `log` receives the printed lines.  For dataset mb the set is data.mb.<rect>_gray (see :class:`MbTrainSet`).
@@ -904,7 +1046,12 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     Checkpoints (:func:`checkpoint_path`, next to the net): `checkpoint_steps` K writes the state every K steps of an
     epoch and at each epoch's end; `stop_after` S writes it at the first chunk boundary after S seconds and raises
     :class:`Stopped`; `resume` continues from the checkpoint if there is one.  A resumed run gives the bits of an
-    uninterrupted one; the checkpoint is deleted once the net file is written."""
+    uninterrupted one; the checkpoint is deleted once the net file is written.
+
+    With `comm` (a rowband.Comm of world > 1 ranks, each calling train with the same arguments and its own `device`) the
+    batches are shared out as :class:`Trainer` says and the run gives the one-GPU bits; only rank 0 prints, writes the
+    checkpoints and the net and runs the evaluation.  The checkpoint does not record the number of ranks: a state written
+    by R ranks resumes on any other count."""
     import torch
 
     from . import t7
@@ -913,6 +1060,10 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
         raise ValueError("action must be train_tr or train_all, got %r" % (action,))
     check(o)
     check_checkpoint_options(checkpoint_steps, stop_after)
+    rank, world = (comm.rank, comm.world) if comm is not None else (0, 1)
+    check_world(world, o)
+    if world == 1:
+        comm = None
     arch = arch_of(o)
     fname = net_path(data_root, dataset, args, arch)
     if os.path.exists(fname):
@@ -937,6 +1088,8 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     tower, head = init_net(stream, o)                                            # :663-736
     if start:                                                                    # the initial weights are replaced
         stream.restore(start["mt_key"], start["mt_pos"], start["carry"])
+    if rank != 0:
+        log = lambda line: None                                                 # noqa: E731
     for line in net_lines(o):
         log(line)
     h = o["bs"] // 2
@@ -944,25 +1097,28 @@ def train(dataset, action, o, args=(), data_root=".", seed=42, device=0, out="ou
     dev = torch.device("cuda", device)
     with torch.cuda.device(dev):
         if mb:
-            tr = Trainer(o, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device, planes=planes)
+            tr = Trainer(o, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device, planes=planes, rank=rank, world=world,
+                         comm=comm)
             build = lambda n, rows: mb.warps(stream, o, rows, tr.ws)                                      # :791-846
         else:
             X0 = torch.from_numpy(np.ascontiguousarray(data.X0, np.float32)).to(dev)
             X1 = torch.from_numpy(np.ascontiguousarray(data.X1, np.float32)).to(dev)
-            tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device)
+            tr = Trainer(o, X0, X1, chunk=CHUNK, loss_cap=max(nsteps, 1), device=device, rank=rank, world=world, comm=comm)
             build = lambda n, rows: make_warps(draw_params(stream, o, n * h), rows, tr.ws)
         try:
             if start:
                 tr.load_state(start["params"], start["momenta"])
             else:
                 tr.set_layers(tower, head)
-            fit(tr, nnz, perm, build, o, stream, epochs=epochs, log=log, ckpt=ckpt, start=start)
+            fit(tr, nnz, perm, build, o, stream, epochs=epochs, log=log, ckpt=ckpt, start=start, comm=comm)
             tower, head = tr.net()
         finally:
             tr.close()
     if mb:                                                                       # the training planes are not needed now
         del planes, tr
         torch.cuda.empty_cache()
+    if rank != 0:                                                                # rank 0 writes and evaluates the net
+        return fname
     os.makedirs(os.path.dirname(fname), exist_ok=True)
     extra = dict(rect=rect, color="gray") if mb else {}
     t7.save_net(fname, tower, head, opt=dict(o, a=action, seed=seed, gpu=device + 1, **extra))   # :883, save_net(0)

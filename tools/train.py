@@ -21,6 +21,13 @@ Checkpoints (none of these three is part of the net's name):
 
 A resumed run prints the remaining epoch lines and writes the net an uninterrupted run would, bit for bit; the checkpoint is
 deleted once the net file is written.  A checkpoint of other options or another training set is refused.
+
+Several GPUs (both architectures, KITTI or Middlebury): one process per GPU under torchrun, each on the GPU of its
+LOCAL_RANK (so -gpu is refused there), NCCL between them.  The epoch lines, the net file and the checkpoints are those of
+one GPU, bit for bit, and a checkpoint written by one rank count resumes on another.  The rank count must be a power of
+two and at most 2 bs; rank 0 prints, writes and runs test_te / submit.
+
+    torchrun --nproc-per-node 8 tools/train.py kitti fast -a train_tr -data_root /data
 """
 import argparse
 import os
@@ -137,6 +144,15 @@ def main(argv=None, arch="fast"):
     from mccnn_b200 import train
 
     prog = MB_TOOL if arch is None else TOOLS[arch]
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    rank = int(os.environ.get("RANK", "0"))
+    try:
+        train.check_world(world, o)
+    except ValueError as e:
+        raise SystemExit("%s: torchrun with %s" % (prog, e))
+    if world > 1 and any(a == "-gpu" or a.startswith("-gpu=") for a in args.argv):
+        raise SystemExit("%s: -gpu under torchrun: each process trains on the GPU of its LOCAL_RANK, and the net records "
+                         "rank 0's GPU 1; leave -gpu out" % prog)
     fname = train.net_path(args.data_root, args.dataset, main_args(args.argv), args.arch)
     if os.path.exists(fname):
         raise SystemExit("%s: %s already exists; remove it first" % (prog, fname))
@@ -146,16 +162,33 @@ def main(argv=None, arch="fast"):
             train.MbTrainSet(args.data_root, args.rect, args.a)
         except (OSError, ValueError) as e:
             raise SystemExit("%s: %s" % (prog, e))
-    print(" ".join(args.argv) + " ", flush=True)                                  # main.lua:6-9
+    if rank == 0:
+        print(" ".join(args.argv) + " ", flush=True)                              # main.lua:6-9
     ckpt = dict(checkpoint_steps=args.checkpoint_steps, stop_after=args.stop_after, resume=args.resume)
+    device, comm = args.device, None
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+
+        from mccnn_b200 import rowband
+
+        device = int(os.environ.get("LOCAL_RANK", "0"))
+        torch.cuda.set_device(device)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", device))
+        comm = rowband.Comm()
     try:
         train.train(args.dataset, args.a, o, args=main_args(args.argv), data_root=args.data_root, seed=args.seed,
-                    device=args.device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True), **rect, **ckpt)
+                    device=device, out=args.out, stereo=stereo, log=lambda s: print(s, flush=True), comm=comm, **rect,
+                    **ckpt)
     except (MemoryError, train.CheckpointError) as e:                            # the mb planes do not fit, a bad checkpoint
         raise SystemExit("%s: %s" % (prog, e))
     except train.Stopped as e:
-        print("%s: %s" % (prog, e), file=sys.stderr, flush=True)
+        if rank == 0:
+            print("%s: %s" % (prog, e), file=sys.stderr, flush=True)
         return train.EX_TEMPFAIL
+    finally:
+        if comm is not None:
+            dist.destroy_process_group()
     return 0
 
 
