@@ -458,8 +458,8 @@ int mccnn_mb_nnz_fill(const float *d0, const unsigned char *mask, int H, int W, 
  * (main.lua:843-846).  Pointers may be host or device unless noted (copies use cudaMemcpyDefault). */
 
 /* One patch of make_patch (main.lua:607-619): m the forward 2x3 matrix as stored in the FloatTensor, contrast and
- * brightness as float, image the 0-based index into the trainer's pair table (for the X0 / X1 creators: into X0 / X1,
- * (n_img, 1, H, W) float32), view 0 = the pair's x0, 1 = its x1. */
+ * brightness as float, image the 0-based index into the trainer's or sampler's pair table, view 0 = the pair's x0, 1 = its
+ * x1. */
 typedef struct {
 	float m[6];
 	float contrast, brightness;
@@ -473,31 +473,75 @@ typedef struct {
 	int H, W;
 } mccnn_train_pair;
 
-/* The sampler alone: out (n, ws, ws) = warpAffine(X[image], m, (ws, ws), INTER_CUBIC, BORDER_CONSTANT 0) * contrast +
- * brightness, bit-identical to OpenCV's float path as oracle/train.py restates it.  DEVICE pointers; an image index
- * outside [0, n_img) gives a NaN patch.  Runs mccnn_train_sample_pairs' kernel on the table {X0[i], X1[i], H, W}. */
-int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n, int ws,
-		       float *out, adcensus_stream_t stream);
+/* What mccnn_trainer_create builds: the arch, main.lua's options of that arch, and the trainer's rank of world ranks. */
+typedef struct {
+	int slow;             /* 0: arch 'fast', 1: arch 'slow' */
+	int l1, fm, bs;
+	float mom;
+	float margin;         /* 'fast' only (Margin2) */
+	int pow;              /* 'fast' only: 1 or 2 */
+	int l2, nh2;          /* 'slow' only */
+	int chunk, loss_cap;
+	int rank, world;      /* world 1 (rank 0): one GPU; >= 2: a data-parallel shard */
+} mccnn_trainer_config;
 
-/* The sampler on a DEVICE table of n_pairs pairs: the source of warps[i] is pairs[image].x0 (view 0) or .x1 (view 1), and
- * its constant-0 border is that pair's own H x W.  A pair index outside [0, n_pairs) gives a NaN patch.  The table is
- * read back to the host once to check it (ADCENSUS_EINVAL for a null plane or a size < 1, ADCENSUS_ELIMIT above 32767),
- * so the call waits for `stream`. */
+/* The sampler alone: out (n, ws, ws) = warpAffine(X, m, (ws, ws), INTER_CUBIC, BORDER_CONSTANT 0) * contrast +
+ * brightness, bit-identical to OpenCV's float path as oracle/train.py restates it, on a DEVICE table of n_pairs pairs: the
+ * source X of warps[i] is pairs[image].x0 (view 0) or .x1 (view 1), and its constant-0 border is that pair's own H x W.
+ * DEVICE pointers; a pair index outside [0, n_pairs) gives a NaN patch.  The table is read back to the host once to check
+ * it (ADCENSUS_EINVAL for a null plane or a size < 1, ADCENSUS_ELIMIT above 32767), so the call waits for `stream`. */
 int mccnn_train_sample_pairs(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws, float *out,
 			     adcensus_stream_t stream);
 
 typedef struct mccnn_trainer mccnn_trainer;
 
-/* net_tr of arch 'fast' (l1 valid 3x3 convolutions 1 -> fm -> .. -> fm, ReLU between them, Normalize2, StereoJoin1) with
- * Margin2(margin, pow) and momentum `mom`, for batches of bs pairs, sampling from the DEVICE images X0 / X1 (kept by the
- * caller for the trainer's lifetime).  Parameters, momenta and gradients are one flat fp32 vector each: per layer W
- * (fm, cin, 3, 3) then b (fm), layer 1 first; all start at 0.  `chunk` bounds the steps of one mccnn_trainer_run,
- * `loss_cap` the per-step losses kept between two mccnn_trainer_reset_losses.  The step is captured once into a CUDA graph
- * of mccnn_trainer_launches_per_step kernels; it has no floating-point atomics, so equal inputs give equal bits.
- * bs even, l1 <= 8, fm <= 128 (else ADCENSUS_ELIMIT, also when a patch's activations exceed shared memory). */
-int mccnn_trainer_create(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom, const float *X0,
-			 const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
-			 adcensus_stream_t stream);
+/* The trainer cfg describes, on `device`, sampling from a table of stereo pairs: `pairs` is a HOST array of n_pairs
+ * records, copied into trainer-owned device memory; the planes it points to are kept by the caller for the trainer's
+ * lifetime.  A warp's image is an index into this table.
+ *
+ * 'fast' (slow 0): net_tr of l1 valid 3x3 convolutions 1 -> fm -> .. -> fm, ReLU between them, Normalize2, StereoJoin1,
+ * with Margin2(margin, pow).
+ * 'slow' (slow 1, main.lua:663-677): l1 valid 3x3 convolutions 1 -> fm -> .. -> fm with a ReLU after every one,
+ * Reshape(bs, 2 fm) (row r = the features of patches 2r and 2r + 1), l2 x [Linear(in, nh2), ReLU], Linear(nh2, 1), Sigmoid,
+ * then BCECriterion2 against the targets 0, 1, 0, 1, ... (main.lua:848-849); the loss of a step is BCECriterion2's output.
+ * Both with momentum `mom`, for batches of bs pairs.  Parameters, momenta and gradients are one flat fp32 vector each: per
+ * tower layer W (fm, cin, 3, 3) then b (fm), layer 1 first, then ('slow') per Linear W (out, in) followed by b (out), in
+ * main.lua's order; all start at 0.  fp32 on the CUDA cores with fixed reduction orders and no floating-point atomics, so
+ * equal inputs give equal bits.  `chunk` bounds the steps of one mccnn_trainer_run or mccnn_trainer_shard_begin,
+ * `loss_cap` the per-step losses kept between two mccnn_trainer_reset_losses.
+ *
+ * The arguments are checked before the first CUDA call, and *h is NULL after any failure.  ADCENSUS_EINVAL: a null h or
+ * cfg; slow not 0 or 1; l1, fm, chunk or loss_cap < 1; bs < 2 or odd; 'fast' pow not 1 or 2; 'slow' l2 or nh2 < 1; world
+ * < 1 or not a power of two; rank outside [0, world); no pairs, a null plane, an H or W < 1.  ADCENSUS_ELIMIT: an H or W
+ * above 32767; l1 > 8; fm > 128; world above 256 or above 2 bs; 'slow' fm not a multiple of 16, l2 > 4, nh2 not 128, 256
+ * or 384, or 2 bs fm ws^2 >= 2^31.  ADCENSUS_ELIMIT also when a 'fast' patch's activations exceed shared memory.
+ *
+ * world 1 (one GPU): the step is captured once into a CUDA graph of mccnn_trainer_launches_per_step kernels, which
+ * mccnn_trainer_run and mccnn_trainer_step_patches launch.
+ *
+ * world >= 2 (data-parallel training): the trainer of rank `rank` of `world` ranks, each on its own device with the same
+ * pair table, parameters and momenta.  A step is three segments, each a captured graph, with two all-gathers the caller
+ * runs on `stream` between them: after segment 0 of SHARD_TOWER_OUT, after segment 1 of SHARD_WGRAD_PART, every rank's
+ * slots (mccnn_trainer_shard_slot) from that rank.  The parameters, momenta and losses are then those of the one-GPU
+ * trainer of the same arch, bit for bit, on every rank.
+ * 'fast': rank r holds the batch's patches n = r, r + world, ... as its patches 0, 1, ...; mccnn_trainer_size's PATCHES,
+ * TOWER and DZ are that share.
+ *   segment 0: the sampler and the tower on the rank's patches; its last layer -> its slot of SHARD_TOWER_OUT;
+ *   segment 1: Normalize2 / StereoJoin1 / Margin2 on the whole batch (every rank the same), the tower's backward pass on
+ *              the rank's patches and its partial weight gradient (levels 128 .. world of wgrad's tree) -> its slot of
+ *              SHARD_WGRAD_PART;
+ *   segment 2: the tree's levels world / 2 .. 1 over the ranks' partials, then the update.
+ * 'slow': the buffers are the whole batch's.  Rank r owns the patches [N r / world, N (r + 1) / world) and in each tower
+ * layer the weight-gradient splits that start in them (mccnn_trainer_slow_shard_plan); it runs the tower on its patches
+ * and on those its splits read past them.
+ *   segment 0: the sampler and the tower forward; SHARD_TOWER_OUT is the last layer (ROWS), the rank's slot its rows;
+ *   segment 1: the Linear layers, BCE and their gradients on the whole batch, the tower backward, the rank's splits of
+ *              each layer's weight gradient; SHARD_WGRAD_PART is the split workspace, one slot per layer (piece);
+ *   segment 2: the splits added in split order, then the update.
+ * mccnn_trainer_run and _step_patches refuse a shard; get / set / size / reset_losses work as for one GPU, and
+ * launches_per_step counts the kernels of the three segments. */
+int mccnn_trainer_create(mccnn_trainer **h, const mccnn_trainer_config *cfg, const mccnn_train_pair *pairs, int n_pairs,
+			 int device, adcensus_stream_t stream);
 int mccnn_trainer_destroy(mccnn_trainer *h);
 
 /* nsteps <= chunk training steps: warps (nsteps, N) mccnn_warp (pinned host or device; it must stay unchanged until the
@@ -508,57 +552,6 @@ int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, dou
 /* One step from given patches ((N, 1, ws, ws) float32) instead of the sampler. */
 int mccnn_trainer_step_patches(mccnn_trainer *h, const float *patches, double lr, adcensus_stream_t stream);
 
-/* net_tr of arch 'slow' (main.lua:663-677): l1 valid 3x3 convolutions 1 -> fm -> .. -> fm with a ReLU after every one,
- * Reshape(bs, 2 fm) (row r = the features of patches 2r and 2r + 1), l2 x [Linear(in, nh2), ReLU], Linear(nh2, 1), Sigmoid,
- * then BCECriterion2 against the targets 0, 1, 0, 1, ... (main.lua:848-849), with momentum `mom`.  The parameter vector
- * holds the tower's layers as for 'fast', then per Linear W (out, in) followed by b (out), in main.lua's order.  fp32 on
- * the CUDA cores with fixed reduction orders and no floating-point atomics.  The handle works with every mccnn_trainer_*
- * call; the loss of a step is BCECriterion2's output.  l1 1..8, fm a multiple of 16 up to 128, l2 1..4, nh2 128, 256 or
- * 384 (else ADCENSUS_ELIMIT). */
-int mccnn_trainer_create_slow(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom, const float *X0,
-			      const float *X1, int n_img, int H, int W, int chunk, int loss_cap, int device,
-			      adcensus_stream_t stream);
-
-/* The two creators above on a table of stereo pairs instead of X0 / X1: `pairs` is a HOST array of n_pairs records, copied
- * into trainer-owned device memory; the planes it points to are kept by the caller for the trainer's lifetime.  A warp's
- * image is an index into this table.  mccnn_trainer_create[_slow] build the table {X0 + i H W, X1 + i H W, H, W} and call
- * these, so both give the same bits from the same planes.  Each pair's planes non-null and H, W >= 1 (else
- * ADCENSUS_EINVAL), H, W <= 32767 (else ADCENSUS_ELIMIT); the other limits are the creators'. */
-int mccnn_trainer_create_pairs(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom,
-			       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
-			       adcensus_stream_t stream);
-int mccnn_trainer_create_slow_pairs(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom,
-				    const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
-				    adcensus_stream_t stream);
-
-/* Data-parallel training: the trainer of rank `rank` of `world` ranks (a power of two, at most 256 and at most 2 bs, else
- * ADCENSUS_ELIMIT), each on its own device with the same pair table, parameters and momenta.  A step is three segments,
- * each a captured graph, with two all-gathers the caller runs on `stream` between them: after segment 0 of
- * SHARD_TOWER_OUT, after segment 1 of SHARD_WGRAD_PART, every rank's slots (mccnn_trainer_shard_slot) from that rank.
- * The parameters, momenta and losses are then those of the one-GPU trainer of the same arch, bit for bit, on every rank.
- *
- * 'fast' (mccnn_trainer_create_shard): rank r holds the batch's patches n = r, r + world, ... as its patches 0, 1, ...;
- * mccnn_trainer_size's PATCHES, TOWER and DZ are that share.
- *   segment 0: the sampler and the tower on the rank's patches; its last layer -> its slot of SHARD_TOWER_OUT;
- *   segment 1: Normalize2 / StereoJoin1 / Margin2 on the whole batch (every rank the same), the tower's backward pass on
- *              the rank's patches and its partial weight gradient (levels 128 .. world of wgrad's tree) -> its slot of
- *              SHARD_WGRAD_PART;
- *   segment 2: the tree's levels world / 2 .. 1 over the ranks' partials, then the update.
- * 'slow' (mccnn_trainer_create_slow_shard): the buffers are the whole batch's.  Rank r owns the patches [N r / world,
- * N (r + 1) / world) and in each tower layer the weight-gradient splits that start in them (mccnn_trainer_slow_shard_plan);
- * it runs the tower on its patches and on those its splits read past them.
- *   segment 0: the sampler and the tower forward; SHARD_TOWER_OUT is the last layer (ROWS), the rank's slot its rows;
- *   segment 1: the Linear layers, BCE and their gradients on the whole batch, the tower backward, the rank's splits of
- *              each layer's weight gradient; SHARD_WGRAD_PART is the split workspace, one slot per layer (piece);
- *   segment 2: the splits added in split order, then the update.
- * mccnn_trainer_run and _step_patches refuse a shard; get / set / size / reset_losses work as for the others, and
- * launches_per_step counts the kernels of the three segments. */
-int mccnn_trainer_create_shard(mccnn_trainer **h, int l1, int fm, int bs, float margin, int pow, float mom,
-			       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
-			       int world, adcensus_stream_t stream);
-int mccnn_trainer_create_slow_shard(mccnn_trainer **h, int l1, int fm, int l2, int nh2, int bs, float mom,
-				    const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
-				    int world, adcensus_stream_t stream);
 /* the next nsteps <= chunk steps' records of the patches the rank samples, (nsteps, its share) mccnn_warp ('fast': the
  * patches rank, rank + world, ...; 'slow': the patches plan[0] .. plan[2] - 1), and the lr; then call the segments 0,
  * 1, 2 once per step, in order */

@@ -883,14 +883,6 @@ static float **train_buffer(mccnn_trainer *h, int what, long *count)
 // ROWS is a view of the tower's last layer (N, fm, 1, 1) = (bs, 2 fm), not an allocation of its own
 static bool owned(int what) { return what != MCCNN_TRAIN_ROWS; }
 
-// the table {X0 + i H W, X1 + i H W, H, W} of the (n_img, 1, H, W) creators
-static std::vector<mccnn_train_pair> stacked_pairs(const float *X0, const float *X1, int n_img, int H, int W)
-{
-	std::vector<mccnn_train_pair> t(n_img);
-	for (int i = 0; i < n_img; i++) t[i] = {X0 + (long)i * H * W, X1 + (long)i * H * W, H, W};
-	return t;
-}
-
 static int check_pairs(const mccnn_train_pair *pairs, int n_pairs)
 {
 	if (!pairs || n_pairs < 1) return ADCENSUS_EINVAL;
@@ -900,30 +892,6 @@ static int check_pairs(const mccnn_train_pair *pairs, int n_pairs)
 		if (p.H > 32767 || p.W > 32767) return ADCENSUS_ELIMIT;
 	}
 	return 0;
-}
-
-static int launch_sample(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws, float *out,
-			 cudaStream_t s)
-{
-	train_sample_kernel<<<adc_div_up((long)n * ws * ws, 128), 128, 0, s>>>(pairs, n_pairs, warps, nullptr, n, ws, out);
-	ADC_CHECK_LAUNCH();
-	return 0;
-}
-
-extern "C" int mccnn_train_sample(const float *X0, const float *X1, int n_img, int H, int W, const mccnn_warp *warps, int n,
-				  int ws, float *out, adcensus_stream_t stream)
-{
-	if (!X0 || !X1 || !warps || !out || n_img < 1 || H < 1 || W < 1 || n < 1 || ws < 1) return ADCENSUS_EINVAL;
-	if ((long)n * ws * ws >= (1l << 31) || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
-	cudaStream_t s = adc_stream(stream);
-	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
-	mccnn_train_pair *d = nullptr;
-	ADC_CUDA(cudaMallocAsync((void **)&d, t.size() * sizeof(mccnn_train_pair), s));
-	// from pageable memory: the call returns once `t` has been read
-	int rc = (int)cudaMemcpyAsync(d, t.data(), t.size() * sizeof(mccnn_train_pair), cudaMemcpyHostToDevice, s);
-	if (!rc) rc = launch_sample(d, n_img, warps, n, ws, out, s);
-	const int rf = (int)cudaFreeAsync(d, s);
-	return rc ? rc : rf;
 }
 
 extern "C" int mccnn_train_sample_pairs(const mccnn_train_pair *pairs, int n_pairs, const mccnn_warp *warps, int n, int ws,
@@ -936,7 +904,10 @@ extern "C" int mccnn_train_sample_pairs(const mccnn_train_pair *pairs, int n_pai
 	ADC_CUDA(cudaMemcpyAsync(t.data(), pairs, t.size() * sizeof(mccnn_train_pair), cudaMemcpyDeviceToHost, s));
 	ADC_CUDA(cudaStreamSynchronize(s));
 	const int rc = check_pairs(t.data(), n_pairs);
-	return rc ? rc : launch_sample(pairs, n_pairs, warps, n, ws, out, s);
+	if (rc) return rc;
+	train_sample_kernel<<<adc_div_up((long)n * ws * ws, 128), 128, 0, s>>>(pairs, n_pairs, warps, nullptr, n, ws, out);
+	ADC_CHECK_LAUNCH();
+	return 0;
 }
 
 extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
@@ -965,11 +936,31 @@ extern "C" int mccnn_trainer_destroy(mccnn_trainer *h)
 	return 0;
 }
 
-static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2, int bs, float margin, int pow, float mom,
-		  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, adcensus_stream_t stream,
-		  int rank = 0, int world = 0)
+// the limits of include/adcensus_b200.h's mccnn_trainer_create, in the order EINVAL, the pair table, ELIMIT
+static int check_config(mccnn_trainer **out, const mccnn_trainer_config *c, const mccnn_train_pair *pairs, int n_pairs)
 {
-	*out = nullptr;
+	if (!out || !c || (c->slow != 0 && c->slow != 1) || c->l1 < 1 || c->fm < 1 || c->bs < 2 || (c->bs % 2) ||
+	    c->chunk < 1 || c->loss_cap < 1 || (c->slow ? c->l2 < 1 || c->nh2 < 1 : c->pow != 1 && c->pow != 2) ||
+	    c->world < 1 || (c->world & (c->world - 1)) || c->rank < 0 || c->rank >= c->world)
+		return ADCENSUS_EINVAL;
+	const int rc = check_pairs(pairs, n_pairs);
+	if (rc) return rc;
+	if (c->l1 > LMAX || c->fm > 128 || c->world > WG_NT || c->world > 2l * c->bs ||
+	    (c->slow && (c->fm % 16 || c->l2 > L2MAX || (c->nh2 != 128 && c->nh2 != 256 && c->nh2 != 384) ||
+			 2l * c->bs * c->fm * (1 + 2 * c->l1) * (1 + 2 * c->l1) >= (1l << 31))))
+		return ADCENSUS_ELIMIT;
+	return 0;
+}
+
+extern "C" int mccnn_trainer_create(mccnn_trainer **out, const mccnn_trainer_config *cfg, const mccnn_train_pair *pairs,
+				    int n_pairs, int device, adcensus_stream_t stream)
+{
+	if (out) *out = nullptr;
+	const int bad = check_config(out, cfg, pairs, n_pairs);
+	if (bad) return bad;
+	// a one-GPU trainer has world 0: run / step_patches and the shard_* calls tell it from a shard by that
+	const int slow = cfg->slow, l1 = cfg->l1, fm = cfg->fm, l2 = cfg->l2, nh2 = cfg->nh2, bs = cfg->bs,
+		  chunk = cfg->chunk, rank = cfg->rank, world = cfg->world > 1 ? cfg->world : 0;
 	mccnn_trainer *h = (mccnn_trainer *)calloc(1, sizeof(mccnn_trainer));
 	if (!h) return ADCENSUS_EINVAL;
 	h->slow = slow;
@@ -999,8 +990,8 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	for (int k = 1; k < l1; k++) h->bufsz = h->bufsz > fm * (L.ws - 2 * k) * (L.ws - 2 * k) ? h->bufsz
 											   : fm * (L.ws - 2 * k) * (L.ws - 2 * k);
 	h->smem = 2 * h->bufsz * (int)sizeof(float);
-	h->device = device; h->chunk = chunk; h->loss_cap = loss_cap; h->n_pairs = n_pairs;
-	h->margin = margin; h->mom = mom; h->pow2 = pow == 2;
+	h->device = device; h->chunk = chunk; h->loss_cap = cfg->loss_cap; h->n_pairs = n_pairs;
+	h->margin = cfg->margin; h->mom = cfg->mom; h->pow2 = cfg->pow == 2;
 	h->neg_lr_host = 0.f;
 	int prev = 0;
 	cudaGetDevice(&prev);
@@ -1058,84 +1049,6 @@ static int create(mccnn_trainer **out, int slow, int l1, int fm, int l2, int nh2
 	return 0;
 }
 
-extern "C" int mccnn_trainer_create(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
-				    const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap,
-				    int device, adcensus_stream_t stream)
-{
-	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || n_img < 1 || H < 1 ||
-	    W < 1 || chunk < 1 || loss_cap < 1)
-		return ADCENSUS_EINVAL;
-	if (l1 > LMAX || fm > 128 || H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
-	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
-	return mccnn_trainer_create_pairs(out, l1, fm, bs, margin, pow, mom, t.data(), n_img, chunk, loss_cap, device, stream);
-}
-
-extern "C" int mccnn_trainer_create_slow(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
-					 const float *X0, const float *X1, int n_img, int H, int W, int chunk, int loss_cap,
-					 int device, adcensus_stream_t stream)
-{
-	if (!out || !X0 || !X1 || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || n_img < 1 || H < 1 ||
-	    W < 1 || chunk < 1 || loss_cap < 1)
-		return ADCENSUS_EINVAL;
-	if (H > 32767 || W > 32767) return ADCENSUS_ELIMIT;
-	const std::vector<mccnn_train_pair> t = stacked_pairs(X0, X1, n_img, H, W);
-	return mccnn_trainer_create_slow_pairs(out, l1, fm, l2, nh2, bs, mom, t.data(), n_img, chunk, loss_cap, device, stream);
-}
-
-extern "C" int mccnn_trainer_create_pairs(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
-					  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
-					  adcensus_stream_t stream)
-{
-	if (!out || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || chunk < 1 || loss_cap < 1)
-		return ADCENSUS_EINVAL;
-	const int rc = check_pairs(pairs, n_pairs);
-	if (rc) return rc;
-	if (l1 > LMAX || fm > 128) return ADCENSUS_ELIMIT;
-	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, pairs, n_pairs, chunk, loss_cap, device, stream);
-}
-
-extern "C" int mccnn_trainer_create_slow_pairs(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
-					       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
-					       adcensus_stream_t stream)
-{
-	if (!out || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || chunk < 1 || loss_cap < 1)
-		return ADCENSUS_EINVAL;
-	const int rc = check_pairs(pairs, n_pairs);
-	if (rc) return rc;
-	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) ||
-	    (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31))
-		return ADCENSUS_ELIMIT;
-	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, pairs, n_pairs, chunk, loss_cap, device, stream);
-}
-
-extern "C" int mccnn_trainer_create_shard(mccnn_trainer **out, int l1, int fm, int bs, float margin, int pow, float mom,
-					  const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device, int rank,
-					  int world, adcensus_stream_t stream)
-{
-	if (!out || l1 < 1 || fm < 1 || bs < 2 || (bs % 2) || (pow != 1 && pow != 2) || chunk < 1 || loss_cap < 1 || world < 1 ||
-	    (world & (world - 1)) || rank < 0 || rank >= world)
-		return ADCENSUS_EINVAL;
-	const int rc = check_pairs(pairs, n_pairs);
-	if (rc) return rc;
-	if (l1 > LMAX || fm > 128 || world > WG_NT || world > 2 * bs) return ADCENSUS_ELIMIT;
-	return create(out, 0, l1, fm, 0, 0, bs, margin, pow, mom, pairs, n_pairs, chunk, loss_cap, device, stream, rank, world);
-}
-
-extern "C" int mccnn_trainer_create_slow_shard(mccnn_trainer **out, int l1, int fm, int l2, int nh2, int bs, float mom,
-					       const mccnn_train_pair *pairs, int n_pairs, int chunk, int loss_cap, int device,
-					       int rank, int world, adcensus_stream_t stream)
-{
-	if (!out || l1 < 1 || fm < 1 || l2 < 1 || nh2 < 1 || bs < 2 || (bs % 2) || chunk < 1 || loss_cap < 1 || world < 1 ||
-	    (world & (world - 1)) || rank < 0 || rank >= world)
-		return ADCENSUS_EINVAL;
-	const int rc = check_pairs(pairs, n_pairs);
-	if (rc) return rc;
-	if (l1 > LMAX || fm > 128 || fm % 16 || l2 > L2MAX || (nh2 != 128 && nh2 != 256 && nh2 != 384) ||
-	    (long)2 * bs * fm * (1 + 2 * l1) * (1 + 2 * l1) >= (1l << 31) || world > WG_NT || world > 2 * bs)
-		return ADCENSUS_ELIMIT;
-	return create(out, 1, l1, fm, l2, nh2, bs, 0.f, 1, mom, pairs, n_pairs, chunk, loss_cap, device, stream, rank, world);
-}
-
 static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
 {
 	const float v = (float)(-lr);                                           // add(-opt.lr, grads[i]): the scalar as float
@@ -1143,6 +1056,15 @@ static int set_lr(mccnn_trainer *h, double lr, cudaStream_t s)
 	h->neg_lr_host = v;
 	ADC_CUDA(cudaMemcpyAsync(h->neg_lr, &h->neg_lr_host, sizeof(float), cudaMemcpyHostToDevice, s));
 	return 0;
+}
+
+// the start of a chunk of nsteps steps: the lr, the steps' nw warp records each, the step counter back to 0
+static int begin_chunk(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr, cudaStream_t s)
+{
+	int rc = set_lr(h, lr, s);
+	if (!rc) rc = (int)cudaMemcpyAsync(h->warps, warps, (size_t)nsteps * h->nw * sizeof(mccnn_warp), cudaMemcpyDefault, s);
+	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, sizeof(int), s);
+	return rc;
 }
 
 extern "C" int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int nsteps, double lr, adcensus_stream_t stream)
@@ -1154,9 +1076,7 @@ extern "C" int mccnn_trainer_run(mccnn_trainer *h, const mccnn_warp *warps, int 
 	int prev = 0;
 	cudaGetDevice(&prev);
 	cudaSetDevice(h->device);
-	int rc = set_lr(h, lr, s);
-	if (!rc) rc = (int)cudaMemcpyAsync(h->warps, warps, (size_t)nsteps * h->L.N * sizeof(mccnn_warp), cudaMemcpyDefault, s);
-	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, sizeof(int), s);
+	int rc = begin_chunk(h, warps, nsteps, lr, s);
 	for (int i = 0; i < nsteps && !rc; i++) rc = (int)cudaGraphLaunch(h->full, s);
 	cudaSetDevice(prev);
 	return rc;
@@ -1172,9 +1092,7 @@ extern "C" int mccnn_trainer_shard_begin(mccnn_trainer *h, const mccnn_warp *war
 	int prev = 0;
 	cudaGetDevice(&prev);
 	cudaSetDevice(h->device);
-	int rc = set_lr(h, lr, s);
-	if (!rc) rc = (int)cudaMemcpyAsync(h->warps, warps, (size_t)nsteps * h->nw * sizeof(mccnn_warp), cudaMemcpyDefault, s);
-	if (!rc) rc = (int)cudaMemsetAsync(h->ctr, 0, sizeof(int), s);
+	const int rc = begin_chunk(h, warps, nsteps, lr, s);
 	cudaSetDevice(prev);
 	return rc;
 }

@@ -27,7 +27,7 @@ read from the sources; parity with Torch7 is unpinned, and it is pinned against 
 
 Dataset mb (main.lua:455-491, 828-841): the training images are every light group ``x_<i>_<j>.bin``, j >= 2, of the
 images the nnz rows name, one device pair per (image, light, exposure) in a table the sampler reads (:class:`MbTrainSet`,
-``mccnn_trainer_create_pairs``).  After the uniforms of :791-818 each sample draws light, exp, the d_exp test, exp_ only
+``mccnn_trainer_create``).  After the uniforms of :791-818 each sample draws light, exp, the d_exp test, exp_ only
 when that test passes, then the d_light test, so a sample takes a variable number of words: ``mccnn_mb_sample_starts``
 finds the boundaries in a buffer of raw words, numpy gathers the columns (:func:`draw_params_mb`), and the words drawn past
 the last sample of a chunk go back to the stream, so chunked building gives the records building everything at once gives.
@@ -418,23 +418,16 @@ def make_warps(p, rows, ws, pairs=None):
 
 
 def sample_patches(X0, X1, warps, ws):
-    """the sampler alone (mccnn_train_sample): X0 / X1 (n_img, 1, H, W) CUDA float32, warps a WARP_DTYPE array ->
-    (len(warps), ws, ws) CUDA float32"""
-    import torch
-
-    from .adcensus import _check, _stream, _t, lib
+    """the sampler alone on the pairs (X0[i, 0], X1[i, 0]): X0 / X1 (n_img, 1, H, W) CUDA float32, warps a WARP_DTYPE
+    array -> (len(warps), ws, ws) CUDA float32"""
+    from .adcensus import _t
 
     name = "sample_patches"
-    p0, p1 = _t(X0, 1, name), _t(X1, 2, name)
+    _t(X0, 1, name)
+    _t(X1, 2, name)
     if X0.shape != X1.shape or X0.dim() != 4 or X0.shape[1] != 1:
         raise ValueError("%s: X0 and X1 must both be (n, 1, H, W)" % name)
-    n_img, _, H, W = X0.shape
-    w = torch.from_numpy(np.ascontiguousarray(warps, WARP_DTYPE).view(np.uint8)).to(X0.device)
-    out = torch.empty((len(warps), ws, ws), dtype=torch.float32, device=X0.device)
-    with torch.cuda.device(X0.device):
-        _check(lib().mccnn_train_sample(p0, p1, n_img, H, W, w.data_ptr(), len(warps), ws, out.data_ptr(), _stream(out)),
-               name)
-    return out
+    return sample_patches_pairs([(X0[i, 0], X1[i, 0]) for i in range(len(X0))], warps, ws)
 
 
 def pair_table(planes):
@@ -467,15 +460,35 @@ def sample_patches_pairs(planes, warps, ws):
     return out
 
 
+class TrainerConfig(ctypes.Structure):
+    """mccnn_trainer_config"""
+
+    _fields_ = [
+        ("slow", ctypes.c_int),
+        ("l1", ctypes.c_int),
+        ("fm", ctypes.c_int),
+        ("bs", ctypes.c_int),
+        ("mom", ctypes.c_float),
+        ("margin", ctypes.c_float),
+        ("pow", ctypes.c_int),
+        ("l2", ctypes.c_int),
+        ("nh2", ctypes.c_int),
+        ("chunk", ctypes.c_int),
+        ("loss_cap", ctypes.c_int),
+        ("rank", ctypes.c_int),
+        ("world", ctypes.c_int),
+    ]
+
+
 class Trainer:
     """csrc/train.cu's trainer: net_tr + Margin2 ('fast') or + BCECriterion2 ('slow', when `o` has l2) and the momentum
-    update on `device`, sampling from X0 / X1 (CUDA), or with `planes` = [(x0, x1)] CUDA (H, W) planes from that table of
-    stereo pairs (a warp's image is then a pair index).
+    update on `device`, sampling from the pairs (X0[i, 0], X1[i, 0]) of X0 / X1 (n_img, 1, H, W) CUDA, or with `planes` =
+    [(x0, x1)] CUDA (H, W) planes from that table of stereo pairs (a warp's image is a pair index).
 
     With `world` > 1, rank `rank` of a data-parallel run whose ranks exchange through `comm` (a rowband.Comm: send / recv
     / exchange / barrier): every rank is given the same records, runs the tower on its share of each batch
     (:func:`shard_warps`) and ends each step with the parameters, momenta and loss of the one-GPU trainer, bit for bit
-    (csrc/train.cu's mccnn_trainer_create_shard / _create_slow_shard)."""
+    (csrc/train.cu's mccnn_trainer_create with world > 1)."""
 
     def __init__(self, o, X0=None, X1=None, chunk=CHUNK, loss_cap=1, device=None, planes=None, rank=0, world=1,
                  comm=None):
@@ -497,48 +510,22 @@ class Trainer:
         self.N = 2 * self.bs
         self._keep = (X0, X1, planes)
         self._h = ctypes.c_void_p()
+        if planes is None:
+            _t(X0, 1, "Trainer")
+            _t(X1, 2, "Trainer")
+            planes = [(X0[i, 0], X1[i, 0]) for i in range(len(X0))]
+        t = pair_table(planes)
+        slow = self.arch == "slow"
+        cfg = TrainerConfig(slow=slow, l1=self.l1, fm=self.fm, bs=self.bs, mom=o["mom"], margin=0 if slow else o["m"],
+                            pow=1 if slow else o["pow"], l2=self.l2 or 0, nh2=self.nh2 or 0, chunk=chunk,
+                            loss_cap=loss_cap, rank=rank, world=world)
         with torch.cuda.device(self.dev):
             self.stream = torch.cuda.current_stream(self.dev)
+            _check(lib().mccnn_trainer_create(ctypes.byref(self._h), ctypes.byref(cfg), t.ctypes.data_as(ctypes.c_void_p),
+                                              len(t), self.dev.index, _stream(src)), "mccnn_trainer_create")
             if world > 1:
-                if planes is None:                                       # mccnn_trainer_create's table of X0 / X1
-                    planes = [(X0[i, 0], X1[i, 0]) for i in range(len(X0))]
-                t = pair_table(planes)
-                tp = t.ctypes.data_as(ctypes.c_void_p)
-                if self.arch == "slow":
-                    _check(lib().mccnn_trainer_create_slow_shard(ctypes.byref(self._h), self.l1, self.fm, self.l2,
-                                                                 self.nh2, self.bs, o["mom"], tp, len(t), chunk, loss_cap,
-                                                                 self.dev.index, rank, world, _stream(src)),
-                           "mccnn_trainer_create_slow_shard")
-                else:
-                    _check(lib().mccnn_trainer_create_shard(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"],
-                                                            o["pow"], o["mom"], tp, len(t), chunk, loss_cap,
-                                                            self.dev.index, rank, world, _stream(src)),
-                           "mccnn_trainer_create_shard")
                 self.n_warps = shard_patches(o, rank, world)[2]
                 self._gathered = [self._shard_slots(w) for w in (SHARD_TOWER_OUT, SHARD_WGRAD_PART)]
-            elif planes is not None:
-                t = pair_table(planes)
-                tp = t.ctypes.data_as(ctypes.c_void_p)
-                if self.arch == "slow":
-                    _check(lib().mccnn_trainer_create_slow_pairs(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2,
-                                                                 self.bs, o["mom"], tp, len(t), chunk, loss_cap, self.dev.index,
-                                                                 _stream(src)),
-                           "mccnn_trainer_create_slow_pairs")
-                else:
-                    _check(lib().mccnn_trainer_create_pairs(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"], o["pow"],
-                                                            o["mom"], tp, len(t), chunk, loss_cap, self.dev.index,
-                                                            _stream(src)),
-                           "mccnn_trainer_create_pairs")
-            elif self.arch == "slow":
-                n_img, _, H, W = X0.shape
-                _check(lib().mccnn_trainer_create_slow(ctypes.byref(self._h), self.l1, self.fm, self.l2, self.nh2, self.bs,
-                                                       o["mom"], _t(X0, 1, "Trainer"), _t(X1, 2, "Trainer"), n_img, H, W,
-                                                       chunk, loss_cap, self.dev.index, _stream(X0)), "mccnn_trainer_create_slow")
-            else:
-                n_img, _, H, W = X0.shape
-                _check(lib().mccnn_trainer_create(ctypes.byref(self._h), self.l1, self.fm, self.bs, o["m"], o["pow"], o["mom"],
-                                                  _t(X0, 1, "Trainer"), _t(X1, 2, "Trainer"), n_img, H, W, chunk, loss_cap,
-                                                  self.dev.index, _stream(X0)), "mccnn_trainer_create")
         self.launches_per_step = lib().mccnn_trainer_launches_per_step(self._h)
 
     def _shard_slots(self, what):

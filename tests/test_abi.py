@@ -124,6 +124,78 @@ def test_round2_entry_points_reject_bad_arguments_without_a_gpu(lib):
     assert lib.mccnn_pipeline_run_batch(None, 1, arr, arr, arr, arr, arr, None) == -1
 
 
+def test_trainer_create_checks_every_limit_without_a_gpu(lib):
+    """mccnn_trainer_create: EINVAL (-1) for the scalars, then the pair table, then ELIMIT (-2), one rule at a time -- all
+    decided before the first CUDA call, with *h NULL after the refusal"""
+    import numpy as np
+
+    from mccnn_b200 import train
+
+    fast = dict(slow=0, l1=4, fm=64, bs=128, mom=0.9, margin=0.2, pow=1, chunk=256, loss_cap=1, rank=0, world=1)
+    slow = dict(slow=1, l1=4, fm=112, bs=128, mom=0.9, l2=4, nh2=384, chunk=256, loss_cap=1, rank=0, world=1)
+    good = np.zeros(2, train.PAIR_DTYPE)
+    good["x0"], good["x1"], good["H"], good["W"] = 1 << 20, 1 << 21, 350, 1242
+
+    def create(base, table=good, n=None, **kw):
+        h = ctypes.c_void_p(16)
+        cfg = train.TrainerConfig(**dict(base, **kw))
+        rc = lib.mccnn_trainer_create(ctypes.byref(h), ctypes.byref(cfg), table.ctypes.data_as(ctypes.c_void_p),
+                                      len(table) if n is None else n, -1, None)
+        assert h.value is None, (base["slow"], kw)
+        return rc
+
+    def pairs(**kw):
+        t = good.copy()
+        for k, v in kw.items():
+            t[k][1] = v
+        return t
+
+    # the valid ones pass every check and reach CUDA, which refuses device -1
+    for base in (fast, slow):
+        assert create(base) > 0 and create(base, rank=1, world=2) > 0 and create(base, world=256) > 0
+    cfg = train.TrainerConfig(**fast)
+    assert lib.mccnn_trainer_create(None, ctypes.byref(cfg), good.ctypes.data_as(ctypes.c_void_p), 2, -1, None) == -1
+    h = ctypes.c_void_p(16)
+    assert lib.mccnn_trainer_create(ctypes.byref(h), None, good.ctypes.data_as(ctypes.c_void_p), 2, -1, None) == -1
+    assert h.value is None
+    for base in (fast, slow):
+        for kw in (dict(slow=2), dict(l1=0), dict(fm=0), dict(bs=0), dict(bs=1), dict(bs=3), dict(chunk=0),
+                   dict(loss_cap=0), dict(world=0), dict(world=3), dict(world=6, rank=1), dict(rank=-1),
+                   dict(rank=1), dict(world=4, rank=4)):
+            assert create(base, **kw) == -1, kw
+        assert create(base, n=0) == -1
+        for t in (pairs(x0=0), pairs(x1=0), pairs(H=0), pairs(W=0)):
+            assert create(base, t) == -1
+        assert create(base, pairs(H=40000)) == -2 and create(base, pairs(W=40000)) == -2
+        for kw in (dict(l1=9), dict(fm=129), dict(world=512, bs=512), dict(world=8, bs=2)):
+            assert create(base, **kw) == -2, kw
+        assert create(base, pairs(W=40000), fm=0) == -1                   # the scalars before the table
+        assert create(base, pairs(H=0), l1=9) == -1                       # the table before the limits
+    for kw in (dict(pow=0), dict(pow=3)):
+        assert create(fast, **kw) == -1, kw
+        assert create(slow, **kw) > 0, kw                                 # read only for 'fast'
+    for kw in (dict(l2=0), dict(nh2=0)):
+        assert create(slow, **kw) == -1, kw
+        assert create(fast, **kw) > 0, kw                                 # read only for 'slow'
+    for kw in (dict(fm=120), dict(l2=5), dict(nh2=200), dict(fm=128, l1=8, bs=29028)):
+        assert create(slow, **kw) == -2, kw
+        assert create(fast, **kw) > 0, kw
+    assert create(slow, fm=128, l1=8, bs=29026) > 0                       # 2 bs fm ws^2 just under 2^31
+
+
+def test_trainer_config_mirrors_the_header():
+    from mccnn_b200 import train
+
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "adcensus_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^}]*)\} mccnn_trainer_config;", src).group(1)
+    want = []
+    for decl in body.split(";"):
+        if decl.strip():
+            ctype, names = decl.split(None, 1)
+            want += [(n.strip(), {"int": ctypes.c_int, "float": ctypes.c_float}[ctype]) for n in names.split(",")]
+    assert train.TrainerConfig._fields_ == want
+
+
 def test_python_mirror_type_errors():
     import torch
 
