@@ -519,15 +519,16 @@ def cbca_volume(kind, H, W, D, direction, seed=0):
     return vol
 
 
-def cbca_f64(x0c, x1c, vol, direction):
+def cbca_f64(x0c, x1c, vol, direction, planes=None):
     """adcensus.cu:343-377 in float64: the tap sums over each output's cross support, as (row runs, then rows); the
-    order does not matter at this precision.  Entries with x + d * direction outside the image are copied."""
+    order does not matter at this precision.  Entries with x + d * direction outside the image are copied.  `planes`:
+    aggregate only these disparities (the others are copied)."""
     D, H, W = vol.shape
     out = np.array(vol, np.float64)
     ys, xs = np.mgrid[0:H, 0:W]
     v = np.nan_to_num(np.asarray(vol, np.float64), nan=0.0)
     m = int(max(pack_maxlen(x0c, x1c), 1))
-    for d in range(D):
+    for d in (range(D) if planes is None else planes):
         sh = d * direction
         xp = xs + sh
         ok = (xp >= 0) & (xp < W)
