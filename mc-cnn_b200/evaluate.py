@@ -80,16 +80,11 @@ def check_options(dataset, at=0, color="gray", debug=False, use_cache=False, mak
                              "...)" % name)
 
 
-def preset_name(dataset, arch):
-    """the census / ad presets of main.lua:146-204 are shared by kitti and kitti2015"""
-    return "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
-
-
 def check_stage_options(dataset, arch, sm_terminate="", sm_skip="", **overrides):
     """Refuse a -sm_terminate / -sm_skip value that is not one of main.lua's step names, or that names a step doing no work
     in the stereo method of (dataset, arch) with `overrides` (pipeline.idle_steps): main.lua would run it and print the
     result of another variant under this one's name -- a wrong row in an ablation table."""
-    opt = pipeline.make_params(preset_name(dataset, arch), arch, sm_terminate=sm_terminate, sm_skip=sm_skip, **overrides)
+    opt = pipeline.make_params(dataset, arch, sm_terminate=sm_terminate, sm_skip=sm_skip, **overrides)
     idle = pipeline.idle_steps(opt)
     for option, name in (("sm_terminate", sm_terminate), ("sm_skip", sm_skip)):
         if name in idle:
@@ -214,25 +209,16 @@ def load_data(dataset, data_root=".", rect="imperfect", color="gray"):
 
 
 class Evaluator:
-    """The network and stereo method of one (dataset, arch), built once: tower and head on `device`, the parameters of
-    main.lua's presets with `overrides`, fix_border's width from the network (main.lua:382-391, 923)."""
+    """The network and stereo method of one (dataset, arch), built once (:class:`frontend.StereoMethod`): tower and head on
+    `device`, the parameters of main.lua's presets with `overrides`, fix_border's width from the network."""
 
     def __init__(self, dataset, arch, net_fname=None, device=0, **overrides):
         check_options(dataset)
-        if arch not in ("fast", "slow", "ad", "census"):
-            raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
         self.dataset, self.arch = dataset, arch
-        self.net = self.tower = self.head = None
-        if arch in ("fast", "slow"):
-            if not net_fname:
-                raise ValueError("arch '%s' needs -net_fname" % arch)
-            self.net = frontend.load_net(net_fname, arch)
-            overrides.setdefault("border", frontend.net_border(self.net))
-        # the census / ad presets of main.lua:146-204 are shared by kitti and kitti2015
-        self.opt = pipeline.make_params(preset_name(dataset, arch), arch, **overrides)
+        self.method = frontend.StereoMethod(dataset, arch, net_fname, **overrides)
+        self.opt = self.method.opt
         self.dev = torch.device("cuda", device)
-        if self.net is not None:
-            self.tower, self.head = frontend.make_stages(self.net, self.dev)
+        self.tower, self.head = self.method.stages(self.dev)
         self.sp = None
 
     @property
@@ -244,15 +230,18 @@ class Evaluator:
         if self.arch != "fast":
             return
         H, W, D = (max(s[k] for s in shapes) for k in range(3))
-        if self.sp is not None and H <= self.sp.H and W <= self.sp.W and D <= self.sp.D:
-            return
-        self.close()
+        if self.sp is not None:
+            if H <= self.sp.H and W <= self.sp.W and D <= self.sp.D:
+                return
+            self.sp.close()
         self.sp = pipeline.StereoPipeline(self.tower.fm, D, H, W, self.opt, device=self.dev.index)
 
     def close(self):
+        """release the pipeline, the feature tower and the scorer head"""
         if self.sp is not None:
             self.sp.close()
             self.sp = None
+        self.method.close()
 
     def stereo_predict(self, x_batch, disp_max):
         """main.lua:929-1082 for one (2,1,H,W) device batch: (H, W) device disparity map"""

@@ -11,10 +11,15 @@ documented arithmetic -- byte values as floats, Y = 0.299 R + 0.587 G + 0.114 B 
 fp32 in that order, mean and the unbiased (n-1) standard deviation accumulated in double, the
 scalar applied in fp32 -- **parity unpinned** for the last bit of the double accumulations; every
 stage after the (2,1,H,W) batch is the bit-exact path of :mod:`pipeline`.
+
+Which stereo method a (dataset, arch, network) runs -- preset, fix_border's width, network stages -- is decided by
+:class:`StereoMethod` for every prediction path.
 """
 import os
 
 import numpy as np
+
+from . import pipeline
 
 
 def load_bytes(path):
@@ -134,19 +139,56 @@ def net_border(net):
     return sum((w.shape[3] - 1) // 2 for w, _ in net.tower)
 
 
-def make_stages(net, device):
-    """The GPU stages of a loaded network on `device` (a torch.device or index): (FeatureTower, ScorerHead or None) --
-    net_te, and for 'slow' net_te2 (main.lua:894-900)."""
-    import torch
+class StereoMethod:
+    """The stereo method of ``main.lua <dataset> <arch> -net_fname N``, decided in one place for every prediction path.
 
-    from .feature_tower import FeatureTower
-    from .scorer_head import ScorerHead
+    The constructor does no GPU work: it checks the arch, loads the network of arch 'fast' / 'slow' from `net_fname` and
+    checks its arch (main.lua:893-901), and sets ``opt``, the preset of (dataset, arch) with `overrides` and fix_border's
+    width from the network (main.lua:382-391, 923; the preset's without a network; an explicit `border` wins).
+    :meth:`stages` then builds the network's GPU stages once, and :meth:`close` releases them."""
 
-    dev = torch.device("cuda", device) if isinstance(device, int) else device
-    with torch.cuda.device(dev):
-        tower = FeatureTower(net.tower, arch=net.arch, device=dev.index)
-        head = ScorerHead(net.head, device=dev.index) if net.arch == "slow" else None
-    return tower, head
+    def __init__(self, dataset, arch, net_fname=None, **overrides):
+        pipeline.check_arch(arch)
+        self.dataset, self.arch = dataset, arch
+        self.net = load_net(net_fname, arch) if net_fname and arch in ("fast", "slow") else None
+        if self.net is not None:
+            overrides.setdefault("border", net_border(self.net))
+        self.overrides = overrides
+        self.opt = self.params()
+        self.tower = self.head = None
+
+    @property
+    def needs_net(self):
+        """arch 'fast' / 'slow' without a network: the tower's input to the stereo method has to come from elsewhere"""
+        return self.arch in ("fast", "slow") and self.net is None
+
+    def params(self, **overrides):
+        """``opt`` with more `overrides`"""
+        return pipeline.make_params(self.dataset, self.arch, **dict(self.overrides, **overrides))
+
+    def stages(self, device):
+        """(FeatureTower, ScorerHead or None) of the network on `device` (a torch.device or index), built on the first call --
+        net_te, and for 'slow' net_te2 (main.lua:894-900); (None, None) for 'ad' / 'census'."""
+        if self.needs_net:
+            raise ValueError("arch '%s' needs -net_fname" % self.arch)
+        if self.net is not None and self.tower is None:
+            import torch
+
+            from .feature_tower import FeatureTower
+            from .scorer_head import ScorerHead
+
+            dev = torch.device("cuda", device) if isinstance(device, int) else device
+            with torch.cuda.device(dev):
+                self.tower = FeatureTower(self.net.tower, arch=self.arch, device=dev.index)
+                self.head = ScorerHead(self.net.head, device=dev.index) if self.arch == "slow" else None
+        return self.tower, self.head
+
+    def close(self):
+        """release the stages :meth:`stages` built"""
+        for st in (self.tower, self.head):
+            if st is not None:
+                st.close()
+        self.tower = self.head = None
 
 
 def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=None, out_dir=None, device=0,
@@ -159,32 +201,28 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     unit-norm tower output; 'ad' / 'census' need neither."""
     import torch
 
-    from . import pipeline
-
-    net = None
-    if arch in ("fast", "slow") and features is None:                          # decided before any GPU work
-        if net_fname is None:
-            raise ValueError("arch '%s' needs -net_fname (or, for 'fast', the tower output in `features`)" % arch)
-        net = load_net(net_fname, arch)                                         # main.lua:893-901
-    elif arch == "slow":
+    method = StereoMethod(dataset, arch, None if features is not None else net_fname, **overrides)   # before any GPU work
+    if method.needs_net and features is None:
+        raise ValueError("arch '%s' needs -net_fname (or, for 'fast', the tower output in `features`)" % arch)
+    if method.needs_net and arch == "slow":
         raise ValueError("arch 'slow' needs -net_fname: the scorer head's weights come with the tower's")
-    elif arch not in ("fast", "ad", "census"):
-        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
 
     batch = make_batch(left, right)
     dev = torch.device("cuda", device)
     x_batch = torch.from_numpy(batch).to(dev)
-    feats = head = None
-    if net is not None:
-        tower, head = make_stages(net, dev)
+    try:
         with torch.cuda.device(dev):
-            feats = tower.forward(x_batch)                                      # main.lua:944 / :957
-    elif arch == "fast":
-        feats = torch.as_tensor(features, dtype=torch.float32).to(dev).contiguous()
-    opt = pipeline.make_params(dataset, arch, **overrides)
-    with torch.cuda.device(dev):
-        disp, volL, volR = pipeline.stereo_predict(x_batch, feats, opt, int(disp_max), want_vols=True, arch=arch, head=head)
-    disp_h = disp.cpu().numpy()
+            tower, head = (None, None) if method.needs_net else method.stages(dev)
+            feats = None
+            if tower is not None:
+                feats = tower.forward(x_batch)                                  # main.lua:944 / :957
+            elif arch == "fast":
+                feats = torch.as_tensor(features, dtype=torch.float32).to(dev).contiguous()
+            disp, volL, volR = pipeline.stereo_predict(x_batch, feats, method.opt, int(disp_max), want_vols=True, arch=arch,
+                                                       head=head)
+        disp_h = disp.cpu().numpy()
+    finally:
+        method.close()
     if out_dir is not None:
         os.makedirs(out_dir, exist_ok=True)
         write_bin(os.path.join(out_dir, "right.bin"), volR.cpu().numpy())       # direction 1 comes first

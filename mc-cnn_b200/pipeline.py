@@ -137,8 +137,20 @@ PRESETS = {
 }
 
 
+ARCHS = ("fast", "slow", "ad", "census")
+
+
+def check_arch(arch):
+    """refuse an architecture main.lua does not have"""
+    if arch not in ARCHS:
+        raise ValueError("arch must be %s or %r" % (", ".join(map(repr, ARCHS[:-1])), ARCHS[-1]))
+
+
 def make_params(dataset="kitti", arch="fast", **overrides):
-    """The preset of (dataset, arch) with `overrides`; ``sm_terminate`` / ``sm_skip`` take main.lua's step names."""
+    """The preset of (dataset, arch) with `overrides`; ``sm_terminate`` / ``sm_skip`` take main.lua's step names.  kitti2015
+    shares kitti's 'ad' and 'census' presets (main.lua:146-204)."""
+    if dataset == "kitti2015" and arch in ("ad", "census"):
+        dataset = "kitti"
     d = dict(PRESETS[(dataset, arch)])
     d.setdefault("sgm_i", 1)
     for k in ("sm_terminate", "sm_skip"):
@@ -159,6 +171,7 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
     Returns disp (1,1,H,W) [, left vol, right vol].
     """
     assert x_batch.is_cuda
+    check_arch(arch)
     H, W = x_batch.size(2), x_batch.size(3)
     dev = x_batch.device
     vols = torch.empty((2, disp_max, H, W), device=dev, dtype=torch.float32)
@@ -181,8 +194,6 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
         vols[1:2].copy_(vr)
         adcensus.fix_border(vols[0:1], opt.border, -1)                            # :981
         adcensus.fix_border(vols[1:2], opt.border, 1)
-    else:
-        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
 
     st = stages(opt)                                                              # -sm_terminate / -sm_skip
     disp = {}

@@ -38,6 +38,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from . import pipeline
+
 
 def split(n, parts, i):
     """[lo, hi) of part i when n items are cut into `parts` nearly equal contiguous pieces"""
@@ -151,6 +153,7 @@ def band_source(ops, x_batch, D, opt, arch, tower=None, head=None):
     (-1 left, 1 right) is not in `dirs` and skipping it saves work; `extends` says whether the volumes of a row are cheap
     enough to compute again on the neighbouring bands ('fast', 'ad', 'census': the first CBCA block then runs on the
     extended band) or not ('slow': every row is scored by exactly one rank, the first block exchanges halo rows)."""
+    pipeline.check_arch(arch)
     H = x_batch.shape[2]
 
     def rows(a, b, m):
@@ -168,8 +171,6 @@ def band_source(ops, x_batch, D, opt, arch, tower=None, head=None):
             return vl, vr
 
         return volumes, True
-    if arch not in ("fast", "slow"):
-        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
     if tower is None or (arch == "slow" and head is None):
         raise ValueError("arch '%s' needs the feature tower%s" % (arch, " and the scorer head" if arch == "slow" else ""))
 
@@ -537,18 +538,13 @@ def predict_pair(left=None, right=None, dataset="kitti", arch="census", disp_max
     for the same images, dataset, arch, network, disp_max and overrides.  Returns the disparity map (H, W) float32 numpy on
     every rank; with `want_vols` also this rank's rows of the left and right volumes, (D, y1 - y0, W) device tensors.
     Every check on the arguments and the network file is made before any GPU work."""
-    from . import frontend, pipeline
+    from . import frontend
 
-    if arch not in ("fast", "slow", "ad", "census"):
-        raise ValueError("arch must be 'fast', 'slow', 'ad' or 'census'")
-    opt = pipeline.make_params(dataset, arch, **overrides)
-    _refuse_stage_options(opt)
-    net = None
-    if arch in ("fast", "slow") and tower is None:
-        if net_fname is None:
-            raise ValueError("arch '%s' needs -net_fname (or the stage objects `tower` / `head`)" % arch)
-        net = frontend.load_net(net_fname, arch)                                     # main.lua:893-901
-    elif arch == "slow" and head is None:
+    method = frontend.StereoMethod(dataset, arch, None if tower is not None else net_fname, **overrides)
+    _refuse_stage_options(method.opt)
+    if method.needs_net and tower is None:
+        raise ValueError("arch '%s' needs -net_fname (or the stage objects `tower` / `head`)" % arch)
+    if arch == "slow" and tower is not None and head is None:
         raise ValueError("arch 'slow' needs the scorer head with the feature tower")
     if x_batch is None:
         x_batch = frontend.make_batch(left, right)                                   # main.lua:1085-1100
@@ -560,18 +556,14 @@ def predict_pair(left=None, right=None, dataset="kitti", arch="census", disp_max
         xb = torch.as_tensor(x_batch, dtype=torch.float32).to(dev).contiguous()
         if xb.dim() != 4 or xb.shape[:2] != (2, 1):
             raise ValueError("x_batch: (2, 1, H, W) expected, got %s" % (tuple(xb.shape),))
-        own = net is not None
-        if own:
-            tower, head = frontend.make_stages(net, dev)
         try:
+            if tower is None:
+                tower, head = method.stages(dev)
             vols = want_vols or out_dir is not None
-            out = band_predict(CudaOps(dev), xb, D, opt, arch, tower, head, comm, chunks, want_vols=vols)
+            out = band_predict(CudaOps(dev), xb, D, method.opt, arch, tower, head, comm, chunks, want_vols=vols)
             disp, volL, volR = out if vols else (out, None, None)
         finally:
-            if own:
-                tower.close()
-                if head is not None:
-                    head.close()
+            method.close()
         disp_h = disp.cpu().numpy()
         if out_dir is not None:
             write_outputs(out_dir, disp_h, volL, volR, comm)

@@ -35,7 +35,7 @@ import torch
 from . import adcensus, dataio, evaluate, frontend, pipeline
 
 METHODS = ("random", "hillclimb_slow", "hillclimb_fast", "hillclimb_dim")
-ARCHS = ("fast", "slow", "ad", "census")
+ARCHS = pipeline.ARCHS
 DATASETS = ("kitti", "kitti2015", "mb")
 
 # hs.py:53-91 -- the same grid for kitti / kitti2015 x slow, ad and census; Python literals kept (int vs float), the log
@@ -202,35 +202,24 @@ SKIP_STEPS = ("cbca", "sgm", "occlusion", "subpixel_enchancement", "median", "bi
 TERMINATE_STEPS = ("cnn", "cbca1", "sgm", "cbca2", "occlusion", "mismatch", "subpixel_enchancement", "median")
 
 
-def preset_name(dataset, arch):
-    """the census / ad presets of main.lua:146-204 are shared by kitti and kitti2015 (as in Evaluator)"""
-    return "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
-
-
 class Searcher:
     """Scores parameter sets of one (dataset, arch, net) on the test_te examples; see the module docstring."""
 
     def __init__(self, dataset, arch, net_fname=None, data_root=".", rect="imperfect", color="gray", device=0):
         evaluate.check_options(dataset, color=color)
-        if arch not in ARCHS:
-            raise SearchError("arch must be 'fast', 'slow', 'ad' or 'census'")
         self.dataset, self.arch = dataset, arch
         self.params = grid(dataset, arch)
-        self.base = {}
-        net = None
-        if arch in ("fast", "slow"):
-            if not net_fname:
-                raise SearchError("arch '%s' needs a net file" % arch)
-            net = frontend.load_net(net_fname, arch)
-            self.base["border"] = frontend.net_border(net)
-        self.opt = pipeline.make_params(preset_name(dataset, arch), arch, **self.base)
+        self.method = frontend.StereoMethod(dataset, arch, net_fname)
+        if self.method.needs_net:
+            raise SearchError("arch '%s' needs a net file" % arch)
+        self.opt = self.method.opt
         self.dev = torch.device("cuda", device)
         self.err_at = dataio.ERR_AT[dataset]
         self.data = evaluate.load_data(dataset, data_root, rect, color)
         self.examples = self.data.examples("test_te")
         self.head_calls = 0
         self.cache_fill_seconds = 0.0
-        self.tower = self.head = self.sp = None
+        self.sp = None
         with torch.cuda.device(self.dev):
             self.x, self.gt, self.shapes, self.ids = [], [], [], []
             for ex in self.examples:
@@ -239,8 +228,7 @@ class Searcher:
                 self.gt.append(torch.from_numpy(self.data.ground_truth(ex, img_width)).to(self.dev))
                 self.shapes.append((x.shape[2], x.shape[3], disp_max))
                 self.ids.append(id_)
-            if net is not None:
-                self.tower, self.head = frontend.make_stages(net, self.dev)
+            self.tower, self.head = self.method.stages(self.dev)
             H, W, D = (max(s[k] for s in self.shapes) for k in range(3))
             self.sp = pipeline.StereoPipeline(self.tower.fm if self.tower else 1, D, H, W, self.opt, device=self.dev.index,
                                               cbca_mode=None if arch == "fast" else "exact")
@@ -255,9 +243,9 @@ class Searcher:
                 self.vols = torch.empty(nv * D * H * W, device=self.dev)
 
     def close(self):
-        for st in (self.sp, self.tower, self.head):
-            if st is not None:
-                st.close()
+        if self.sp is not None:
+            self.sp.close()
+        self.method.close()
         self.sp = self.tower = self.head = None
 
     def _views(self, buf, i):
@@ -344,7 +332,7 @@ class Searcher:
         unknown = set(overrides) - set(n for n, _ in pipeline.Params._fields_)
         if unknown:
             raise SearchError("unknown parameter(s) %s" % ", ".join(sorted(unknown)))
-        return pipeline.make_params(preset_name(self.dataset, self.arch), self.arch, **dict(self.base, **overrides))
+        return self.method.params(**overrides)
 
     def score(self, overrides):
         """(score, [err per example]) of one parameter set: err = bad / valid pixels (main.lua:1224-1236), score =

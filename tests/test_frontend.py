@@ -1,5 +1,10 @@
 """CPU: the image front end of `-a predict` (main.lua:1084-1100): PNG loading, grey conversion,
-standardisation.  (The GPU part of predict() is covered in tests/test_gpu_parity.py.)"""
+standardisation, and the host phase of the stereo method's resolver.  (The GPU part of predict() is covered in
+tests/test_gpu_parity.py.)"""
+import os
+import subprocess
+import sys
+
 import numpy as np
 import pytest
 
@@ -92,3 +97,73 @@ def test_predict_refuses_bad_net_arguments_before_any_gpu_work(tmp_path):
     with pytest.raises(t7.T7Error):
         frontend.predict("no-such-left.png", "no-such-right.png", "kitti", "fast", disp_max=8,
                          net_fname=str(_png(tmp_path, "x.png", np.zeros((4, 4), np.uint8), "L")))
+
+
+DEPTHS = (2, 4, 5)
+
+
+@pytest.fixture(scope="module")
+def nets(tmp_path_factory):
+    """{(arch, depth): .t7 file} of random networks with `depth` 3x3 layers, a scorer head for 'slow'"""
+    from mccnn_b200 import t7
+    from oracle import feature_tower as oft
+    from oracle import scorer_head as osh
+
+    tmp = tmp_path_factory.mktemp("nets")
+    rng = np.random.default_rng(0)
+    out = {}
+    for arch in ("fast", "slow"):
+        for depth in DEPTHS:
+            out[arch, depth] = str(tmp / ("%s_%d.t7" % (arch, depth)))
+            t7.save_net(out[arch, depth], oft.make_weights(rng, l1=depth, fm=8),
+                        osh.make_weights(rng, 8, 16, 2) if arch == "slow" else None)
+    return out
+
+
+@pytest.mark.parametrize("border", [None, 7])
+@pytest.mark.parametrize("depth", (None,) + DEPTHS)
+@pytest.mark.parametrize("arch", ["fast", "slow", "ad", "census"])
+@pytest.mark.parametrize("dataset", ["kitti", "kitti2015", "mb"])
+def test_stereo_method_parameters(nets, dataset, arch, depth, border):
+    """the preset of (dataset, arch) -- kitti's for kitti2015 ad / census (main.lua:146-204) -- with fix_border's width from
+    the net for 'fast' / 'slow' (main.lua:382-391, 923: one per 3x3 layer), the preset's without a net, an explicit border
+    over both; 'ad' / 'census' take no net"""
+    from mccnn_b200 import pipeline
+
+    net_fname = nets["slow" if arch == "slow" else "fast", depth] if depth else None
+    takes_net = arch in ("fast", "slow") and depth is not None
+    over = {} if border is None else {"border": border}
+    method = frontend.StereoMethod(dataset, arch, net_fname, **over)
+    preset = "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
+    want = border if border is not None else depth if takes_net else pipeline.PRESETS[preset, arch]["border"]
+    assert method.opt.as_dict() == pipeline.make_params(preset, arch, border=want).as_dict()
+    assert method.needs_net == (arch in ("fast", "slow") and not takes_net)
+    assert method.tower is None and method.head is None
+
+
+def test_kitti2015_shares_the_kitti_ad_and_census_presets():
+    from mccnn_b200 import pipeline
+
+    for arch in ("ad", "census"):
+        assert pipeline.make_params("kitti2015", arch).as_dict() == pipeline.make_params("kitti", arch).as_dict()
+    assert pipeline.make_params("kitti2015", "census", L1=2).as_dict() == pipeline.make_params("kitti", "census", L1=2).as_dict()
+
+
+def test_stereo_method_host_phase_makes_no_cuda_call(nets):
+    """in a fresh process, so that no other test has initialised CUDA before"""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    code = ("import sys, torch\nsys.path.insert(0, %r)\nimport mccnn_b200\nfrom mccnn_b200 import frontend\n"
+            "for arch, f in %r:\n    frontend.StereoMethod('kitti', arch, f, L1=3)\n"
+            "print(torch.cuda.is_initialized())\n" % (root, [(a, f) for (a, _), f in sorted(nets.items())]))
+    r = subprocess.run([sys.executable, "-c", code], cwd=root, capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, r.stderr[-2000:]
+    assert r.stdout.split() == ["False"]
+
+
+def test_stereo_method_refusals(nets):
+    with pytest.raises(ValueError, match="arch must be 'fast', 'slow', 'ad' or 'census'"):
+        frontend.StereoMethod("kitti", "sad")
+    with pytest.raises(ValueError, match="'fast' network"):
+        frontend.StereoMethod("kitti", "slow", nets["fast", 4])
+    with pytest.raises(ValueError, match="arch 'slow' needs -net_fname"):
+        frontend.StereoMethod("kitti", "slow").stages(0)             # refused before the device is touched

@@ -36,7 +36,7 @@ def test_predict_from_net_file(tmp_path, arch):
     xb = torch.from_numpy(frontend.make_batch(lp, rp)).to("cuda:0")
     tower = feature_tower.FeatureTower(layers, arch=arch)
     head = scorer_head.ScorerHead(head_layers) if arch == "slow" else None
-    opt = pipeline.make_params("kitti", arch)
+    opt = pipeline.make_params("kitti", arch, border=3)                # fix_border's width of the 3-layer net
     want, wl, wr = pipeline.stereo_predict(xb, tower.forward(xb), opt, D, want_vols=True, arch=arch, head=head)
     torch.cuda.synchronize()
     assert disp.shape == (H, W) and np.isfinite(disp).all()

@@ -151,11 +151,7 @@ def _run_capturing_maps(monkeypatch, *args, **kw):
 
 
 def _frontend_map(world, files, dataset, arch, disp_max):
-    kw = {}
-    if arch in ("fast", "slow"):
-        kw = dict(net_fname=world["nets"][arch], border=frontend.net_border(frontend.load_net(world["nets"][arch], arch)))
-    preset = "kitti" if dataset == "kitti2015" and arch in ("ad", "census") else dataset
-    return frontend.predict(files[0], files[1], dataset=preset, arch=arch, disp_max=disp_max, **kw)
+    return frontend.predict(files[0], files[1], dataset=dataset, arch=arch, disp_max=disp_max, net_fname=world["nets"].get(arch))
 
 
 @pytest.mark.parametrize("dataset,arch,disp_max", [("kitti", "fast", 228), ("kitti2015", "fast", 228), ("kitti", "census", 228),

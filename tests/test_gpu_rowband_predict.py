@@ -58,10 +58,9 @@ def test_band_volumes_equal_rows_of_the_whole_image(tmp_path, arch, H, W, D):
     dev = torch.device("cuda", 0)
     lp, rp = _images(tmp_path, H, W)
     xb = torch.from_numpy(frontend.make_batch(lp, rp)).to(dev)
-    tower = head = feats = None
-    if arch in ("fast", "slow"):
-        tower, head = frontend.make_stages(frontend.load_net(_net(str(tmp_path / "net.t7"), arch), arch), dev)
-        feats = tower.forward(xb)
+    method = frontend.StereoMethod("kitti", arch, _net(str(tmp_path / "net.t7"), arch) if arch in ("fast", "slow") else None)
+    tower, head = method.stages(dev)
+    feats = tower.forward(xb) if tower is not None else None
     opt = pipeline.make_params("kitti", arch)
     # the volumes as main.lua holds them at :986: the chain stopped right after the matching cost
     _, wantL, wantR = pipeline.stereo_predict(xb, feats, pipeline.make_params("kitti", arch, sm_terminate="cnn"), D,
@@ -82,12 +81,12 @@ def test_band_volumes_equal_rows_of_the_whole_image(tmp_path, arch, H, W, D):
         if not extends:
             assert covered == H
     torch.cuda.synchronize()
+    method.close()
 
 
 def _frontend_files(tmp_path, lp, rp, arch, D, net):
     out = str(tmp_path / "frontend")
-    over = {"border": frontend.net_border(frontend.load_net(net, arch))} if net else {}
-    frontend.predict(lp, rp, "kitti", arch, disp_max=D, out_dir=out, net_fname=net, **over)
+    frontend.predict(lp, rp, "kitti", arch, disp_max=D, out_dir=out, net_fname=net)
     torch.cuda.synchronize()
     return out
 

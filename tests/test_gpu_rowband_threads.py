@@ -167,31 +167,23 @@ def test_band_predict_matches_the_whole_image(pair, arch):
     tmp, lp, rp, nets = pair
     xb = torch.from_numpy(frontend.make_batch(lp, rp)).to(dev())
     opt = pipeline.make_params("kitti", arch)
-    net = frontend.load_net(nets[arch], arch) if arch in ("fast", "slow") else None
-    feats = head = None
-    if net is not None:
-        tower, head = frontend.make_stages(net, dev())
-        feats = tower.forward(xb)
+    method = frontend.StereoMethod("kitti", arch, nets.get(arch))
+    tower, head = method.stages(dev())
+    feats = tower.forward(xb) if tower is not None else None
     want, wantL, wantR = pipeline.stereo_predict(xb, feats, opt, D_IMG, want_vols=True, arch=arch, head=head)
     torch.cuda.synchronize()
-    if net is not None:
-        tower.close()
-        if head is not None:
-            head.close()
+    method.close()
     del feats
 
     def rank(comm):
-        t = h = None
-        if net is not None:
-            t, h = frontend.make_stages(net, dev())
+        m = frontend.StereoMethod("kitti", arch, nets.get(arch))
+        t, h = m.stages(dev())
         try:
             d, vl, vr = rowband.band_predict(rowband.CudaOps(dev()), xb, D_IMG, opt, arch, t, h, comm, want_vols=True)
             return d.cpu(), vl.cpu(), vr.cpu()
         finally:
             torch.cuda.current_stream().synchronize()
-            for s in (t, h):
-                if s is not None:
-                    s.close()
+            m.close()
 
     for r, (d, vl, vr) in enumerate(run_ranks(WORLD, rank, device=dev())):
         y0, y1 = rowband.split(H_IMG, WORLD, r)
@@ -205,10 +197,9 @@ def test_predict_pair_writes_frontend_predict_files(pair, arch):
     tmp, lp, rp, nets = pair
     net = nets.get(arch)
     want = _frontend_files(tmp / arch, lp, rp, arch, D_IMG, net)
-    over = {"border": frontend.net_border(frontend.load_net(net, arch))} if net else {}
     out = str(tmp / arch / "rowband")
     run_ranks(WORLD, lambda comm: rowband.predict_pair(lp, rp, "kitti", arch, disp_max=D_IMG, net_fname=net, comm=comm,
-                                                       device=dev(), out_dir=out, **over), device=dev())
+                                                       device=dev(), out_dir=out), device=dev())
     _assert_same_files(out, want)
 
 

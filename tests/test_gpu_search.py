@@ -118,13 +118,12 @@ def test_set_params_equals_a_fresh_pipeline(dataset, arch, cbca, overlap):
     else:
         forced = [dict(blur_sigma=10.0, pi1=1.0, pi2=32.0)]
     points = _points(dataset, arch, 10, seed=11 + PRESETS.index((dataset, arch)), forced=forced)
-    preset = search.preset_name(dataset, arch)
-    base = pipeline.make_params(preset, arch, blur_sigma=1.0)          # smallest Gaussian: 10.0 must grow the buffer
+    base = pipeline.make_params(dataset, arch, blur_sigma=1.0)          # smallest Gaussian: 10.0 must grow the buffer
     sp = pipeline.StereoPipeline(C, CREATED[2], CREATED[0], CREATED[1], base)
     _configure(sp, cbca, overlap)
     ins = {s: _pair(s, seed=s[1]) for s in (CREATED, SMALL)}
     for k, pt in enumerate(points):
-        opt = pipeline.make_params(preset, arch, **pt)
+        opt = pipeline.make_params(dataset, arch, **pt)
         shape = SMALL if k % 3 == 1 else CREATED
         fresh = pipeline.StereoPipeline(C, shape[2], shape[0], shape[1], opt)
         _configure(fresh, cbca, overlap)
@@ -135,7 +134,7 @@ def test_set_params_equals_a_fresh_pipeline(dataset, arch, cbca, overlap):
     # the twin lanes of run_batch follow set_params: a batch at the created shape, then re-targeted again
     pairs = [_pair(CREATED, seed=s) for s in (1, 2, 3)]
     for pt in points[-2:]:
-        opt = pipeline.make_params(preset, arch, **pt)
+        opt = pipeline.make_params(dataset, arch, **pt)
         sp.set_params(opt)
         got = sp.run_batch(pairs)
         torch.cuda.synchronize()
@@ -191,7 +190,7 @@ def _chain_case(world, dataset, arch, shape, seed):
     views, _ = synth._scene_views(rng, h, w, d)
     xb = _t(views[:, None])
     feats = head = None
-    opt = pipeline.make_params(search.preset_name(dataset, arch), arch)
+    opt = pipeline.make_params(dataset, arch)
     if arch == "slow":
         tl, hl = world["layers"]["slow"]
         tower = feature_tower.FeatureTower(tl, arch="slow")

@@ -221,7 +221,7 @@ def test_tool_refuses_a_net_of_the_other_arch(tmp_path):
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import predict_rowband
-    from mccnn_b200 import t7
+    from mccnn_b200 import frontend, t7
     from oracle import feature_tower as oft
 
     net = str(tmp_path / "fast.t7")
@@ -229,7 +229,8 @@ def test_tool_refuses_a_net_of_the_other_arch(tmp_path):
     with pytest.raises(SystemExit, match="'fast' network"):
         predict_rowband.parse_args(["kitti", "slow", "-left", "l", "-right", "r", "-disp_max", "8", "-net_fname", net])
     args, over = predict_rowband.parse_args(["kitti", "fast", "-left", "l", "-right", "r", "-disp_max", "8", "-net_fname", net])
-    assert over == {"border": 2} and args.out == "."
+    assert over == {} and args.out == "."
+    assert frontend.StereoMethod(args.dataset, args.arch, args.net_fname, **over).opt.border == 2      # the net's, not 4
 
 
 def test_predict_pair_refuses_before_any_gpu_work(tmp_path):

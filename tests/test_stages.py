@@ -131,7 +131,7 @@ def test_steps_that_do_no_work_are_refused(dataset, arch, option, name, over):
     with pytest.raises(ValueError, match="-%s %s: that step does no work in the %s %s" % (option, name, dataset, arch)):
         evaluate.check_stage_options(dataset, arch, **dict(over, **{option: name}))
     # the same variant is still a valid pipeline parameter set: it equals another variant (test_mb_no_op_variants...)
-    pipeline.make_params(evaluate.preset_name(dataset, arch), arch, **dict(over, **{option: name}))
+    pipeline.make_params(dataset, arch, **dict(over, **{option: name}))
 
 
 def test_idle_steps_follow_the_parameters():
@@ -236,7 +236,7 @@ def test_ablation_variants():
         pipeline.make_params("kitti", "fast", **ov)
     # steps that do no work are left out, as run_main.py refuses them
     for dataset, arch in (("kitti", "fast"), ("kitti2015", "slow"), ("mb", "census"), ("mb", "fast"), ("kitti", "ad")):
-        opt = pipeline.make_params(evaluate.preset_name(dataset, arch), arch)
+        opt = pipeline.make_params(dataset, arch)
         labels = [l for l, _ in search.ablation_variants(opt)]
         idle = pipeline.idle_steps(opt)
         assert labels == ["full"] + ["-sm_skip " + s for s in sc.SKIP if s not in idle] + [

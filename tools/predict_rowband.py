@@ -28,17 +28,15 @@ def parse_args(argv=None):
     for k in ("sm_terminate", "sm_skip"):
         if k in overrides:
             raise SystemExit("predict_rowband.py: -%s is not supported: the row bands run the full chain (use run_main.py)" % k)
-    if args.arch in ("fast", "slow"):
-        if not args.net_fname:
-            raise SystemExit("predict_rowband.py: arch '%s' needs -net_fname" % args.arch)
-        import mccnn_b200  # noqa: F401
-        from mccnn_b200 import frontend
+    import mccnn_b200  # noqa: F401
+    from mccnn_b200 import frontend
 
-        try:
-            net = frontend.load_net(args.net_fname, args.arch)
-        except ValueError as e:
-            raise SystemExit("predict_rowband.py: %s" % e)
-        overrides.setdefault("border", frontend.net_border(net))          # as run_main.py -a predict
+    try:
+        method = frontend.StereoMethod(args.dataset, args.arch, args.net_fname or None, **overrides)
+    except ValueError as e:
+        raise SystemExit("predict_rowband.py: %s" % e)
+    if method.needs_net:
+        raise SystemExit("predict_rowband.py: arch '%s' needs -net_fname" % args.arch)
     return args, overrides
 
 

@@ -84,8 +84,6 @@ def main(argv=None):
     if args.a == "predict":
         if not (args.left and args.right and args.disp_max):
             raise SystemExit("run_main.py: -a predict needs -left, -right and -disp_max")
-        if args.arch in ("fast", "slow") and args.net_fname:
-            overrides.setdefault("border", frontend.net_border(frontend.load_net(args.net_fname, args.arch)))
         frontend.predict(args.left, args.right, dataset=args.dataset, arch=args.arch, disp_max=args.disp_max,
                          out_dir=".", device=args.device, net_fname=args.net_fname or None, **overrides)
         return 0
