@@ -312,6 +312,39 @@ int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D, const flo
 			       const float *imgL, const float *imgR, float *disp, float *outL, float *outR,
 			       adcensus_stream_t stream);
 
+/* ---- confidence, LR map, sparse maps and sparsification counts (csrc/confidence.cu; DESIGN §19) ---------------------------
+ * An addition beyond the reference.  Margin confidence of a (D,H,W) volume at each pixel: d1 = the arg-min of
+ * mccnn_argmin_pitched (first strict minimum, NaN skipped, 0 when nothing is below +inf) with value c1; c2 = the minimum by
+ * the same rule over the d with |d - d1| >= 2; conf = c2 - c1 in float when both are below +inf, else 0.  The confidence
+ * belongs to the integer winner: sub-pixel refinement, median and bilateral filtering move the disparity, not its confidence.
+ *
+ * mccnn_pipeline_run_shape_conf / _run_volumes_conf: mccnn_pipeline_run_shape / _run_volumes that also write conf (H,W),
+ * the margin confidence of the final left volume (what volL / outL receives), and lr (H,W), main.lua:1056's outlier map
+ * (0 consistent, 1 mismatch, 2 occlusion) of the two winner-take-all maps; for lr, direction +1 and the LR check run even
+ * when -sm_terminate / -sm_skip would skip them.  conf and lr may be NULL; with both NULL the calls are the plain ones (same
+ * launches, same bits), and disp never changes with them.  ADCENSUS_EINVAL, before any launch, for lr with lr_check == 0
+ * and as the plain calls. */
+int mccnn_pipeline_run_shape_conf(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+				  const float *imgL, const float *imgR, float *disp, float *conf, float *lr, float *volL,
+				  float *volR, adcensus_stream_t stream);
+int mccnn_pipeline_run_volumes_conf(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
+				    const float *imgL, const float *imgR, float *disp, float *conf, float *lr, float *outL,
+				    float *outR, adcensus_stream_t stream);
+/* The arg-min (disp) and the margin confidence (conf) of a contiguous (D,H,W) volume in one read; disp bit-identical to
+ * mccnn_argmin.  H <= 65535. */
+int mccnn_margin_confidence(const float *vol, float *disp, float *conf, int D, int H, int W, adcensus_stream_t stream);
+/* out = disp at the n_keep pixels of largest conf (ties: lower row-major index first), `invalid` elsewhere.  Pixels are
+ * ordered by conf's float bits, which order like the values (NaN above +inf).  1 <= n_keep <= H*W (else ADCENSUS_EINVAL),
+ * H*W < 2^32 (else ADCENSUS_ELIMIT); out must not alias disp or conf.  Exact and deterministic.  Asynchronous. */
+int mccnn_sparsify(const float *disp, const float *conf, float *out, int H, int W, long long n_keep, float invalid,
+		   adcensus_stream_t stream);
+/* The counts of the sparsification curve of pred against gt (H,W): counts[0] = M, the pixels with gt != 0 (main.lua:1230);
+ * counts[1] = B, the bad ones among them (|gt - pred| > err_at); counts[1 + k], k = 1..20 = the bad ones among the first
+ * n_k = ceil(k M / 20) of the M pixels ordered as mccnn_sparsify orders them.  counts: 22 long longs in device memory.
+ * Exact and deterministic.  Asynchronous. */
+int mccnn_sparsification_counts(const float *pred, const float *conf, const float *gt, int H, int W, float err_at,
+				long long *counts, adcensus_stream_t stream);
+
 /* Host-buffer call (what a non-CUDA caller binds): copies inputs H2D, runs,
  * copies disp back, and returns after the result is in disp_host. */
 int mccnn_pipeline_run_host(mccnn_pipeline *p, const float *featL_host, const float *featR_host,

@@ -41,6 +41,7 @@ int adc_stereo_join(const float *input_L, const float *input_R, float *output_L,
 int adc_fill_invalid(float *volL, float *volR, int D, int H, int W, int ld, cudaStream_t s);
 int adc_fix_border(float *vol, int D, int H, int W, int ld, int n, int direction, cudaStream_t s);
 int adc_argmin_pitched(const float *vol, float *disp, int D, int H, int W, int ld, cudaStream_t s);
+int adc_argmin_conf_pitched(const float *vol, float *disp, float *conf, int D, int H, int W, int ld, cudaStream_t s);
 int adc_subpixel(const float *d0, const float *c2, float *out, int H, int W, int ld, int disp_max, cudaStream_t s);
 
 // Private volume layout: (D, H, ld), ld = W rounded up to a multiple of 4 floats.  Every row then starts on a
@@ -202,10 +203,11 @@ Stages stages_of(const mccnn_params &o)
 	return st;
 }
 
-// direction +1 is consumed only by the outlier map of the interpolations (or a caller that wants the right volume)
-bool needs_right(const mccnn_params &o, const Stages &st, const float *volR)
+// direction +1 is consumed only by the outlier map of the interpolations (or a caller that wants the right volume or the
+// outlier map itself)
+bool needs_right(const mccnn_params &o, const Stages &st, const float *volR, const float *lr)
 {
-	return (o.lr_check && (st.occlusion || st.mismatch)) || volR;
+	return (o.lr_check && (st.occlusion || st.mismatch)) || volR || lr;
 }
 
 // gaussian(blur_sigma) (main.lua:1078 gaussian(opt.blur_sigma):cuda()) into p->gauss; the buffer grows only when the kernel
@@ -428,9 +430,10 @@ static int run_build_volumes(mccnn_pipeline *p, int H, int W, int D, const float
 }
 
 // main.lua:986-1082 from the two volumes in the private buffers (the right one only when it is consumed); nl = the
-// launches that built them
+// launches that built them.  conf: the margin confidence of the final left volume, from direction -1's arg-min (same
+// launch count); lr: main.lua:1056's outlier map, for which direction +1 and the LR check run if nothing else needs them.
 static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, const float *imgR, float *disp, float *volL,
-		     float *volR, int nl, cudaStream_t s)
+		     float *volR, float *conf, float *lr, int nl, cudaStream_t s)
 {
 	const int ld = (W + 3) & ~3;
 	const long HW = (long)H * W, V = (long)D * H * ld;
@@ -503,7 +506,11 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 			STEP(cbca(cur, spare, direction, ds));
 			float *t = cur; cur = spare; spare = t; nl += 1;
 		}
-		STEP(adc_argmin_pitched(cur, direction == 1 ? dispR : dispL, D, H, W, ld, ds)); nl += 1; // :1049-1050
+		if (direction == -1 && conf)                                                             // :1049-1050
+			STEP(adc_argmin_conf_pitched(cur, dispL, conf, D, H, W, ld, ds));
+		else
+			STEP(adc_argmin_pitched(cur, direction == 1 ? dispR : dispL, D, H, W, ld, ds));
+		nl += 1;
 		float *dst = direction == 1 ? volR : volL;                                               // :1042-1047
 		if (dst) STEP((int)cudaMemcpy2DAsync(dst, (size_t)W * 4, cur, (size_t)ld * 4, (size_t)W * 4, (size_t)D * H,
 						     cudaMemcpyDeviceToDevice, ds));
@@ -512,7 +519,7 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 	};
 	// main.lua:954-955: without the LR check (mb) only direction -1 is consumed, unless the caller asks for the
 	// right volume (`-a predict` writes right.bin); with it, only when an interpolation reads the outlier map
-	const bool need_right = needs_right(o, st, volR);
+	const bool need_right = needs_right(o, st, volR, lr);
 	if (!need_right) {
 		STEP(run_direction(1, s, volsL, p->bufA, p->bufC, p->sgmtab));
 	} else if (!p->overlap) {
@@ -530,8 +537,8 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 	}
 
 	const float *curd = dispL;                                                                   // disp[2]
-	float *outlier = m + 2 * HW;
-	if (st.occlusion || st.mismatch) {                                                           // :1056 (unread otherwise)
+	float *outlier = lr ? lr : m + 2 * HW;
+	if (st.occlusion || st.mismatch || lr) {                                                     // :1056 (unread otherwise)
 		STEP(adcensus_outlier_detection(dispL, dispR, outlier, H, W, D, s)); nl += 1;
 	}
 	if (st.occlusion) {                                                                          // :1058
@@ -562,19 +569,21 @@ static int run_chain(mccnn_pipeline *p, int H, int W, int D, const float *imgL, 
 }
 
 static int pipeline_run_at(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
-			   const float *imgL, const float *imgR, float *disp, float *volL, float *volR, cudaStream_t s)
+			   const float *imgL, const float *imgR, float *disp, float *volL, float *volR, float *conf, float *lr,
+			   cudaStream_t s)
 {
 	int nl = 0;
 	STEP(run_fits(p, H, W, D));
 	STEP(run_build_volumes(p, H, W, D, featL, featR, s, &nl));
-	return run_chain(p, H, W, D, imgL, imgR, disp, volL, volR, nl, s);
+	return run_chain(p, H, W, D, imgL, imgR, disp, volL, volR, conf, lr, nl, s);
 }
 
-extern "C" int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
-					  const float *imgL, const float *imgR, float *disp, float *outL, float *outR,
-					  adcensus_stream_t stream)
+extern "C" int mccnn_pipeline_run_volumes_conf(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
+					       const float *imgL, const float *imgR, float *disp, float *conf, float *lr, float *outL,
+					       float *outR, adcensus_stream_t stream)
 {
 	if (!p || !volL || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
+	if (lr && !p->prm.lr_check) return ADCENSUS_EINVAL;                    // main.lua has no LR check there
 	if (!volR && (p->prm.lr_check || outR)) return ADCENSUS_EINVAL;       // direction +1 is run: it needs its volume
 	if (H < 1 || W < 1 || D < 1 || p->prm.border + 1 > W) return ADCENSUS_EINVAL;
 	if (H > p->H || W > p->W || D > p->D) return ADCENSUS_ELIMIT;
@@ -585,9 +594,16 @@ extern "C" int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D
 	const long V = (long)D * H * ld;
 	const size_t row = (size_t)W * sizeof(float), pitch = (size_t)ld * sizeof(float);
 	ADC_CUDA(cudaMemcpy2DAsync(p->vols, pitch, volL, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
-	if (needs_right(p->prm, stages_of(p->prm), outR))                      // only then is the right volume read
+	if (needs_right(p->prm, stages_of(p->prm), outR, lr))                  // only then is the right volume read
 		ADC_CUDA(cudaMemcpy2DAsync(p->vols + V, pitch, volR, row, row, (size_t)D * H, cudaMemcpyDeviceToDevice, s));
-	return run_chain(p, H, W, D, imgL, imgR, disp, outL, outR, 0, s);
+	return run_chain(p, H, W, D, imgL, imgR, disp, outL, outR, conf, lr, 0, s);
+}
+
+extern "C" int mccnn_pipeline_run_volumes(mccnn_pipeline *p, int H, int W, int D, const float *volL, const float *volR,
+					  const float *imgL, const float *imgR, float *disp, float *outL, float *outR,
+					  adcensus_stream_t stream)
+{
+	return mccnn_pipeline_run_volumes_conf(p, H, W, D, volL, volR, imgL, imgR, disp, nullptr, nullptr, outL, outR, stream);
 }
 
 extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const float *featR,
@@ -596,18 +612,26 @@ extern "C" int mccnn_pipeline_run(mccnn_pipeline *p, const float *featL, const f
 {
 	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
 	DeviceGuard g(p->device);
-	return pipeline_run_at(p, p->H, p->W, p->D, featL, featR, imgL, imgR, disp, volL, volR, adc_stream(stream));
+	return pipeline_run_at(p, p->H, p->W, p->D, featL, featR, imgL, imgR, disp, volL, volR, nullptr, nullptr, adc_stream(stream));
+}
+
+extern "C" int mccnn_pipeline_run_shape_conf(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
+					     const float *imgL, const float *imgR, float *disp, float *conf, float *lr, float *volL,
+					     float *volR, adcensus_stream_t stream)
+{
+	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
+	if (lr && !p->prm.lr_check) return ADCENSUS_EINVAL;
+	if (H < 1 || W < 1 || D < 1 || p->prm.border + 1 > W) return ADCENSUS_EINVAL;
+	if (H > p->H || W > p->W || D > p->D) return ADCENSUS_ELIMIT;
+	DeviceGuard g(p->device);
+	return pipeline_run_at(p, H, W, D, featL, featR, imgL, imgR, disp, volL, volR, conf, lr, adc_stream(stream));
 }
 
 extern "C" int mccnn_pipeline_run_shape(mccnn_pipeline *p, int H, int W, int D, const float *featL, const float *featR,
 					const float *imgL, const float *imgR, float *disp, float *volL, float *volR,
 					adcensus_stream_t stream)
 {
-	if (!p || !featL || !featR || !imgL || !imgR || !disp) return ADCENSUS_EINVAL;
-	if (H < 1 || W < 1 || D < 1 || p->prm.border + 1 > W) return ADCENSUS_EINVAL;
-	if (H > p->H || W > p->W || D > p->D) return ADCENSUS_ELIMIT;
-	DeviceGuard g(p->device);
-	return pipeline_run_at(p, H, W, D, featL, featR, imgL, imgR, disp, volL, volR, adc_stream(stream));
+	return mccnn_pipeline_run_shape_conf(p, H, W, D, featL, featR, imgL, imgR, disp, nullptr, nullptr, volL, volR, stream);
 }
 
 static int host_staging(mccnn_pipeline *p)

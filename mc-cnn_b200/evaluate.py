@@ -243,20 +243,23 @@ class Evaluator:
             self.sp = None
         self.method.close()
 
-    def stereo_predict(self, x_batch, disp_max):
-        """main.lua:929-1082 for one (2,1,H,W) device batch: (H, W) device disparity map"""
+    def stereo_predict(self, x_batch, disp_max, conf=None, lr=None):
+        """main.lua:929-1082 for one (2,1,H,W) device batch: (H, W) device disparity map.  `conf` / `lr`: (H, W) device
+        tensors that receive the margin confidence and the LR check's outlier map (mc-cnn_b200/confidence.py)."""
         with torch.cuda.device(self.dev):
             if self.arch == "fast":
                 feats = self.tower.forward(x_batch)
-                return self.sp.run_shape(feats[0], feats[1], x_batch[0, 0], x_batch[1, 0], disp_max=disp_max)
+                return self.sp.run_shape(feats[0], feats[1], x_batch[0, 0], x_batch[1, 0], disp_max=disp_max, conf=conf,
+                                         lr=lr)
             feats = self.tower.forward(x_batch) if self.arch == "slow" else None
-            return pipeline.stereo_predict(x_batch, feats, self.opt, disp_max, arch=self.arch, head=self.head)[0, 0]
+            return pipeline.stereo_predict(x_batch, feats, self.opt, disp_max, arch=self.arch, head=self.head, conf=conf,
+                                           lr=lr)[0, 0]
 
-    def timed(self, x_batch, disp_max):
+    def timed(self, x_batch, disp_max, conf=None):
         """main.lua:1195-1200: (pred, runtime in seconds) with the device synchronised before and after"""
         torch.cuda.synchronize(self.dev)
         t0 = time.perf_counter()
-        pred = self.stereo_predict(x_batch, disp_max)
+        pred = self.stereo_predict(x_batch, disp_max) if conf is None else self.stereo_predict(x_batch, disp_max, conf=conf)
         torch.cuda.synchronize(self.dev)
         return pred, time.perf_counter() - t0
 
@@ -295,6 +298,39 @@ class Evaluator:
         if verbose:
             print(lua_num(mean), flush=True)
         return TestResult(out, mean)
+
+    def sparsification(self, action="test_te", data_root=".", data=None, rect="imperfect", color="gray", err_at=None,
+                       verbose=True):
+        """The sparsification curve of each example's map under its margin confidence (an addition beyond the reference,
+        mc-cnn_b200/confidence.py): per example ``id\terr\tauc\tauc_opt`` (err = test()'s, e_20 of the curve), then
+        ``mean`` and the three means.  `err_at` defaults to main.lua's for the dataset.  Returns [(id, Sparsification)]."""
+        from . import confidence
+
+        if action not in ("test_te", "test_all"):
+            raise ValueError("sparsification() runs test_te or test_all, not %r" % (action,))
+        data = data or load_data(self.dataset, data_root, rect, color)
+        err_at = dataio.ERR_AT[self.dataset] if err_at is None else err_at
+        examples = data.examples(action)
+        self.prepare([data.shape_of(ex) for ex in examples])
+        out = []
+        for ex in examples:
+            x, disp_max, id_, _, img_width = data.example(ex)
+            x_batch = torch.from_numpy(x).to(self.dev)
+            conf = torch.empty(x.shape[2:], device=self.dev)
+            pred = self.stereo_predict(x_batch, disp_max, conf=conf)
+            if torch.isnan(pred).any():                                                         # main.lua:1224
+                raise ValueError("example %s: the prediction contains NaN" % (id_,))
+            gt = torch.from_numpy(np.ascontiguousarray(data.ground_truth(ex, img_width), np.float32)).to(self.dev)
+            with torch.cuda.device(self.dev):
+                res = confidence.sparsification(pred.contiguous(), conf, gt.contiguous(), err_at)
+            out.append((id_, res))
+            if verbose:
+                print("\t".join([str(id_)] + [lua_num(v) for v in (res.curve[-1], res.auc, res.auc_opt)]), flush=True)
+        if verbose:
+            means = [(sum(f(r) for _, r in out) / len(out)) if out else float("nan")
+                     for f in (lambda r: r.curve[-1], lambda r: r.auc, lambda r: r.auc_opt)]
+            print("\t".join(["mean"] + [lua_num(v) for v in means]), flush=True)
+        return out
 
     def submit(self, data_root=".", out="out", data=None, rect="imperfect", color="gray"):
         """``-a submit`` (main.lua:1107-1120, 1202-1222, 1288-1290): KITTI PNG16 maps (kitti2015 under disp_0/), Middlebury

@@ -192,13 +192,15 @@ class StereoMethod:
 
 
 def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=None, out_dir=None, device=0,
-            net_fname=None, **overrides):
+            net_fname=None, confidence=False, **overrides):
     """``main.lua <dataset> <arch> -a predict -net_fname N -left L -right R -disp_max D`` from the image files on:
     returns disp (H,W) float32 (numpy).  With `out_dir`, writes right.bin and left.bin ((1,D,H,W), in
     that order, main.lua:1042-1047) and disp.bin ((1,1,H,W), :1103) there.  arch 'fast' / 'slow' take the trained
     network from `net_fname` (the reference's ascii .t7, main.lua:893-901, read by :mod:`t7`) and run it on the GPU
     (feature tower, and for 'slow' the scorer head); arch 'fast' alternatively accepts `features` (2,C,H,W), the
-    unit-norm tower output; 'ad' / 'census' need neither."""
+    unit-norm tower output; 'ad' / 'census' need neither.  With `confidence` (an addition beyond the reference), also writes
+    conf.bin, the margin confidence of the left volume (mc-cnn_b200/confidence.py), and for presets with the LR check lr.bin,
+    main.lua:1056's outlier map, both (1,1,H,W) float32, each announced by a ``Writing`` line in main.lua's format."""
     import torch
 
     method = StereoMethod(dataset, arch, None if features is not None else net_fname, **overrides)   # before any GPU work
@@ -218,8 +220,11 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
                 feats = tower.forward(x_batch)                                  # main.lua:944 / :957
             elif arch == "fast":
                 feats = torch.as_tensor(features, dtype=torch.float32).to(dev).contiguous()
+            H, W = x_batch.shape[2:]
+            conf = torch.empty((H, W), device=dev) if confidence else None
+            lr = torch.empty((H, W), device=dev) if confidence and method.opt.lr_check else None
             disp, volL, volR = pipeline.stereo_predict(x_batch, feats, method.opt, int(disp_max), want_vols=True, arch=arch,
-                                                       head=head)
+                                                       head=head, conf=conf, lr=lr)
         disp_h = disp.cpu().numpy()
     finally:
         method.close()
@@ -228,4 +233,8 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
         write_bin(os.path.join(out_dir, "right.bin"), volR.cpu().numpy())       # direction 1 comes first
         write_bin(os.path.join(out_dir, "left.bin"), volL.cpu().numpy())
         write_bin(os.path.join(out_dir, "disp.bin"), disp_h)
+        for name, t in (("conf", conf), ("lr", lr)):
+            if t is not None:
+                print("Writing %s.bin, 1 x 1 x %d x %d" % (name, H, W), flush=True)
+                write_bin(os.path.join(out_dir, name + ".bin"), t.cpu().numpy())
     return disp_h[0, 0]

@@ -30,7 +30,7 @@ from collections import OrderedDict, namedtuple
 
 import numpy as np
 
-from . import batch, dataio, evaluate, frontend, predict_kitti, preprocess
+from . import batch, confidence, dataio, evaluate, frontend, predict_kitti, preprocess
 
 DATASETS = ("kitti", "kitti2015")
 GT_OCC = {"kitti": "disp_occ", "kitti2015": "disp_occ_0"}
@@ -305,16 +305,22 @@ def _world():
 
 
 def evaluate_training(dataset, net_fname, arch="fast", data_root=".", disp_max=predict_kitti.DISP_MAX, out=None, device=0,
-                      prefetch=True, verbose=True, **overrides):
+                      prefetch=True, verbose=True, density=None, **overrides):
     """The net over every raw training pair of `dataset` under `data_root` (predict_kitti.py test's loop, on CUDA device
     `device`; `overrides` change the stereo method's preset as in Evaluator), each map scored by devkit_counts.  With `out`,
     each map is also written in submission layout (refused when `out` is not empty), so that score_dir(dataset, out, ...)
-    gives the same numbers.  Returns the Scores on rank 0, None on other ranks."""
+    gives the same numbers.  With `density` in (0, 1] (an addition beyond the reference), each map is first made sparse,
+    keeping the ceil(density H W) pixels of largest margin confidence (:func:`confidence.sparsify`, 0 elsewhere): what is
+    scored and written is the sparse map, whose dropped pixels the devkit fills by its background interpolation.  Returns
+    the Scores on rank 0, None on other ranks."""
+    import torch
     import torch.distributed as dist
 
     _check_dataset(dataset)
     if int(disp_max) < 1:
         raise ValueError("disp_max must be at least 1, got %r" % (disp_max,))
+    if density is not None:
+        confidence.check_density(density)
     files = training_files(data_root, dataset)
     shapes = predict_kitti.scan([f[:3] for f in files])
     check_maps([(None,) + f[2:] for f in files], shapes)
@@ -334,7 +340,14 @@ def evaluate_training(dataset, net_fname, arch="fast", data_root=".", disp_max=p
     def compute(i):
         left, right, noc = pre.get(i)
         occ, obj = pre_maps.get(i)
-        pred = ev.stereo_predict(frontend.make_batch_cuda(left, right, ev.dev), disp_max)
+        x_batch = frontend.make_batch_cuda(left, right, ev.dev)
+        if density is None:
+            pred = ev.stereo_predict(x_batch, disp_max)
+        else:
+            conf = torch.empty(x_batch.shape[2:], device=ev.dev)
+            pred = ev.stereo_predict(x_batch, disp_max, conf=conf)
+            with torch.cuda.device(ev.dev):
+                pred = confidence.sparsify(pred, conf, density, 0.0)
         c = devkit_counts(pred, noc, occ, obj)
         if out is not None:
             H, W = shapes[i]

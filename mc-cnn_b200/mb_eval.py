@@ -27,7 +27,7 @@ from collections import OrderedDict, namedtuple
 
 import numpy as np
 
-from . import dataio, evaluate, preprocess
+from . import confidence, dataio, evaluate, preprocess
 
 REGIONS = ("nonocc", "all")
 # the count layout of mccnn_mb_evaldisp (include/adcensus_b200.h): counts[r, k], r 0 = nonocc, 1 = all
@@ -251,16 +251,21 @@ def score_dir(out, data_root=".", res="F", alg=None, device=0, verbose=True):
     return rep.done()
 
 
-def evaluate_training(arch, net_fname=None, data_root=".", res="F", out=None, device=0, verbose=True, **overrides):
+def evaluate_training(arch, net_fname=None, data_root=".", res="F", out=None, device=0, verbose=True, density=None,
+                      **overrides):
     """The net over the 15 MiddEval3 ``trainingH`` pairs, read from the raw files (grey views through the GPU read_im of
     preprocess_mb, disp_max = the scene's ndisp), each map predicted by evaluate.Evaluator at the mb preset of `arch`
     (`overrides` as in Evaluator) on CUDA device `device` and scored at resolution `res`.  With `out` (refused when not
     empty), each map and its runtime are also written as Evaluator.submit writes them, ``out/trainingH/<scene>/
     disp0<method>.pfm`` (rows bottom-up) and ``time<method>.txt``, so that score_dir(out, ...) prints the same lines.
-    Prints one line per scene and the line of means; returns the Scores."""
+    Prints one line per scene and the line of means; returns the Scores.  With `density` in (0, 1] (an addition beyond the
+    reference), each map keeps the ceil(density H W) pixels of largest margin confidence and holds +inf, the SDK's invalid
+    value, elsewhere (:func:`confidence.sparsify`, after the timed region); that map is scored and written."""
     import torch
 
     _check_res(res)
+    if density is not None:
+        confidence.check_density(density)
     todo = []
     for s in training_scenes(data_root):
         d = scene_dir(data_root, s)
@@ -279,7 +284,10 @@ def evaluate_training(arch, net_fname=None, data_root=".", res="F", out=None, de
         with torch.cuda.device(ev.dev):
             for s, views, size, ndisp, gt, mask in todo:
                 x = preprocess._mb_views(dict(groups=[(views, (2,))], half=False), "gray", ev.dev)[0]
-                pred, runtime = ev.timed(torch.from_numpy(np.ascontiguousarray(x)).to(ev.dev), ndisp)
+                conf = None if density is None else torch.empty(size, device=ev.dev)
+                pred, runtime = ev.timed(torch.from_numpy(np.ascontiguousarray(x)).to(ev.dev), ndisp, conf=conf)
+                if conf is not None:
+                    pred = confidence.sparsify(pred, conf, density, float("inf"))
                 rep.add(s, *_score(pred, gt, mask, ndisp, ev.dev))
                 if out is not None:
                     base = os.path.join(out, "trainingH", s)

@@ -160,7 +160,7 @@ def make_params(dataset="kitti", arch="fast", **overrides):
     return Params(**d)
 
 
-def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast", head=None):
+def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast", head=None, conf=None, lr=None):
     """main.lua:929-1082 through the adcensus.* operators.
 
     x_batch  (2,1,H,W) standardised images (left, right); arch 'fast': features (2,C,H,W) the tower
@@ -168,10 +168,15 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
     (main.lua:932-942), `features` is ignored; arch 'slow' (main.lua:956-981): features (2,fm,H,W) = the accurate
     architecture's tower output and `head` a :class:`mccnn_b200.scorer_head.ScorerHead` (net_te2), which scores every
     disparity into both volumes.  opt a :class:`Params`.
+    `conf` / `lr` (H, W) device tensors or None (an addition beyond the reference, DESIGN §19): receive the margin
+    confidence of the final left volume (:func:`confidence.margin`) and main.lua:1056's outlier map (0 consistent,
+    1 mismatch, 2 occlusion; only with the LR check, computed even when -sm_terminate / -sm_skip leave it unused).
     Returns disp (1,1,H,W) [, left vol, right vol].
     """
     assert x_batch.is_cuda
     check_arch(arch)
+    if lr is not None and not opt.lr_check:
+        raise adcensus.AdcensusError("stereo_predict: lr needs the LR check (kitti / kitti2015); main.lua has none for mb")
     H, W = x_batch.size(2), x_batch.size(3)
     dev = x_batch.device
     vols = torch.empty((2, disp_max, H, W), device=dev, dtype=torch.float32)
@@ -228,10 +233,16 @@ def stereo_predict(x_batch, features, opt, disp_max, want_vols=False, arch="fast
             out_vols[direction] = vol.clone()                                     # :1042-1047
         disp[1 if direction == 1 else 2] = adcensus.argmin(vol)                   # :1049-1050
 
+    if conf is not None:
+        from . import confidence
+
+        conf.view(H, W).copy_(confidence.margin(vol)[1].view(H, W))
     d = disp[2]
     if opt.lr_check:                                                              # :1054-1066
         outlier = torch.zeros_like(d)
         adcensus.outlier_detection(disp[2], disp[1], outlier, disp_max)
+        if lr is not None:
+            lr.view(H, W).copy_(outlier.view(H, W))
         if st["occlusion"]:
             d = adcensus.interpolate_occlusion(d, outlier)
         if st["mismatch"]:
@@ -318,11 +329,13 @@ class StereoPipeline:
         adcensus._check(rc, n)
         return disp
 
-    def run_shape(self, featL, featR, imgL, imgR, disp_max=None, disp=None, volL=None, volR=None):
+    def run_shape(self, featL, featR, imgL, imgR, disp_max=None, disp=None, volL=None, volR=None, conf=None, lr=None):
         """:meth:`run` at a smaller shape than the created one (mccnn_pipeline_run_shape): H, W from ``imgL``, D =
         ``disp_max`` (default: the created D); every tensor must be contiguous at that shape.  Same results, bit for bit,
         as a pipeline created at this shape, without allocating: one pipeline created at the largest (H, W, D) of a dataset
-        serves all of its images.  Asynchronous on torch's current stream."""
+        serves all of its images.  ``conf`` / ``lr`` (H, W) receive the margin confidence and the LR check's outlier map
+        (mccnn_pipeline_run_shape_conf; ``lr`` only with the LR check); ``disp`` is the same with or without them.
+        Asynchronous on torch's current stream."""
         n = "mccnn_pipeline_run_shape"
         if imgL.dim() != 2:
             raise adcensus.AdcensusError("%s: imgL must be (H, W), got %s" % (n, tuple(imgL.shape)))
@@ -331,23 +344,34 @@ class StereoPipeline:
         if disp is None:
             disp = torch.empty((H, W), device=imgL.device, dtype=torch.float32)
         want = [("featL", featL, (self.C, H, W)), ("featR", featR, (self.C, H, W)), ("imgR", imgR, (H, W)),
-                ("disp", disp, (H, W)), ("volL", volL, (D, H, W)), ("volR", volR, (D, H, W))]
+                ("disp", disp, (H, W)), ("volL", volL, (D, H, W)), ("volR", volR, (D, H, W)), ("conf", conf, (H, W)),
+                ("lr", lr, (H, W))]
         for name, t, shape in want:
             if t is not None and tuple(t.shape) != shape:
                 raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
+        self._check_lr(lr, n)
         with torch.cuda.device(imgL.device):
-            rc = adcensus.lib().mccnn_pipeline_run_shape(self._h, H, W, D, adcensus._t(featL, 1, n), adcensus._t(featR, 2, n),
-                                                         adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
-                                                         adcensus._t(disp, 5, n), adcensus._t(volL, 6, n, optional=True),
-                                                         adcensus._t(volR, 7, n, optional=True), adcensus._stream(imgL))
+            ptrs = (adcensus._t(featL, 1, n), adcensus._t(featR, 2, n), adcensus._t(imgL, 3, n), adcensus._t(imgR, 4, n),
+                    adcensus._t(disp, 5, n))
+            vols = (adcensus._t(volL, 6, n, optional=True), adcensus._t(volR, 7, n, optional=True))
+            if conf is None and lr is None:
+                rc = adcensus.lib().mccnn_pipeline_run_shape(self._h, H, W, D, *ptrs, *vols, adcensus._stream(imgL))
+            else:
+                rc = adcensus.lib().mccnn_pipeline_run_shape_conf(self._h, H, W, D, *ptrs, adcensus._t(conf, 8, n, optional=True),
+                                                                  adcensus._t(lr, 9, n, optional=True), *vols,
+                                                                  adcensus._stream(imgL))
         adcensus._check(rc, n)
         return disp
 
-    def run_volumes(self, volL, volR, imgL, imgR, disp_max=None, disp=None, outL=None, outR=None):
+    def _check_lr(self, lr, n):
+        if lr is not None and not self.params.lr_check:
+            raise adcensus.AdcensusError("%s: lr needs the LR check (kitti / kitti2015); main.lua has none for mb" % n)
+
+    def run_volumes(self, volL, volR, imgL, imgR, disp_max=None, disp=None, outL=None, outR=None, conf=None, lr=None):
         """The chain of :meth:`run_shape` from given cost volumes (mccnn_pipeline_run_volumes): volL / volR (D, H, W) or
         (1, D, H, W) device tensors as main.lua holds them at :986 (NaN fill, fix_border applied); they are not modified.
         ``volR`` may be None when the parameters have no LR check and ``outR`` is None.  H, W from ``imgL``, D = ``disp_max``
-        (default: the created D).  Asynchronous on torch's current stream."""
+        (default: the created D).  ``conf`` / ``lr`` as in :meth:`run_shape`.  Asynchronous on torch's current stream."""
         n = "mccnn_pipeline_run_volumes"
         if imgL.dim() != 2:
             raise adcensus.AdcensusError("%s: imgL must be (H, W), got %s" % (n, tuple(imgL.shape)))
@@ -358,17 +382,23 @@ class StereoPipeline:
         vol = lambda t: t[0] if t is not None and t.dim() == 4 and t.shape[0] == 1 else t
         volL, volR = vol(volL), vol(volR)
         want = [("volL", volL, (D, H, W)), ("volR", volR, (D, H, W)), ("imgR", imgR, (H, W)), ("disp", disp, (H, W)),
-                ("outL", outL, (D, H, W)), ("outR", outR, (D, H, W))]
+                ("outL", outL, (D, H, W)), ("outR", outR, (D, H, W)), ("conf", conf, (H, W)), ("lr", lr, (H, W))]
         for name, t, shape in want:
             if t is not None and tuple(t.shape) != shape:
                 raise adcensus.AdcensusError("%s: %s must be %s, got %s" % (n, name, shape, tuple(t.shape)))
         if volR is None and (self.params.lr_check or outR is not None):
             raise adcensus.AdcensusError("%s: volR is needed (LR check or outR)" % n)
+        self._check_lr(lr, n)
         ptrs = (adcensus._t(volL, 1, n), adcensus._t(volR, 2, n, optional=True), adcensus._t(imgL, 3, n),
-                adcensus._t(imgR, 4, n), adcensus._t(disp, 5, n), adcensus._t(outL, 6, n, optional=True),
-                adcensus._t(outR, 7, n, optional=True))
+                adcensus._t(imgR, 4, n), adcensus._t(disp, 5, n))
+        outs = (adcensus._t(outL, 6, n, optional=True), adcensus._t(outR, 7, n, optional=True))
         with torch.cuda.device(imgL.device):
-            rc = adcensus.lib().mccnn_pipeline_run_volumes(self._h, H, W, D, *ptrs, adcensus._stream(imgL))
+            if conf is None and lr is None:
+                rc = adcensus.lib().mccnn_pipeline_run_volumes(self._h, H, W, D, *ptrs, *outs, adcensus._stream(imgL))
+            else:
+                rc = adcensus.lib().mccnn_pipeline_run_volumes_conf(self._h, H, W, D, *ptrs, adcensus._t(conf, 8, n, optional=True),
+                                                                    adcensus._t(lr, 9, n, optional=True), *outs,
+                                                                    adcensus._stream(imgL))
         adcensus._check(rc, n)
         return disp
 

@@ -25,6 +25,9 @@ prints.
 Deliberate deviations from predict_kitti.lua: KITTI 2015 and archs other than 'fast' are accepted; missing files, views of
 different sizes and a ground truth of another size are refused before any GPU work; ``submit`` refuses a non-empty output
 directory (as Evaluator.submit does) and also writes 2015 maps, under ``out/disp_0/``.
+
+An addition beyond the reference: ``submit`` with `density` p in (0, 1] writes sparse maps, the ceil(p H W) pixels of
+largest margin confidence and 0 (the PNG16 invalid value) elsewhere (:func:`confidence.sparsify`).
 """
 import concurrent.futures
 import os
@@ -32,7 +35,7 @@ from collections import namedtuple
 
 import numpy as np
 
-from . import batch, dataio, evaluate, frontend, preprocess
+from . import batch, confidence, dataio, evaluate, frontend, preprocess
 
 ACTIONS = ("test", "submit")
 DISP_MAX = 228                          # predict_kitti.lua:37
@@ -175,7 +178,7 @@ def check_out(out):
 
 
 def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", out="out", disp_max=DISP_MAX, device=0,
-                  prefetch=True, verbose=True, **overrides):
+                  prefetch=True, verbose=True, density=None, **overrides):
     """predict_kitti.lua's `test` or `submit` on the raw `dataset` ('kitti' or 'kitti2015') under `data_root` on CUDA device
     `device`; `overrides` change the stereo method's preset as in Evaluator.  Returns, on rank 0, the TestResult (errors per
     training pair, mean) or the list of written files; None on other ranks.  `prefetch` False decodes each pair in turn."""
@@ -188,6 +191,10 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
         raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
     if int(disp_max) < 1:
         raise ValueError("disp_max must be at least 1, got %r" % (disp_max,))
+    if density is not None:
+        if action != "submit":
+            raise ValueError("density applies to the maps submit writes; %s writes none" % action)
+        confidence.check_density(density)
     files = pair_files(data_root, dataset, action)
     shapes = scan(files)
     distributed = dist.is_initialized() and dist.get_world_size() > 1
@@ -205,9 +212,16 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
     def compute(i):
         left, right, gt = pre.get(i)
         x_batch = frontend.make_batch_cuda(left, right, ev.dev)
-        pred = ev.stereo_predict(x_batch, disp_max)
+        if density is None:
+            pred = ev.stereo_predict(x_batch, disp_max)
+        else:
+            conf = torch.empty(x_batch.shape[2:], device=ev.dev)
+            pred = ev.stereo_predict(x_batch, disp_max, conf=conf)
         if action == "test":
             return error_counts(pred, gt).cpu()
+        if density is not None:
+            with torch.cuda.device(ev.dev):
+                pred = confidence.sparsify(pred, conf, density, 0.0)
         H, W = shapes[i]
         f = dataio.write_kitti_submission(pred.cpu().numpy(), H, W, out, i, dataset)
         assert f == submission_file(i)

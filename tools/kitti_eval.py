@@ -32,6 +32,8 @@ def parser():
     p.add_argument("-disp_max", type=int, default=228)
     p.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
     p.add_argument("-out", default=None, help="also write the maps here, in submission layout")
+    p.add_argument("-density", type=float, default=None,
+                   help="keep this share of each map's pixels, the most confident ones, in (0, 1]")
     s = sub.add_parser("score", help="score PNG16 maps in submission layout")
     s.add_argument("dataset", choices=("kitti", "kitti2015"))
     s.add_argument("pred_dir")
@@ -50,6 +52,8 @@ def parse_args(argv=None):
             raise SystemExit("kitti_eval.py: arch '%s' needs -net_fname" % args.arch)
         if args.disp_max < 1:
             raise SystemExit("kitti_eval.py: -disp_max must be at least 1")
+        if args.density is not None and not 0 < args.density <= 1:
+            raise SystemExit("kitti_eval.py: -density must be in (0, 1]")
     elif not os.path.isdir(args.pred_dir):
         raise SystemExit("kitti_eval.py: %s is not a directory" % args.pred_dir)
     return args
@@ -71,7 +75,7 @@ def main(argv=None):
     try:
         if args.action == "predict":
             kitti_eval.evaluate_training(args.dataset, args.net_fname or None, args.arch, data_root=args.data_root,
-                                         disp_max=args.disp_max, out=args.out, device=device)
+                                         disp_max=args.disp_max, out=args.out, device=device, density=args.density)
         else:
             kitti_eval.score_dir(args.dataset, args.pred_dir, data_root=args.data_root, device=device)
     finally:

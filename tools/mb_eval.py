@@ -31,6 +31,8 @@ def parser():
     p.add_argument("-res", choices=("F", "H"), default="F")
     p.add_argument("-out", default=None, help="also write the maps here, in -a submit's layout")
     p.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    p.add_argument("-density", type=float, default=None,
+                   help="keep this share of each map's pixels, the most confident ones, +inf elsewhere; in (0, 1]")
     s = sub.add_parser("score", help="score the maps of a directory in -a submit's layout")
     s.add_argument("out")
     s.add_argument("-data_root", default=".")
@@ -48,6 +50,8 @@ def parse_args(argv=None):
     if args.action == "predict":
         if args.arch in ("fast", "slow") and not args.net_fname:
             raise SystemExit("mb_eval.py: arch '%s' needs -net_fname" % args.arch)
+        if args.density is not None and not 0 < args.density <= 1:
+            raise SystemExit("mb_eval.py: -density must be in (0, 1]")
     elif not os.path.isdir(args.out):
         raise SystemExit("mb_eval.py: %s is not a directory" % args.out)
     return args
@@ -60,7 +64,7 @@ def main(argv=None):
 
     if args.action == "predict":
         mb_eval.evaluate_training(args.arch, args.net_fname or None, data_root=args.data_root, res=args.res, out=args.out,
-                                  device=args.gpu - 1)
+                                  device=args.gpu - 1, density=args.density)
     else:
         mb_eval.score_dir(args.out, data_root=args.data_root, res=args.res, alg=args.alg, device=args.gpu - 1)
     return 0

@@ -9,7 +9,9 @@
 ``out/%06d_10.png`` (kitti) or ``out/disp_0/%06d_10.png`` (kitti2015) for every testing pair and prints its index.  The raw
 archives are read from ``<data_root>/data.kitti/unzip`` or ``data.kitti2015/unzip``, as preprocess_kitti.py reads them.
 -gpu is 1-based as in main.lua.  Under torchrun each process takes the GPU of its LOCAL_RANK and the pairs are shared
-round-robin; the output is the one a single process prints.  See mc-cnn_b200/predict_kitti.py.
+round-robin; the output is the one a single process prints.  `submit -density p` (an addition beyond the reference) keeps
+the ceil(p H W) pixels of largest margin confidence in each map and writes 0, the invalid value, elsewhere.  See
+mc-cnn_b200/predict_kitti.py.
 """
 import argparse
 import os
@@ -28,6 +30,7 @@ def parser():
     ap.add_argument("-out", default="out")
     ap.add_argument("-disp_max", type=int, default=228)
     ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    ap.add_argument("-density", type=float, default=None, help="submit: keep this share of each map's pixels, in (0, 1]")
     return ap
 
 
@@ -40,6 +43,11 @@ def parse_args(argv=None):
         raise SystemExit("predict_kitti.py: -disp_max must be at least 1")
     if args.gpu < 1:
         raise SystemExit("predict_kitti.py: -gpu is 1-based")
+    if args.density is not None:
+        if args.action != "submit":
+            raise SystemExit("predict_kitti.py: -density applies to the maps submit writes; test writes none")
+        if not 0 < args.density <= 1:
+            raise SystemExit("predict_kitti.py: -density must be in (0, 1]")
     return args
 
 
@@ -58,7 +66,7 @@ def main(argv=None):
         device = int(os.environ.get("LOCAL_RANK", "0"))
     try:
         predict_kitti(args.action, args.dataset, net_fname=args.net_fname or None, arch=args.arch, data_root=args.data_root,
-                      out=args.out, disp_max=args.disp_max, device=device)
+                      out=args.out, disp_max=args.disp_max, device=device, density=args.density)
     finally:
         if world > 1:
             dist.destroy_process_group()

@@ -6,11 +6,13 @@
     python tools/run_main.py kitti fast -a time -net_fname N [-tiny]
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70
     python tools/run_main.py kitti fast -a test_te -net_fname N -sm_skip sgm          # or -sm_terminate cbca1, ...
+    python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -confidence
 
 Option names are main.lua's (-gpu is 1-based as there); -L1 ... -blur_t override the stereo method's preset
 (main.lua:70-295); -sm_terminate / -sm_skip stop after / leave out one step of it (main.lua:953-1082; unknown step
 names, and steps that do no work with these parameters, are refused).  Datasets are read relative to -data_root (default: the working directory), as main.lua reads them
-relative to its own.  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
+relative to its own.  -confidence (an addition beyond the reference, -a predict only) also writes conf.bin, the margin
+confidence of each pixel, and with the LR check lr.bin, main.lua:1056's outlier map (mc-cnn_b200/confidence.py).  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
 what each action computes and where it deliberately differs from main.lua.
 """
 import argparse
@@ -49,6 +51,7 @@ def parser():
         ap.add_argument("-" + name, nargs="?", const=True, default=False, type=_flag)
     ap.add_argument("-sm_terminate", default="")
     ap.add_argument("-sm_skip", default="")
+    ap.add_argument("-confidence", nargs="?", const=True, default=False, type=_flag)
     for name, typ in PRESET_OPTIONS.items():
         ap.add_argument("-" + name, type=typ, default=None)
     return ap
@@ -65,6 +68,8 @@ def parse_args(argv=None):
         raise SystemExit("run_main.py: unknown action -a %s (%s)" % (args.a, ", ".join(ACTIONS)))
     if args.gpu < 1:
         raise SystemExit("run_main.py: -gpu is 1-based")
+    if args.confidence and args.a != "predict":
+        raise SystemExit("run_main.py: -confidence writes conf.bin next to -a predict's outputs; -a %s writes none" % args.a)
     evaluate.check_options(args.dataset, at=args.at, color=args.color, debug=args.debug, use_cache=args.use_cache,
                            make_cache=args.make_cache)
     overrides = {k: getattr(args, k) for k in PRESET_OPTIONS if getattr(args, k) is not None}
@@ -85,7 +90,8 @@ def main(argv=None):
         if not (args.left and args.right and args.disp_max):
             raise SystemExit("run_main.py: -a predict needs -left, -right and -disp_max")
         frontend.predict(args.left, args.right, dataset=args.dataset, arch=args.arch, disp_max=args.disp_max,
-                         out_dir=".", device=args.device, net_fname=args.net_fname or None, **overrides)
+                         out_dir=".", device=args.device, net_fname=args.net_fname or None, confidence=args.confidence,
+                         **overrides)
         return 0
     ev = evaluate.Evaluator(args.dataset, args.arch, net_fname=args.net_fname or None, device=args.device, **overrides)
     try:
