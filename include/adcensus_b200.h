@@ -731,6 +731,43 @@ int mccnn_mb_evaldisp(const float *disp, int h, int w, const float *gt, int Hg, 
 		      int maxdisp, long long *counts, double *sums, float *quantiles, void *scratch,
 		      adcensus_stream_t stream);
 
+/* ---- metric depth, point clouds and depth metrics (csrc/depth.cu, depth.py; DESIGN §20) ---------------------------------
+ * An addition beyond the reference.  A disparity d (H,W) at pixel (x, y) is valid when it is finite and s = d + doffs > 0
+ * (fp32 add); then, each operation rounded once in fp32 and in this order, Z = fB / s, X = ((x - cx) * Z) / f,
+ * Y = ((y - cy) * Z) / f, where fB is f * baseline computed in double and rounded once to float by the caller.  max_depth
+ * (> 0; +inf for none) also makes Z > max_depth invalid.  Every entry checks, before any launch: H, W >= 1, f > 0, fB > 0,
+ * finite f, fB, cx, cy, doffs, max_depth > 0 (else ADCENSUS_EINVAL); H * W < 2^31 (else ADCENSUS_ELIMIT).  DEVICE pointers;
+ * asynchronous on `stream`.
+ *
+ * mccnn_disp_to_depth: Z (H,W), and X, Y (H,W) unless both are NULL; NaN at invalid pixels. */
+int mccnn_disp_to_depth(const float *disp, int H, int W, float f, float cx, float cy, float fB, float doffs, float max_depth,
+			float *Z, float *X, float *Y, adcensus_stream_t stream);
+/* mccnn_point_cloud_count: the number of valid pixels, to count (one DEVICE int64).
+ * mccnn_point_cloud_fill: one binary little-endian PLY vertex record per valid pixel, in row-major order, packed 15 bytes
+ * apiece (float x, y, z; uchar red, green, blue) into out (16-byte aligned, at least 15 cap bytes); records past cap are
+ * dropped.  The colour is rgb (H,W,3) R, G, B bytes (nch 3) or (H,W) grey bytes repeated three times (nch 1).  The order is
+ * fixed (per-block counts, an exclusive 64-bit scan over the blocks, then the fill): the same bytes on every run. */
+int mccnn_point_cloud_count(const float *disp, int H, int W, float fB, float doffs, float max_depth, long long *count,
+			    adcensus_stream_t stream);
+int mccnn_point_cloud_fill(const float *disp, const unsigned char *rgb, int nch, int H, int W, float f, float cx, float cy, float fB,
+			   float doffs, float max_depth, unsigned char *out, long long cap, adcensus_stream_t stream);
+/* The depth metrics of pred against the ground-truth disparity gt (H,W), both turned into depth by the rule above without
+ * the cap; with pred_depth != 0, pred already holds depths in metres, valid where finite and > 0 (a depth map read back).  S = the pixels whose gt depth Zg is valid and lies in [min_depth, max_depth] (fp32 compares; 0 < min_depth <=
+ * max_depth, else ADCENSUS_EINVAL).  Over S and a valid predicted depth Z, clamped to [min_depth, max_depth] in fp32, in
+ * float64: sums[0] = sum |Z - Zg| / Zg, sums[1] = sum (Z - Zg)^2 / Zg, sums[2] = sum (Z - Zg)^2, sums[3] = sum (log Z -
+ * log Zg)^2, each block summing a fixed range in a fixed order and one block adding the block sums in a fixed order (the
+ * same bits on every run and GPU); counts (int64) as below, with r = max(Z / Zg, Zg / Z) in double. */
+enum {
+	MCCNN_DEPTH_GT,          /* |S| */
+	MCCNN_DEPTH_N,           /* |S and a valid prediction| */
+	MCCNN_DEPTH_A1,          /* ... with r < 1.25 */
+	MCCNN_DEPTH_A2,          /* r < 1.25^2 */
+	MCCNN_DEPTH_A3,          /* r < 1.25^3 */
+	MCCNN_DEPTH_NCOUNT
+};
+int mccnn_depth_metrics(const float *pred, int pred_depth, const float *gt, int H, int W, float fB, float doffs, float min_depth,
+			float max_depth, long long *counts, double *sums, adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,11 +10,15 @@ write and `main.lua` reads back, the error metric of `-a test_te`, and the submi
 * ``bad_pixel_rate``: share of ground-truth pixels whose error exceeds ``err_at`` (3 px KITTI,
   1 px Middlebury; main.lua:400, 453, 1228-1236);
 * ``kitti_submission_image``: the prediction pasted into the bottom rows of the full-size frame
-  (main.lua:1203-1205).
+  (main.lua:1203-1205);
+* ``read_calib`` / ``write_depth_png16``: the KITTI 2012, KITTI 2015 and MiddEval3 calibration files, and KITTI's depth
+  map format (DESIGN §20, an addition beyond the reference).
 
 Plain numpy / PIL host code: nothing here touches the GPU.
 """
 import os
+import re
+from collections import namedtuple
 
 import numpy as np
 
@@ -135,3 +139,95 @@ def write_kitti_submission(pred, img_height, img_width, out_dir, idx, dataset="k
     fname = os.path.join(path, "%06d_10.png" % idx)
     write_png16(kitti_submission_image(pred, img_height, img_width), fname)
     return fname
+
+
+# ---- calibration and depth maps (DESIGN §20) ------------------------------------------------------------------------------
+
+Calib = namedtuple("Calib", "f cx cy baseline doffs width height")
+Calib.__doc__ = """A rectified stereo pair's camera: focal length f and principal point (cx, cy) in pixels, baseline in metres,
+doffs (the x-difference of the two principal points) in pixels, and the image size the file states (None when it states
+none)."""
+
+CALIB_KINDS = ("kitti", "kitti2015", "mb")
+# the two projection matrices of each KITTI calibration file: the grey pair (2012) and the colour pair (2015)
+_KITTI_P = {"kitti": ("P0", "P1"), "kitti2015": ("P_rect_02", "P_rect_03")}
+
+
+def _calib_entries(path):
+    """{key: value text} of a calibration file's ``key: value`` (KITTI) or ``key=value`` (Middlebury) lines"""
+    out = {}
+    with open(path) as f:
+        for line in f:
+            m = re.match(r"\s*([A-Za-z_][A-Za-z0-9_]*)\s*[:=]\s*(.*?)\s*$", line)
+            if m:
+                out[m.group(1)] = m.group(2)
+    return out
+
+
+def _numbers(path, entries, key, n):
+    """the n numbers of `key`, refused when the key is missing or does not hold exactly n numbers"""
+    if key not in entries:
+        raise ValueError("%s: missing key %s" % (path, key))
+    try:
+        v = [float(t) for t in entries[key].replace("[", " ").replace("]", " ").replace(";", " ").split()]
+    except ValueError:
+        v = []
+    if len(v) != n or not all(np.isfinite(v)):
+        raise ValueError("%s: %s must hold %d finite numbers, got %r" % (path, key, n, entries[key]))
+    return v
+
+
+def read_calib(path, kind):
+    """The :data:`Calib` of a calibration file (DESIGN §20).  kind 'kitti': KITTI 2012's ``calib/%06d.txt``, the grey
+    pair P0 / P1; 'kitti2015': ``calib_cam_to_cam/%06d.txt``, the colour pair P_rect_02 / P_rect_03 and the size S_rect_02
+    when present; 'mb': a MiddEval3 scene's ``calib.txt`` (cam0, doffs, baseline in millimetres, width, height).  KITTI:
+    f = P[0,0], cx = P[0,2], cy = P[1,2] of the left matrix, baseline = (P_left[0,3] - P_right[0,3]) / f, doffs = 0.
+    Refuses a missing key, a malformed matrix, f <= 0 and baseline <= 0, naming the file and the key."""
+    if kind not in CALIB_KINDS:
+        raise ValueError("calibration kind must be one of %s, got %r" % (", ".join(CALIB_KINDS), kind))
+    e = _calib_entries(path)
+    width = height = None
+    if kind == "mb":
+        cam0 = _numbers(path, e, "cam0", 9)
+        f, cx, cy = cam0[0], cam0[2], cam0[5]
+        baseline = _numbers(path, e, "baseline", 1)[0] / 1000.0
+        doffs = _numbers(path, e, "doffs", 1)[0]
+        width, height = (int(_numbers(path, e, k, 1)[0]) for k in ("width", "height"))
+        fkey, bkey = "cam0", "baseline"
+    else:
+        kl, kr = _KITTI_P[kind]
+        pl, pr = _numbers(path, e, kl, 12), _numbers(path, e, kr, 12)
+        f, cx, cy = pl[0], pl[2], pl[6]
+        baseline = (pl[3] - pr[3]) / f if f > 0 else 0.0
+        doffs = 0.0
+        if kind == "kitti2015" and "S_rect_02" in e:
+            width, height = (int(v) for v in _numbers(path, e, "S_rect_02", 2))
+        fkey, bkey = kl, "%s / %s" % (kl, kr)
+    if not f > 0:
+        raise ValueError("%s: %s gives f = %g, must be > 0" % (path, fkey, f))
+    if not baseline > 0:
+        raise ValueError("%s: %s gives baseline = %g m, must be > 0" % (path, bkey, baseline))
+    return Calib(f, cx, cy, baseline, doffs, width, height)
+
+
+def check_calib_size(cal, H, W, path):
+    """refuses a calibration whose stated image size is not (H, W): nothing is rescaled"""
+    if cal.width is not None and (cal.width, cal.height) != (W, H):
+        raise ValueError("%s: calibration for %dx%d images, the image is %dx%d" % (path, cal.width, cal.height, W, H))
+
+
+def write_depth_png16(Z, fname):
+    """KITTI's depth map format: uint16 = round(Z * 256) (Z in metres, float64 product), 0 where Z has no depth (NaN) or
+    rounds to 0; values past the uint16 range are clamped"""
+    from PIL import Image
+
+    Z = np.asarray(Z, dtype=np.float32)
+    assert Z.ndim == 2
+    v = np.rint(np.nan_to_num(Z.astype(np.float64) * 256.0, nan=0.0, posinf=65535.0, neginf=0.0))
+    Image.fromarray(np.clip(v, 0, 65535).astype(np.uint16)).save(fname, format="PNG")
+
+
+def read_depth_png16(fname):
+    """:func:`write_depth_png16`'s inverse: float32 (H, W) metres, NaN where the file holds 0"""
+    v = read_png16_raw(fname)
+    return np.where(v == 0, np.float32(np.nan), v.astype(np.float32) / np.float32(256.0)).astype(np.float32)

@@ -19,7 +19,8 @@ import os
 
 import numpy as np
 
-from . import pipeline
+from . import confidence as confidence_
+from . import dataio, depth, pipeline
 
 
 def load_bytes(path):
@@ -192,7 +193,7 @@ class StereoMethod:
 
 
 def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=None, out_dir=None, device=0,
-            net_fname=None, confidence=False, **overrides):
+            net_fname=None, confidence=False, calib=None, ply=False, max_depth=None, density=None, **overrides):
     """``main.lua <dataset> <arch> -a predict -net_fname N -left L -right R -disp_max D`` from the image files on:
     returns disp (H,W) float32 (numpy).  With `out_dir`, writes right.bin and left.bin ((1,D,H,W), in
     that order, main.lua:1042-1047) and disp.bin ((1,1,H,W), :1103) there.  arch 'fast' / 'slow' take the trained
@@ -200,9 +201,22 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     (feature tower, and for 'slow' the scorer head); arch 'fast' alternatively accepts `features` (2,C,H,W), the
     unit-norm tower output; 'ad' / 'census' need neither.  With `confidence` (an addition beyond the reference), also writes
     conf.bin, the margin confidence of the left volume (mc-cnn_b200/confidence.py), and for presets with the LR check lr.bin,
-    main.lua:1056's outlier map, both (1,1,H,W) float32, each announced by a ``Writing`` line in main.lua's format."""
+    main.lua:1056's outlier map, both (1,1,H,W) float32, each announced by a ``Writing`` line in main.lua's format.
+
+    With `calib`, a :data:`dataio.Calib` of the pair (an addition beyond the reference, DESIGN §20), also writes depth.bin,
+    the metric depth of disp ((1,1,H,W) float32, NaN = no depth, Z > `max_depth` dropped), and with `ply` points.ply, the
+    point cloud coloured from the left image's bytes.  `density` (with `confidence`) keeps in both only the pixels
+    confidence.sparsify keeps."""
     import torch
 
+    if (ply or max_depth is not None or density is not None) and calib is None:
+        raise ValueError("ply, max_depth and density apply to the depth outputs, which need calib")
+    if density is not None and not confidence:
+        raise ValueError("density ranks pixels by their confidence: it needs confidence")
+    colour = None
+    if calib is not None:
+        colour = load_bytes(left) if isinstance(left, (str, os.PathLike)) else np.asarray(left)
+        dataio.check_calib_size(calib, colour.shape[0], colour.shape[1], "calib")
     method = StereoMethod(dataset, arch, None if features is not None else net_fname, **overrides)   # before any GPU work
     if method.needs_net and features is None:
         raise ValueError("arch '%s' needs -net_fname (or, for 'fast', the tower output in `features`)" % arch)
@@ -225,6 +239,12 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
             lr = torch.empty((H, W), device=dev) if confidence and method.opt.lr_check else None
             disp, volL, volR = pipeline.stereo_predict(x_batch, feats, method.opt, int(disp_max), want_vols=True, arch=arch,
                                                        head=head, conf=conf, lr=lr)
+            Z = pts = None
+            if calib is not None:
+                dmap = disp.reshape(H, W) if density is None else confidence_.sparsify(disp.reshape(H, W), conf, density)
+                Z = depth.depth(dmap, calib, max_depth)
+                if ply:
+                    pts = depth.point_cloud(dmap, calib, colour, max_depth=max_depth)
         disp_h = disp.cpu().numpy()
     finally:
         method.close()
@@ -237,4 +257,10 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
             if t is not None:
                 print("Writing %s.bin, 1 x 1 x %d x %d" % (name, H, W), flush=True)
                 write_bin(os.path.join(out_dir, name + ".bin"), t.cpu().numpy())
+        if Z is not None:
+            print("Writing depth.bin, 1 x 1 x %d x %d" % (H, W), flush=True)
+            write_bin(os.path.join(out_dir, "depth.bin"), Z.cpu().numpy())
+        if pts is not None:
+            print("Writing points.ply, %d points" % pts.n, flush=True)
+            depth.write_ply(os.path.join(out_dir, "points.ply"), pts)
     return disp_h[0, 0]

@@ -28,6 +28,12 @@ directory (as Evaluator.submit does) and also writes 2015 maps, under ``out/disp
 
 An addition beyond the reference: ``submit`` with `density` p in (0, 1] writes sparse maps, the ceil(p H W) pixels of
 largest margin confidence and 0 (the PNG16 invalid value) elsewhere (:func:`confidence.sparsify`).
+
+Another addition: with `depth`, either action also writes each pair's metric depth as ``out/depth_0/%06d_10.png`` (KITTI's
+depth format, dataio.write_depth_png16: round(Z * 256), 0 = none), and with `ply` its coloured point cloud as
+``out/points_0/%06d_10.ply`` (:mod:`depth`), both from the map submit writes (the sparse one under `density`).  The
+calibration is read from beside the images: ``calib/%06d.txt`` (2012, in the data archive) or ``calib_cam_to_cam/%06d.txt``
+(2015, from the calibration archive data_scene_flow_calib.zip unpacked into the same ``unzip/`` directory).
 """
 import concurrent.futures
 import os
@@ -36,6 +42,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import batch, confidence, dataio, evaluate, frontend, preprocess
+from . import depth as depth_
 
 ACTIONS = ("test", "submit")
 DISP_MAX = 228                          # predict_kitti.lua:37
@@ -110,6 +117,43 @@ class Prefetch:
             self.pool.shutdown(wait=True)
 
 
+CALIB_DIR = {"kitti": "calib", "kitti2015": "calib_cam_to_cam"}
+
+
+def calib_file(left, dataset):
+    """the calibration file of the pair whose left image is `left` (``<sub>/image_*/%06d_10.png``)"""
+    sub = os.path.dirname(os.path.dirname(left))
+    return os.path.join(sub, CALIB_DIR[dataset], os.path.basename(left)[:6] + ".txt")
+
+
+def read_calibs(files, shapes, dataset):
+    """the :data:`dataio.Calib` of every pair, refused (naming the file) when missing, malformed or of another size"""
+    out = []
+    for (left, _, _), (H, W) in zip(files, shapes):
+        path = calib_file(left, dataset)
+        if not os.path.isfile(path):
+            raise FileNotFoundError("missing calibration file %s" % path)
+        cal = dataio.read_calib(path, dataset)
+        dataio.check_calib_size(cal, H, W, path)
+        out.append(cal)
+    return out
+
+
+def depth_files(out, i):
+    """(depth PNG, point cloud) of pair i"""
+    return (os.path.join(out, "depth_0", "%06d_10.png" % i), os.path.join(out, "points_0", "%06d_10.ply" % i))
+
+
+def write_depth(pred, left, cal, out, i, ply):
+    """pair i's depth PNG, and with `ply` its point cloud, from the device map `pred`"""
+    fz, fp = depth_files(out, i)
+    os.makedirs(os.path.dirname(fz), exist_ok=True)
+    dataio.write_depth_png16(depth_.depth(pred, cal).cpu().numpy(), fz)
+    if ply:
+        os.makedirs(os.path.dirname(fp), exist_ok=True)
+        depth_.write_ply(fp, depth_.point_cloud(pred, cal, left))
+
+
 def error_counts(disp, gt16, err_at=ERR_AT):
     """(bad, valid) pixel counts of one device map against its PNG16 ground truth (mccnn_kitti_error_count): disp (H, W) CUDA
     float32, gt16 (H, W) uint16 values (numpy, or an int16 / uint16 torch tensor).  Returns a (2,) int64 CUDA tensor."""
@@ -178,10 +222,11 @@ def check_out(out):
 
 
 def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", out="out", disp_max=DISP_MAX, device=0,
-                  prefetch=True, verbose=True, density=None, **overrides):
+                  prefetch=True, verbose=True, density=None, depth=False, ply=False, **overrides):
     """predict_kitti.lua's `test` or `submit` on the raw `dataset` ('kitti' or 'kitti2015') under `data_root` on CUDA device
     `device`; `overrides` change the stereo method's preset as in Evaluator.  Returns, on rank 0, the TestResult (errors per
-    training pair, mean) or the list of written files; None on other ranks.  `prefetch` False decodes each pair in turn."""
+    training pair, mean) or the list of written files; None on other ranks.  `prefetch` False decodes each pair in turn.
+    `depth` / `ply` also write the depth maps / point clouds (module docstring)."""
     import torch
     import torch.distributed as dist
 
@@ -195,10 +240,13 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
         if action != "submit":
             raise ValueError("density applies to the maps submit writes; %s writes none" % action)
         confidence.check_density(density)
+    if ply and not depth:
+        raise ValueError("ply writes the point clouds of the depth maps: it needs depth")
     files = pair_files(data_root, dataset, action)
     shapes = scan(files)
+    calibs = read_calibs(files, shapes, dataset) if depth else None
     distributed = dist.is_initialized() and dist.get_world_size() > 1
-    if action == "submit":
+    if action == "submit" or depth:
         check_out(out)
         if distributed:
             dist.barrier()                      # every rank has looked at `out` before any rank writes to it
@@ -218,10 +266,16 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
             conf = torch.empty(x_batch.shape[2:], device=ev.dev)
             pred = ev.stereo_predict(x_batch, disp_max, conf=conf)
         if action == "test":
+            if depth:
+                with torch.cuda.device(ev.dev):
+                    write_depth(pred, left, calibs[i], out, i, ply)
             return error_counts(pred, gt).cpu()
         if density is not None:
             with torch.cuda.device(ev.dev):
                 pred = confidence.sparsify(pred, conf, density, 0.0)
+        if depth:
+            with torch.cuda.device(ev.dev):
+                write_depth(pred, left, calibs[i], out, i, ply)
         H, W = shapes[i]
         f = dataio.write_kitti_submission(pred.cpu().numpy(), H, W, out, i, dataset)
         assert f == submission_file(i)

@@ -10,7 +10,9 @@
 archives are read from ``<data_root>/data.kitti/unzip`` or ``data.kitti2015/unzip``, as preprocess_kitti.py reads them.
 -gpu is 1-based as in main.lua.  Under torchrun each process takes the GPU of its LOCAL_RANK and the pairs are shared
 round-robin; the output is the one a single process prints.  `submit -density p` (an addition beyond the reference) keeps
-the ceil(p H W) pixels of largest margin confidence in each map and writes 0, the invalid value, elsewhere.  See
+the ceil(p H W) pixels of largest margin confidence in each map and writes 0, the invalid value, elsewhere.  `-depth`
+(also an addition) writes each pair's metric depth as ``out/depth_0/%06d_10.png`` (KITTI's depth format), and with `-ply`
+its coloured point cloud as ``out/points_0/%06d_10.ply``, from the calibration files beside the images.  See
 mc-cnn_b200/predict_kitti.py.
 """
 import argparse
@@ -31,6 +33,8 @@ def parser():
     ap.add_argument("-disp_max", type=int, default=228)
     ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
     ap.add_argument("-density", type=float, default=None, help="submit: keep this share of each map's pixels, in (0, 1]")
+    ap.add_argument("-depth", action="store_true", help="also write out/depth_0/%%06d_10.png, the metric depth")
+    ap.add_argument("-ply", action="store_true", help="with -depth: also write out/points_0/%%06d_10.ply")
     return ap
 
 
@@ -48,6 +52,8 @@ def parse_args(argv=None):
             raise SystemExit("predict_kitti.py: -density applies to the maps submit writes; test writes none")
         if not 0 < args.density <= 1:
             raise SystemExit("predict_kitti.py: -density must be in (0, 1]")
+    if args.ply and not args.depth:
+        raise SystemExit("predict_kitti.py: -ply writes the point clouds of the depth maps; it needs -depth")
     return args
 
 
@@ -66,7 +72,8 @@ def main(argv=None):
         device = int(os.environ.get("LOCAL_RANK", "0"))
     try:
         predict_kitti(args.action, args.dataset, net_fname=args.net_fname or None, arch=args.arch, data_root=args.data_root,
-                      out=args.out, disp_max=args.disp_max, device=device, density=args.density)
+                      out=args.out, disp_max=args.disp_max, device=device, density=args.density, depth=args.depth,
+                      ply=args.ply)
     finally:
         if world > 1:
             dist.destroy_process_group()

@@ -7,12 +7,17 @@
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70
     python tools/run_main.py kitti fast -a test_te -net_fname N -sm_skip sgm          # or -sm_terminate cbca1, ...
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -confidence
+    python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -calib calib/000000.txt -ply
 
 Option names are main.lua's (-gpu is 1-based as there); -L1 ... -blur_t override the stereo method's preset
 (main.lua:70-295); -sm_terminate / -sm_skip stop after / leave out one step of it (main.lua:953-1082; unknown step
 names, and steps that do no work with these parameters, are refused).  Datasets are read relative to -data_root (default: the working directory), as main.lua reads them
 relative to its own.  -confidence (an addition beyond the reference, -a predict only) also writes conf.bin, the margin
-confidence of each pixel, and with the LR check lr.bin, main.lua:1056's outlier map (mc-cnn_b200/confidence.py).  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
+confidence of each pixel, and with the LR check lr.bin, main.lua:1056's outlier map (mc-cnn_b200/confidence.py).
+-calib FILE (also an addition, -a predict only; KITTI 2012 calib/%06d.txt, KITTI 2015 calib_cam_to_cam/%06d.txt or a
+MiddEval3 calib.txt, by dataset) also writes depth.bin, the metric depth of each pixel in metres (NaN = none), and with -ply
+points.ply, the coloured point cloud; -max_depth M drops depths past M metres, and -density p (with -confidence) keeps only
+the ceil(p H W) most confident pixels in both (mc-cnn_b200/depth.py).  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
 what each action computes and where it deliberately differs from main.lua.
 """
 import argparse
@@ -52,6 +57,10 @@ def parser():
     ap.add_argument("-sm_terminate", default="")
     ap.add_argument("-sm_skip", default="")
     ap.add_argument("-confidence", nargs="?", const=True, default=False, type=_flag)
+    ap.add_argument("-calib", default="")
+    ap.add_argument("-ply", nargs="?", const=True, default=False, type=_flag)
+    ap.add_argument("-max_depth", type=float, default=None)
+    ap.add_argument("-density", type=float, default=None)
     for name, typ in PRESET_OPTIONS.items():
         ap.add_argument("-" + name, type=typ, default=None)
     return ap
@@ -70,6 +79,17 @@ def parse_args(argv=None):
         raise SystemExit("run_main.py: -gpu is 1-based")
     if args.confidence and args.a != "predict":
         raise SystemExit("run_main.py: -confidence writes conf.bin next to -a predict's outputs; -a %s writes none" % args.a)
+    if args.calib and args.a != "predict":
+        raise SystemExit("run_main.py: -calib writes depth.bin next to -a predict's outputs; -a %s writes none" % args.a)
+    if (args.ply or args.max_depth is not None or args.density is not None) and not args.calib:
+        raise SystemExit("run_main.py: -ply, -max_depth and -density apply to the depth outputs, which need -calib")
+    if args.max_depth is not None and not args.max_depth > 0:
+        raise SystemExit("run_main.py: -max_depth must be > 0")
+    if args.density is not None:
+        if not args.confidence:
+            raise SystemExit("run_main.py: -density keeps the most confident pixels; it needs -confidence")
+        if not 0 < args.density <= 1:
+            raise SystemExit("run_main.py: -density must be in (0, 1]")
     evaluate.check_options(args.dataset, at=args.at, color=args.color, debug=args.debug, use_cache=args.use_cache,
                            make_cache=args.make_cache)
     overrides = {k: getattr(args, k) for k in PRESET_OPTIONS if getattr(args, k) is not None}
@@ -84,14 +104,18 @@ def parse_args(argv=None):
 def main(argv=None):
     args, overrides = parse_args(argv)
     import mccnn_b200  # noqa: F401
-    from mccnn_b200 import evaluate, frontend
+    from mccnn_b200 import dataio, evaluate, frontend
 
     if args.a == "predict":
         if not (args.left and args.right and args.disp_max):
             raise SystemExit("run_main.py: -a predict needs -left, -right and -disp_max")
+        depth_opts = {}
+        if args.calib:
+            depth_opts = dict(calib=dataio.read_calib(args.calib, args.dataset), ply=args.ply, max_depth=args.max_depth,
+                              density=args.density)
         frontend.predict(args.left, args.right, dataset=args.dataset, arch=args.arch, disp_max=args.disp_max,
                          out_dir=".", device=args.device, net_fname=args.net_fname or None, confidence=args.confidence,
-                         **overrides)
+                         **depth_opts, **overrides)
         return 0
     ev = evaluate.Evaluator(args.dataset, args.arch, net_fname=args.net_fname or None, device=args.device, **overrides)
     try:
