@@ -768,6 +768,18 @@ enum {
 int mccnn_depth_metrics(const float *pred, int pred_depth, const float *gt, int H, int W, float fB, float doffs, float min_depth,
 			float max_depth, long long *counts, double *sums, adcensus_stream_t stream);
 
+/* ---- LiDAR scans projected into sparse depth maps (csrc/depth.cu, depth.py; DESIGN §21) ---------------------------------
+ * An addition beyond the reference.  mccnn_velo_depth_map: pts (n, 4) float32 x, y, z, reflectance (DEVICE, 16-byte
+ * aligned), P the 3x4 row-major velodyne-to-image matrix (12 HOST floats, read during the call), depth (H,W) float32
+ * (DEVICE).  Each point, in fp32 with every operation rounded once: x' = ((P00 x + P01 y) + P02 z) + P03, likewise y' and z'
+ * from rows 1 and 2; kept when min_depth < z' < +inf; its pixel u = rint(x' / z') - 1, v = rint(y' / z') - 1 (rint: to
+ * nearest, ties to even), kept inside [0, W) x [0, H).  Each pixel gets the smallest z' of its points (the smallest index
+ * breaks a tie) and 0 when it has none: the same bits on every run and GPU.  Refuses a NULL or unaligned pointer, n < 0,
+ * H or W < 1, min_depth < 0 or not finite, a non-finite P entry (ADCENSUS_EINVAL); H * W >= 2^31 or n >= 2^32
+ * (ADCENSUS_ELIMIT).  pts may be NULL when n == 0.  Asynchronous on `stream`. */
+int mccnn_velo_depth_map(const float *pts, long long n, const float *P, int H, int W, float min_depth, float *depth,
+			 adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

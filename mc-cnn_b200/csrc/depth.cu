@@ -13,6 +13,10 @@
 //   16-byte words; only the partial first and last words are written bytewise, so every global byte has one writer.
 // * mccnn_depth_metrics: per pixel (the prediction a disparity or already a depth) the integer counts and four float64 terms; each block sums a fixed range of CHUNK pixels
 //   in a fixed order, one block adds the block sums in a fixed order: no float atomics, the same bits on every GPU.
+// * mccnn_velo_depth_map (DESIGN §21): a LiDAR scan projected into an (H, W) depth map.  The keys are cleared to all ones,
+//   each kept point atomicMin-s the 64-bit key (float bits of its z, its index) of its pixel, and one pass decodes the
+//   keys.  z > 0, so its bits order like its value: the smallest z wins, the smallest index breaks a tie, and the result
+//   does not depend on the order of the atomics.
 #include <math.h>
 
 #include <algorithm>
@@ -276,6 +280,44 @@ __global__ void __launch_bounds__(THREADS) metrics_finish_kernel(const double *_
 	if (tid < NSUM) sums[tid] = sh[tid][0];
 }
 
+// ---- LiDAR scans projected into a sparse depth map (DESIGN §21) ----
+
+constexpr unsigned long long NO_POINT = ~0ull;   // every key's high word is a finite float's bits, never all ones
+
+struct Proj {
+	float p[12];                                   // row-major 3x4
+};
+
+// r . (x, y, z, 1) in fp32, each operation rounded once, left to right
+__device__ __forceinline__ float proj_row(const float *r, float x, float y, float z)
+{
+	return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r[0], x), __fmul_rn(r[1], y)), __fmul_rn(r[2], z)), r[3]);
+}
+
+// each point's key (z bits << 32 | index) min-ed into the key of its pixel
+__global__ void velo_key_kernel(const float4 *__restrict__ pts, long long n, Proj P, int H, int W, float min_depth,
+				unsigned long long *__restrict__ key)
+{
+	for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+		const float4 q = pts[i];
+		const float z = proj_row(P.p + 8, q.x, q.y, q.z);
+		if (!(z > min_depth && z < CUDART_INF_F)) continue;
+		const float fu = rintf(__fdiv_rn(proj_row(P.p, q.x, q.y, q.z), z));
+		const float fv = rintf(__fdiv_rn(proj_row(P.p + 4, q.x, q.y, q.z), z));
+		if (!(fu >= 1.f && fu <= (float)W && fv >= 1.f && fv <= (float)H)) continue;
+		const long p = (long)((int)fv - 1) * W + ((int)fu - 1);
+		atomicMin(key + p, (unsigned long long)__float_as_uint(z) << 32 | (unsigned long long)i);
+	}
+}
+
+__global__ void velo_decode_kernel(const unsigned long long *__restrict__ key, long n, float *__restrict__ depth)
+{
+	for (long p = (long)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (long)gridDim.x * blockDim.x) {
+		const unsigned long long k = key[p];
+		depth[p] = k == NO_POINT ? 0.f : __uint_as_float((unsigned)(k >> 32));
+	}
+}
+
 long grid_for(long n) { return std::min<long>((n + THREADS - 1) / THREADS, (long)adc_num_sms() * 8); }
 
 // the checks every entry shares: sizes, H * W < 2^31, f and fB > 0, finite cx, cy, doffs, max_depth > 0 (+inf: no cap)
@@ -370,6 +412,33 @@ int mccnn_depth_metrics(const float *pred, int pred_depth, const float *gt, int 
 		rc = (int)cudaPeekAtLastError();
 	}
 	const int rf = adc_scratch_free(part, s);
+	return rc ? rc : rf;
+}
+
+int mccnn_velo_depth_map(const float *pts, long long n, const float *P, int H, int W, float min_depth, float *depth,
+			 adcensus_stream_t stream)
+{
+	if ((n && !pts) || ((uintptr_t)pts & 15) || !P || !depth || n < 0 || H < 1 || W < 1 || !(min_depth >= 0.f) ||
+	    !isfinite(min_depth))
+		return ADCENSUS_EINVAL;
+	if ((long)H * W >= (1l << 31) || n >= (1ll << 32)) return ADCENSUS_ELIMIT;
+	Proj pr;
+	for (int k = 0; k < 12; k++) {
+		if (!isfinite(P[k])) return ADCENSUS_EINVAL;
+		pr.p[k] = P[k];
+	}
+	const long npx = (long)H * W;
+	cudaStream_t s = adc_stream(stream);
+	unsigned long long *key = nullptr;
+	int rc = adc_scratch_alloc((void **)&key, sizeof(unsigned long long) * npx, s);
+	if (rc) return rc;
+	rc = (int)cudaMemsetAsync(key, 0xff, sizeof(unsigned long long) * npx, s);
+	if (!rc) {
+		if (n) velo_key_kernel<<<grid_for(n), THREADS, 0, s>>>((const float4 *)pts, n, pr, H, W, min_depth, key);
+		velo_decode_kernel<<<grid_for(npx), THREADS, 0, s>>>(key, npx, depth);
+		rc = (int)cudaPeekAtLastError();
+	}
+	const int rf = adc_scratch_free(key, s);
 	return rc ? rc : rf;
 }
 

@@ -12,7 +12,9 @@ write and `main.lua` reads back, the error metric of `-a test_te`, and the submi
 * ``kitti_submission_image``: the prediction pasted into the bottom rows of the full-size frame
   (main.lua:1203-1205);
 * ``read_calib`` / ``write_depth_png16``: the KITTI 2012, KITTI 2015 and MiddEval3 calibration files, and KITTI's depth
-  map format (DESIGN §20, an addition beyond the reference).
+  map format (DESIGN §20, an addition beyond the reference);
+* ``read_calib(date, 'kitti_raw')`` / ``read_velodyne`` / ``raw_frames``: a KITTI raw drive's calibration, Velodyne scans
+  and frame list (DESIGN §21, an addition beyond the reference).
 
 Plain numpy / PIL host code: nothing here touches the GPU.
 """
@@ -148,9 +150,14 @@ Calib.__doc__ = """A rectified stereo pair's camera: focal length f and principa
 doffs (the x-difference of the two principal points) in pixels, and the image size the file states (None when it states
 none)."""
 
-CALIB_KINDS = ("kitti", "kitti2015", "mb")
-# the two projection matrices of each KITTI calibration file: the grey pair (2012) and the colour pair (2015)
-_KITTI_P = {"kitti": ("P0", "P1"), "kitti2015": ("P_rect_02", "P_rect_03")}
+RawCalib = namedtuple("RawCalib", Calib._fields + ("velo",))
+RawCalib.__doc__ = """A KITTI raw drive's grey pair (the :data:`Calib` fields) and velo, the 3x4 velodyne-to-image matrix
+P_rect_00 R_rect_00 [R|T]_velo_to_cam as a tuple of 12 float64, row-major (DESIGN §21)."""
+
+CALIB_KINDS = ("kitti", "kitti2015", "mb", "kitti_raw")
+# the two projection matrices of each KITTI calibration file: the grey pair (2012 and raw drives), the colour pair (2015)
+_KITTI_P = {"kitti": ("P0", "P1"), "kitti2015": ("P_rect_02", "P_rect_03"), "kitti_raw": ("P_rect_00", "P_rect_01")}
+RAW_CAM, RAW_VELO = "calib_cam_to_cam.txt", "calib_velo_to_cam.txt"
 
 
 def _calib_entries(path):
@@ -177,14 +184,35 @@ def _numbers(path, entries, key, n):
     return v
 
 
+def velo_to_image(P, R_rect, R, T):
+    """P (12) . R_rect (9, padded to 4x4) . [R (9) | T (3)] (padded to 4x4), the top 3x4 of the product as 12 float64,
+    row-major, in this operation order (DESIGN §21): B[i][j] = (R_rect[i][0] A[0][j] + R_rect[i][1] A[1][j]) +
+    R_rect[i][2] A[2][j] with A = [R|T]; M[i][j] = (P[i][0] B[0][j] + P[i][1] B[1][j]) + P[i][2] B[2][j], plus P[i][3]
+    when j = 3."""
+    A = [[R[3 * i + j] for j in range(3)] + [T[i]] for i in range(3)]
+    B = [[(R_rect[3 * i] * A[0][j] + R_rect[3 * i + 1] * A[1][j]) + R_rect[3 * i + 2] * A[2][j] for j in range(4)]
+         for i in range(3)]
+    M = []
+    for i in range(3):
+        for j in range(4):
+            m = (P[4 * i] * B[0][j] + P[4 * i + 1] * B[1][j]) + P[4 * i + 2] * B[2][j]
+            M.append(m + P[4 * i + 3] if j == 3 else m)
+    return tuple(M)
+
+
 def read_calib(path, kind):
     """The :data:`Calib` of a calibration file (DESIGN §20).  kind 'kitti': KITTI 2012's ``calib/%06d.txt``, the grey
     pair P0 / P1; 'kitti2015': ``calib_cam_to_cam/%06d.txt``, the colour pair P_rect_02 / P_rect_03 and the size S_rect_02
     when present; 'mb': a MiddEval3 scene's ``calib.txt`` (cam0, doffs, baseline in millimetres, width, height).  KITTI:
     f = P[0,0], cx = P[0,2], cy = P[1,2] of the left matrix, baseline = (P_left[0,3] - P_right[0,3]) / f, doffs = 0.
+    'kitti_raw' (DESIGN §21): `path` is a raw drive's date directory; its ``calib_cam_to_cam.txt`` gives the grey pair
+    P_rect_00 / P_rect_01, the size S_rect_00 and R_rect_00, its ``calib_velo_to_cam.txt`` R and T, and the result is a
+    :data:`RawCalib` whose velo is :func:`velo_to_image`.
     Refuses a missing key, a malformed matrix, f <= 0 and baseline <= 0, naming the file and the key."""
     if kind not in CALIB_KINDS:
         raise ValueError("calibration kind must be one of %s, got %r" % (", ".join(CALIB_KINDS), kind))
+    if kind == "kitti_raw":
+        return _read_raw_calib(path)
     e = _calib_entries(path)
     width = height = None
     if kind == "mb":
@@ -208,6 +236,73 @@ def read_calib(path, kind):
     if not baseline > 0:
         raise ValueError("%s: %s gives baseline = %g m, must be > 0" % (path, bkey, baseline))
     return Calib(f, cx, cy, baseline, doffs, width, height)
+
+
+def _read_raw_calib(date_dir):
+    cam, velo = os.path.join(date_dir, RAW_CAM), os.path.join(date_dir, RAW_VELO)
+    for p in (cam, velo):
+        if not os.path.isfile(p):
+            raise FileNotFoundError("missing calibration file %s" % p)
+    e, ev = _calib_entries(cam), _calib_entries(velo)
+    pl, pr = _numbers(cam, e, "P_rect_00", 12), _numbers(cam, e, "P_rect_01", 12)
+    width, height = (int(v) for v in _numbers(cam, e, "S_rect_00", 2))
+    R_rect = _numbers(cam, e, "R_rect_00", 9)
+    R, T = _numbers(velo, ev, "R", 9), _numbers(velo, ev, "T", 3)
+    f, cx, cy = pl[0], pl[2], pl[6]
+    if not f > 0:
+        raise ValueError("%s: P_rect_00 gives f = %g, must be > 0" % (cam, f))
+    baseline = (pl[3] - pr[3]) / f
+    if not baseline > 0:
+        raise ValueError("%s: P_rect_00 / P_rect_01 gives baseline = %g m, must be > 0" % (cam, baseline))
+    if not (width > 0 and height > 0):
+        raise ValueError("%s: S_rect_00 gives a %dx%d image" % (cam, width, height))
+    return RawCalib(f, cx, cy, baseline, 0.0, width, height, velo_to_image(pl, R_rect, R, T))
+
+
+def read_velodyne(path):
+    """a KITTI raw scan ``velodyne_points/data/%010d.bin``: (N, 4) float32 x, y, z, reflectance (little-endian); a file whose
+    size is not a multiple of 16 bytes is refused"""
+    size = os.path.getsize(path)
+    if size % 16:
+        raise ValueError("%s: %d bytes, not a whole number of 16-byte points" % (path, size))
+    return np.fromfile(path, dtype="<f4").reshape(-1, 4).astype(np.float32, copy=False)
+
+
+RAW_LEFT, RAW_RIGHT, RAW_SCAN = ("image_00", "data", "%010d.png"), ("image_01", "data", "%010d.png"), \
+    ("velodyne_points", "data", "%010d.bin")
+
+
+def raw_file(drive_dir, what, i):
+    """the file of frame i of a raw drive: what is RAW_LEFT, RAW_RIGHT or RAW_SCAN"""
+    return os.path.join(drive_dir, what[0], what[1], what[2] % i)
+
+
+def _raw_indices(drive_dir, what):
+    d = os.path.join(drive_dir, what[0], what[1])
+    ext = what[2][-4:]
+    if not os.path.isdir(d):
+        return set()
+    return {int(f[:-4]) for f in os.listdir(d) if f.endswith(ext) and len(f) == 14 and f[:10].isdigit()}
+
+
+def raw_frames(drive_dir, velodyne=False):
+    """The ascending frame indices of a KITTI raw drive (``<date>/<date>_drive_<nnnn>_sync``) that have both grey images
+    (``image_00/data/%010d.png``, ``image_01/data/%010d.png``) and, with `velodyne`, the scan.  Refuses a drive with no
+    frame, or one where some frames lack one of these files, naming the frames."""
+    sets = [_raw_indices(drive_dir, RAW_LEFT), _raw_indices(drive_dir, RAW_RIGHT)]
+    names = ["image_00", "image_01"]
+    if velodyne:
+        sets.append(_raw_indices(drive_dir, RAW_SCAN))
+        names.append("velodyne_points")
+    every = set.union(*sets)
+    both = set.intersection(*sets)
+    if every != both:
+        miss = ["%s lacks %s" % (n, ", ".join("%010d" % i for i in sorted(every - s)[:5]) + (" ..." if len(every - s) > 5 else ""))
+                for n, s in zip(names, sets) if every - s]
+        raise ValueError("%s: frames missing on one side: %s" % (drive_dir, "; ".join(miss)))
+    if not both:
+        raise ValueError("%s: no frames (image_00/data/%%010d.png and image_01/data/%%010d.png)" % drive_dir)
+    return sorted(both)
 
 
 def check_calib_size(cal, H, W, path):

@@ -6,6 +6,7 @@ DESIGN §20).
     pts = point_cloud(disp, cal, left_u8, conf=None, density=None)      # Cloud(data, n): device bytes, vertex count
     write_ply("scene.ply", pts)
     m = metrics(disp, gt_disp, cal, min_depth=1e-3, max_depth=80.0)     # DepthMetrics
+    Zs = velo_depth(scan, raw_cal, H, W)                                  # a LiDAR scan's depth map, 0 = none (DESIGN §21)
 
 A disparity d at pixel (x, y) is valid when it is finite and d + doffs > 0 (fp32 add); then, in fp32 with each operation
 rounded once and in this order, Z = fB / (d + doffs), X = ((x - cx) * Z) / f, Y = ((y - cy) * Z) / f, where fB is the
@@ -180,3 +181,38 @@ def metrics(disp, gt, cal, min_depth=MIN_DEPTH, max_depth=KITTI_MAX_DEPTH, is_de
     """:data:`DepthMetrics` of `disp` against the ground-truth disparity `gt` under `cal` (see the module docstring)"""
     c, s = counts(disp, gt, cal, min_depth, max_depth, is_depth)
     return metrics_of(c.cpu(), s.cpu())
+
+
+def velo_depth(pts, cal, H, W, min_depth=MIN_DEPTH):
+    """The (H, W) CUDA float32 depth map of the CUDA LiDAR scan `pts` ((N, 4) float32: x, y, z, reflectance) under
+    ``cal.velo`` (a :data:`dataio.RawCalib`, or any 12 numbers of a row-major 3x4 matrix, rounded once to fp32): each pixel
+    the smallest camera depth z > min_depth of the points projecting onto it, 0 where none does (mccnn_velo_depth_map,
+    DESIGN §21)."""
+    n = "mccnn_velo_depth_map"
+    if not isinstance(pts, torch.Tensor) or not pts.is_cuda or pts.dtype != torch.float32:
+        raise adcensus.AdcensusError("%s: pts must be a CUDA float32 tensor" % n)
+    if pts.dim() != 2 or pts.size(1) != 4:
+        raise adcensus.AdcensusError("%s: pts must be (N, 4), got %s" % (n, tuple(pts.shape)))
+    velo = getattr(cal, "velo", cal)
+    P = np.asarray(velo, dtype=np.float64).reshape(-1).astype(np.float32)
+    if P.size != 12:
+        raise ValueError("%s: a 3x4 matrix expected, got %d numbers" % (n, P.size))
+    if not min_depth >= 0:
+        raise ValueError("min_depth must be >= 0, got %r" % (min_depth,))
+    p = pts.contiguous()
+    if p.data_ptr() % 16:
+        p = p.clone()
+    Z = torch.empty((int(H), int(W)), device=p.device, dtype=torch.float32)
+    with torch.cuda.device(p.device):
+        adcensus._check(adcensus.lib().mccnn_velo_depth_map(p.data_ptr() if p.numel() else None, p.size(0),
+                                                            P.ctypes.data, int(H), int(W), _f32(min_depth), Z.data_ptr(),
+                                                            adcensus._stream(p)), n)
+    return Z
+
+
+def disparity_of_depth(Z, cal):
+    """the disparity fB / Z (fp32) of a CUDA depth map `Z` with doffs 0, NaN where Z is not > 0: mccnn_disp_to_depth, the
+    same map in the other direction.  It turns a scan's depth map into the ground-truth disparity :func:`metrics` takes."""
+    if float(cal.doffs) != 0.0:
+        raise ValueError("a depth map becomes a disparity this way only when doffs = 0, got %r" % (cal.doffs,))
+    return depth(Z, cal)

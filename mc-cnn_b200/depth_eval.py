@@ -103,7 +103,7 @@ def _score(pred, gts, cal, dataset, is_depth=False):
     return out
 
 
-def report(dataset, names, compute, rank=None, world=None, verbose=True):
+def report(dataset, names, compute, rank=None, world=None, verbose=True, ncol=None):
     """batch.run_sharded over the pairs; rank 0 prints one line per pair and the line of means and returns the Scores"""
     import torch.distributed as dist
 
@@ -117,7 +117,8 @@ def report(dataset, names, compute, rank=None, world=None, verbose=True):
         rows.append(_unpack(t))
         if verbose:
             print(line(name, rows[-1]), flush=True)
-    mean = [sum(r[k] for r in rows) / len(rows) if rows else float("nan") for k in range(len(columns(dataset)))]
+    ncol = len(columns(dataset)) if ncol is None else ncol
+    mean = [sum(r[k] for r in rows) / len(rows) if rows else float("nan") for k in range(ncol)]
     if verbose:
         print(line("mean", mean), flush=True)
     return Scores(list(names), rows, mean)
@@ -206,3 +207,116 @@ def score_dir(dataset, pred_dir, data_root=".", source="disp", device=0, verbose
             return _score(pred, gts, cal, dataset, is_depth=source == "depth")
 
     return report(dataset, [p[0] for p in pairs], compute, rank, world, verbose)
+
+
+# ---- KITTI raw drives against the projected Velodyne scans (DESIGN §21) ------------------------------------------------------
+
+RAW_COLUMNS = ["lidar_%s" % m for m in depth.METRICS]
+# the published crop rectangles, fractions of (H, H, W, W): rows [top, bottom), columns [left, right) (Garg et al. 2016;
+# Eigen et al. 2014)
+CROPS = {"garg": (0.40810811, 0.99189189, 0.03594771, 0.96405229), "eigen": (0.3324324, 0.91351351, 0.0359477, 0.96405229)}
+
+
+def crop_box(crop, H, W):
+    """(top, bottom, left, right) of crop 'garg' / 'eigen' at H x W: each fraction times the size in float64, truncated"""
+    if crop not in CROPS:
+        raise ValueError("crop must be garg, eigen or none, got %r" % (crop,))
+    a, b, c, d = CROPS[crop]
+    return int(a * H), int(b * H), int(c * W), int(d * W)
+
+
+def lidar_gt(scan, cal, H, W, device, min_depth=depth.MIN_DEPTH, crop="none"):
+    """the ground-truth disparity of a frame: its scan (host (N, 4) float32) projected into an H x W depth map
+    (depth.velo_depth), 0 outside the crop rectangle, turned into the disparity fB / Z (NaN where no point) that
+    depth.metrics takes"""
+    import torch
+
+    Z = depth.velo_depth(torch.from_numpy(scan).to(device), cal, H, W, min_depth)
+    if crop != "none":
+        t, b, l, r = crop_box(crop, H, W)
+        for rows, cols in ((slice(0, t), slice(None)), (slice(b, None), slice(None)), (slice(None), slice(0, l)),
+                           (slice(None), slice(r, None))):
+            Z[rows, cols] = 0.0
+    return depth.disparity_of_depth(Z, cal)
+
+
+def _check_raw(min_depth, max_depth, crop):
+    if not (0 < min_depth <= max_depth):
+        raise ValueError("need 0 < min_depth <= max_depth, got %r, %r" % (min_depth, max_depth))
+    if crop != "none":
+        crop_box(crop, 1, 1)
+
+
+def _raw_inputs(frames):
+    """(pair files, shapes, calibrations) of the frames, refused before any GPU work as predict_raw refuses them"""
+    from . import predict_raw
+
+    files = predict_raw.pair_files(frames)
+    shapes = predict_kitti.scan(files)
+    return files, shapes, predict_raw.read_calibs(frames, shapes)
+
+
+def evaluate_raw(dataset, arch, frames, net_fname=None, disp_max=predict_kitti.DISP_MAX, min_depth=depth.MIN_DEPTH,
+                 max_depth=depth.KITTI_MAX_DEPTH, crop="none", device=0, prefetch=True, verbose=True, **overrides):
+    """The net over each raw frame of `frames` (predict_raw.Frame list; predict_raw.drive_frames(..., velodyne=True) or
+    read_list), each map scored against the frame's projected scan (:func:`lidar_gt`) by depth.metrics with `min_depth` and
+    `max_depth`.  Prints one line per frame (predict_raw.frame_name, then the RAW_COLUMNS values) and the line of means;
+    returns the Scores on rank 0, None on other ranks."""
+    from . import predict_raw
+
+    _check_raw(min_depth, max_depth, crop)
+    files, shapes, cals = _raw_inputs(frames)
+    rank, world = _world()
+    run = predict_kitti.PairRunner(files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch,
+                                   **overrides)
+
+    def compute(i):
+        import torch
+
+        fr = frames[i]
+        cal = cals[predict_raw.date_dir(fr.drive)]
+        _, _, _, pred, _ = run.predict(i)
+        with torch.cuda.device(run.dev):
+            gt = lidar_gt(dataio.read_velodyne(dataio.raw_file(fr.drive, dataio.RAW_SCAN, fr.index)), cal, *shapes[i],
+                          run.dev, min_depth, crop)
+            return list(depth.metrics(pred, gt, cal, min_depth, max_depth))
+
+    try:
+        run.prepare()
+        return report("raw", [predict_raw.frame_name(f) for f in frames], compute, rank, world, verbose, len(RAW_COLUMNS))
+    finally:
+        run.close()
+
+
+def score_raw(frames, pred_dir, source="disp", min_depth=depth.MIN_DEPTH, max_depth=depth.KITTI_MAX_DEPTH, crop="none",
+              device=0, verbose=True):
+    """Scores the maps predict_raw wrote under `pred_dir` (``<drive>/disp/%010d.png``, or with `source` 'depth'
+    ``<drive>/depth/%010d.png``) for `frames` against their projected scans, as :func:`evaluate_raw` does.  Every frame
+    needs its map."""
+    import torch
+
+    from . import predict_raw
+
+    if source not in ("disp", "depth"):
+        raise ValueError("source must be 'disp' or 'depth', got %r" % (source,))
+    _check_raw(min_depth, max_depth, crop)
+    maps = [predict_raw.out_file(pred_dir, fr, source) for fr in frames]
+    for f in maps:
+        if not os.path.isfile(f):
+            raise FileNotFoundError("missing map %s" % f)
+    _, shapes, cals = _raw_inputs(frames)
+    rank, world = _world()
+    dev = torch.device("cuda", device)
+
+    def compute(i):
+        fr = frames[i]
+        m = dataio.read_depth_png16(maps[i]) if source == "depth" else dataio.read_png16(maps[i])
+        if m.shape != tuple(shapes[i]):
+            raise ValueError("%s is %dx%d, the images %dx%d" % (maps[i], *m.shape, *shapes[i]))
+        cal = cals[predict_raw.date_dir(fr.drive)]
+        with torch.cuda.device(dev):
+            gt = lidar_gt(dataio.read_velodyne(dataio.raw_file(fr.drive, dataio.RAW_SCAN, fr.index)), cal, *shapes[i], dev,
+                          min_depth, crop)
+            return list(depth.metrics(torch.from_numpy(m).to(dev), gt, cal, min_depth, max_depth, is_depth=source == "depth"))
+
+    return report("raw", [predict_raw.frame_name(f) for f in frames], compute, rank, world, verbose, len(RAW_COLUMNS))

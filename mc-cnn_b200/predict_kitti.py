@@ -94,6 +94,7 @@ class Prefetch:
 
     def __init__(self, files, order, enabled=True):
         self.files, self.order = files, list(order)
+        self.pos = {i: k for k, i in enumerate(self.order)}
         self.pool = concurrent.futures.ThreadPoolExecutor(max_workers=1) if enabled else None
         self.pending = {}
 
@@ -105,7 +106,7 @@ class Prefetch:
         if self.pool is None:
             return decode(self.files[i])
         self._start(i)
-        k = self.order.index(i) + 1
+        k = self.pos[i] + 1
         if k < len(self.order):
             self._start(self.order[k])
         return self.pending.pop(i).result()
@@ -115,6 +116,38 @@ class Prefetch:
             for f in self.pending.values():
                 f.cancel()
             self.pool.shutdown(wait=True)
+
+
+class PairRunner:
+    """The stereo method of (dataset, arch, net) over a list of pairs, shared by every tool that predicts a sequence of
+    image files: one :class:`evaluate.Evaluator` prepared at the largest (H, W, disp_max) of `shapes`, and this rank's
+    pairs (``batch.shard_indices`` of `rank`, `world`) decoded one ahead in a background thread (:class:`Prefetch`).
+    :meth:`predict` gives one pair's device map; :meth:`close` releases both."""
+
+    def __init__(self, files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch=True, **overrides):
+        self.ev = evaluate.Evaluator(dataset, arch, net_fname=net_fname, device=device, **overrides)
+        self.dev = self.ev.dev
+        self.disp_max = int(disp_max)
+        self.pre = Prefetch(files, batch.shard_indices(len(files), rank, world), enabled=prefetch)
+        self.shapes = [(H, W, self.disp_max) for H, W in shapes]
+
+    def prepare(self):
+        self.ev.prepare(self.shapes)
+
+    def predict(self, i, conf=False):
+        """(left bytes, right bytes, ground truth or None, the (H, W) device map, its margin confidence or None) of pair i"""
+        import torch
+
+        left, right, gt = self.pre.get(i)
+        x_batch = frontend.make_batch_cuda(left, right, self.dev)
+        if not conf:
+            return left, right, gt, self.ev.stereo_predict(x_batch, self.disp_max), None
+        c = torch.empty(x_batch.shape[2:], device=self.dev)
+        return left, right, gt, self.ev.stereo_predict(x_batch, self.disp_max, conf=c), c
+
+    def close(self):
+        self.pre.close()
+        self.ev.close()
 
 
 CALIB_DIR = {"kitti": "calib", "kitti2015": "calib_cam_to_cam"}
@@ -250,31 +283,23 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
         check_out(out)
         if distributed:
             dist.barrier()                      # every rank has looked at `out` before any rank writes to it
-    ev = evaluate.Evaluator(dataset, arch, net_fname=net_fname, device=device, **overrides)
     rank = dist.get_rank() if distributed else 0
     world = dist.get_world_size() if distributed else 1
-    pre = Prefetch(files, batch.shard_indices(len(files), rank, world), enabled=prefetch)
-    disp_max = int(disp_max)
+    run = PairRunner(files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch, **overrides)
     submission_file = lambda i: os.path.join(out if dataset == "kitti" else os.path.join(out, "disp_0"), "%06d_10.png" % i)
 
     def compute(i):
-        left, right, gt = pre.get(i)
-        x_batch = frontend.make_batch_cuda(left, right, ev.dev)
-        if density is None:
-            pred = ev.stereo_predict(x_batch, disp_max)
-        else:
-            conf = torch.empty(x_batch.shape[2:], device=ev.dev)
-            pred = ev.stereo_predict(x_batch, disp_max, conf=conf)
+        left, _, gt, pred, conf = run.predict(i, conf=density is not None)
         if action == "test":
             if depth:
-                with torch.cuda.device(ev.dev):
+                with torch.cuda.device(run.dev):
                     write_depth(pred, left, calibs[i], out, i, ply)
             return error_counts(pred, gt).cpu()
         if density is not None:
-            with torch.cuda.device(ev.dev):
+            with torch.cuda.device(run.dev):
                 pred = confidence.sparsify(pred, conf, density, 0.0)
         if depth:
-            with torch.cuda.device(ev.dev):
+            with torch.cuda.device(run.dev):
                 write_depth(pred, left, calibs[i], out, i, ply)
         H, W = shapes[i]
         f = dataio.write_kitti_submission(pred.cpu().numpy(), H, W, out, i, dataset)
@@ -282,8 +307,7 @@ def predict_kitti(action, dataset, net_fname=None, arch="fast", data_root=".", o
         return torch.tensor([i])
 
     try:
-        ev.prepare([(H, W, disp_max) for H, W in shapes])
+        run.prepare()
         return report(action, len(files), compute, rank, world, submission_file, verbose)
     finally:
-        pre.close()
-        ev.close()
+        run.close()

@@ -74,13 +74,15 @@ def _standardise(x):
     return ((x - x.mean()) / x.std(ddof=1)).astype(np.float32)
 
 
-def _scene_views(rng, H, W, D, n_views=2):
+def _scene_views(rng, H, W, D, n_views=2, levels=None):
     """(views (n_views, H, W), gt (H, W)): standardised grey views of one natural scene, view 0 the left image, every other
     view the right image (views 2, 3 ... with their own brightness and noise, like Middlebury's extra exposures / lights).
-    Left pixel x matches right pixel x - gt; gt is piecewise constant in [1, D) and 0 (invalid) on about 10% of the pixels."""
+    Left pixel x matches right pixel x - gt; gt is piecewise constant in [1, D) (or drawn from the integers `levels`) and 0
+    (invalid) on about 10% of the pixels."""
     dmax = max(2, min(D, W // 3))
     gy, gx = (H + 15) // 16, (W + 47) // 48
-    gt = np.kron(rng.integers(1, dmax, size=(gy, gx)), np.ones((16, 48), np.int64))[:H, :W]
+    blocks = rng.integers(1, dmax, size=(gy, gx)) if levels is None else np.asarray(levels)[rng.integers(0, len(levels), (gy, gx))]
+    gt = np.kron(blocks, np.ones((16, 48), np.int64))[:H, :W]
     ext = W + D
     scene = natural_image(rng, H, ext)
     cols = np.arange(W)[None, :] + D
@@ -163,6 +165,76 @@ def write_kitti_raw(root, dataset="kitti", n_tr=41, n_te=2, H=375, widths=(1242,
                 frac = (slant[:H, :W] * (np.arange(W)[None, :] % 48) // 48) / np.float32(256)
                 dataio.write_png16(np.where(gt > 0, gt + frac, 0).astype(np.float32), os.path.join(unzip, sub, names[2], fname))
     return unzip
+
+
+# A raw drive's camera: f B = 384 exactly, and every disparity of RAW_LEVELS gives a depth 384 / d that is exact in fp32 and
+# turns back into d exactly, so a scan sampled from the true depth scores 0 against the true disparity.
+RAW_F, RAW_B = 768.0, 0.5
+RAW_LEVELS = (6, 8, 12, 16, 24, 32, 48)
+# velodyne (x forward, y left, z up) to camera 0 (x right, y down, z forward), no offset
+RAW_VELO_R = (0.0, -1.0, 0.0, 0.0, 0.0, -1.0, 1.0, 0.0, 0.0)
+
+
+def raw_calib_text(H, W, f=RAW_F, B=RAW_B, R_rect=(1, 0, 0, 0, 1, 0, 0, 0, 1), R=RAW_VELO_R, T=(0.0, 0.0, 0.0)):
+    """(calib_cam_to_cam.txt, calib_velo_to_cam.txt) of a raw drive's date directory, in KITTI's key: value layout"""
+    cx, cy = W / 2 - 0.25, H / 2 + 0.5
+    num = lambda v: " ".join(repr(float(x)) for x in v)
+    P0 = (f, 0, cx, 0, 0, f, cy, 0, 0, 0, 1, 0)
+    P1 = (f, 0, cx, -f * B, 0, f, cy, 0, 0, 0, 1, 0)
+    cam = ["calib_time: 09-Jan-2012 13:57:47", "corner_dist: 9.950000e-02"]
+    for k in ("00", "01", "02", "03"):
+        cam += ["S_%s: 1.392000e+03 5.120000e+02" % k, "K_%s: %s" % (k, num((f, 0, cx, 0, f, cy, 0, 0, 1))),
+                "S_rect_%s: %d %d" % (k, W, H), "R_rect_%s: %s" % (k, num(R_rect)),
+                "P_rect_%s: %s" % (k, num(P1 if k in ("01", "03") else P0))]
+    velo = ["calib_time: 15-Mar-2012 11:37:16", "R: %s" % num(R), "T: %s" % num(T),
+            "delta_f: 0.000000e+00 0.000000e+00", "delta_c: 0.000000e+00 0.000000e+00"]
+    return "\n".join(cam) + "\n", "\n".join(velo) + "\n"
+
+
+def write_kitti_drive(root, date="2011_09_26", drive=1, n=3, H=40, W=150, seed=0, D=64, levels=RAW_LEVELS, every=3):
+    """A seeded KITTI raw drive under ``root/<date>/<date>_drive_<drive>_sync``: grey rectified pairs
+    ``image_00/data/%010d.png`` / ``image_01/data/%010d.png`` whose left pixel x matches right pixel x - gt (gt piecewise
+    constant over `levels`, 0 on about 10% of the pixels), the date directory's calibration (:func:`raw_calib_text`, written
+    once per date) and per frame a velodyne scan ``velodyne_points/data/%010d.bin`` sampled from the same scene: a point at
+    the true depth 384 / gt for one pixel in `every` where gt > 0, placed where the projection rule of DESIGN §21 maps it to
+    that pixel, plus points hidden behind them on the same pixels, points behind the camera and points outside the image.
+    Returns (drive directory, [gt (H, W) float32 per frame])."""
+    import os
+
+    from PIL import Image
+
+    rng = np.random.default_rng(seed)
+    date_dir = os.path.join(root, date)
+    drive_dir = os.path.join(date_dir, "%s_drive_%04d_sync" % (date, drive))
+    for sub in ("image_00", "image_01", "velodyne_points"):
+        os.makedirs(os.path.join(drive_dir, sub, "data"), exist_ok=True)
+    cam, velo = raw_calib_text(H, W)
+    for name, text in (("calib_cam_to_cam.txt", cam), ("calib_velo_to_cam.txt", velo)):
+        if not os.path.exists(os.path.join(date_dir, name)):
+            with open(os.path.join(date_dir, name), "w") as f:
+                f.write(text)
+    cx, cy = W / 2 - 0.25, H / 2 + 0.5
+    fB = np.float32(RAW_F * RAW_B)
+    byte = lambda a: np.clip(np.rint(128 + 40 * a), 0, 255).astype(np.uint8)
+    gts = []
+    for k in range(n):
+        views, gt = _scene_views(rng, H, W, D, levels=levels)
+        for v, sub in zip(views, ("image_00", "image_01")):
+            Image.fromarray(byte(v), "L").save(os.path.join(drive_dir, sub, "data", "%010d.png" % k), format="PNG")
+        ys, xs = np.nonzero((gt > 0) & (rng.integers(0, every, gt.shape) == 0))
+        z = (fB / gt[ys, xs].astype(np.float32)).astype(np.float32)
+        X = (xs + 1 - cx) * z.astype(np.float64) / RAW_F            # the image coordinate u + 1 of pixel u (DESIGN §21)
+        Y = (ys + 1 - cy) * z.astype(np.float64) / RAW_F
+        pts = [np.stack([z, -X, -Y], 1)]
+        m = rng.random(len(z)) < 0.2                                 # hidden: the same ray, further away
+        pts.append(np.stack([z[m] * 1.5, -X[m] * 1.5, -Y[m] * 1.5], 1))
+        pts.append(np.stack([-rng.uniform(1, 50, 50), rng.uniform(-20, 20, 50), rng.uniform(-2, 2, 50)], 1))
+        pts.append(np.stack([rng.uniform(5, 50, 50), rng.uniform(200, 400, 50), rng.uniform(-2, 2, 50)], 1))
+        xyz = np.concatenate(pts).astype(np.float32)
+        scan = np.concatenate([xyz, rng.uniform(0, 1, (len(xyz), 1)).astype(np.float32)], 1)
+        scan[rng.permutation(len(scan))].astype("<f4").tofile(os.path.join(drive_dir, "velodyne_points", "data", "%010d.bin" % k))
+        gts.append(gt.astype(np.float32))
+    return drive_dir, gts
 
 
 def write_kitti_eval_maps(unzip, dataset="kitti", seed=0):
