@@ -780,6 +780,29 @@ int mccnn_depth_metrics(const float *pred, int pred_depth, const float *gt, int 
 int mccnn_velo_depth_map(const float *pts, long long n, const float *P, int H, int W, float min_depth, float *depth,
 			 adcensus_stream_t stream);
 
+/* ---- stereo rectification of calibrated raw cameras (csrc/rectify.cu, rectify.py; DESIGN §22) -------------------------
+ * An addition beyond the reference.  mccnn_rectify_pair: both views of a raw pair, left and right (H,W) grey or (H,W,3)
+ * R, G, B bytes (nch 1 or 3, DEVICE), rectified in one launch into out_left and out_right (Ho,Wo[,3]) bytes (DEVICE), and
+ * with a non-NULL `valid` the left view's validity (Ho,Wo) bytes, 1 valid and 0 not.  params_left / params_right: the
+ * MCCNN_RECTIFY_NPARAM HOST floats of each camera, read during the call: iR = inv(P[:, :3] R) row-major (computed in
+ * float64 and rounded once to fp32), fx, fy, cx, cy of K, then k1 k2 p1 p2 k3 k4 k5 k6 (missing ones 0).
+ * Output pixel (u, v), in fp32 with every operation rounded once, in this order (OpenCV's initUndistortRectifyMap model):
+ *   X = (iR00 u + iR01 v) + iR02, Y and Z likewise from rows 1 and 2;  x = X / Z, y = Y / Z;  r2 = x x + y y;
+ *   rad = (1 + r2 (k1 + r2 (k2 + r2 k3))) / (1 + r2 (k4 + r2 (k5 + r2 k6)));
+ *   xd = x rad + (2 p1 x y + p2 (r2 + 2 x x));  yd = y rad + (p1 (r2 + 2 y y) + 2 p2 x y)  (products left to right);
+ *   sx = fx xd + cx, sy = fy yd + cy.
+ * Sampling: x0 = floor(sx), a = sx - x0, y0 = floor(sy), b = sy - y0; the taps x0, x0 + 1, y0, y0 + 1 clamped into the raw
+ * image (the border replicated); v = (1 - b) ((1 - a) I00 + a I01) + b ((1 - a) I10 + a I11), the byte rint(v) (ties to
+ * even), the colour channels sharing the weights.  Valid: -0.5 <= sx < W - 0.5 and -0.5 <= sy < H - 0.5.  Where Z <= 0 or
+ * sx or sy is not finite the pixel is invalid and its bytes are 0.  The same bytes on every run and GPU.
+ * Refuses, before any launch: a NULL pointer (valid excepted), an output overlapping an input or another output, nch not 1
+ * or 3, a non-finite parameter, H, W, Ho or Wo < 1 (ADCENSUS_EINVAL); H W nch or Ho Wo nch >= 2^31 (ADCENSUS_ELIMIT).
+ * Asynchronous on `stream`. */
+#define MCCNN_RECTIFY_NPARAM 21
+int mccnn_rectify_pair(const unsigned char *left, const unsigned char *right, int nch, int H, int W, const float *params_left,
+		       const float *params_right, int Ho, int Wo, unsigned char *out_left, unsigned char *out_right,
+		       unsigned char *valid, adcensus_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

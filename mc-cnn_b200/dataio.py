@@ -14,7 +14,9 @@ write and `main.lua` reads back, the error metric of `-a test_te`, and the submi
 * ``read_calib`` / ``write_depth_png16``: the KITTI 2012, KITTI 2015 and MiddEval3 calibration files, and KITTI's depth
   map format (DESIGN §20, an addition beyond the reference);
 * ``read_calib(date, 'kitti_raw')`` / ``read_velodyne`` / ``raw_frames``: a KITTI raw drive's calibration, Velodyne scans
-  and frame list (DESIGN §21, an addition beyond the reference).
+  and frame list (DESIGN §21, an addition beyond the reference);
+* ``read_rectification``: a raw stereo pair's intrinsics, distortion and rectification, from a KITTI raw date directory or
+  OpenCV FileStorage YAML files (DESIGN §22, an addition beyond the reference).
 
 Plain numpy / PIL host code: nothing here touches the GPU.
 """
@@ -309,6 +311,172 @@ def check_calib_size(cal, H, W, path):
     """refuses a calibration whose stated image size is not (H, W): nothing is rescaled"""
     if cal.width is not None and (cal.width, cal.height) != (W, H):
         raise ValueError("%s: calibration for %dx%d images, the image is %dx%d" % (path, cal.width, cal.height, W, H))
+
+
+# ---- rectification of calibrated raw cameras (DESIGN §22) ----------------------------------------------------------------
+
+CameraRect = namedtuple("CameraRect", "K D R P size rect_size")
+CameraRect.__doc__ = """One raw camera and its rectification, float64: K the 3x3 intrinsics (9 numbers, row-major), D its 0, 4, 5 or 8
+distortion coefficients in OpenCV's order k1 k2 p1 p2 [k3 [k4 k5 k6]], R the 3x3 rectifying rotation (9), P the 3x4
+rectified projection (12), size the raw image size (W, H) and rect_size the rectified one (W', H')."""
+
+RECT_KINDS = ("kitti_raw", "opencv")
+RAW_EXTRACT = "_extract"                 # a KITTI raw drive of unrectified images: <date>/<date>_drive_<nnnn>_extract
+
+
+class StereoRect(namedtuple("StereoRect", "left right")):
+    """A raw stereo pair's two :data:`CameraRect`; :attr:`calib` is the :data:`Calib` of the rectified pair."""
+
+    __slots__ = ()
+
+    @property
+    def calib(self):
+        """f = P1[0,0], cx = P1[0,2], cy = P1[1,2], baseline = (P1[0,3] - P2[0,3]) / f, doffs = P2[0,2] - P1[0,2], the size
+        rect_size"""
+        p1, p2 = self.left.P, self.right.P
+        return Calib(p1[0], p1[2], p1[6], (p1[3] - p2[3]) / p1[0], p2[2] - p1[2], *self.left.rect_size)
+
+    def check_size(self, H, W, path):
+        """refuses raw images that are not (H, W) = the cameras' size"""
+        for side, cam in (("left", self.left), ("right", self.right)):
+            if tuple(cam.size) != (W, H):
+                raise ValueError("%s: %s camera calibrated for %dx%d images, the image is %dx%d"
+                                 % (path, side, cam.size[0], cam.size[1], W, H))
+
+
+def _all_numbers(path, text, key):
+    try:
+        v = [float(t) for t in text.replace("[", " ").replace("]", " ").replace(";", " ").replace(",", " ").split()]
+    except ValueError:
+        raise ValueError("%s: %s must hold numbers, got %r" % (path, key, text)) from None
+    if not all(np.isfinite(v)):
+        raise ValueError("%s: %s must hold finite numbers, got %r" % (path, key, text))
+    return v
+
+
+def _opencv_entries(paths):
+    """{key: (numbers, file)} of the !!opencv-matrix entries (and scalar numbers) of OpenCV FileStorage YAML files, later
+    files overriding earlier ones.  A matrix whose data does not hold rows * cols numbers is refused."""
+    out = {}
+    for path in paths:
+        with open(path) as f:
+            text = f.read()
+        if not text.startswith("%YAML"):
+            raise ValueError("%s: not an OpenCV FileStorage YAML file (no %%YAML header)" % path)
+        blocks, key = {}, None
+        for line in text.splitlines()[1:]:
+            m = re.match(r"([A-Za-z_][A-Za-z0-9_]*)\s*:(.*)$", line)
+            if m:
+                key = m.group(1)
+                blocks[key] = [m.group(2)]
+            elif key is not None and line[:1].isspace():
+                blocks[key].append(line)
+            else:
+                key = None                       # '---' and anything else at the top level ends an entry
+        for key, lines in blocks.items():
+            body = "\n".join(lines)
+            if "!!opencv-matrix" in body:
+                fields = dict(re.findall(r"^\s*(rows|cols|dt)\s*:\s*(\S+)", body, re.M))
+                data = re.search(r"data\s*:\s*\[(.*?)\]", body, re.S)
+                if "rows" not in fields or "cols" not in fields or data is None:
+                    raise ValueError("%s: %s is not an opencv-matrix with rows, cols and data" % (path, key))
+                v = _all_numbers(path, data.group(1), key)
+                rows, cols = int(fields["rows"]), int(fields["cols"])
+                if len(v) != rows * cols:
+                    raise ValueError("%s: %s is %dx%d but holds %d numbers" % (path, key, rows, cols, len(v)))
+                out[key] = (v, path)
+            else:
+                try:
+                    out[key] = ([float(body.strip())], path)
+                except ValueError:
+                    pass                         # strings and nested maps are not calibration numbers
+    return out
+
+
+def _camera(src, keys, n_expected, size, rect_size):
+    """the :data:`CameraRect` of `keys` (K, D, R, P names) in `src` {key: (numbers, file)}; checks the counts and K"""
+    vals = []
+    for k, n in zip(keys, n_expected):
+        names = k if isinstance(k, tuple) else (k,)
+        hit = next((nm for nm in names if nm in src), None)
+        if hit is None:
+            raise ValueError("%s: missing key %s" % (src["__file__"], " or ".join(names)))
+        v, path = src[hit]
+        if n is None:
+            if len(v) not in (0, 4, 5, 8):
+                raise ValueError("%s: %s holds %d distortion coefficients; 0, 4, 5 or 8 are supported" % (path, hit, len(v)))
+        elif len(v) != n:
+            raise ValueError("%s: %s must hold %d numbers, got %d" % (path, hit, n, len(v)))
+        vals.append((tuple(float(x) for x in v), hit, path))
+    (K, kname, kpath), (D, _, _), (R, rname, _), (P, pname, ppath) = vals
+    if K[1] != 0 or K[3] != 0:
+        raise ValueError("%s: %s has skew; a zero-skew camera matrix is expected" % (kpath, kname))
+    if K[6:] != (0.0, 0.0, 1.0):
+        raise ValueError("%s: %s's last row is %s, not (0, 0, 1)" % (kpath, kname, K[6:]))
+    M = np.asarray(P, np.float64).reshape(3, 4)[:, :3] @ np.asarray(R, np.float64).reshape(3, 3)
+    if not np.linalg.cond(M) < 1e12:
+        raise ValueError("%s: %s[:, :3] . %s is singular" % (ppath, pname, rname))
+    return CameraRect(K, D, R, P, tuple(size), tuple(rect_size))
+
+
+def _check_pair(rect, path, p1name, p2name):
+    """the refusals of a rectified pair: f <= 0, baseline <= 0, a vertical rig, rectified sizes that differ"""
+    p1, p2 = rect.left.P, rect.right.P
+    if not p1[0] > 0:
+        raise ValueError("%s: %s gives f = %g, must be > 0" % (path, p1name, p1[0]))
+    if p1[4:] != p2[4:] or p2[7] != 0:
+        raise ValueError("%s: %s and %s differ in rows 1 and 2 or %s[1,3] != 0: a vertical rig, which is not supported"
+                         % (path, p1name, p2name, p2name))
+    if not rect.calib.baseline > 0:
+        raise ValueError("%s: %s / %s gives baseline = %g, must be > 0" % (path, p1name, p2name, rect.calib.baseline))
+    if rect.left.rect_size != rect.right.rect_size:
+        raise ValueError("%s: the rectified sizes differ, %s and %s" % (path, rect.left.rect_size, rect.right.rect_size))
+    return rect
+
+
+def _size(path, e, key):
+    v = _numbers(path, e, key, 2)
+    if not all(x == int(x) and x >= 1 for x in v):
+        raise ValueError("%s: %s must hold two positive whole numbers, got %r" % (path, key, e[key]))
+    return int(v[0]), int(v[1])
+
+
+def read_rectification(path, kind, size=None):
+    """The :class:`StereoRect` of a raw stereo pair (DESIGN §22).  kind 'kitti_raw': `path` is a KITTI raw date directory;
+    its ``calib_cam_to_cam.txt`` gives K_0i, D_0i, R_rect_0i, P_rect_0i, S_0i and S_rect_0i of the grey cameras 00 and 01.
+    kind 'opencv': `path` is an OpenCV FileStorage YAML file or a list of them, merged (e.g. stereo_calib's intrinsics.yml
+    and extrinsics.yml), holding M1 or K1, D1, M2 or K2, D2, R1, R2, P1, P2; `size` (W, H) is the images' size, and the
+    rectified size equals it.  Refuses, naming the file and the key: a missing key or a wrong count of numbers, a distortion
+    count other than 0, 4, 5 or 8, a K with skew or whose last row is not (0, 0, 1), a singular P[:, :3] R, f <= 0,
+    baseline <= 0, a vertical rig (the two P's rows 1 and 2 differ, or P2[1,3] != 0) and rectified sizes that differ."""
+    if kind not in RECT_KINDS:
+        raise ValueError("rectification kind must be one of %s, got %r" % (", ".join(RECT_KINDS), kind))
+    if kind == "kitti_raw":
+        if size is not None:
+            raise ValueError("kitti_raw: the raw size comes from S_00 / S_01, not from `size`")
+        cam = os.path.join(path, RAW_CAM)
+        if not os.path.isfile(cam):
+            raise FileNotFoundError("missing calibration file %s" % cam)
+        e = _calib_entries(cam)
+        src = {k: (_all_numbers(cam, v, k), cam) for k, v in e.items() if k[:2] in ("K_", "D_", "R_", "P_", "S_")}
+        src["__file__"] = cam
+        cams = []
+        for i in ("00", "01"):
+            cams.append(_camera(src, ("K_" + i, "D_" + i, "R_rect_" + i, "P_rect_" + i), (9, None, 9, 12),
+                                _size(cam, e, "S_" + i), _size(cam, e, "S_rect_" + i)))
+        return _check_pair(StereoRect(*cams), cam, "P_rect_00", "P_rect_01")
+    paths = [path] if isinstance(path, (str, os.PathLike)) else list(path)
+    if not paths:
+        raise ValueError("opencv: no calibration file given")
+    if size is None or len(size) != 2 or not all(int(s) == s and s >= 1 for s in size):
+        raise ValueError("opencv: the images' size (W, H) is needed, got %r" % (size,))
+    size = (int(size[0]), int(size[1]))
+    src = _opencv_entries(paths)
+    src["__file__"] = " + ".join(str(p) for p in paths)
+    cams = [_camera(src, (("M%d" % i, "K%d" % i), "D%d" % i, "R%d" % i, "P%d" % i), (9, None, 9, 12), size, size)
+            for i in (1, 2)]
+    where = src["P1"][1] if src["P1"][1] == src["P2"][1] else src["__file__"]
+    return _check_pair(StereoRect(*cams), where, "P1", "P2")
 
 
 def write_depth_png16(Z, fname):

@@ -251,6 +251,7 @@ def _raw_inputs(frames):
     """(pair files, shapes, calibrations) of the frames, refused before any GPU work as predict_raw refuses them"""
     from . import predict_raw
 
+    predict_raw.check_synced(sorted({fr.drive for fr in frames}))
     files = predict_raw.pair_files(frames)
     shapes = predict_kitti.scan(files)
     return files, shapes, predict_raw.read_calibs(frames, shapes)

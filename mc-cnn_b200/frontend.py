@@ -193,7 +193,8 @@ class StereoMethod:
 
 
 def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=None, out_dir=None, device=0,
-            net_fname=None, confidence=False, calib=None, ply=False, max_depth=None, density=None, **overrides):
+            net_fname=None, confidence=False, calib=None, ply=False, max_depth=None, density=None, rectify=None,
+            **overrides):
     """``main.lua <dataset> <arch> -a predict -net_fname N -left L -right R -disp_max D`` from the image files on:
     returns disp (H,W) float32 (numpy).  With `out_dir`, writes right.bin and left.bin ((1,D,H,W), in
     that order, main.lua:1042-1047) and disp.bin ((1,1,H,W), :1103) there.  arch 'fast' / 'slow' take the trained
@@ -206,15 +207,28 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     With `calib`, a :data:`dataio.Calib` of the pair (an addition beyond the reference, DESIGN §20), also writes depth.bin,
     the metric depth of disp ((1,1,H,W) float32, NaN = no depth, Z > `max_depth` dropped), and with `ply` points.ply, the
     point cloud coloured from the left image's bytes.  `density` (with `confidence`) keeps in both only the pixels
-    confidence.sparsify keeps."""
+    confidence.sparsify keeps.
+
+    With `rectify`, a :class:`dataio.StereoRect` of the raw cameras (DESIGN §22), the views are first rectified on the GPU
+    (rectify.rectify) and the unchanged path runs on the rectified bytes: every output lies on the rectified grid, `calib`
+    is rectify.calib (passing both is refused), the point cloud is coloured from the rectified left bytes, and the pixels
+    outside the left view's validity mask have no disparity (NaN in disp.bin and in every map made from it), so no depth and
+    no vertex either."""
     import torch
 
+    if rectify is not None:
+        if calib is not None:
+            raise ValueError("rectify defines the calibration of the rectified pair: pass rectify or calib, not both")
+        calib = rectify.calib
     if (ply or max_depth is not None or density is not None) and calib is None:
         raise ValueError("ply, max_depth and density apply to the depth outputs, which need calib")
     if density is not None and not confidence:
         raise ValueError("density ranks pixels by their confidence: it needs confidence")
     colour = None
-    if calib is not None:
+    if rectify is not None:
+        left, right = (load_bytes(v) if isinstance(v, (str, os.PathLike)) else np.asarray(v) for v in (left, right))
+        rectify.check_size(left.shape[0], left.shape[1], "rectify")
+    elif calib is not None:
         colour = load_bytes(left) if isinstance(left, (str, os.PathLike)) else np.asarray(left)
         dataio.check_calib_size(calib, colour.shape[0], colour.shape[1], "calib")
     method = StereoMethod(dataset, arch, None if features is not None else net_fname, **overrides)   # before any GPU work
@@ -223,9 +237,16 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
     if method.needs_net and arch == "slow":
         raise ValueError("arch 'slow' needs -net_fname: the scorer head's weights come with the tower's")
 
-    batch = make_batch(left, right)
     dev = torch.device("cuda", device)
-    x_batch = torch.from_numpy(batch).to(dev)
+    valid = None
+    if rectify is not None:
+        from .rectify import rectify as rectify_pair
+
+        left, right, valid = rectify_pair(left, right, rectify, dev)
+        colour = left
+        x_batch = make_batch_cuda(left, right, dev)
+    else:
+        x_batch = torch.from_numpy(make_batch(left, right)).to(dev)
     try:
         with torch.cuda.device(dev):
             tower, head = (None, None) if method.needs_net else method.stages(dev)
@@ -239,6 +260,8 @@ def predict(left, right, dataset="kitti", arch="census", disp_max=70, features=N
             lr = torch.empty((H, W), device=dev) if confidence and method.opt.lr_check else None
             disp, volL, volR = pipeline.stereo_predict(x_batch, feats, method.opt, int(disp_max), want_vols=True, arch=arch,
                                                        head=head, conf=conf, lr=lr)
+            if valid is not None:                                               # before density and depth
+                disp = disp.masked_fill(valid.reshape(disp.shape) == 0, float("nan"))
             Z = pts = None
             if calib is not None:
                 dmap = disp.reshape(H, W) if density is None else confidence_.sparsify(disp.reshape(H, W), conf, density)

@@ -41,7 +41,7 @@ from collections import namedtuple
 
 import numpy as np
 
-from . import batch, confidence, dataio, evaluate, frontend, preprocess
+from . import batch, confidence, dataio, evaluate, frontend, preprocess, rectify
 from . import depth as depth_
 
 ACTIONS = ("test", "submit")
@@ -122,14 +122,20 @@ class PairRunner:
     """The stereo method of (dataset, arch, net) over a list of pairs, shared by every tool that predicts a sequence of
     image files: one :class:`evaluate.Evaluator` prepared at the largest (H, W, disp_max) of `shapes`, and this rank's
     pairs (``batch.shard_indices`` of `rank`, `world`) decoded one ahead in a background thread (:class:`Prefetch`).
-    :meth:`predict` gives one pair's device map; :meth:`close` releases both."""
+    :meth:`predict` gives one pair's device map; :meth:`close` releases both.
 
-    def __init__(self, files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch=True, **overrides):
+    `rects` (DESIGN §22), one :class:`dataio.StereoRect` or None per pair: a pair that has one is decoded on the host as
+    usual, rectified on the device (rectify.rectify) before make_batch_cuda, and its map is NaN outside the left view's
+    validity mask; `shapes` are then the rectified shapes the pipeline runs at."""
+
+    def __init__(self, files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch=True, rects=None,
+                 **overrides):
         self.ev = evaluate.Evaluator(dataset, arch, net_fname=net_fname, device=device, **overrides)
         self.dev = self.ev.dev
         self.disp_max = int(disp_max)
         self.pre = Prefetch(files, batch.shard_indices(len(files), rank, world), enabled=prefetch)
         self.shapes = [(H, W, self.disp_max) for H, W in shapes]
+        self.rects = rects
 
     def prepare(self):
         self.ev.prepare(self.shapes)
@@ -139,11 +145,19 @@ class PairRunner:
         import torch
 
         left, right, gt = self.pre.get(i)
+        rect = self.rects[i] if self.rects is not None else None
+        if rect is not None:
+            left, right, valid = rectify.rectify(left, right, rect, self.dev)
         x_batch = frontend.make_batch_cuda(left, right, self.dev)
-        if not conf:
-            return left, right, gt, self.ev.stereo_predict(x_batch, self.disp_max), None
-        c = torch.empty(x_batch.shape[2:], device=self.dev)
-        return left, right, gt, self.ev.stereo_predict(x_batch, self.disp_max, conf=c), c
+        c = None
+        if conf:
+            c = torch.empty(x_batch.shape[2:], device=self.dev)
+            pred = self.ev.stereo_predict(x_batch, self.disp_max, conf=c)
+        else:
+            pred = self.ev.stereo_predict(x_batch, self.disp_max)
+        if rect is not None:
+            pred = pred.masked_fill(valid == 0, float("nan"))
+        return left, right, gt, pred, c
 
     def close(self):
         self.pre.close()

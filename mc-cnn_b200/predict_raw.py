@@ -12,6 +12,12 @@ pipeline at the largest shape, the next pair's PNGs decoded while the GPU works.
 process per GPU) the frames of all drives, in drive then frame order, go round-robin over the ranks; each rank writes its
 own frames' files and rank 0 prints every frame's line in order.
 
+A drive whose name ends in ``_extract`` (KITTI's unsynced+unrectified archives, the same image layout) is read as
+unrectified (DESIGN §22): each frame is rectified on the GPU by dataio.read_rectification(date, 'kitti_raw') to S_rect_00
+before the unchanged stereo method, its outputs lie on the rectified grid with the calibration that rectification defines,
+and the pixels outside the left view's validity mask have no disparity, depth or vertex (0 in the disparity PNG).  Its
+raw images must be of size S_00 / S_01.
+
 Outputs under ``out/<drive>/``: ``disp/%010d.png`` (KITTI's PNG16, dataio.write_png16), ``depth/%010d.png``
 (dataio.write_depth_png16 of depth.depth), ``points/%010d.ply`` (depth.point_cloud coloured by the left image) and
 ``conf/%010d.bin`` (the margin confidence, (1, 1, H, W) float32 in main.lua's .bin layout).  `density` p keeps, in the
@@ -64,6 +70,7 @@ def read_list(path, data_root):
             if len(parts) != 2 or not parts[1].isdigit() or parts[0].count("/") != 1:
                 raise ValueError("%s:%d: '<date>/<drive> <frame>' expected, got %r" % (path, k, line.rstrip("\n")))
             fr = Frame(os.path.join(data_root, parts[0]), int(parts[1]))
+            check_synced([fr.drive])
             for what in (dataio.RAW_LEFT, dataio.RAW_RIGHT, dataio.RAW_SCAN):
                 p = dataio.raw_file(fr.drive, what, fr.index)
                 if not os.path.isfile(p):
@@ -78,6 +85,35 @@ def pair_files(frames):
     """[(left, right, None)] of the frames, as predict_kitti.Prefetch decodes them"""
     return [(dataio.raw_file(fr.drive, dataio.RAW_LEFT, fr.index), dataio.raw_file(fr.drive, dataio.RAW_RIGHT, fr.index), None)
             for fr in frames]
+
+
+def is_extract(drive):
+    """whether `drive` is an unrectified KITTI raw drive (its name ends in ``_extract``)"""
+    return drive_name(drive).endswith(dataio.RAW_EXTRACT)
+
+
+def check_synced(drives):
+    """refuses unrectified (``_extract``) drives where a drive is scored against its Velodyne scans"""
+    for d in drives:
+        if is_extract(d):
+            raise ValueError("%s is an unrectified (_extract) drive: its scans are text files, not synchronised with the "
+                             "cameras, so it cannot be scored against them; use the drive's _sync version" % d)
+
+
+def read_rects(frames, shapes):
+    """[dataio.StereoRect of its date, or None] per frame: the rectification of every frame of an ``_extract`` drive, each
+    date's refused when it is missing or malformed or its raw size is not the frame's"""
+    rects, out = {}, []
+    for fr, (H, W) in zip(frames, shapes):
+        if not is_extract(fr.drive):
+            out.append(None)
+            continue
+        d = date_dir(fr.drive)
+        if d not in rects:
+            rects[d] = dataio.read_rectification(d, "kitti_raw")
+        rects[d].check_size(H, W, os.path.join(d, dataio.RAW_CAM))
+        out.append(rects[d])
+    return out
 
 
 def read_calibs(frames, shapes):
@@ -137,13 +173,16 @@ def predict_raw(dataset, arch, drives, net_fname=None, out="out", disp=False, de
     frames = drive_frames(drives, every)
     files = pair_files(frames)
     shapes = predict_kitti.scan(files)
-    cals = read_calibs(frames, shapes)
+    rects = read_rects(frames, shapes)
+    synced = [k for k, r in enumerate(rects) if r is None]
+    cals = read_calibs([frames[k] for k in synced], [shapes[k] for k in synced])
+    shapes = [s if r is None else r.left.rect_size[::-1] for s, r in zip(shapes, rects)]
     check_out(out, drives)
     rank, world = _world()
     if world > 1:
         dist.barrier()                          # every rank has looked at `out` before any rank writes to it
     run = predict_kitti.PairRunner(files, shapes, dataset, arch, net_fname, disp_max, device, rank, world, prefetch,
-                                   **overrides)
+                                   rects=rects if any(rects) else None, **overrides)
 
     def path(fr, kind):
         p = out_file(out, fr, kind)
@@ -158,12 +197,14 @@ def predict_raw(dataset, arch, drives, net_fname=None, out="out", disp=False, de
                 frontend.write_bin(path(fr, "conf"), conf.reshape(1, 1, *conf.shape).cpu().numpy())
             if density is not None:
                 pred = confidence_.sparsify(pred, conf, density, 0.0)
-            cal = cals[date_dir(fr.drive)]
+            cal = cals[date_dir(fr.drive)] if rects[i] is None else rects[i].calib
             if depth:
                 dataio.write_depth_png16(depth_.depth(pred, cal).cpu().numpy(), path(fr, "depth"))
             if ply:
                 depth_.write_ply(path(fr, "points"), depth_.point_cloud(pred, cal, left))
             if disp:
+                if rects[i] is not None:                        # no disparity outside the mask: 0 in KITTI's PNG16
+                    pred = pred.nan_to_num(nan=0.0, posinf=float("inf"), neginf=float("-inf"))
                 dataio.write_png16(pred.cpu().numpy(), path(fr, "disp"))
         return torch.tensor([i])
 

@@ -237,6 +237,116 @@ def write_kitti_drive(root, date="2011_09_26", drive=1, n=3, H=40, W=150, seed=0
     return drive_dir, gts
 
 
+# An unrectified drive's rigs (DESIGN §22): raw cameras with a moderate 5-coefficient distortion and a small rectifying
+# rotation each.  'kitti': the rectified grid lies inside the larger raw image, as KITTI's S_rect_00 does; 'alpha1': P is
+# zoomed out, like OpenCV's stereoRectify with alpha = 1, so the rectified grid (the raw size) reaches past the raw image.
+# Focal lengths scale with the image: P's f = W 25/24 (200 at W = 192), K's fx, fy = Wraw 35/36, Wraw 26/27 (210, 208 at 216).
+EXTRACT_B = 0.5
+EXTRACT_D = ((-0.15, 0.04, 0.0006, -0.0004, 0.0), (-0.14, 0.035, -0.0005, 0.0003, 0.0))
+EXTRACT_ROT = ((0.004, -0.006, 0.003), (0.002, -0.004, 0.001))
+EXTRACT_RIGS = {"kitti": 1.0, "alpha1": 0.68}                   # P's focal length over W 25/24
+
+
+def _rodrigues(r):
+    r = np.asarray(r, np.float64)
+    t = np.linalg.norm(r)
+    k = r / t
+    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(t) * Kx + (1 - np.cos(t)) * Kx @ Kx
+
+
+def extract_cameras(H, W, Hraw, Wraw, rig="kitti"):
+    """[(K, D, R, P) float64 per grey camera 00, 01] of an unrectified drive whose rectified grid is H x W and raw images
+    Hraw x Wraw; P_rect_01 = P_rect_00 with P[0,3] = -f EXTRACT_B"""
+    f = W * 25 / 24 * EXTRACT_RIGS[rig]
+    P0 = np.array([[f, 0, W / 2 - 0.25, 0], [0, f, H / 2 + 0.5, 0], [0, 0, 1, 0]])
+    P1 = P0.copy()
+    P1[0, 3] = -f * EXTRACT_B
+    cams = []
+    for k, P in enumerate((P0, P1)):
+        K = np.array([[Wraw * 35 / 36, 0, Wraw / 2 - 0.5 + 0.3 * (1 - 2 * k)], [0, Wraw * 26 / 27, Hraw / 2 + 0.2], [0, 0, 1]])
+        cams.append((K, np.array(EXTRACT_D[k]), _rodrigues(EXTRACT_ROT[k]), P))
+    return cams
+
+
+def extract_calib_text(H, W, Hraw, Wraw, rig="kitti"):
+    """(calib_cam_to_cam.txt, calib_velo_to_cam.txt) of an unrectified drive's date directory: K_0i, D_0i, R_rect_0i,
+    P_rect_0i, S_0i and S_rect_0i of the grey cameras (:func:`extract_cameras`), and raw_calib_text's velodyne file"""
+    num = lambda v: " ".join("%.12e" % float(x) for x in np.asarray(v).reshape(-1))
+    cam = ["calib_time: 09-Jan-2012 13:57:47", "corner_dist: 9.950000e-02"]
+    for i, (K, D, R, P) in enumerate(extract_cameras(H, W, Hraw, Wraw, rig)):
+        k = "0%d" % i
+        cam += ["S_%s: %s" % (k, num((Wraw, Hraw))), "K_%s: %s" % (k, num(K)), "D_%s: %s" % (k, num(D)),
+                "R_%s: %s" % (k, num(np.eye(3))), "T_%s: %s" % (k, num((-EXTRACT_B * i, 0, 0))),
+                "S_rect_%s: %s" % (k, num((W, H))), "R_rect_%s: %s" % (k, num(R)), "P_rect_%s: %s" % (k, num(P))]
+    return "\n".join(cam) + "\n", raw_calib_text(H, W)[1]
+
+
+def unrectify(scene, K, D, R, P, Hraw, Wraw, iters=30):
+    """The raw (Hraw, Wraw) float image of a rectified float `scene`: each raw pixel undistorted iteratively in float64,
+    rotated by R, projected by P[:, :3] onto the rectified grid, and `scene` sampled there bilinearly (clamped edges)."""
+    v, u = np.meshgrid(np.arange(Hraw, dtype=np.float64), np.arange(Wraw, dtype=np.float64), indexing="ij")
+    k1, k2, p1, p2, k3 = D
+    xd, yd = (u - K[0, 2]) / K[0, 0], (v - K[1, 2]) / K[1, 1]
+    x, y = xd.copy(), yd.copy()
+    for _ in range(iters):
+        r2 = x * x + y * y
+        rad = 1 + r2 * (k1 + r2 * (k2 + r2 * k3))
+        x = (xd - (2 * p1 * x * y + p2 * (r2 + 2 * x * x))) / rad
+        y = (yd - (p1 * (r2 + 2 * y * y) + 2 * p2 * x * y)) / rad
+    q = np.einsum("ij,jhw->ihw", P[:, :3] @ R, np.stack([x, y, np.ones_like(x)]))
+    sx, sy = q[0] / q[2], q[1] / q[2]
+    H, W = scene.shape
+    x0 = np.clip(np.floor(sx), 0, W - 1).astype(np.int64)
+    y0 = np.clip(np.floor(sy), 0, H - 1).astype(np.int64)
+    x1, y1 = np.minimum(x0 + 1, W - 1), np.minimum(y0 + 1, H - 1)
+    a, b = np.clip(sx - np.floor(sx), 0, 1), np.clip(sy - np.floor(sy), 0, 1)
+    a = np.where((sx < 0) | (sx > W - 1), 0, a)
+    b = np.where((sy < 0) | (sy > H - 1), 0, b)
+    return (1 - b) * ((1 - a) * scene[y0, x0] + a * scene[y0, x1]) + b * ((1 - a) * scene[y1, x0] + a * scene[y1, x1])
+
+
+def write_kitti_extract_drive(root, date="2011_09_26", drive=1, n=3, H=64, W=192, Hraw=80, Wraw=216, seed=0, D=64,
+                              levels=RAW_LEVELS, rig="kitti", sync=False):
+    """A seeded unrectified KITTI raw drive under ``root/<date>/<date>_drive_<drive>_extract``: per frame a rectified scene
+    of _scene_views (H x W, left pixel x matching right pixel x - gt, gt piecewise constant over `levels`, 0 on about 10% of
+    the pixels) made raw by :func:`unrectify` with the cameras of :func:`extract_cameras` (`rig` 'kitti' or 'alpha1') and
+    written as grey bytes ``image_00/data/%010d.png`` / ``image_01/data/%010d.png`` (Hraw x Wraw), and the date directory's
+    :func:`extract_calib_text` (written once per date).  With `sync`, also ``<date>_drive_<drive>_sync`` holding the same
+    scenes' rectified bytes.  Returns (extract drive directory, [gt (H, W) float32 per frame], sync drive directory or
+    None)."""
+    import os
+
+    from PIL import Image
+
+    rng = np.random.default_rng(seed)
+    date_dir = os.path.join(root, date)
+    out = os.path.join(date_dir, "%s_drive_%04d_extract" % (date, drive))
+    sync_dir = os.path.join(date_dir, "%s_drive_%04d_sync" % (date, drive)) if sync else None
+    for d in (out, sync_dir):
+        for sub in ("image_00", "image_01"):
+            if d is not None:
+                os.makedirs(os.path.join(d, sub, "data"), exist_ok=True)
+    cam, velo = extract_calib_text(H, W, Hraw, Wraw, rig)
+    for name, text in (("calib_cam_to_cam.txt", cam), ("calib_velo_to_cam.txt", velo)):
+        if not os.path.exists(os.path.join(date_dir, name)):
+            with open(os.path.join(date_dir, name), "w") as f:
+                f.write(text)
+    cams = extract_cameras(H, W, Hraw, Wraw, rig)
+    byte = lambda a: np.clip(np.rint(a), 0, 255).astype(np.uint8)
+    gts = []
+    for k in range(n):
+        views, gt = _scene_views(rng, H, W, D, levels=levels)
+        for v, sub, (K, Dk, R, P) in zip(views, ("image_00", "image_01"), cams):
+            scene = 128.0 + 40.0 * v.astype(np.float64)
+            raw = unrectify(scene, K, Dk, R, P, Hraw, Wraw)
+            Image.fromarray(byte(raw), "L").save(os.path.join(out, sub, "data", "%010d.png" % k), format="PNG")
+            if sync_dir is not None:
+                Image.fromarray(byte(scene), "L").save(os.path.join(sync_dir, sub, "data", "%010d.png" % k), format="PNG")
+        gts.append(gt.astype(np.float32))
+    return out, gts, sync_dir
+
+
 def write_kitti_eval_maps(unzip, dataset="kitti", seed=0):
     """The ground truth the devkits' metrics read besides disp_noc, next to a write_kitti_raw tree (`unzip` is what it
     returned): ``training/disp_occ/`` (``disp_occ_0/`` for 'kitti2015') is disp_noc with its invalid pixels filled in

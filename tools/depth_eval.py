@@ -86,6 +86,13 @@ def parse_args(argv=None):
         for d in args.drive:
             if not os.path.isdir(d):
                 raise SystemExit("depth_eval.py: %s is not a directory" % d)
+        import mccnn_b200  # noqa: F401
+        from mccnn_b200.predict_raw import check_synced
+
+        try:
+            check_synced(args.drive)
+        except ValueError as e:
+            raise SystemExit("depth_eval.py: %s" % e)
         if args.raw_action == "predict":
             if args.arch in ("fast", "slow") and not args.net_fname:
                 raise SystemExit("depth_eval.py: arch '%s' needs -net_fname" % args.arch)

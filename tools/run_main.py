@@ -8,6 +8,8 @@
     python tools/run_main.py kitti fast -a test_te -net_fname N -sm_skip sgm          # or -sm_terminate cbca1, ...
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -confidence
     python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -calib calib/000000.txt -ply
+    python tools/run_main.py kitti census -a predict -left L.png -right R.png -disp_max 70 -rectify intrinsics.yml \
+        -rectify extrinsics.yml -ply
 
 Option names are main.lua's (-gpu is 1-based as there); -L1 ... -blur_t override the stereo method's preset
 (main.lua:70-295); -sm_terminate / -sm_skip stop after / leave out one step of it (main.lua:953-1082; unknown step
@@ -17,7 +19,11 @@ confidence of each pixel, and with the LR check lr.bin, main.lua:1056's outlier 
 -calib FILE (also an addition, -a predict only; KITTI 2012 calib/%06d.txt, KITTI 2015 calib_cam_to_cam/%06d.txt or a
 MiddEval3 calib.txt, by dataset) also writes depth.bin, the metric depth of each pixel in metres (NaN = none), and with -ply
 points.ply, the coloured point cloud; -max_depth M drops depths past M metres, and -density p (with -confidence) keeps only
-the ceil(p H W) most confident pixels in both (mc-cnn_b200/depth.py).  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
+the ceil(p H W) most confident pixels in both (mc-cnn_b200/depth.py).  -rectify FILE [-rectify FILE2] (also an addition,
+-a predict only, instead of -calib) takes raw views of a calibrated rig: OpenCV FileStorage YAML files holding M1/K1, D1,
+M2/K2, D2, R1, R2, P1, P2 (stereo_calib's intrinsics.yml and extrinsics.yml); the pair is rectified on the GPU first, every
+output lies on the rectified grid, the depth uses the calibration P1 / P2 define, and the pixels outside the left view's
+validity mask have no disparity (NaN), depth or vertex (mc-cnn_b200/rectify.py).  Training (-a train_tr / train_all) is not part of this tool.  See mc-cnn_b200/evaluate.py for
 what each action computes and where it deliberately differs from main.lua.
 """
 import argparse
@@ -58,6 +64,7 @@ def parser():
     ap.add_argument("-sm_skip", default="")
     ap.add_argument("-confidence", nargs="?", const=True, default=False, type=_flag)
     ap.add_argument("-calib", default="")
+    ap.add_argument("-rectify", action="append", default=[])
     ap.add_argument("-ply", nargs="?", const=True, default=False, type=_flag)
     ap.add_argument("-max_depth", type=float, default=None)
     ap.add_argument("-density", type=float, default=None)
@@ -81,8 +88,17 @@ def parse_args(argv=None):
         raise SystemExit("run_main.py: -confidence writes conf.bin next to -a predict's outputs; -a %s writes none" % args.a)
     if args.calib and args.a != "predict":
         raise SystemExit("run_main.py: -calib writes depth.bin next to -a predict's outputs; -a %s writes none" % args.a)
-    if (args.ply or args.max_depth is not None or args.density is not None) and not args.calib:
-        raise SystemExit("run_main.py: -ply, -max_depth and -density apply to the depth outputs, which need -calib")
+    if args.rectify and args.a != "predict":
+        raise SystemExit("run_main.py: -rectify rectifies -a predict's raw pair; -a %s reads no raw pair" % args.a)
+    if args.rectify and args.calib:
+        raise SystemExit("run_main.py: -rectify defines the rectified pair's calibration; give -rectify or -calib, not both")
+    if len(args.rectify) > 2:
+        raise SystemExit("run_main.py: -rectify takes one or two files (e.g. intrinsics.yml and extrinsics.yml)")
+    for f in args.rectify:
+        if not os.path.isfile(f):
+            raise SystemExit("run_main.py: -rectify %s is not a file" % f)
+    if (args.ply or args.max_depth is not None or args.density is not None) and not (args.calib or args.rectify):
+        raise SystemExit("run_main.py: -ply, -max_depth and -density apply to the depth outputs, which need -calib or -rectify")
     if args.max_depth is not None and not args.max_depth > 0:
         raise SystemExit("run_main.py: -max_depth must be > 0")
     if args.density is not None:
@@ -104,7 +120,7 @@ def parse_args(argv=None):
 def main(argv=None):
     args, overrides = parse_args(argv)
     import mccnn_b200  # noqa: F401
-    from mccnn_b200 import dataio, evaluate, frontend
+    from mccnn_b200 import dataio, evaluate, frontend, predict_kitti
 
     if args.a == "predict":
         if not (args.left and args.right and args.disp_max):
@@ -113,6 +129,10 @@ def main(argv=None):
         if args.calib:
             depth_opts = dict(calib=dataio.read_calib(args.calib, args.dataset), ply=args.ply, max_depth=args.max_depth,
                               density=args.density)
+        if args.rectify:
+            H, W = predict_kitti.scan([(args.left, args.right, None)])[0]
+            depth_opts = dict(rectify=dataio.read_rectification(args.rectify, "opencv", size=(W, H)), ply=args.ply,
+                              max_depth=args.max_depth, density=args.density)
         frontend.predict(args.left, args.right, dataset=args.dataset, arch=args.arch, disp_max=args.disp_max,
                          out_dir=".", device=args.device, net_fname=args.net_fname or None, confidence=args.confidence,
                          **depth_opts, **overrides)
