@@ -803,6 +803,42 @@ int mccnn_rectify_pair(const unsigned char *left, const unsigned char *right, in
 		       const float *params_right, int Ho, int Wo, unsigned char *out_left, unsigned char *out_right,
 		       unsigned char *valid, adcensus_stream_t stream);
 
+/* ---- posed frames fused into one world-frame voxel map (csrc/fusion.cu, fusion.py; DESIGN §23) ------------------------
+ * An addition beyond the reference.  A table of voxels of edge `voxel` metres, each holding n_pix (int64), n_frames (the
+ * frames that put a pixel in it, int64), three float64 sums of world points and three int64 sums of colour bytes.
+ * mccnn_fusion_create: an empty table on CUDA device `device`; refuses voxel not finite or <= 0 and a device that does
+ * not exist (ADCENSUS_EINVAL).  Every other call makes that device current for its duration.
+ * mccnn_fusion_add: one frame.  disp (H,W) float32 and rgb (H,W[,3]) bytes (nch 1 or 3) are DEVICE; f, cx, cy, fB, doffs
+ * and max_depth as mccnn_point_cloud_fill; pose12 the 12 HOST float64 of a row-major [R | t] taking the frame's camera
+ * point into the world, read during the call.  A pixel valid under §20's rule has the camera point (X, Y, Z) of its
+ * point-cloud vertex and the world point w_k = ((R_k0 X + R_k1 Y) + R_k2 Z) + t_k in float64, each operation rounded once;
+ * its voxel index is floor(w / voxel) (float64 division) per axis.  When each index lies in [-2^20, 2^20) its key is
+ * ((ix + 2^20) << 42) | ((iy + 2^20) << 21) | (iz + 2^20), else it counts as outside and is dropped.  Each voxel's partial
+ * starts at +0.0 and adds its pixels in row-major order; the table's sum starts at +0.0 and adds the frames' partials in
+ * the order they were added.  stats (3 DEVICE int64) receives the frame's pixels in the table, its pixels outside the key
+ * range and the table's voxel count afterwards.  One int64 is read back (the stream is synchronised) to size the table,
+ * which grows by reallocation.  Refuses NULL pointers, nch not 1 or 3, H or W < 1, a camera as mccnn_point_cloud_fill
+ * refuses, a non-finite pose entry (ADCENSUS_EINVAL) and H W nch >= 2^31 (ADCENSUS_ELIMIT), before any launch.
+ * mccnn_fusion_size: the voxel count (-1 for NULL).
+ * mccnn_fusion_count: the voxels with n_frames >= min_frames (min_frames >= 1), to count (one DEVICE int64).
+ * mccnn_fusion_fill: one 15-byte PLY vertex record per such voxel in ascending key order (records past cap are dropped):
+ * the position float32(sum / n_pix) per axis, divided in float64, and the colour (C + n_pix / 2) / n_pix per channel in
+ * integers.  Blocks count their voxels, one block scans the counts in block order (64-bit), then the fill: the same bytes
+ * on every run and GPU.
+ * mccnn_fusion_table: the table in ascending key order into DEVICE arrays of mccnn_fusion_size entries: keys, npix,
+ * nframes, and sums and colours as three planes (x, y, z / r, g, b) of that many entries each.
+ * All asynchronous on `stream` except the read-back of mccnn_fusion_add. */
+typedef struct mccnn_fusion mccnn_fusion;
+int mccnn_fusion_create(mccnn_fusion **out, double voxel, int device);
+int mccnn_fusion_add(mccnn_fusion *h, const float *disp, const unsigned char *rgb, int nch, int H, int W, float f, float cx, float cy,
+		     float fB, float doffs, float max_depth, const double *pose12, long long *stats, adcensus_stream_t stream);
+long long mccnn_fusion_size(const mccnn_fusion *h);
+int mccnn_fusion_count(const mccnn_fusion *h, int min_frames, long long *count, adcensus_stream_t stream);
+int mccnn_fusion_fill(const mccnn_fusion *h, int min_frames, unsigned char *out, long long cap, adcensus_stream_t stream);
+int mccnn_fusion_table(const mccnn_fusion *h, unsigned long long *keys, long long *npix, long long *nframes, double *sums,
+		       long long *colours, adcensus_stream_t stream);
+void mccnn_fusion_destroy(mccnn_fusion *h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,7 @@
 
 #include <algorithm>
 
+#include "camera.cuh"
 #include "common.cuh"
 
 namespace {
@@ -31,21 +32,6 @@ constexpr long CHUNK = (long)THREADS * ITEMS;    // pixels per block
 constexpr int REC = 15;                          // bytes per PLY vertex: float x, y, z, uchar r, g, b
 constexpr int SCAN_THREADS = 1024;
 constexpr unsigned FULL = 0xffffffffu;
-
-struct Cam {
-	float f, cx, cy, fB, doffs, max_depth;
-};
-
-// Z of disparity d, or false when d has no depth (not finite, d + doffs <= 0, Z > max_depth)
-__device__ __forceinline__ bool depth_of(float d, const Cam &c, float *z)
-{
-	const float s = __fadd_rn(d, c.doffs);
-	if (!(isfinite(d) && s > 0.f)) return false;
-	*z = __fdiv_rn(c.fB, s);
-	return *z <= c.max_depth;
-}
-
-__device__ __forceinline__ float lateral(int u, float c0, float z, float f) { return __fdiv_rn(__fmul_rn(__fsub_rn((float)u, c0), z), f); }
 
 __global__ void depth_kernel(const float *__restrict__ disp, long n, int W, Cam c, float *__restrict__ Z, float *__restrict__ X,
 			     float *__restrict__ Y)

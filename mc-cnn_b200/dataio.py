@@ -307,6 +307,93 @@ def raw_frames(drive_dir, velodyne=False):
     return sorted(both)
 
 
+# ---- poses of a raw drive (DESIGN §23) ------------------------------------------------------------------------------------
+
+RAW_OXTS = ("oxts", "data", "%010d.txt")
+RAW_IMU = "calib_imu_to_velo.txt"
+OXTS_FIELDS = 30
+EARTH_RADIUS = 6378137.0                 # the KITTI raw devkit's er
+
+
+def read_oxts(path):
+    """One OXTS record ``oxts/data/%010d.txt``: its 30 numbers as float64 (lat, lon, alt, roll, pitch, yaw, ...).  Refuses,
+    naming the file, a record that does not hold exactly 30 finite numbers and a latitude with |lat| >= 90."""
+    with open(path) as f:
+        text = f.read()
+    try:
+        v = [float(t) for t in text.split()]
+    except ValueError:
+        raise ValueError("%s: an OXTS record holds %d numbers, got %r" % (path, OXTS_FIELDS, text[:80])) from None
+    if len(v) != OXTS_FIELDS or not all(np.isfinite(v)):
+        raise ValueError("%s: an OXTS record holds %d finite numbers, got %d" % (path, OXTS_FIELDS, len(v)))
+    if not abs(v[0]) < 90:
+        raise ValueError("%s: latitude %r is not in (-90, 90)" % (path, v[0]))
+    return np.asarray(v, np.float64)
+
+
+def _rigid(R, T):
+    M = np.eye(4)
+    M[:3, :3] = np.asarray(R, np.float64).reshape(3, 3)
+    M[:3, 3] = T
+    return M
+
+
+def oxts_pose(rec, scale):
+    """the 4x4 IMU pose of one OXTS record (the devkit's convertOxtsToPose): Mercator t = (s er lon pi/180,
+    s er ln(tan((90 + lat) pi/360)), alt) and R = Rz(yaw) Ry(pitch) Rx(roll), s = `scale`"""
+    lat, lon, alt, rx, ry, rz = (float(x) for x in rec[:6])
+    t = (scale * EARTH_RADIUS * lon * np.pi / 180, scale * EARTH_RADIUS * np.log(np.tan((90 + lat) * np.pi / 360)), alt)
+    c, s = np.cos, np.sin
+    Rx = np.array([[1, 0, 0], [0, c(rx), -s(rx)], [0, s(rx), c(rx)]])
+    Ry = np.array([[c(ry), 0, s(ry)], [0, 1, 0], [-s(ry), 0, c(ry)]])
+    Rz = np.array([[c(rz), -s(rz), 0], [s(rz), c(rz), 0], [0, 0, 1]])
+    return _rigid(Rz @ Ry @ Rx, t)
+
+
+def camera_to_imu(date_dir):
+    """inv(T_imu->velo) inv(T_velo->cam) inv(R_rect_00), 4x4 float64: a point of the rectified left camera in the IMU frame.
+    Reads R_rect_00 (calib_cam_to_cam.txt), R and T of calib_velo_to_cam.txt and of calib_imu_to_velo.txt; refuses a
+    missing file or key, naming it."""
+    cam, velo, imu = (os.path.join(date_dir, n) for n in (RAW_CAM, RAW_VELO, RAW_IMU))
+    for p in (cam, velo, imu):
+        if not os.path.isfile(p):
+            raise FileNotFoundError("missing calibration file %s" % p)
+    e, ev, ei = _calib_entries(cam), _calib_entries(velo), _calib_entries(imu)
+    R_rect = _rigid(_numbers(cam, e, "R_rect_00", 9), (0, 0, 0))
+    velo_cam = _rigid(_numbers(velo, ev, "R", 9), _numbers(velo, ev, "T", 3))
+    imu_velo = _rigid(_numbers(imu, ei, "R", 9), _numbers(imu, ei, "T", 3))
+    return np.linalg.inv(imu_velo) @ np.linalg.inv(velo_cam) @ np.linalg.inv(R_rect)
+
+
+def raw_poses(drive_dir, frames):
+    """[4x4 float64 per frame of `frames`]: each takes a point of that frame's rectified left camera (DESIGN §20's X, Y, Z)
+    into the drive's world frame, the rectified left camera of frames[0] (so its pose is I).  C_i = T_i camera_to_imu, T_i
+    the frame's :func:`oxts_pose` with the Mercator scale cos(lat0 pi/180) of frames[0]'s latitude; W_i = inv(C_0) C_i
+    (DESIGN §23).  Refuses a missing calibration file or key and a frame without its OXTS record, naming them, before
+    reading any image."""
+    frames = list(frames)
+    if not frames:
+        raise ValueError("%s: no frames to pose" % drive_dir)
+    c2i = camera_to_imu(os.path.dirname(os.path.normpath(drive_dir)))
+    recs = []
+    for i in frames:
+        p = raw_file(drive_dir, RAW_OXTS, i)
+        if not os.path.isfile(p):
+            raise FileNotFoundError("%s: frame %010d has no OXTS record %s" % (drive_dir, i, p))
+        recs.append(read_oxts(p))
+    scale = np.cos(recs[0][0] * np.pi / 180)
+    T = [oxts_pose(r, scale) for r in recs]
+    # inv(C_0) C_i = inv(c2i) (inv(T_0) T_i) c2i, with inv(T_0) T_i = [R_0' R_i | R_0' (t_i - t_0)]: the Mercator
+    # translations (~1e6 m) are subtracted before anything else touches them
+    R0, t0 = T[0][:3, :3], T[0][:3, 3]
+    i2c = np.linalg.inv(c2i)
+    out = [np.eye(4)]
+    for t in T[1:]:
+        rel = _rigid((R0.T @ t[:3, :3]).ravel(), R0.T @ (t[:3, 3] - t0))
+        out.append(i2c @ rel @ c2i)
+    return out
+
+
 def check_calib_size(cal, H, W, path):
     """refuses a calibration whose stated image size is not (H, W): nothing is rescaled"""
     if cal.width is not None and (cal.width, cal.height) != (W, H):

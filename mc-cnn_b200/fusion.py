@@ -1,0 +1,253 @@
+"""The stereo depth of posed frames fused into one world-frame point cloud on the GPU (an addition beyond the reference;
+DESIGN §23).
+
+    fu = Fusion(voxel=0.1, device=0)
+    fu.add(disp, cal, left, pose)              # pose: 4x4 (or its top 3x4) camera-to-world, float64
+    pts = fu.cloud(min_frames=2)               # a depth.Cloud: one vertex per voxel seen by >= 2 frames
+    depth.write_ply("map.ply", pts)
+    t = fu.table()                             # numpy: keys, n_pix, n_frames, sums (n, 3), colours (n, 3)
+    fu.stats                                   # FusionStats(pixels, outside, voxels)
+    fu.close()
+
+    fuse_drive("kitti", "census", ["/data/raw/2011_09_26/2011_09_26_drive_0002_sync"], out="O", voxel=0.1)
+    # O/2011_09_26_drive_0002_sync/fused.ply, posed by the drive's OXTS records (dataio.raw_poses)
+
+A pixel contributes when §20's depth rule makes it valid (max_depth included).  Its camera point (X, Y, Z) is its
+depth.point_cloud vertex; its world point w = R (X, Y, Z) + t is computed in float64 with each operation rounded once and
+no FMA; its voxel is floor(w / voxel) per axis.  A voxel keeps n_pix, n_frames (frames that put a pixel in it), float64
+sums of w and int64 sums of the colour bytes; a frame's partial adds its pixels in row-major order from +0.0 and the table
+adds the frames' partials in the order they were added, so the result has the same bits on every run and GPU.  Points
+whose voxel index lies outside [-2^20, 2^20) on some axis are counted in stats.outside and dropped.  The cloud has one
+vertex per voxel with n_frames >= min_frames, in ascending key order: float32(sum / n_pix) and (C + n_pix // 2) // n_pix.
+"""
+import ctypes
+import math
+import os
+from collections import namedtuple
+
+import numpy as np
+import torch
+
+from . import adcensus, confidence as confidence_, dataio, depth, predict_kitti, predict_raw
+
+KEY_BITS = 21
+KEY_HALF = 1 << 20
+FUSED = "fused.ply"
+
+FusionStats = namedtuple("FusionStats", "pixels outside voxels")
+FusionStats.__doc__ = """pixels: the pixels added to the table, outside: the valid pixels dropped because their voxel lies outside the
+key range, voxels: the table's voxel count"""
+FusionTable = namedtuple("FusionTable", "keys n_pix n_frames sums colours")
+FusionTable.__doc__ = """The table in ascending key order: keys (n,) uint64, n_pix and n_frames (n,) int64, sums (n, 3) float64 of the
+world points, colours (n, 3) int64 sums of the R, G, B bytes"""
+DriveSummary = namedtuple("DriveSummary", "drive frames pixels outside voxels vertices")
+
+
+def check_voxel(voxel):
+    if not (isinstance(voxel, (int, float)) and math.isfinite(voxel) and voxel > 0):
+        raise ValueError("voxel must be a finite edge length > 0 in metres, got %r" % (voxel,))
+    return float(voxel)
+
+
+def check_min_frames(min_frames):
+    if not (isinstance(min_frames, int) and min_frames >= 1):
+        raise ValueError("min_frames must be an integer >= 1, got %r" % (min_frames,))
+    return min_frames
+
+
+def pose12(pose):
+    """the 12 float64 of a camera-to-world pose's [R | t], row-major: a 4x4 matrix whose last row is (0, 0, 0, 1), or its
+    3x4 top; refuses other shapes and non-finite entries"""
+    P = np.asarray(pose, np.float64)
+    if P.shape == (4, 4):
+        if not np.array_equal(P[3], [0.0, 0.0, 0.0, 1.0]):
+            raise ValueError("a 4x4 pose's last row must be (0, 0, 0, 1), got %s" % (P[3],))
+        P = P[:3]
+    if P.shape != (3, 4):
+        raise ValueError("a pose is 4x4 or 3x4, got %s" % (P.shape,))
+    if not np.isfinite(P).all():
+        raise ValueError("a pose must be finite")
+    return np.ascontiguousarray(P.reshape(12))
+
+
+def key_index(keys):
+    """(ix, iy, iz) int64 arrays of voxel keys"""
+    k = np.asarray(keys, np.uint64)
+    m = np.uint64((1 << KEY_BITS) - 1)
+    return tuple((((k >> np.uint64(s)) & m).astype(np.int64) - KEY_HALF) for s in (2 * KEY_BITS, KEY_BITS, 0))
+
+
+class Fusion:
+    """One world-frame voxel map on CUDA device `device` (mccnn_fusion_*): frames are added in order, the map read out as a
+    cloud or a table (module docstring)."""
+
+    def __init__(self, voxel, device=0):
+        self.voxel = check_voxel(voxel)
+        self.dev = torch.device("cuda", int(device))
+        self._h = ctypes.c_void_p()
+        with torch.cuda.device(self.dev):
+            adcensus._check(adcensus.lib().mccnn_fusion_create(ctypes.byref(self._h), self.voxel, self.dev.index),
+                            "mccnn_fusion_create")
+        self._totals = torch.zeros(2, dtype=torch.int64, device=self.dev)
+        self.frames = 0
+
+    def _handle(self):
+        if not self._h:
+            raise ValueError("the fusion map is closed")
+        return self._h
+
+    def add(self, disp, cal, left, pose, max_depth=None, conf=None, density=None):
+        """Fuse one frame: `disp` its CUDA disparity map, `cal` its dataio.Calib, `left` its decoded left image ((H, W) or
+        (H, W, 3) uint8, host or device), `pose` its camera-to-world matrix.  With `conf` and `density`, only the pixels
+        confidence.sparsify keeps."""
+        if (conf is None) != (density is None):
+            raise ValueError("conf and density go together")
+        h = self._handle()
+        P = pose12(pose)
+        name = "mccnn_fusion_add"
+        d, H, W = depth._map(disp, "disp", name)
+        if d.device != self.dev:
+            raise ValueError("%s: disp is on %s, the map on %s" % (name, d.device, self.dev))
+        rgb, nch = depth._colour(left, H, W, self.dev)
+        cap = depth._cap(max_depth)
+        stats = torch.empty(3, dtype=torch.int64, device=self.dev)
+        with torch.cuda.device(self.dev):
+            if conf is not None:
+                d = confidence_.sparsify(d, conf, density)
+            adcensus._check(adcensus.lib().mccnn_fusion_add(
+                h, d.data_ptr(), rgb.data_ptr(), nch, H, W, depth._f32(cal.f), depth._f32(cal.cx), depth._f32(cal.cy),
+                depth.fB(cal), depth._f32(cal.doffs), cap, P.ctypes.data, stats.data_ptr(), adcensus._stream(d)), name)
+            self._totals += stats[:2]
+        self.frames += 1
+
+    @property
+    def stats(self):
+        """:data:`FusionStats` of every frame added so far (one device-to-host copy)"""
+        p, o = (int(v) for v in self._totals.cpu().tolist())
+        return FusionStats(p, o, int(adcensus.lib().mccnn_fusion_size(self._handle())))
+
+    def cloud(self, min_frames=1):
+        """the :data:`depth.Cloud` of the voxels seen by at least `min_frames` frames: one int64 is read back (the count),
+        the records stay on the device"""
+        check_min_frames(min_frames)
+        h, lib = self._handle(), adcensus.lib()
+        with torch.cuda.device(self.dev):
+            s = torch.cuda.current_stream(self.dev).cuda_stream
+            count = torch.empty(1, dtype=torch.int64, device=self.dev)
+            adcensus._check(lib.mccnn_fusion_count(h, min_frames, count.data_ptr(), s), "mccnn_fusion_count")
+            n = int(count.item())
+            data = torch.empty(max(1, n) * depth.REC, dtype=torch.uint8, device=self.dev)
+            adcensus._check(lib.mccnn_fusion_fill(h, min_frames, data.data_ptr(), n, s), "mccnn_fusion_fill")
+        return depth.Cloud(data[:n * depth.REC], n)
+
+    def table(self):
+        """the :data:`FusionTable` as numpy arrays"""
+        h, lib = self._handle(), adcensus.lib()
+        n = int(lib.mccnn_fusion_size(h))
+        with torch.cuda.device(self.dev):
+            buf = torch.empty(max(1, 9 * n), dtype=torch.int64, device=self.dev)
+            p, e = buf.data_ptr(), buf.element_size()
+            adcensus._check(lib.mccnn_fusion_table(h, p, p + n * e, p + 2 * n * e, p + 3 * n * e, p + 6 * n * e,
+                                                   torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_fusion_table")
+            a = buf[:9 * n].cpu().numpy()
+        return FusionTable(a[:n].view(np.uint64).copy(), a[n:2 * n].copy(), a[2 * n:3 * n].copy(),
+                           a[3 * n:6 * n].view(np.float64).reshape(3, n).T.copy(), a[6 * n:].reshape(3, n).T.copy())
+
+    def close(self):
+        if self._h:
+            torch.cuda.synchronize(self.dev)
+            adcensus.lib().mccnn_fusion_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def fused_file(out, drive):
+    return os.path.join(out, predict_raw.drive_name(drive), FUSED)
+
+
+def check_drives(drives, out):
+    """the refusals of fuse_drive that need no GPU: _extract drives and an existing fused.ply"""
+    for d in drives:
+        if predict_raw.is_extract(d):
+            raise ValueError("%s is an unrectified (_extract) drive: its OXTS records run at their own rate, not one per "
+                             "image, so its frames cannot be posed; use the drive's _sync version" % d)
+        f = fused_file(out, d)
+        if os.path.exists(f):
+            raise ValueError("%s exists; fusion does not overwrite a map" % f)
+
+
+def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_frames=1, max_depth=None, every=1,
+               confidence=False, density=None, disp_max=predict_kitti.DISP_MAX, device=0, prefetch=True, verbose=True,
+               **overrides):
+    """The stereo method over every `every`-th frame of each `_sync` drive in `drives`, in frame order on one device, each
+    drive's frames fused into ``out/<drive>/fused.ply`` in its own world frame (dataio.raw_poses: the drive's first fused
+    frame).  Prints ``<date>/<drive> <frame>`` per frame and one summary line per drive; returns the
+    :data:`DriveSummary` list.  Everything that can be refused is refused before any GPU work."""
+    import torch.distributed as dist
+
+    if dataset not in predict_raw.DATASETS:
+        raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
+    voxel = check_voxel(voxel)
+    check_min_frames(min_frames)
+    depth._cap(max_depth)
+    if int(disp_max) < 1:
+        raise ValueError("disp_max must be at least 1, got %r" % (disp_max,))
+    if density is not None:
+        if not confidence:
+            raise ValueError("density ranks pixels by their confidence: it needs confidence")
+        confidence_.check_density(density)
+    if dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError("fusion adds the frames in order on one device; run it in one process")
+    if not drives:
+        raise ValueError("no drive given")
+    check_drives(drives, out)
+    frames = predict_raw.drive_frames(drives, every)
+    poses = {}
+    for d in drives:
+        idx = [fr.index for fr in frames if fr.drive == d]
+        poses.update(zip(((d, i) for i in idx), dataio.raw_poses(d, idx)))
+    files = predict_raw.pair_files(frames)
+    shapes = predict_kitti.scan(files)
+    cals = predict_raw.read_calibs(frames, shapes)
+    run = predict_kitti.PairRunner(files, shapes, dataset, arch, net_fname, disp_max, device, 0, 1, prefetch, **overrides)
+    out_sums = []
+    fu = None
+    try:
+        run.prepare()
+        for i, fr in enumerate(frames):
+            if fu is None:
+                fu = Fusion(voxel, run.dev.index)
+            left, _, _, pred, conf = run.predict(i, conf=confidence)
+            fu.add(pred, cals[predict_raw.date_dir(fr.drive)], left, poses[(fr.drive, fr.index)], max_depth=max_depth,
+                   conf=conf if density is not None else None, density=density)
+            if verbose:
+                print(predict_raw.frame_name(fr), flush=True)
+            if i + 1 == len(frames) or frames[i + 1].drive != fr.drive:
+                pts = fu.cloud(min_frames)
+                path = fused_file(out, fr.drive)
+                os.makedirs(os.path.dirname(path), exist_ok=True)
+                depth.write_ply(path, pts)
+                st = fu.stats
+                s = DriveSummary("%s/%s" % (os.path.basename(predict_raw.date_dir(fr.drive)), predict_raw.drive_name(fr.drive)),
+                                 fu.frames, st.pixels, st.outside, st.voxels, pts.n)
+                out_sums.append(s)
+                if verbose:
+                    print("%s: frames %d pixels %d outside %d voxels %d vertices %d" % s, flush=True)
+                fu.close()
+                fu = None
+    finally:
+        if fu is not None:
+            fu.close()
+        run.close()
+    return out_sums

@@ -601,3 +601,146 @@ def write_mb_eval_gt(unzip, seed=0):
         full = np.kron(gt, np.ones((2, 2), np.float32)) * 2 + rng.uniform(-0.9, 0.9, (2 * h, 2 * w)).astype(np.float32)
         write("trainingF", s, *holes_and_mask(np.maximum(full, 0), 0.08))
     return len(scenes)
+
+
+# A posed drive (DESIGN §23): textured planes of one static world, seen from a camera moving forward while it yaws.  The
+# world frame is the first frame's rectified left camera (x right, y down, z forward); each plane is (normal, offset):
+# n . x = offset.  Ground, a wall ahead and two side walls.
+POSED_PLANES = (((0.0, 1.0, 0.0), 1.65), ((0.0, 0.0, 1.0), 14.0), ((1.0, 0.0, 0.0), 3.5), ((1.0, 0.0, 0.0), -4.0))
+# the plane's in-plane texture axes (indices of x, y, z)
+_POSED_AXES = ((0, 2), (0, 1), (2, 1), (2, 1))
+POSED_B = 0.5
+POSED_LATLON = (49.011212804408, 8.4228850417969, 112.83)         # the first frame's GPS position (Karlsruhe)
+POSED_RPY = (0.021, -0.013, 0.61)                                 # its roll, pitch, yaw
+POSED_IMU_ROT, POSED_IMU_T = (0.012, -0.021, 0.017), (-0.8086759, 0.3195559, -0.7997231)
+POSED_R_RECT_ROT = (0.003, -0.002, 0.001)
+
+
+def _hash01(i, j, k):
+    """a value in [0, 1) per integer lattice point (i, j) of texture k"""
+    m = np.uint64(0xFFFFFFFF)
+    h = (i.astype(np.uint64) * np.uint64(73856093)) ^ (j.astype(np.uint64) * np.uint64(19349663)) ^ np.uint64(k * 83492791 + 1)
+    h &= m
+    h = ((h ^ (h >> np.uint64(13))) * np.uint64(1274126177)) & m
+    h ^= h >> np.uint64(16)
+    return h.astype(np.float64) / 4294967296.0
+
+
+def _value_noise(a, b, cell, k):
+    ga, gb = a / cell, b / cell
+    i, j = np.floor(ga), np.floor(gb)
+    fa, fb = ga - i, gb - j
+    i, j = i.astype(np.int64), j.astype(np.int64)
+    v = lambda di, dj: _hash01(i + di, j + dj, k)
+    return (1 - fb) * ((1 - fa) * v(0, 0) + fa * v(1, 0)) + fb * ((1 - fa) * v(0, 1) + fa * v(1, 1))
+
+
+def posed_texture(p, plane):
+    """the grey level in [0, 255] of world points p (..., 3) on plane `plane`: a function of world position only"""
+    a, b = p[..., _POSED_AXES[plane][0]], p[..., _POSED_AXES[plane][1]]
+    return 30.0 + 195.0 * (0.6 * _value_noise(a, b, 0.04, 2 * plane) + 0.4 * _value_noise(a, b, 0.15, 2 * plane + 1))
+
+
+def posed_camera_poses(n, step=0.4, yaw=np.radians(1.5)):
+    """[4x4 camera-to-world float64] of n frames: the first is I, each next one `step` metres ahead along its heading and
+    turned by `yaw` about the camera's vertical (y) axis"""
+    out, R, t = [], np.eye(3), np.zeros(3)
+    Ry = np.array([[np.cos(yaw), 0, np.sin(yaw)], [0, 1, 0], [-np.sin(yaw), 0, np.cos(yaw)]])
+    for _ in range(n):
+        M = np.eye(4)
+        M[:3, :3], M[:3, 3] = R, t
+        out.append(M)
+        t = t + R @ np.array([0.0, 0.0, step])
+        R = R @ Ry.T
+    return out
+
+
+def posed_render(pose, H, W, f, cx, cy, shift=0.0):
+    """(Z (H, W) camera depth of the nearest plane hit, plane id (H, W) int8, grey float) of the camera at `pose` moved by
+    `shift` metres along its own x axis (the right camera: the baseline)"""
+    v, u = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    dc = np.stack([(u - cx) / f, (v - cy) / f, np.ones_like(u)], -1)
+    R, t = pose[:3, :3], pose[:3, 3] + pose[:3, :3] @ np.array([shift, 0.0, 0.0])
+    dw = dc @ R.T
+    Z = np.full((H, W), np.inf)
+    pid = np.full((H, W), -1, np.int8)
+    for k, (nrm, off) in enumerate(POSED_PLANES):
+        nrm = np.asarray(nrm)
+        den = dw @ nrm
+        with np.errstate(divide="ignore", invalid="ignore"):
+            s = (off - nrm @ t) / den
+        hit = (s > 0) & (s < Z)
+        Z = np.where(hit, s, Z)
+        pid = np.where(hit, k, pid).astype(np.int8)
+    grey = np.zeros((H, W))
+    for k in range(len(POSED_PLANES)):
+        m = pid == k
+        grey[m] = posed_texture(t + dw[m] * Z[m][:, None], k)
+    return Z, pid, grey
+
+
+def _rpy(R):
+    """(roll, pitch, yaw) with R = Rz(yaw) Ry(pitch) Rx(roll)"""
+    return np.arctan2(R[2, 1], R[2, 2]), np.arctan2(-R[2, 0], np.hypot(R[0, 0], R[1, 0])), np.arctan2(R[1, 0], R[0, 0])
+
+
+def posed_oxts(imu_poses, lat0):
+    """[30 numbers per frame] of IMU poses (4x4, Mercator translation at the scale of latitude lat0): lat, lon, alt, roll,
+    pitch, yaw by the inverse Mercator projection, the rest velocities, accelerations and status fields"""
+    from . import dataio
+
+    s = np.cos(lat0 * np.pi / 180)
+    out = []
+    for T in imu_poses:
+        mx, my, alt = T[:3, 3]
+        lon = mx * 180 / (np.pi * s * dataio.EARTH_RADIUS)
+        lat = 360 / np.pi * np.arctan(np.exp(my / (s * dataio.EARTH_RADIUS))) - 90
+        out.append([lat, lon, alt, *_rpy(T[:3, :3])] + [0.0] * 17 + [0.05, 0.02, 4, 10, 4, 4, 0])
+    return out
+
+
+def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5)):
+    """A KITTI raw ``_sync`` drive whose frames view the static world of POSED_PLANES from known poses
+    (:func:`posed_camera_poses`): grey pairs ``image_00`` / ``image_01`` rendered by ray casting (nearest plane hit, the
+    grey level a function of the world position, so the two views agree), the date directory's calibration (f = W,
+    baseline POSED_B, a small R_rect_00, velo-to-cam RAW_VELO_R, and calib_imu_to_velo.txt with a rotation and
+    translation), and ``oxts/data/%010d.txt`` records whose poses, through dataio.raw_poses, are the camera poses.
+    Returns (drive directory, [exact disparity fB / Z (H, W) float32], [plane id (H, W) int8], [camera pose 4x4])."""
+    import os
+
+    from PIL import Image
+
+    from . import dataio
+
+    date_dir = os.path.join(root, date)
+    drive_dir = os.path.join(date_dir, "%s_drive_%04d_sync" % (date, drive))
+    for sub in ("image_00", "image_01", "oxts"):
+        os.makedirs(os.path.join(drive_dir, sub, "data"), exist_ok=True)
+    f = float(W)
+    cam, velo = raw_calib_text(H, W, f=f, B=POSED_B, R_rect=_rodrigues(POSED_R_RECT_ROT).ravel())
+    num = lambda v: " ".join(repr(float(x)) for x in np.asarray(v).reshape(-1))
+    imu = "calib_time: 25-May-2012 16:47:16\nR: %s\nT: %s\n" % (num(_rodrigues(POSED_IMU_ROT)), num(POSED_IMU_T))
+    for name, text in ((dataio.RAW_CAM, cam), (dataio.RAW_VELO, velo), (dataio.RAW_IMU, imu)):
+        if not os.path.exists(os.path.join(date_dir, name)):
+            with open(os.path.join(date_dir, name), "w") as fh:
+                fh.write(text)
+    cal = dataio.read_calib(date_dir, "kitti_raw")
+    c2i = dataio.camera_to_imu(date_dir)
+    lat0 = POSED_LATLON[0]
+    T0 = dataio.oxts_pose(np.array(POSED_LATLON + POSED_RPY), np.cos(lat0 * np.pi / 180))
+    C0 = T0 @ c2i
+    poses = posed_camera_poses(n, step, yaw)
+    fB = cal.f * cal.baseline
+    disps, pids = [], []
+    byte = lambda a: np.clip(np.rint(a), 0, 255).astype(np.uint8)
+    for k, P in enumerate(poses):
+        Z, pid, grey = posed_render(P, H, W, cal.f, cal.cx, cal.cy)
+        _, _, grey_r = posed_render(P, H, W, cal.f, cal.cx, cal.cy, shift=cal.baseline)
+        Image.fromarray(byte(grey), "L").save(os.path.join(drive_dir, "image_00", "data", "%010d.png" % k), format="PNG")
+        Image.fromarray(byte(grey_r), "L").save(os.path.join(drive_dir, "image_01", "data", "%010d.png" % k), format="PNG")
+        disps.append((fB / Z).astype(np.float32))
+        pids.append(pid)
+    for k, rec in enumerate(posed_oxts([C0 @ P @ np.linalg.inv(c2i) for P in poses], lat0)):
+        with open(os.path.join(drive_dir, "oxts", "data", "%010d.txt" % k), "w") as fh:
+            fh.write(" ".join(repr(float(x)) if isinstance(x, float) else str(x) for x in rec) + "\n")
+    return drive_dir, disps, pids, poses

@@ -1,0 +1,87 @@
+"""Fuse each KITTI raw drive's stereo depth into one world-frame point cloud, posed by the drive's OXTS records (an
+addition beyond the reference).
+
+    python tools/fuse_raw.py kitti census -drive /data/raw/2011_09_26/2011_09_26_drive_0002_sync -out O -voxel 0.1 \\
+        [-min_frames 2] [-max_depth 40] [-every k] [-confidence -density p] [-disp_max 228] [-gpu 1] [-net_fname N]
+
+Each frame of each drive is predicted with the presets of `dataset` (kitti or kitti2015), in frame order on one GPU, and
+added to the drive's voxel map (edge -voxel metres) at its pose: the frame's GPS/IMU record ``oxts/data/%010d.txt`` and the
+date directory's calib_imu_to_velo.txt, calib_velo_to_cam.txt and calib_cam_to_cam.txt.  The world frame is the rectified
+left camera of the drive's first fused frame.  ``O/<drive>/fused.ply`` gets one vertex per voxel seen by at least
+-min_frames frames: the mean of its points and of their colours.  -max_depth drops farther pixels, -density p keeps the
+ceil(p H W) most confident pixels of each map (with -confidence).  The line ``<date>/<drive> <frame>`` is printed for each
+frame, then one summary line per drive.  Refused before any GPU work: _extract drives, a missing OXTS or calibration file,
+an existing fused.ply, and running under torchrun with more than one process.  -gpu is 1-based as in main.lua.  See
+mc-cnn_b200/fusion.py.
+"""
+import argparse
+import math
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def parser():
+    ap = argparse.ArgumentParser(prog="fuse_raw.py", description=__doc__.splitlines()[0])
+    ap.add_argument("dataset", choices=("kitti", "kitti2015"))
+    ap.add_argument("arch", choices=("fast", "slow", "census", "ad"))
+    ap.add_argument("-net_fname", default="")
+    ap.add_argument("-drive", action="append", default=[], help="a drive directory <date>/<date>_drive_<nnnn>_sync; repeatable")
+    ap.add_argument("-out", default="out")
+    ap.add_argument("-voxel", type=float, required=True, help="the voxel edge in metres")
+    ap.add_argument("-min_frames", type=int, default=1, help="write the voxels seen by at least this many frames")
+    ap.add_argument("-max_depth", type=float, default=None, help="drop pixels farther than this many metres")
+    ap.add_argument("-confidence", action="store_true", help="compute each map's margin confidence (for -density)")
+    ap.add_argument("-density", type=float, default=None, help="with -confidence: keep this share of each map's pixels, in (0, 1]")
+    ap.add_argument("-every", type=int, default=1)
+    ap.add_argument("-disp_max", type=int, default=228)
+    ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    return ap
+
+
+def parse_args(argv=None):
+    """Refuses what cannot run before any file or GPU is touched."""
+    args = parser().parse_args(argv)
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise SystemExit("fuse_raw.py: fusion adds the frames in order on one GPU; run it as one process, not under torchrun")
+    if args.arch in ("fast", "slow") and not args.net_fname:
+        raise SystemExit("fuse_raw.py: arch '%s' needs -net_fname" % args.arch)
+    if not args.drive:
+        raise SystemExit("fuse_raw.py: give at least one -drive")
+    if not (math.isfinite(args.voxel) and args.voxel > 0):
+        raise SystemExit("fuse_raw.py: -voxel must be a finite length > 0 in metres")
+    if args.min_frames < 1:
+        raise SystemExit("fuse_raw.py: -min_frames must be at least 1")
+    if args.max_depth is not None and not args.max_depth > 0:
+        raise SystemExit("fuse_raw.py: -max_depth must be > 0")
+    if args.density is not None:
+        if not args.confidence:
+            raise SystemExit("fuse_raw.py: -density ranks pixels by their confidence; it needs -confidence")
+        if not 0 < args.density <= 1:
+            raise SystemExit("fuse_raw.py: -density must be in (0, 1]")
+    if args.every < 1:
+        raise SystemExit("fuse_raw.py: -every must be at least 1")
+    if args.disp_max < 1:
+        raise SystemExit("fuse_raw.py: -disp_max must be at least 1")
+    if args.gpu < 1:
+        raise SystemExit("fuse_raw.py: -gpu is 1-based")
+    for d in args.drive:
+        if not os.path.isdir(d):
+            raise SystemExit("fuse_raw.py: %s is not a directory" % d)
+    return args
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    import mccnn_b200  # noqa: F401
+    from mccnn_b200.fusion import fuse_drive
+
+    fuse_drive(args.dataset, args.arch, args.drive, net_fname=args.net_fname or None, out=args.out, voxel=args.voxel,
+               min_frames=args.min_frames, max_depth=args.max_depth, every=args.every, confidence=args.confidence,
+               density=args.density, disp_max=args.disp_max, device=args.gpu - 1)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
