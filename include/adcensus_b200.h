@@ -839,6 +839,47 @@ int mccnn_fusion_table(const mccnn_fusion *h, unsigned long long *keys, long lon
 		       long long *colours, adcensus_stream_t stream);
 void mccnn_fusion_destroy(mccnn_fusion *h);
 
+/* ---- posed frames fused into a truncated signed distance field (csrc/tsdf.cu, fusion.py; DESIGN §24) -------------------
+ * An addition beyond the reference.  A table of bricks of 8^3 voxels of edge `voxel` metres, truncation `trunc` metres.
+ * A brick's key is §23's key of its index floor(i / 8), i = floor(w / voxel) the voxel index; each voxel holds S (float64),
+ * n (the frames that updated it), nc and three colour byte sums (int32): MCCNN_TSDF_BRICK_BYTES per brick.
+ * mccnn_tsdf_create: an empty field on CUDA device `device`; refuses voxel not finite or <= 0, trunc not finite or < voxel
+ * and a device that does not exist (ADCENSUS_EINVAL), and ceil(trunc / (4 voxel)) > 64 (ADCENSUS_ELIMIT).
+ * mccnn_tsdf_add: one frame, its arguments as mccnn_fusion_add's.  With K = ceil(trunc / (4 voxel)) and s = fp32(trunc / K),
+ * each valid pixel of depth Z allocates the bricks of its ray points at z = Z + fp32(j) s (fp32), j = -K .. K, z > 0,
+ * placed as fusion places a pixel; points whose brick lies outside [-2^20, 2^20) on some axis are counted.  Then every
+ * voxel of every brick: centre c = (i + 0.5) voxel, q = R^T (c - t) in float64 (((R_0a d_0 + R_1a d_1) + R_2a d_2), d =
+ * c - t), skipped unless q_z > 0 and the pixel (floor((q_x / q_z) f + cx + 0.5), likewise y) lies in the image and has a
+ * depth Z; eta = Z - q_z; skipped when eta < -trunc; else S += min(eta, trunc) / trunc, n += 1, and when |eta| < trunc the
+ * pixel's colour bytes are added and nc += 1.  stats (2 DEVICE int64) receives the frame's valid pixels and its points
+ * outside the key range.  One int64 is read back (the stream is synchronised).  Refuses what mccnn_fusion_add refuses,
+ * and (ADCENSUS_ELIMIT) H W (2K + 1) >= 2^31 and a frame beyond the 2^23-th.
+ * mccnn_tsdf_bricks: the brick count (-1 for NULL).  mccnn_tsdf_pool_bytes: the bytes the brick pool holds (-1 for NULL).
+ * mccnn_tsdf_table: the field in ascending key order into DEVICE arrays: keys (bricks), then per voxel (brick, z, y, x):
+ * S, n, nc (bricks 512 each) and colours (bricks 512 3, r g b interleaved).
+ * mccnn_tsdf_mesh_count: the vertex and face counts (2 DEVICE int64) of the mesh of the voxels with n >= min_frames.
+ * mccnn_tsdf_mesh_fill: its 15-byte PLY vertex records (vertices past vcap dropped; vcap < 2^31) and int32 faces (3 per
+ * face, faces past fcap dropped): marching tetrahedra on the Kuhn split, DESIGN §24's order and orientation.
+ * mccnn_tsdf_render: the (H,W) DEVICE float32 depth map seen from pose12 under f, cx, cy: the first zero crossing, from
+ * positive to negative, of the trilinear field sampled at camera depths fp32(k voxel), k >= 1, up to max_depth (may be
+ * +inf); NaN where none.  The brick bounds are read back (the stream is synchronised).  Refuses min_frames < 1, H or W < 1,
+ * a bad camera or pose and, with max_depth +inf, a singular R (ADCENSUS_EINVAL).
+ * All asynchronous on `stream` except the read-backs named. */
+#define MCCNN_TSDF_BRICK_BYTES 14336
+typedef struct mccnn_tsdf mccnn_tsdf;
+int mccnn_tsdf_create(mccnn_tsdf **out, double voxel, double trunc, int device);
+int mccnn_tsdf_add(mccnn_tsdf *h, const float *disp, const unsigned char *rgb, int nch, int H, int W, float f, float cx, float cy,
+		   float fB, float doffs, float max_depth, const double *pose12, long long *stats, adcensus_stream_t stream);
+long long mccnn_tsdf_bricks(const mccnn_tsdf *h);
+long long mccnn_tsdf_pool_bytes(const mccnn_tsdf *h);
+int mccnn_tsdf_table(const mccnn_tsdf *h, unsigned long long *keys, double *S, int *n, int *nc, int *colours, adcensus_stream_t stream);
+int mccnn_tsdf_mesh_count(const mccnn_tsdf *h, int min_frames, long long *counts, adcensus_stream_t stream);
+int mccnn_tsdf_mesh_fill(const mccnn_tsdf *h, int min_frames, unsigned char *verts, long long vcap, int *faces, long long fcap,
+			 adcensus_stream_t stream);
+int mccnn_tsdf_render(const mccnn_tsdf *h, int min_frames, int H, int W, float f, float cx, float cy, float max_depth,
+		      const double *pose12, float *depth, adcensus_stream_t stream);
+void mccnn_tsdf_destroy(mccnn_tsdf *h);
+
 #ifdef __cplusplus
 }
 #endif

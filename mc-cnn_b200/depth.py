@@ -146,6 +146,50 @@ def read_ply(path):
     return rec["xyz"].copy(), rec["rgb"].copy()
 
 
+MESH_HEADER = PLY_HEADER.replace("end_header\n", "element face %d\nproperty list uchar int vertex_indices\nend_header\n")
+FACE_REC = np.dtype([("n", "u1"), ("v", "<i4", 3)])     # a face: the count 3, then three int32 vertex indices
+
+Mesh = namedtuple("Mesh", "data n faces")  # data: (n * 15,) CUDA uint8 vertex records; faces: (F, 3) CUDA int32
+
+
+def mesh_ply_bytes(nv, nf):
+    """the PLY header of a mesh of nv vertices and nf triangles"""
+    return (MESH_HEADER % (nv, nf)).encode("ascii")
+
+
+def write_mesh_ply(path, mesh):
+    """`mesh` (a :data:`Mesh`) as a binary little-endian PLY file: :func:`write_ply`'s vertex element, then ``element face``
+    with ``property list uchar int vertex_indices`` (13 bytes per triangle)"""
+    body = mesh.data.cpu().numpy() if hasattr(mesh.data, "cpu") else np.asarray(mesh.data, np.uint8)
+    faces = mesh.faces.cpu().numpy() if hasattr(mesh.faces, "cpu") else np.asarray(mesh.faces, np.int32)
+    rec = np.zeros(len(faces), FACE_REC)
+    rec["n"], rec["v"] = 3, faces.reshape(-1, 3)
+    with open(path, "wb") as f:
+        f.write(mesh_ply_bytes(mesh.n, len(faces)))
+        f.write(memoryview(np.ascontiguousarray(body)))
+        f.write(memoryview(rec))
+
+
+def read_mesh_ply(path):
+    """(xyz (n, 3) float32, rgb (n, 3) uint8, faces (F, 3) int32) of a file :func:`write_mesh_ply` wrote"""
+    with open(path, "rb") as f:
+        raw = f.read()
+    end = raw.index(b"end_header\n") + len(b"end_header\n")
+    head = raw[:end]
+    try:
+        nv = int(head.split(b"element vertex ")[1].split(b"\n")[0])
+        nf = int(head.split(b"element face ")[1].split(b"\n")[0])
+    except (IndexError, ValueError):
+        raise ValueError("%s: not a mesh of this format" % path) from None
+    if head != mesh_ply_bytes(nv, nf) or len(raw) != end + REC * nv + FACE_REC.itemsize * nf:
+        raise ValueError("%s: not a mesh of this format" % path)
+    rec = np.frombuffer(raw, np.dtype([("xyz", "<f4", 3), ("rgb", "u1", 3)]), count=nv, offset=end)
+    fr = np.frombuffer(raw, FACE_REC, count=nf, offset=end + REC * nv)
+    if nf and not (fr["n"] == 3).all():
+        raise ValueError("%s: a face is not a triangle" % path)
+    return rec["xyz"].copy(), rec["rgb"].copy(), fr["v"].astype(np.int32)
+
+
 def counts(disp, gt, cal, min_depth=MIN_DEPTH, max_depth=KITTI_MAX_DEPTH, is_depth=False):
     """(counts (NCOUNT,) int64, sums (NSUM,) float64) CUDA tensors of mccnn_depth_metrics: `disp` and the ground-truth
     disparity `gt` (0 or non-finite = none), CUDA float32 maps of one shape.  max_depth None: no cap.  With `is_depth`,

@@ -12,6 +12,14 @@ DESIGN §23).
     fuse_drive("kitti", "census", ["/data/raw/2011_09_26/2011_09_26_drive_0002_sync"], out="O", voxel=0.1)
     # O/2011_09_26_drive_0002_sync/fused.ply, posed by the drive's OXTS records (dataio.raw_poses)
 
+    ts = TSDF(voxel=0.1, trunc=None, device=0)  # a truncated signed distance field (DESIGN §24), trunc 4 voxel by default
+    ts.add(disp, cal, left, pose)               # as Fusion.add
+    m = ts.mesh(min_frames=1)                   # a depth.Mesh: vertex records and int32 faces on the device
+    depth.write_mesh_ply("map.ply", m)
+    Z = ts.render(cal, pose, H, W)              # CUDA (H, W) fp32 depth of the field seen from pose, NaN = no surface
+    ts.table(); ts.stats; ts.close()            # TSDFTable numpy arrays, TSDFStats(pixels, outside, bricks, pool_bytes)
+    fuse_drive(..., mesh=True, score=True)      # O/<drive>/mesh.ply, and each frame scored against its scan
+
 A pixel contributes when §20's depth rule makes it valid (max_depth included).  Its camera point (X, Y, Z) is its
 depth.point_cloud vertex; its world point w = R (X, Y, Z) + t is computed in float64 with each operation rounded once and
 no FMA; its voxel is floor(w / voxel) per axis.  A voxel keeps n_pix, n_frames (frames that put a pixel in it), float64
@@ -33,6 +41,9 @@ from . import adcensus, confidence as confidence_, dataio, depth, predict_kitti,
 KEY_BITS = 21
 KEY_HALF = 1 << 20
 FUSED = "fused.ply"
+MESHED = "mesh.ply"
+VOX = 512                                  # voxels per brick of the TSDF, local order (z, y, x)
+MAX_TSDF_FRAMES = 1 << 23                  # the int32 colour sums of a voxel cannot overflow up to this many frames
 
 FusionStats = namedtuple("FusionStats", "pixels outside voxels")
 FusionStats.__doc__ = """pixels: the pixels added to the table, outside: the valid pixels dropped because their voxel lies outside the
@@ -41,6 +52,13 @@ FusionTable = namedtuple("FusionTable", "keys n_pix n_frames sums colours")
 FusionTable.__doc__ = """The table in ascending key order: keys (n,) uint64, n_pix and n_frames (n,) int64, sums (n, 3) float64 of the
 world points, colours (n, 3) int64 sums of the R, G, B bytes"""
 DriveSummary = namedtuple("DriveSummary", "drive frames pixels outside voxels vertices")
+TSDFStats = namedtuple("TSDFStats", "pixels outside bricks pool_bytes")
+TSDFStats.__doc__ = """pixels: the valid pixels integrated, outside: the ray points dropped because their brick lies outside the key
+range, bricks: the table's brick count, pool_bytes: the bytes its brick pool holds"""
+TSDFTable = namedtuple("TSDFTable", "keys S n nc colours")
+TSDFTable.__doc__ = """The field in ascending brick-key order: keys (b,) uint64, then per voxel (b, 8, 8, 8) indexed (brick, z, y, x):
+S float64, n and nc int32, and colours (b, 8, 8, 8, 3) int32 sums of the R, G, B bytes"""
+MeshSummary = namedtuple("MeshSummary", "drive frames pixels outside bricks vertices faces scores")
 
 
 def check_voxel(voxel):
@@ -53,6 +71,16 @@ def check_min_frames(min_frames):
     if not (isinstance(min_frames, int) and min_frames >= 1):
         raise ValueError("min_frames must be an integer >= 1, got %r" % (min_frames,))
     return min_frames
+
+
+def check_trunc(trunc, voxel):
+    """the truncation in metres: 4 voxel when None, else finite, >= voxel and at most 256 voxel (2K + 1 <= 129 ray points
+    per pixel)"""
+    if trunc is None:
+        return 4.0 * voxel
+    if not (isinstance(trunc, (int, float)) and math.isfinite(trunc) and voxel <= trunc <= 256 * voxel):
+        raise ValueError("trunc must be a finite length in [voxel, 256 voxel] (voxel %r) in metres, got %r" % (voxel, trunc))
+    return float(trunc)
 
 
 def pose12(pose):
@@ -172,29 +200,155 @@ class Fusion:
             pass
 
 
-def fused_file(out, drive):
-    return os.path.join(out, predict_raw.drive_name(drive), FUSED)
+class TSDF:
+    """One truncated signed distance field on CUDA device `device` (mccnn_tsdf_*, DESIGN §24): frames are added in order at
+    their poses; the field is read out as a mesh, a depth map seen from any pose, or a table."""
+
+    def __init__(self, voxel, trunc=None, device=0):
+        self.voxel = check_voxel(voxel)
+        self.trunc = check_trunc(trunc, self.voxel)
+        self.dev = torch.device("cuda", int(device))
+        self._h = ctypes.c_void_p()
+        with torch.cuda.device(self.dev):
+            adcensus._check(adcensus.lib().mccnn_tsdf_create(ctypes.byref(self._h), self.voxel, self.trunc, self.dev.index),
+                            "mccnn_tsdf_create")
+        self._totals = torch.zeros(2, dtype=torch.int64, device=self.dev)
+        self.frames = 0
+
+    def _handle(self):
+        if not self._h:
+            raise ValueError("the TSDF is closed")
+        return self._h
+
+    def add(self, disp, cal, left, pose, max_depth=None, conf=None, density=None):
+        """Integrate one frame; the arguments are :meth:`Fusion.add`'s."""
+        if (conf is None) != (density is None):
+            raise ValueError("conf and density go together")
+        h = self._handle()
+        if self.frames >= MAX_TSDF_FRAMES:
+            raise ValueError("a TSDF takes at most 2^23 frames")
+        P = pose12(pose)
+        name = "mccnn_tsdf_add"
+        d, H, W = depth._map(disp, "disp", name)
+        if d.device != self.dev:
+            raise ValueError("%s: disp is on %s, the field on %s" % (name, d.device, self.dev))
+        rgb, nch = depth._colour(left, H, W, self.dev)
+        cap = depth._cap(max_depth)
+        stats = torch.empty(2, dtype=torch.int64, device=self.dev)
+        with torch.cuda.device(self.dev):
+            if conf is not None:
+                d = confidence_.sparsify(d, conf, density)
+            adcensus._check(adcensus.lib().mccnn_tsdf_add(
+                h, d.data_ptr(), rgb.data_ptr(), nch, H, W, depth._f32(cal.f), depth._f32(cal.cx), depth._f32(cal.cy),
+                depth.fB(cal), depth._f32(cal.doffs), cap, P.ctypes.data, stats.data_ptr(), adcensus._stream(d)), name)
+            self._totals += stats
+        self.frames += 1
+
+    @property
+    def stats(self):
+        """:data:`TSDFStats` of every frame added so far (one device-to-host copy)"""
+        h, lib = self._handle(), adcensus.lib()
+        p, o = (int(v) for v in self._totals.cpu().tolist())
+        return TSDFStats(p, o, int(lib.mccnn_tsdf_bricks(h)), int(lib.mccnn_tsdf_pool_bytes(h)))
+
+    def mesh(self, min_frames=1):
+        """the :data:`depth.Mesh` of the voxels seen by at least `min_frames` frames: two int64 are read back (the counts),
+        the vertex records and faces stay on the device"""
+        check_min_frames(min_frames)
+        h, lib = self._handle(), adcensus.lib()
+        with torch.cuda.device(self.dev):
+            s = torch.cuda.current_stream(self.dev).cuda_stream
+            counts = torch.empty(2, dtype=torch.int64, device=self.dev)
+            adcensus._check(lib.mccnn_tsdf_mesh_count(h, min_frames, counts.data_ptr(), s), "mccnn_tsdf_mesh_count")
+            nv, nf = (int(v) for v in counts.cpu().tolist())
+            if nv >= 1 << 31:
+                raise ValueError("the mesh has %d vertices; int32 faces index fewer than 2^31" % nv)
+            data = torch.empty(max(1, nv) * depth.REC, dtype=torch.uint8, device=self.dev)
+            faces = torch.empty((max(1, nf), 3), dtype=torch.int32, device=self.dev)
+            adcensus._check(lib.mccnn_tsdf_mesh_fill(h, min_frames, data.data_ptr(), nv, faces.data_ptr(), nf, s),
+                            "mccnn_tsdf_mesh_fill")
+        return depth.Mesh(data[:nv * depth.REC], nv, faces[:nf])
+
+    def render(self, cal, pose, H, W, min_frames=1, max_depth=None):
+        """the CUDA (H, W) float32 depth map of the field seen from camera-to-world `pose` under `cal`'s f, cx, cy: each
+        pixel's first zero crossing from positive to negative, NaN where none"""
+        check_min_frames(min_frames)
+        h = self._handle()
+        P = pose12(pose)
+        if not (int(H) >= 1 and int(W) >= 1):
+            raise ValueError("H and W must be >= 1, got %r, %r" % (H, W))
+        Z = torch.empty((int(H), int(W)), dtype=torch.float32, device=self.dev)
+        with torch.cuda.device(self.dev):
+            adcensus._check(adcensus.lib().mccnn_tsdf_render(
+                h, min_frames, int(H), int(W), depth._f32(cal.f), depth._f32(cal.cx), depth._f32(cal.cy),
+                depth._cap(max_depth), P.ctypes.data, Z.data_ptr(), torch.cuda.current_stream(self.dev).cuda_stream),
+                "mccnn_tsdf_render")
+        return Z
+
+    def table(self):
+        """the :data:`TSDFTable` as numpy arrays"""
+        h, lib = self._handle(), adcensus.lib()
+        b = int(lib.mccnn_tsdf_bricks(h))
+        with torch.cuda.device(self.dev):
+            keys = torch.empty(max(1, b), dtype=torch.int64, device=self.dev)
+            S = torch.empty(max(1, b * VOX), dtype=torch.float64, device=self.dev)
+            n, nc = (torch.empty(max(1, b * VOX), dtype=torch.int32, device=self.dev) for _ in range(2))
+            col = torch.empty(max(1, 3 * b * VOX), dtype=torch.int32, device=self.dev)
+            adcensus._check(lib.mccnn_tsdf_table(h, keys.data_ptr(), S.data_ptr(), n.data_ptr(), nc.data_ptr(), col.data_ptr(),
+                                                 torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_tsdf_table")
+            get = lambda t, m: t[:m].cpu().numpy()
+            return TSDFTable(get(keys, b).view(np.uint64).copy(), get(S, b * VOX).reshape(b, 8, 8, 8),
+                             get(n, b * VOX).reshape(b, 8, 8, 8), get(nc, b * VOX).reshape(b, 8, 8, 8),
+                             get(col, 3 * b * VOX).reshape(b, 8, 8, 8, 3))
+
+    def close(self):
+        if self._h:
+            torch.cuda.synchronize(self.dev)
+            adcensus.lib().mccnn_tsdf_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
-def check_drives(drives, out):
-    """the refusals of fuse_drive that need no GPU: _extract drives and an existing fused.ply"""
+def fused_file(out, drive, mesh=False):
+    return os.path.join(out, predict_raw.drive_name(drive), MESHED if mesh else FUSED)
+
+
+def check_drives(drives, out, mesh=False):
+    """the refusals of fuse_drive that need no GPU: _extract drives and an existing fused.ply (mesh.ply with `mesh`)"""
     for d in drives:
         if predict_raw.is_extract(d):
             raise ValueError("%s is an unrectified (_extract) drive: its OXTS records run at their own rate, not one per "
                              "image, so its frames cannot be posed; use the drive's _sync version" % d)
-        f = fused_file(out, d)
+        f = fused_file(out, d, mesh)
         if os.path.exists(f):
             raise ValueError("%s exists; fusion does not overwrite a map" % f)
 
 
 def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_frames=1, max_depth=None, every=1,
                confidence=False, density=None, disp_max=predict_kitti.DISP_MAX, device=0, prefetch=True, verbose=True,
-               **overrides):
+               mesh=False, trunc=None, score=False, crop="none", min_depth=depth.MIN_DEPTH, **overrides):
     """The stereo method over every `every`-th frame of each `_sync` drive in `drives`, in frame order on one device, each
     drive's frames fused into ``out/<drive>/fused.ply`` in its own world frame (dataio.raw_poses: the drive's first fused
     frame).  Prints ``<date>/<drive> <frame>`` per frame and one summary line per drive; returns the
-    :data:`DriveSummary` list.  Everything that can be refused is refused before any GPU work."""
+    :data:`DriveSummary` list.  With `mesh`, the frames go into a :class:`TSDF` of truncation `trunc` instead, and
+    ``out/<drive>/mesh.ply`` gets its mesh (a :data:`MeshSummary` per drive); with `score` as well, each frame's stereo
+    depth and the field rendered at its pose are scored against its projected scan (depth_eval.lidar_gt, `crop`,
+    `min_depth`, max_depth 80 m): one line per frame, the stereo then the fused lidar_* values, then the line of means.
+    Everything that can be refused is refused before any GPU work."""
     import torch.distributed as dist
+
+    from . import depth_eval
 
     if dataset not in predict_raw.DATASETS:
         raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
@@ -207,12 +361,18 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
         if not confidence:
             raise ValueError("density ranks pixels by their confidence: it needs confidence")
         confidence_.check_density(density)
+    if not mesh and (trunc is not None or score):
+        raise ValueError("trunc and score apply to the distance field: they need mesh")
+    if mesh:
+        trunc = check_trunc(trunc, voxel)
+    if score:
+        depth_eval._check_raw(min_depth, depth.KITTI_MAX_DEPTH, crop)
     if dist.is_initialized() and dist.get_world_size() > 1:
         raise ValueError("fusion adds the frames in order on one device; run it in one process")
     if not drives:
         raise ValueError("no drive given")
-    check_drives(drives, out)
-    frames = predict_raw.drive_frames(drives, every)
+    check_drives(drives, out, mesh)
+    frames = predict_raw.drive_frames(drives, every, velodyne=score)
     poses = {}
     for d in drives:
         idx = [fr.index for fr in frames if fr.drive == d]
@@ -221,29 +381,53 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
     shapes = predict_kitti.scan(files)
     cals = predict_raw.read_calibs(frames, shapes)
     run = predict_kitti.PairRunner(files, shapes, dataset, arch, net_fname, disp_max, device, 0, 1, prefetch, **overrides)
+
+    def gt_of(i):
+        fr = frames[i]
+        return depth_eval.lidar_gt(dataio.read_velodyne(dataio.raw_file(fr.drive, dataio.RAW_SCAN, fr.index)),
+                                   cals[predict_raw.date_dir(fr.drive)], *shapes[i], run.dev, min_depth, crop)
+
     out_sums = []
     fu = None
+    stereo = []                            # the drive's per-frame stereo counts (score)
     try:
         run.prepare()
         for i, fr in enumerate(frames):
             if fu is None:
-                fu = Fusion(voxel, run.dev.index)
+                fu = TSDF(voxel, trunc, run.dev.index) if mesh else Fusion(voxel, run.dev.index)
+                first = i
+            cal = cals[predict_raw.date_dir(fr.drive)]
             left, _, _, pred, conf = run.predict(i, conf=confidence)
-            fu.add(pred, cals[predict_raw.date_dir(fr.drive)], left, poses[(fr.drive, fr.index)], max_depth=max_depth,
+            fu.add(pred, cal, left, poses[(fr.drive, fr.index)], max_depth=max_depth,
                    conf=conf if density is not None else None, density=density)
+            if score:
+                with torch.cuda.device(run.dev):
+                    stereo.append(depth.counts(pred, gt_of(i), cal, min_depth, depth.KITTI_MAX_DEPTH))
             if verbose:
                 print(predict_raw.frame_name(fr), flush=True)
             if i + 1 == len(frames) or frames[i + 1].drive != fr.drive:
-                pts = fu.cloud(min_frames)
-                path = fused_file(out, fr.drive)
+                name = "%s/%s" % (os.path.basename(predict_raw.date_dir(fr.drive)), predict_raw.drive_name(fr.drive))
+                path = fused_file(out, fr.drive, mesh)
                 os.makedirs(os.path.dirname(path), exist_ok=True)
-                depth.write_ply(path, pts)
-                st = fu.stats
-                s = DriveSummary("%s/%s" % (os.path.basename(predict_raw.date_dir(fr.drive)), predict_raw.drive_name(fr.drive)),
-                                 fu.frames, st.pixels, st.outside, st.voxels, pts.n)
+                if mesh:
+                    m = fu.mesh(min_frames)
+                    depth.write_mesh_ply(path, m)
+                    st = fu.stats
+                    s = MeshSummary(name, fu.frames, st.pixels, st.outside, st.bricks, m.n, int(m.faces.shape[0]), None)
+                    if verbose:
+                        print("%s: frames %d pixels %d outside %d bricks %d vertices %d faces %d" % s[:7], flush=True)
+                    if score:
+                        s = s._replace(scores=_score_drive(fu, frames[first:i + 1], first, cals, shapes, poses, stereo, gt_of,
+                                                           min_frames, max_depth, min_depth, verbose))
+                else:
+                    pts = fu.cloud(min_frames)
+                    depth.write_ply(path, pts)
+                    st = fu.stats
+                    s = DriveSummary(name, fu.frames, st.pixels, st.outside, st.voxels, pts.n)
+                    if verbose:
+                        print("%s: frames %d pixels %d outside %d voxels %d vertices %d" % s, flush=True)
                 out_sums.append(s)
-                if verbose:
-                    print("%s: frames %d pixels %d outside %d voxels %d vertices %d" % s, flush=True)
+                stereo = []
                 fu.close()
                 fu = None
     finally:
@@ -251,3 +435,29 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
             fu.close()
         run.close()
     return out_sums
+
+
+def _score_drive(ts, frames, first, cals, shapes, poses, stereo, gt_of, min_frames, max_depth, min_depth, verbose):
+    """each frame's stereo counts and the field rendered at its pose, scored against its scan: one depth_eval line per
+    frame (the stereo then the fused lidar_* values) and the line of means; returns depth_eval.Scores"""
+    from . import depth_eval
+
+    names, rows = [], []
+    for k, fr in enumerate(frames):
+        cal = cals[predict_raw.date_dir(fr.drive)]
+        H, W = shapes[first + k]
+        with torch.cuda.device(ts.dev):
+            Z = ts.render(cal, poses[(fr.drive, fr.index)], H, W, min_frames, max_depth)
+            c, s = depth.counts(Z, gt_of(first + k), cal, min_depth, depth.KITTI_MAX_DEPTH, is_depth=True)
+            row = list(depth.metrics_of(*(t.cpu() for t in stereo[k]))) + list(depth.metrics_of(c.cpu(), s.cpu()))
+        names.append(predict_raw.frame_name(fr))
+        rows.append(row)
+        if verbose:
+            print(depth_eval.line(names[-1], row), flush=True)
+    mean = [sum(r[j] for r in rows) / len(rows) for j in range(len(SCORE_COLUMNS))]
+    if verbose:
+        print(depth_eval.line("mean", mean), flush=True)
+    return depth_eval.Scores(names, rows, mean)
+
+
+SCORE_COLUMNS = ["stereo_lidar_%s" % m for m in depth.METRICS] + ["fused_lidar_%s" % m for m in depth.METRICS]

@@ -699,13 +699,27 @@ def posed_oxts(imu_poses, lat0):
     return out
 
 
-def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5)):
+def posed_scan(pose, H, W, cal, every=2):
+    """(N, 4) float32 velodyne scan of the planes seen from the camera at `pose`: one point per `every`-th pixel in each
+    direction, on the plane hit along the ray of image coordinate u + 1 (DESIGN §21's projection puts it on pixel u), taken
+    through R_rect_00 and RAW_VELO_R into the velodyne frame; reflectance 0.5"""
+    cx, cy = cal.cx - 1.0, cal.cy - 1.0
+    Z = posed_render(pose, H, W, cal.f, cx, cy)[0][::every, ::every]
+    v, u = np.meshgrid(np.arange(0, H, every, dtype=np.float64), np.arange(0, W, every, dtype=np.float64), indexing="ij")
+    ok = np.isfinite(Z)
+    z = Z[ok]
+    p_rect = np.stack([(u[ok] - cx) * z / cal.f, (v[ok] - cy) * z / cal.f, z], 1)
+    p_velo = p_rect @ _rodrigues(POSED_R_RECT_ROT) @ np.asarray(RAW_VELO_R).reshape(3, 3)
+    return np.concatenate([p_velo, np.full((len(z), 1), 0.5)], 1).astype(np.float32)
+
+
+def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5), velodyne=False):
     """A KITTI raw ``_sync`` drive whose frames view the static world of POSED_PLANES from known poses
     (:func:`posed_camera_poses`): grey pairs ``image_00`` / ``image_01`` rendered by ray casting (nearest plane hit, the
     grey level a function of the world position, so the two views agree), the date directory's calibration (f = W,
     baseline POSED_B, a small R_rect_00, velo-to-cam RAW_VELO_R, and calib_imu_to_velo.txt with a rotation and
-    translation), and ``oxts/data/%010d.txt`` records whose poses, through dataio.raw_poses, are the camera poses.
-    Returns (drive directory, [exact disparity fB / Z (H, W) float32], [plane id (H, W) int8], [camera pose 4x4])."""
+    translation), and ``oxts/data/%010d.txt`` records whose poses, through dataio.raw_poses, are the camera poses.  With
+    `velodyne`, also ``velodyne_points/data/%010d.bin`` per frame (:func:`posed_scan`).  Returns (drive directory, [exact disparity fB / Z (H, W) float32], [plane id (H, W) int8], [camera pose 4x4])."""
     import os
 
     from PIL import Image
@@ -743,4 +757,8 @@ def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, 
     for k, rec in enumerate(posed_oxts([C0 @ P @ np.linalg.inv(c2i) for P in poses], lat0)):
         with open(os.path.join(drive_dir, "oxts", "data", "%010d.txt" % k), "w") as fh:
             fh.write(" ".join(repr(float(x)) if isinstance(x, float) else str(x) for x in rec) + "\n")
+    if velodyne:
+        os.makedirs(os.path.join(drive_dir, "velodyne_points", "data"), exist_ok=True)
+        for k, P in enumerate(poses):
+            posed_scan(P, H, W, cal).astype("<f4").tofile(os.path.join(drive_dir, "velodyne_points", "data", "%010d.bin" % k))
     return drive_dir, disps, pids, poses

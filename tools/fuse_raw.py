@@ -13,6 +13,16 @@ ceil(p H W) most confident pixels of each map (with -confidence).  The line ``<d
 frame, then one summary line per drive.  Refused before any GPU work: _extract drives, a missing OXTS or calibration file,
 an existing fused.ply, and running under torchrun with more than one process.  -gpu is 1-based as in main.lua.  See
 mc-cnn_b200/fusion.py.
+
+    python tools/fuse_raw.py kitti census -drive D -out O -voxel 0.1 -mesh [-trunc 0.4] [-score [-crop garg] [-min_depth 1]]
+
+-mesh runs the same frames into a truncated signed distance field (DESIGN §24, truncation -trunc metres, 4 -voxel by
+default, at most 256 -voxel) and writes ``O/<drive>/mesh.ply`` instead: a triangle mesh of its zero level set over the voxels seen by at least
+-min_frames frames, then one summary line per drive.  -score (with -mesh) then renders the field at each fused frame's
+pose and scores it against that frame's Velodyne scan as depth_eval.py raw does (-crop none|garg|eigen, -min_depth,
+max_depth 80 m), next to the frame's own stereo depth: one line per frame, the stereo then the fused lidar_* values, then
+the line of means.  Refused as well: -trunc not finite, below -voxel or above 256 -voxel, -trunc or -score without -mesh, an existing
+mesh.ply, and -score on a drive whose frames lack scans.
 """
 import argparse
 import math
@@ -37,6 +47,11 @@ def parser():
     ap.add_argument("-every", type=int, default=1)
     ap.add_argument("-disp_max", type=int, default=228)
     ap.add_argument("-gpu", type=int, default=1, help="1-based GPU number, as in main.lua")
+    ap.add_argument("-mesh", action="store_true", help="fuse into a truncated signed distance field and write mesh.ply")
+    ap.add_argument("-trunc", type=float, default=None, help="with -mesh: the truncation in metres (default 4 -voxel)")
+    ap.add_argument("-score", action="store_true", help="with -mesh: score the field's depth at each frame against its scan")
+    ap.add_argument("-crop", choices=("none", "garg", "eigen"), default="none", help="with -score: the crop rectangle")
+    ap.add_argument("-min_depth", type=float, default=1e-3, help="with -score: the nearest scored depth in metres")
     return ap
 
 
@@ -66,6 +81,14 @@ def parse_args(argv=None):
         raise SystemExit("fuse_raw.py: -disp_max must be at least 1")
     if args.gpu < 1:
         raise SystemExit("fuse_raw.py: -gpu is 1-based")
+    if args.trunc is not None and not args.mesh:
+        raise SystemExit("fuse_raw.py: -trunc is the distance field's truncation; it needs -mesh")
+    if args.score and not args.mesh:
+        raise SystemExit("fuse_raw.py: -score renders the distance field; it needs -mesh")
+    if args.trunc is not None and not (math.isfinite(args.trunc) and args.voxel <= args.trunc <= 256 * args.voxel):
+        raise SystemExit("fuse_raw.py: -trunc must be a finite length in metres, from -voxel to 256 -voxel")
+    if args.score and not 0 < args.min_depth <= 80.0:
+        raise SystemExit("fuse_raw.py: -min_depth must be in (0, 80]")
     for d in args.drive:
         if not os.path.isdir(d):
             raise SystemExit("fuse_raw.py: %s is not a directory" % d)
@@ -79,7 +102,9 @@ def main(argv=None):
 
     fuse_drive(args.dataset, args.arch, args.drive, net_fname=args.net_fname or None, out=args.out, voxel=args.voxel,
                min_frames=args.min_frames, max_depth=args.max_depth, every=args.every, confidence=args.confidence,
-               density=args.density, disp_max=args.disp_max, device=args.gpu - 1)
+               density=args.density, disp_max=args.disp_max, device=args.gpu - 1,
+               **(dict(mesh=True, trunc=args.trunc, score=args.score, crop=args.crop, min_depth=args.min_depth)
+                  if args.mesh else {}))
     return 0
 
 
