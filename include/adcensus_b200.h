@@ -880,6 +880,35 @@ int mccnn_tsdf_render(const mccnn_tsdf *h, int min_frames, int H, int W, float f
 		      const double *pose12, float *depth, adcensus_stream_t stream);
 void mccnn_tsdf_destroy(mccnn_tsdf *h);
 
+/* ---- frame-to-model tracking against the distance field (csrc/track.cu, track.py; DESIGN §25) ------------------------
+ * An addition beyond the reference.  A handle owns two pyramids of MCCNN_TRACK_LEVELS levels at one (H, W): the source
+ * (a frame's disparity) and the model (a depth map TSDF.render returned).  Level l keeps the full-resolution pixels
+ * (2^l x, 2^l y) and is ceil(H / 2^l) x ceil(W / 2^l); each pixel has a float64 vertex (the fp32 camera.cuh bits of §20's
+ * rule) and a float64 normal, NaN where there is none.
+ * mccnn_track_create: refuses H or W < 1 and a device that does not exist (ADCENSUS_EINVAL), H W >= 2^31 (ADCENSUS_ELIMIT).
+ * mccnn_track_source: the source pyramid of the DEVICE (H,W) disparity map under a camera as mccnn_tsdf_add takes it.
+ * mccnn_track_model: the model pyramid of the DEVICE (H,W) depth map `depth` (NaN = no vertex) under f, cx, cy; the step
+ * projects into the model with this camera.
+ * mccnn_track_step: one projective point-to-plane ICP reduce at `level` for the source-to-model pose pose12 ([R | t]):
+ * sums (28 host float64) receives the upper triangle of J^T J row by row, J^T r and r^2 over the inlier pixels, summed in
+ * DESIGN §25's fixed tree; counts (2 host int64) the inliers and the level's source vertices.  One device-to-host copy;
+ * the stream is synchronised.  Refuses (ADCENSUS_EINVAL) a level outside [0, MCCNN_TRACK_LEVELS), a non-finite pose,
+ * delta not finite or <= 0, cos_theta outside [-1, 1], NULL outputs, and a handle without both pyramids.
+ * mccnn_track_maps: a level's vertices and normals (`which` 0 source, 1 model) into two DEVICE arrays of 3 planes (x, y,
+ * z) of ceil(H / 2^l) ceil(W / 2^l) float64 each.
+ * Every argument is checked before any launch; all asynchronous on `stream` except the step's read-back. */
+#define MCCNN_TRACK_LEVELS 3
+#define MCCNN_TRACK_SUMS 28
+typedef struct mccnn_track mccnn_track;
+int mccnn_track_create(mccnn_track **out, int H, int W, int device);
+int mccnn_track_source(mccnn_track *h, const float *disp, float f, float cx, float cy, float fB, float doffs, float max_depth,
+		       adcensus_stream_t stream);
+int mccnn_track_model(mccnn_track *h, const float *depth, float f, float cx, float cy, adcensus_stream_t stream);
+int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double *sums,
+		     long long *counts, adcensus_stream_t stream);
+int mccnn_track_maps(const mccnn_track *h, int which, int level, double *vertices, double *normals, adcensus_stream_t stream);
+void mccnn_track_destroy(mccnn_track *h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libadcensus_b200.so")
-SOURCES = ["common.cu", "stereo_join.cu", "stereo_join_tma.cu", "cross_cbca.cu", "cbca_tma.cu", "sgm.cu", "post.cu", "adcensus_cost.cu", "scorer_head.cu", "feature_tower.cu", "pipeline.cu", "preprocess.cu", "preprocess_mb.cu", "frontend.cu", "train.cu", "render.cu", "kitti_eval.cu", "mb_eval.cu", "confidence.cu", "depth.cu", "rectify.cu", "fusion.cu", "tsdf.cu"]
+SOURCES = ["common.cu", "stereo_join.cu", "stereo_join_tma.cu", "cross_cbca.cu", "cbca_tma.cu", "sgm.cu", "post.cu", "adcensus_cost.cu", "scorer_head.cu", "feature_tower.cu", "pipeline.cu", "preprocess.cu", "preprocess_mb.cu", "frontend.cu", "train.cu", "render.cu", "kitti_eval.cu", "mb_eval.cu", "confidence.cu", "depth.cu", "rectify.cu", "fusion.cu", "tsdf.cu", "track.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-diag-suppress", "177", "-std=c++17", "--compiler-options", "-fPIC", "-I" + INCLUDE, "-I" + CSRC]
 

@@ -1,0 +1,372 @@
+// track.cu -- frame-to-model tracking against the distance field, for sm_90a (DESIGN §25; an addition beyond the
+// reference).
+//
+// A handle owns two three-level pyramids at one (H, W): the source (a new frame's disparity) and the model (the depth
+// TSDF.render returns at the previous pose).  Level l keeps the full-resolution pixels (2^l x, 2^l y); each level holds
+// float64 vertex and normal planes, NaN where there is none.  mccnn_track_step runs one projective point-to-plane ICP
+// reduce: each source pixel's 28 float64 terms (the upper triangle of J^T J, J^T r, r^2) are summed in a fixed tree --
+// chunks of 1024 pixels in row-major order, stride halving inside each chunk, then the same over the chunk sums padded to
+// a power of two -- so the sums have the same bits on every run and GPU and can be restated in numpy.  The inlier count is
+// an integer, summed by atomics.  One device-to-host copy per step returns the sums and the counts.
+#include <math.h>
+
+#include "camera.cuh"
+#include "keysort.cuh"
+
+namespace {
+
+constexpr int LEVELS = MCCNN_TRACK_LEVELS;
+constexpr int NS = MCCNN_TRACK_SUMS;              // 21 + 6 + 1
+constexpr int CH = 1024;                          // pixels per chunk
+constexpr int RT = 256;                           // threads per chunk: 4 pixels each
+constexpr int RED = 1024;                         // threads of the chunk-sum reduction
+
+__device__ __forceinline__ double dnan() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+struct Maps {
+	double *v[3], *n[3];                          // x, y, z planes of the vertices and the normals
+};
+
+Maps maps_at(double *base, long long np)
+{
+	Maps m;
+	for (int a = 0; a < 3; a++) {
+		m.v[a] = base + a * np;
+		m.n[a] = base + (3 + a) * np;
+	}
+	return m;
+}
+
+// a level's vertex from the full-resolution pixel (2^l x, 2^l y): of its disparity by §20's rule (source), or of the
+// rendered depth, NaN = none (model); fp32 camera.cuh bits promoted to float64.  `nvert` counts the source's vertices.
+__global__ void __launch_bounds__(256) vertex_kernel(const float *__restrict__ src, int is_depth, int W, int l, int hl, int wl,
+						     Cam c, Maps m, unsigned long long *__restrict__ nvert)
+{
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	const long long np = (long long)hl * wl;
+	bool ok = false;
+	if (i < np) {
+		const int x = (int)(i % wl) << l, y = (int)(i / wl) << l;
+		const float s = src[(long long)y * W + x];
+		float z = s;
+		ok = is_depth ? !isnan(s) : depth_of(s, c, &z);
+		m.v[0][i] = ok ? (double)lateral(x, c.cx, z, c.f) : dnan();
+		m.v[1][i] = ok ? (double)lateral(y, c.cy, z, c.f) : dnan();
+		m.v[2][i] = ok ? (double)z : dnan();
+	}
+	const int k = __syncthreads_count(ok);
+	if (nvert && threadIdx.x == 0 && k) atomicAdd(nvert, (unsigned long long)k);
+}
+
+// n = (V(x+1, y) - V(x, y)) x (V(x, y+1) - V(x, y)), normalised, flipped to face the camera; NaN when a vertex is missing
+// or |n| is 0 or not finite.  float64, each operation rounded once, no FMA.
+__global__ void __launch_bounds__(256) normal_kernel(int hl, int wl, Maps m)
+{
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= (long long)hl * wl) return;
+	const int x = (int)(i % wl), y = (int)(i / wl);
+	double n[3] = {dnan(), dnan(), dnan()};
+	if (x + 1 < wl && y + 1 < hl && !isnan(m.v[0][i]) && !isnan(m.v[0][i + 1]) && !isnan(m.v[0][i + wl])) {
+		double p[3], a[3], b[3];
+		for (int k = 0; k < 3; k++) {
+			p[k] = m.v[k][i];
+			a[k] = __dsub_rn(m.v[k][i + 1], p[k]);
+			b[k] = __dsub_rn(m.v[k][i + wl], p[k]);
+		}
+		const double c0 = __dsub_rn(__dmul_rn(a[1], b[2]), __dmul_rn(a[2], b[1]));
+		const double c1 = __dsub_rn(__dmul_rn(a[2], b[0]), __dmul_rn(a[0], b[2]));
+		const double c2 = __dsub_rn(__dmul_rn(a[0], b[1]), __dmul_rn(a[1], b[0]));
+		const double len = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(c0, c0), __dmul_rn(c1, c1)), __dmul_rn(c2, c2)));
+		if (len > 0.0 && len <= 1.7976931348623157e308) {
+			n[0] = __ddiv_rn(c0, len);
+			n[1] = __ddiv_rn(c1, len);
+			n[2] = __ddiv_rn(c2, len);
+			const double dot = __dadd_rn(__dadd_rn(__dmul_rn(n[0], p[0]), __dmul_rn(n[1], p[1])), __dmul_rn(n[2], p[2]));
+			if (dot > 0.0)
+				for (int k = 0; k < 3; k++) n[k] = -n[k];
+		}
+	}
+	for (int k = 0; k < 3; k++) m.n[k][i] = n[k];
+}
+
+struct Step {
+	int hl, wl;
+	double f, cx, cy, scale;                     // the model camera, and 2^-l
+	double d2, cos_t;                            // delta^2, cos(theta)
+};
+
+// pixel i's Jacobian row J and residual r (zero, and false, when the pixel is skipped)
+__device__ __forceinline__ bool pixel_term(long long i, const Maps &S, const Maps &M, const Pose &T, const Step &st, double *J)
+{
+	for (int k = 0; k < 7; k++) J[k] = 0.0;
+	if (i >= (long long)st.hl * st.wl) return false;
+	const double n0 = S.n[0][i];
+	if (isnan(n0)) return false;                 // no source normal (and so no source vertex)
+	double q[3], ns[3];
+	to_world(S.v[0][i], S.v[1][i], S.v[2][i], T, q);
+	const double *r = T.r;
+	for (int a = 0; a < 3; a++)
+		ns[a] = __dadd_rn(__dadd_rn(__dmul_rn(r[4 * a], n0), __dmul_rn(r[4 * a + 1], S.n[1][i])), __dmul_rn(r[4 * a + 2], S.n[2][i]));
+	if (!(q[2] > 0.0)) return false;
+	const double u = floor(__dadd_rn(__dmul_rn(__dadd_rn(__dmul_rn(__ddiv_rn(q[0], q[2]), st.f), st.cx), st.scale), 0.5));
+	const double v = floor(__dadd_rn(__dmul_rn(__dadd_rn(__dmul_rn(__ddiv_rn(q[1], q[2]), st.f), st.cy), st.scale), 0.5));
+	if (!(u >= 0.0 && u < st.wl && v >= 0.0 && v < st.hl)) return false;
+	const long long j = (long long)v * st.wl + (long long)u;
+	const double nm[3] = {M.n[0][j], M.n[1][j], M.n[2][j]};
+	if (isnan(nm[0])) return false;              // no model normal (and so no model vertex)
+	const double d[3] = {__dsub_rn(q[0], M.v[0][j]), __dsub_rn(q[1], M.v[1][j]), __dsub_rn(q[2], M.v[2][j])};
+	const double dd = __dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2]));
+	const double c = __dadd_rn(__dadd_rn(__dmul_rn(ns[0], nm[0]), __dmul_rn(ns[1], nm[1])), __dmul_rn(ns[2], nm[2]));
+	if (!(dd <= st.d2 && c >= st.cos_t)) return false;
+	J[0] = __dsub_rn(__dmul_rn(q[1], nm[2]), __dmul_rn(q[2], nm[1]));
+	J[1] = __dsub_rn(__dmul_rn(q[2], nm[0]), __dmul_rn(q[0], nm[2]));
+	J[2] = __dsub_rn(__dmul_rn(q[0], nm[1]), __dmul_rn(q[1], nm[0]));
+	J[3] = nm[0];
+	J[4] = nm[1];
+	J[5] = nm[2];
+	J[6] = __dadd_rn(__dadd_rn(__dmul_rn(nm[0], d[0]), __dmul_rn(nm[1], d[1])), __dmul_rn(nm[2], d[2]));
+	return true;
+}
+
+// the first two halvings of the four pixels' term J_a J_b (J[6] is r): (P0 + P2) + (P1 + P3), pixel p at t + 256 p
+__device__ __forceinline__ double quad(const double (*J)[7], int a, int b)
+{
+	return __dadd_rn(__dadd_rn(__dmul_rn(J[0][a], J[0][b]), __dmul_rn(J[2][a], J[2][b])),
+			 __dadd_rn(__dmul_rn(J[1][a], J[1][b]), __dmul_rn(J[3][a], J[3][b])));
+}
+
+// one block per chunk of 1024 pixels: thread t holds pixels t, t + 256, t + 512, t + 768 and takes the first two
+// halvings in registers ((a_t + a_t+512) + (a_t+256 + a_t+768)); strides 128, 64 and 32 go through shared memory and
+// 16 .. 1 through warp shuffles.  The chunk's 28 sums go to part[k P + chunk]; the inliers to *inliers.
+__global__ void __launch_bounds__(RT) step_kernel(Maps S, Maps M, Pose T, Step st, double *__restrict__ part, int P,
+						  unsigned long long *__restrict__ inliers)
+{
+	__shared__ double sh[NS * 128];
+	const long long base = (long long)blockIdx.x * CH + threadIdx.x;
+	double J[4][7];
+	int cnt = 0;
+#pragma unroll
+	for (int p = 0; p < 4; p++) cnt += pixel_term(base + p * RT, S, M, T, st, J[p]);
+	double s[NS];
+	{
+		int k = 0;
+#pragma unroll
+		for (int a = 0; a < 6; a++)
+#pragma unroll
+			for (int b = a; b < 6; b++, k++) s[k] = quad(J, a, b);
+#pragma unroll
+		for (int a = 0; a < 6; a++) s[21 + a] = quad(J, a, 6);
+		s[27] = quad(J, 6, 6);
+	}
+#pragma unroll
+	for (int stride = 128; stride >= 32; stride >>= 1) {
+		const int t = threadIdx.x;
+		if (t >= stride && t < 2 * stride)
+#pragma unroll
+			for (int k = 0; k < NS; k++) sh[k * stride + t - stride] = s[k];
+		__syncthreads();
+		if (t < stride)
+#pragma unroll
+			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], sh[k * stride + t]);
+		__syncthreads();
+	}
+	if (threadIdx.x < 32) {
+#pragma unroll
+		for (int off = 16; off >= 1; off >>= 1)
+#pragma unroll
+			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], __shfl_down_sync(0xffffffffu, s[k], off));
+		if (threadIdx.x == 0)
+#pragma unroll
+			for (int k = 0; k < NS; k++) part[(long long)k * P + blockIdx.x] = s[k];
+	}
+	const int total = __reduce_add_sync(0xffffffffu, cnt);
+	if ((threadIdx.x & 31) == 0 && total) atomicAdd(inliers, (unsigned long long)total);
+}
+
+// the chunk sums padded with +0.0 to P (a power of two), reduced by stride halving in place; out = the 28 sums, then the
+// inliers and the level's source vertices as int64
+__global__ void __launch_bounds__(RED) chunk_reduce_kernel(double *__restrict__ part, int n, int P,
+							   const unsigned long long *__restrict__ inliers,
+							   const unsigned long long *__restrict__ nvert, double *__restrict__ out)
+{
+	for (long long e = threadIdx.x; e < (long long)NS * (P - n); e += RED) part[(e / (P - n)) * P + n + e % (P - n)] = 0.0;
+	__syncthreads();
+	for (int stride = P >> 1; stride >= 1; stride >>= 1) {
+		for (long long e = threadIdx.x; e < (long long)NS * stride; e += RED) {
+			const long long k = e / stride, i = e % stride;
+			part[k * P + i] = __dadd_rn(part[k * P + i], part[k * P + i + stride]);
+		}
+		__syncthreads();
+	}
+	if (threadIdx.x < NS) out[threadIdx.x] = part[(long long)threadIdx.x * P];
+	if (threadIdx.x == 0) {
+		((long long *)out)[NS] = (long long)*inliers;
+		((long long *)out)[NS + 1] = (long long)*nvert;
+	}
+}
+
+bool camera_ok(float f, float cx, float cy) { return f > 0.f && isfinite(f) && isfinite(cx) && isfinite(cy); }
+
+}  // namespace
+
+struct mccnn_track {
+	int H, W, device;
+	int hl[LEVELS], wl[LEVELS];
+	long long off[LEVELS];                        // each level's first double in a pyramid
+	long long pyr;                                // doubles per pyramid
+	int P;                                        // chunk sums per term: the level-0 chunk count rounded up to 2^k
+	double *mem;                                  // source pyramid, model pyramid, chunk sums, out
+	unsigned long long *ctr;                      // inliers, then the source vertices per level
+	double *host;                                 // pinned: the 30 values read back per step
+	float mf, mcx, mcy;                           // the model's camera
+	bool have_source, have_model;
+};
+
+namespace {
+
+Maps level_maps(const mccnn_track *h, int which, int l)
+{
+	return maps_at(h->mem + which * h->pyr + h->off[l], (long long)h->hl[l] * h->wl[l]);
+}
+
+int build_pyramid(mccnn_track *h, int which, const float *src, const Cam &c, cudaStream_t s)
+{
+	if (which == 0) ADC_CUDA(cudaMemsetAsync(h->ctr + 1, 0, 8 * LEVELS, s));
+	for (int l = 0; l < LEVELS; l++) {
+		const long long np = (long long)h->hl[l] * h->wl[l];
+		const Maps m = level_maps(h, which, l);
+		vertex_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(src, which, h->W, l, h->hl[l], h->wl[l], c, m,
+								  which == 0 ? h->ctr + 1 + l : nullptr);
+		normal_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(h->hl[l], h->wl[l], m);
+	}
+	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mccnn_track_create(mccnn_track **out, int H, int W, int device)
+{
+	if (!out) return ADCENSUS_EINVAL;
+	*out = nullptr;
+	if (H < 1 || W < 1) return ADCENSUS_EINVAL;
+	if ((long long)H * W >= (1ll << 31)) return ADCENSUS_ELIMIT;
+	int ndev = 0;
+	ADC_CUDA(cudaGetDeviceCount(&ndev));
+	if (device < 0 || device >= ndev) return ADCENSUS_EINVAL;
+	DeviceScope dev(device);
+	if (dev.rc) return dev.rc;
+	mccnn_track *h = new mccnn_track();
+	h->H = H;
+	h->W = W;
+	h->device = device;
+	long long at = 0;
+	for (int l = 0; l < LEVELS; l++) {
+		h->hl[l] = (H + (1 << l) - 1) >> l;
+		h->wl[l] = (W + (1 << l) - 1) >> l;
+		h->off[l] = at;
+		at += 6ll * h->hl[l] * h->wl[l];
+	}
+	h->pyr = at;
+	const long long chunks = ((long long)H * W + CH - 1) / CH;
+	h->P = 1;
+	while (h->P < chunks) h->P <<= 1;
+	const size_t bytes = 8 * (size_t)(2 * h->pyr + (long long)NS * h->P + NS + 2) + 8 * (1 + LEVELS);
+	cudaError_t e = cudaMalloc(&h->mem, bytes);
+	if (e == cudaSuccess) e = cudaMallocHost(&h->host, 8 * (NS + 2));
+	if (e != cudaSuccess) {
+		if (h->mem) cudaFree(h->mem);
+		delete h;
+		return (int)e;
+	}
+	h->ctr = (unsigned long long *)(h->mem + 2 * h->pyr + (long long)NS * h->P + NS + 2);
+	*out = h;
+	return 0;
+}
+
+int mccnn_track_source(mccnn_track *h, const float *disp, float f, float cx, float cy, float fB, float doffs, float max_depth,
+		       adcensus_stream_t stream)
+{
+	if (!h || !disp || !camera_ok(f, cx, cy) || !(fB > 0.f && isfinite(fB) && isfinite(doffs) && max_depth > 0.f))
+		return ADCENSUS_EINVAL;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	const int rc = build_pyramid(h, 0, disp, Cam{f, cx, cy, fB, doffs, max_depth}, adc_stream(stream));
+	if (!rc) h->have_source = true;
+	return rc;
+}
+
+int mccnn_track_model(mccnn_track *h, const float *depth, float f, float cx, float cy, adcensus_stream_t stream)
+{
+	if (!h || !depth || !camera_ok(f, cx, cy)) return ADCENSUS_EINVAL;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	const int rc = build_pyramid(h, 1, depth, Cam{f, cx, cy, 1.f, 0.f, INFINITY}, adc_stream(stream));
+	if (!rc) {
+		h->have_model = true;
+		h->mf = f;
+		h->mcx = cx;
+		h->mcy = cy;
+	}
+	return rc;
+}
+
+int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double *sums,
+		     long long *counts, adcensus_stream_t stream)
+{
+	if (!h || !sums || !counts || level < 0 || level >= LEVELS || !h->have_source || !h->have_model) return ADCENSUS_EINVAL;
+	if (!(delta > 0.0 && isfinite(delta) && cos_theta >= -1.0 && cos_theta <= 1.0)) return ADCENSUS_EINVAL;
+	Pose T;
+	int rc = check_pose(pose12, &T);
+	if (rc) return rc;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	cudaStream_t s = adc_stream(stream);
+	const int hl = h->hl[level], wl = h->wl[level];
+	const int n = (int)(((long long)hl * wl + CH - 1) / CH);
+	int P = 1;
+	while (P < n) P <<= 1;
+	double *part = h->mem + 2 * h->pyr, *out = part + (long long)NS * h->P;
+	const Step st{hl, wl, (double)h->mf, (double)h->mcx, (double)h->mcy, ldexp(1.0, -level), delta * delta, cos_theta};
+	ADC_CUDA(cudaMemsetAsync(h->ctr, 0, 8, s));
+	step_kernel<<<n, RT, 0, s>>>(level_maps(h, 0, level), level_maps(h, 1, level), T, st, part, P, h->ctr);
+	chunk_reduce_kernel<<<1, RED, 0, s>>>(part, n, P, h->ctr, h->ctr + 1 + level, out);
+	ADC_CHECK_LAUNCH();
+	ADC_CUDA(cudaMemcpyAsync(h->host, out, 8 * (NS + 2), cudaMemcpyDeviceToHost, s));
+	ADC_CUDA(cudaStreamSynchronize(s));
+	for (int k = 0; k < NS; k++) sums[k] = h->host[k];
+	counts[0] = ((const long long *)h->host)[NS];
+	counts[1] = ((const long long *)h->host)[NS + 1];
+	return 0;
+}
+
+int mccnn_track_maps(const mccnn_track *h, int which, int level, double *vertices, double *normals, adcensus_stream_t stream)
+{
+	if (!h || !vertices || !normals || which < 0 || which > 1 || level < 0 || level >= LEVELS) return ADCENSUS_EINVAL;
+	if (!(which ? h->have_model : h->have_source)) return ADCENSUS_EINVAL;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	const size_t b = 24 * (size_t)h->hl[level] * h->wl[level];
+	const double *p = h->mem + which * h->pyr + h->off[level];
+	cudaStream_t s = adc_stream(stream);
+	ADC_CUDA(cudaMemcpyAsync(vertices, p, b, cudaMemcpyDeviceToDevice, s));
+	ADC_CUDA(cudaMemcpyAsync(normals, p + 3ll * h->hl[level] * h->wl[level], b, cudaMemcpyDeviceToDevice, s));
+	return 0;
+}
+
+void mccnn_track_destroy(mccnn_track *h)
+{
+	if (!h) return;
+	{
+		DeviceScope dev(h->device);
+		if (!dev.rc) {
+			if (h->mem) cudaFree(h->mem);
+			if (h->host) cudaFreeHost(h->host);
+		}
+	}
+	delete h;
+}
+
+}  // extern "C"

@@ -19,6 +19,7 @@ DESIGN §23).
     Z = ts.render(cal, pose, H, W)              # CUDA (H, W) fp32 depth of the field seen from pose, NaN = no surface
     ts.table(); ts.stats; ts.close()            # TSDFTable numpy arrays, TSDFStats(pixels, outside, bricks, pool_bytes)
     fuse_drive(..., mesh=True, score=True)      # O/<drive>/mesh.ply, and each frame scored against its scan
+    fuse_drive(..., mesh=True, poses="track")   # posed by tracking against the field (DESIGN §25): O/<drive>/poses.txt
 
 A pixel contributes when §20's depth rule makes it valid (max_depth included).  Its camera point (X, Y, Z) is its
 depth.point_cloud vertex; its world point w = R (X, Y, Z) + t is computed in float64 with each operation rounded once and
@@ -42,6 +43,7 @@ KEY_BITS = 21
 KEY_HALF = 1 << 20
 FUSED = "fused.ply"
 MESHED = "mesh.ply"
+POSES = "poses.txt"
 VOX = 512                                  # voxels per brick of the TSDF, local order (z, y, x)
 MAX_TSDF_FRAMES = 1 << 23                  # the int32 colour sums of a voxel cannot overflow up to this many frames
 
@@ -58,7 +60,11 @@ range, bricks: the table's brick count, pool_bytes: the bytes its brick pool hol
 TSDFTable = namedtuple("TSDFTable", "keys S n nc colours")
 TSDFTable.__doc__ = """The field in ascending brick-key order: keys (b,) uint64, then per voxel (b, 8, 8, 8) indexed (brick, z, y, x):
 S float64, n and nc int32, and colours (b, 8, 8, 8, 3) int32 sums of the R, G, B bytes"""
-MeshSummary = namedtuple("MeshSummary", "drive frames pixels outside bricks vertices faces scores")
+MeshSummary = namedtuple("MeshSummary", "drive frames pixels outside bricks vertices faces scores poses lost traj",
+                         defaults=(None, 0, None))
+MeshSummary.__doc__ = """one drive's TSDF: frames integrated, pixels, outside, bricks, mesh vertices and faces; scores (with score);
+poses (the drive's camera-to-world poses), lost (the frames tracking lost) and traj (track.TrajectoryMetrics against the
+OXTS poses, with traj) when the frames were tracked"""
 
 
 def check_voxel(voxel):
@@ -324,8 +330,13 @@ def fused_file(out, drive, mesh=False):
     return os.path.join(out, predict_raw.drive_name(drive), MESHED if mesh else FUSED)
 
 
-def check_drives(drives, out, mesh=False):
-    """the refusals of fuse_drive that need no GPU: _extract drives and an existing fused.ply (mesh.ply with `mesh`)"""
+def poses_file(out, drive):
+    return os.path.join(out, predict_raw.drive_name(drive), POSES)
+
+
+def check_drives(drives, out, mesh=False, tracked=False):
+    """the refusals of fuse_drive that need no GPU: _extract drives and an existing fused.ply (mesh.ply with `mesh`; and
+    poses.txt with `tracked`)"""
     for d in drives:
         if predict_raw.is_extract(d):
             raise ValueError("%s is an unrectified (_extract) drive: its OXTS records run at their own rate, not one per "
@@ -333,11 +344,14 @@ def check_drives(drives, out, mesh=False):
         f = fused_file(out, d, mesh)
         if os.path.exists(f):
             raise ValueError("%s exists; fusion does not overwrite a map" % f)
+        if tracked and os.path.exists(poses_file(out, d)):
+            raise ValueError("%s exists; tracking does not overwrite a trajectory" % poses_file(out, d))
 
 
 def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_frames=1, max_depth=None, every=1,
                confidence=False, density=None, disp_max=predict_kitti.DISP_MAX, device=0, prefetch=True, verbose=True,
-               mesh=False, trunc=None, score=False, crop="none", min_depth=depth.MIN_DEPTH, **overrides):
+               mesh=False, trunc=None, score=False, crop="none", min_depth=depth.MIN_DEPTH, poses="oxts", traj=False,
+               **overrides):
     """The stereo method over every `every`-th frame of each `_sync` drive in `drives`, in frame order on one device, each
     drive's frames fused into ``out/<drive>/fused.ply`` in its own world frame (dataio.raw_poses: the drive's first fused
     frame).  Prints ``<date>/<drive> <frame>`` per frame and one summary line per drive; returns the
@@ -345,10 +359,15 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
     ``out/<drive>/mesh.ply`` gets its mesh (a :data:`MeshSummary` per drive); with `score` as well, each frame's stereo
     depth and the field rendered at its pose are scored against its projected scan (depth_eval.lidar_gt, `crop`,
     `min_depth`, max_depth 80 m): one line per frame, the stereo then the fused lidar_* values, then the line of means.
-    Everything that can be refused is refused before any GPU work."""
+    `poses` 'track' or 'refine' (with `mesh`) poses each frame after a drive's first by tracking it against the field
+    rendered at the previous frame's pose (track.Tracker, DESIGN §25), predicted by constant velocity ('track', no OXTS
+    needed) or by the OXTS increment ('refine'); a lost frame is printed ``<date>/<drive> <frame> lost``, keeps its
+    prediction and is not integrated; ``out/<drive>/poses.txt`` gets the poses, and `traj` prints one line of
+    track.trajectory_metrics against the OXTS poses per drive.  Scores are taken at the tracked poses.  Everything that can
+    be refused is refused before any GPU work."""
     import torch.distributed as dist
 
-    from . import depth_eval
+    from . import depth_eval, track as track_
 
     if dataset not in predict_raw.DATASETS:
         raise ValueError("dataset must be 'kitti' or 'kitti2015', got %r" % (dataset,))
@@ -363,6 +382,13 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
         confidence_.check_density(density)
     if not mesh and (trunc is not None or score):
         raise ValueError("trunc and score apply to the distance field: they need mesh")
+    if poses not in track_.MODES:
+        raise ValueError("poses must be 'oxts', 'track' or 'refine', got %r" % (poses,))
+    tracked = poses != "oxts"
+    if tracked and not mesh:
+        raise ValueError("poses %r tracks each frame against the distance field: it needs mesh" % poses)
+    if traj and not tracked:
+        raise ValueError("traj compares tracked poses with the OXTS poses: it needs poses 'track' or 'refine'")
     if mesh:
         trunc = check_trunc(trunc, voxel)
     if score:
@@ -371,12 +397,13 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
         raise ValueError("fusion adds the frames in order on one device; run it in one process")
     if not drives:
         raise ValueError("no drive given")
-    check_drives(drives, out, mesh)
+    check_drives(drives, out, mesh, tracked)
     frames = predict_raw.drive_frames(drives, every, velodyne=score)
-    poses = {}
-    for d in drives:
-        idx = [fr.index for fr in frames if fr.drive == d]
-        poses.update(zip(((d, i) for i in idx), dataio.raw_poses(d, idx)))
+    oxts = {}
+    if poses != "track" or traj:
+        for d in drives:
+            idx = [fr.index for fr in frames if fr.drive == d]
+            oxts.update(zip(((d, i) for i in idx), dataio.raw_poses(d, idx)))
     files = predict_raw.pair_files(frames)
     shapes = predict_kitti.scan(files)
     cals = predict_raw.read_calibs(frames, shapes)
@@ -388,23 +415,43 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
                                    cals[predict_raw.date_dir(fr.drive)], *shapes[i], run.dev, min_depth, crop)
 
     out_sums = []
-    fu = None
+    fu = tracker = None
     stereo = []                            # the drive's per-frame stereo counts (score)
+    used = oxts if not tracked else {}     # each frame's pose
     try:
         run.prepare()
         for i, fr in enumerate(frames):
             if fu is None:
                 fu = TSDF(voxel, trunc, run.dev.index) if mesh else Fusion(voxel, run.dev.index)
                 first = i
+                est, lost = [], []
             cal = cals[predict_raw.date_dir(fr.drive)]
             left, _, _, pred, conf = run.predict(i, conf=confidence)
-            fu.add(pred, cal, left, poses[(fr.drive, fr.index)], max_depth=max_depth,
-                   conf=conf if density is not None else None, density=density)
+            is_lost = False
+            if tracked:
+                if i == first:
+                    pose = np.eye(4)
+                else:
+                    H, W = (int(v) for v in shapes[i])
+                    if tracker is None or (tracker.H, tracker.W) != (H, W):
+                        if tracker is not None:
+                            tracker.close()
+                        tracker = track_.Tracker(H, W, run.dev.index)
+                    Z = fu.render(cal, est[-1], H, W, 1, max_depth)
+                    O = [oxts[(fr.drive, f.index)] for f in frames[first:i + 1]] if poses == "refine" else None
+                    pose, _, is_lost = tracker.track(pred, cal, Z, est[-1], track_.predict(poses, est, O), max_depth)
+                est.append(pose)
+                used[(fr.drive, fr.index)] = pose
+                if is_lost:
+                    lost.append(fr.index)
+            if not is_lost:
+                fu.add(pred, cal, left, used[(fr.drive, fr.index)], max_depth=max_depth,
+                       conf=conf if density is not None else None, density=density)
             if score:
                 with torch.cuda.device(run.dev):
                     stereo.append(depth.counts(pred, gt_of(i), cal, min_depth, depth.KITTI_MAX_DEPTH))
             if verbose:
-                print(predict_raw.frame_name(fr), flush=True)
+                print(predict_raw.frame_name(fr) + (" lost" if is_lost else ""), flush=True)
             if i + 1 == len(frames) or frames[i + 1].drive != fr.drive:
                 name = "%s/%s" % (os.path.basename(predict_raw.date_dir(fr.drive)), predict_raw.drive_name(fr.drive))
                 path = fused_file(out, fr.drive, mesh)
@@ -416,8 +463,16 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
                     s = MeshSummary(name, fu.frames, st.pixels, st.outside, st.bricks, m.n, int(m.faces.shape[0]), None)
                     if verbose:
                         print("%s: frames %d pixels %d outside %d bricks %d vertices %d faces %d" % s[:7], flush=True)
+                    if tracked:
+                        track_.write_poses(poses_file(out, fr.drive), est)
+                        s = s._replace(poses=est, lost=len(lost))
+                        if traj:
+                            s = s._replace(traj=track_.trajectory_metrics(
+                                est, [oxts[(fr.drive, f.index)] for f in frames[first:i + 1]]))
+                            if verbose:
+                                print(track_.metrics_line(name, s.traj), flush=True)
                     if score:
-                        s = s._replace(scores=_score_drive(fu, frames[first:i + 1], first, cals, shapes, poses, stereo, gt_of,
+                        s = s._replace(scores=_score_drive(fu, frames[first:i + 1], first, cals, shapes, used, stereo, gt_of,
                                                            min_frames, max_depth, min_depth, verbose))
                 else:
                     pts = fu.cloud(min_frames)
@@ -433,6 +488,8 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
     finally:
         if fu is not None:
             fu.close()
+        if tracker is not None:
+            tracker.close()
         run.close()
     return out_sums
 

@@ -713,13 +713,15 @@ def posed_scan(pose, H, W, cal, every=2):
     return np.concatenate([p_velo, np.full((len(z), 1), 0.5)], 1).astype(np.float32)
 
 
-def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5), velodyne=False):
+def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5), velodyne=False,
+                            no_oxts=False):
     """A KITTI raw ``_sync`` drive whose frames view the static world of POSED_PLANES from known poses
     (:func:`posed_camera_poses`): grey pairs ``image_00`` / ``image_01`` rendered by ray casting (nearest plane hit, the
     grey level a function of the world position, so the two views agree), the date directory's calibration (f = W,
     baseline POSED_B, a small R_rect_00, velo-to-cam RAW_VELO_R, and calib_imu_to_velo.txt with a rotation and
     translation), and ``oxts/data/%010d.txt`` records whose poses, through dataio.raw_poses, are the camera poses.  With
-    `velodyne`, also ``velodyne_points/data/%010d.bin`` per frame (:func:`posed_scan`).  Returns (drive directory, [exact disparity fB / Z (H, W) float32], [plane id (H, W) int8], [camera pose 4x4])."""
+    `velodyne`, also ``velodyne_points/data/%010d.bin`` per frame (:func:`posed_scan`).  With `no_oxts`, no ``oxts/``
+    directory (a drive only tracking can pose).  Returns (drive directory, [exact disparity fB / Z (H, W) float32], [plane id (H, W) int8], [camera pose 4x4])."""
     import os
 
     from PIL import Image
@@ -728,7 +730,7 @@ def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, 
 
     date_dir = os.path.join(root, date)
     drive_dir = os.path.join(date_dir, "%s_drive_%04d_sync" % (date, drive))
-    for sub in ("image_00", "image_01", "oxts"):
+    for sub in ("image_00", "image_01") + (() if no_oxts else ("oxts",)):
         os.makedirs(os.path.join(drive_dir, sub, "data"), exist_ok=True)
     f = float(W)
     cam, velo = raw_calib_text(H, W, f=f, B=POSED_B, R_rect=_rodrigues(POSED_R_RECT_ROT).ravel())
@@ -754,7 +756,7 @@ def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, 
         Image.fromarray(byte(grey_r), "L").save(os.path.join(drive_dir, "image_01", "data", "%010d.png" % k), format="PNG")
         disps.append((fB / Z).astype(np.float32))
         pids.append(pid)
-    for k, rec in enumerate(posed_oxts([C0 @ P @ np.linalg.inv(c2i) for P in poses], lat0)):
+    for k, rec in enumerate([] if no_oxts else posed_oxts([C0 @ P @ np.linalg.inv(c2i) for P in poses], lat0)):
         with open(os.path.join(drive_dir, "oxts", "data", "%010d.txt" % k), "w") as fh:
             fh.write(" ".join(repr(float(x)) if isinstance(x, float) else str(x) for x in rec) + "\n")
     if velodyne:

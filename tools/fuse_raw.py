@@ -23,6 +23,16 @@ pose and scores it against that frame's Velodyne scan as depth_eval.py raw does 
 max_depth 80 m), next to the frame's own stereo depth: one line per frame, the stereo then the fused lidar_* values, then
 the line of means.  Refused as well: -trunc not finite, below -voxel or above 256 -voxel, -trunc or -score without -mesh, an existing
 mesh.ply, and -score on a drive whose frames lack scans.
+
+    python tools/fuse_raw.py kitti census -drive D -out O -voxel 0.05 -mesh -poses track|refine [-traj] [-score]
+
+-poses track (with -mesh) poses each frame after the drive's first by tracking it against the field rendered at the
+previous frame's pose (DESIGN §25): projective point-to-plane ICP on three levels, predicted by constant velocity, so the
+drive needs no oxts/.  -poses refine predicts by the OXTS increment instead.  A frame tracking loses prints
+``<date>/<drive> <frame> lost``, keeps its prediction and is not integrated.  ``O/<drive>/poses.txt`` gets the poses
+(KITTI odometry format).  -traj (which needs oxts/) prints one line per drive against the OXTS poses: ate, rpe_t, rpe_r,
+t_err (%) and r_err (deg/m) over 100 .. 800 m segments, and their count.  -score scores renders at the tracked poses.
+Refused as well: -poses track or refine without -mesh, -traj without them, and an existing poses.txt.
 """
 import argparse
 import math
@@ -52,6 +62,9 @@ def parser():
     ap.add_argument("-score", action="store_true", help="with -mesh: score the field's depth at each frame against its scan")
     ap.add_argument("-crop", choices=("none", "garg", "eigen"), default="none", help="with -score: the crop rectangle")
     ap.add_argument("-min_depth", type=float, default=1e-3, help="with -score: the nearest scored depth in metres")
+    ap.add_argument("-poses", choices=("oxts", "track", "refine"), default="oxts",
+                    help="the frames' poses: the OXTS records, or tracked against the field (with -mesh)")
+    ap.add_argument("-traj", action="store_true", help="with -poses track or refine: print the trajectory's errors against OXTS")
     return ap
 
 
@@ -87,6 +100,10 @@ def parse_args(argv=None):
         raise SystemExit("fuse_raw.py: -score renders the distance field; it needs -mesh")
     if args.trunc is not None and not (math.isfinite(args.trunc) and args.voxel <= args.trunc <= 256 * args.voxel):
         raise SystemExit("fuse_raw.py: -trunc must be a finite length in metres, from -voxel to 256 -voxel")
+    if args.poses != "oxts" and not args.mesh:
+        raise SystemExit("fuse_raw.py: -poses %s tracks each frame against the distance field; it needs -mesh" % args.poses)
+    if args.traj and args.poses == "oxts":
+        raise SystemExit("fuse_raw.py: -traj compares tracked poses with OXTS; it needs -poses track or refine")
     if args.score and not 0 < args.min_depth <= 80.0:
         raise SystemExit("fuse_raw.py: -min_depth must be in (0, 80]")
     for d in args.drive:
@@ -103,8 +120,8 @@ def main(argv=None):
     fuse_drive(args.dataset, args.arch, args.drive, net_fname=args.net_fname or None, out=args.out, voxel=args.voxel,
                min_frames=args.min_frames, max_depth=args.max_depth, every=args.every, confidence=args.confidence,
                density=args.density, disp_max=args.disp_max, device=args.gpu - 1,
-               **(dict(mesh=True, trunc=args.trunc, score=args.score, crop=args.crop, min_depth=args.min_depth)
-                  if args.mesh else {}))
+               **(dict(mesh=True, trunc=args.trunc, score=args.score, crop=args.crop, min_depth=args.min_depth,
+                       poses=args.poses, traj=args.traj) if args.mesh else {}))
     return 0
 
 
