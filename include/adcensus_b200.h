@@ -907,6 +907,24 @@ int mccnn_track_model(mccnn_track *h, const float *depth, float f, float cx, flo
 int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double *sums,
 		     long long *counts, adcensus_stream_t stream);
 int mccnn_track_maps(const mccnn_track *h, int which, int level, double *vertices, double *normals, adcensus_stream_t stream);
+/* The photometric term (DESIGN §26).  Its memory is allocated by the first mccnn_track_intensity, so a tracker that never
+ * uses it is no larger.
+ * mccnn_track_intensity: the intensity pyramid of the DEVICE (H,W) grey (nch 1) or (H,W,3) R, G, B (nch 3) byte image
+ * `img`: `which` 0 the source (the frame's left image), 1 the reference (the left image of the frame the model was
+ * rendered at), which also gets its g_x and g_y planes.  Refuses which outside {0, 1} and nch outside {1, 3}.
+ * mccnn_track_step_photometric: mccnn_track_step's reduce, plus the photometric term of each pixel in the same pass and
+ * tree: sums (56 host float64) receives the 28 geometric sums (mccnn_track_step's bits), then the 28 photometric ones;
+ * counts (3 host int64) the geometric inliers, the photometric inliers and the level's source vertices.  One
+ * device-to-host copy; the stream is synchronised.  Refuses what mccnn_track_step refuses, g_min or rho not finite or < 0,
+ * and a handle without both intensity pyramids.
+ * mccnn_track_intensity_maps: a level's intensities (ceil(H / 2^l) ceil(W / 2^l) float32) into the DEVICE array I, and for
+ * the reference its g_x and g_y (float64 each, NaN on the level's border) into gx and gy, which must be NULL for the
+ * source. */
+int mccnn_track_intensity(mccnn_track *h, int which, const unsigned char *img, int nch, adcensus_stream_t stream);
+int mccnn_track_step_photometric(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double g_min,
+				 double rho, double *sums, long long *counts, adcensus_stream_t stream);
+int mccnn_track_intensity_maps(const mccnn_track *h, int which, int level, float *I, double *gx, double *gy,
+			       adcensus_stream_t stream);
 void mccnn_track_destroy(mccnn_track *h);
 
 #ifdef __cplusplus

@@ -8,6 +8,10 @@
 // chunks of 1024 pixels in row-major order, stride halving inside each chunk, then the same over the chunk sums padded to
 // a power of two -- so the sums have the same bits on every run and GPU and can be restated in numpy.  The inlier count is
 // an integer, summed by atomics.  One device-to-host copy per step returns the sums and the counts.
+//
+// The photometric term (DESIGN §26): intensity pyramids of the frame's left image and of the previous frame's (with its
+// gradients), allocated on first use; mccnn_track_step_photometric reduces each pixel's geometric terms and then its
+// photometric ones through the same tree and shared buffer, in one pass and one read-back.
 #include <math.h>
 
 #include "camera.cuh"
@@ -183,25 +187,214 @@ __global__ void __launch_bounds__(RT) step_kernel(Maps S, Maps M, Pose T, Step s
 	if ((threadIdx.x & 31) == 0 && total) atomicAdd(inliers, (unsigned long long)total);
 }
 
+// rows of chunk sums (row k at part[k P]) padded with +0.0 from n to P (a power of two), reduced by stride halving in
+// place; one block of RED threads
+__device__ __forceinline__ void halve_rows(double *__restrict__ part, int rows, int n, int P)
+{
+	for (long long e = threadIdx.x; e < (long long)rows * (P - n); e += RED) part[(e / (P - n)) * P + n + e % (P - n)] = 0.0;
+	__syncthreads();
+	for (int stride = P >> 1; stride >= 1; stride >>= 1) {
+		for (long long e = threadIdx.x; e < (long long)rows * stride; e += RED) {
+			const long long k = e / stride, i = e % stride;
+			part[k * P + i] = __dadd_rn(part[k * P + i], part[k * P + i + stride]);
+		}
+		__syncthreads();
+	}
+}
+
 // the chunk sums padded with +0.0 to P (a power of two), reduced by stride halving in place; out = the 28 sums, then the
 // inliers and the level's source vertices as int64
 __global__ void __launch_bounds__(RED) chunk_reduce_kernel(double *__restrict__ part, int n, int P,
 							   const unsigned long long *__restrict__ inliers,
 							   const unsigned long long *__restrict__ nvert, double *__restrict__ out)
 {
-	for (long long e = threadIdx.x; e < (long long)NS * (P - n); e += RED) part[(e / (P - n)) * P + n + e % (P - n)] = 0.0;
-	__syncthreads();
-	for (int stride = P >> 1; stride >= 1; stride >>= 1) {
-		for (long long e = threadIdx.x; e < (long long)NS * stride; e += RED) {
-			const long long k = e / stride, i = e % stride;
-			part[k * P + i] = __dadd_rn(part[k * P + i], part[k * P + i + stride]);
-		}
-		__syncthreads();
-	}
+	halve_rows(part, NS, n, P);
 	if (threadIdx.x < NS) out[threadIdx.x] = part[(long long)threadIdx.x * P];
 	if (threadIdx.x == 0) {
 		((long long *)out)[NS] = (long long)*inliers;
 		((long long *)out)[NS + 1] = (long long)*nvert;
+	}
+}
+
+// ---- the photometric term (DESIGN §26) ----
+
+// level 0 of an intensity pyramid: the byte, or ((R + G) + B) / 3, in fp32
+__global__ void __launch_bounds__(256) grey_kernel(const unsigned char *__restrict__ img, int nch, long long np, float *__restrict__ I)
+{
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= np) return;
+	if (nch == 1) {
+		I[i] = (float)img[i];
+	} else {
+		const unsigned char *p = img + 3 * i;
+		I[i] = __fdiv_rn(__fadd_rn(__fadd_rn((float)p[0], (float)p[1]), (float)p[2]), 3.0f);
+	}
+}
+
+// (L(a - 1) / 4 + L(a) / 2) + L(a + 1) / 4 along a row (step 1) or a column (step w) of level L, indices clamped to [0, n)
+__device__ __forceinline__ float blur3(const float *L, int a, int n, long long step)
+{
+	const float l = L[(long long)max(a - 1, 0) * step], c = L[(long long)a * step], r = L[(long long)min(a + 1, n - 1) * step];
+	return __fadd_rn(__fadd_rn(__fmul_rn(0.25f, l), __fmul_rn(0.5f, c)), __fmul_rn(0.25f, r));
+}
+
+// level l + 1 (h2 x w2) of level l (h x w): the [1/4 1/2 1/4] blur at even pixels, the three rows' blurs first
+__global__ void __launch_bounds__(256) down_kernel(const float *__restrict__ L, int h, int w, float *__restrict__ out, int h2, int w2)
+{
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= (long long)h2 * w2) return;
+	const int x = 2 * (int)(i % w2), y = 2 * (int)(i / w2);
+	float r[3];
+#pragma unroll
+	for (int k = 0; k < 3; k++) r[k] = blur3(L + (long long)min(max(y - 1 + k, 0), h - 1) * w, x, w, 1);
+	out[i] = __fadd_rn(__fadd_rn(__fmul_rn(0.25f, r[0]), __fmul_rn(0.5f, r[1])), __fmul_rn(0.25f, r[2]));
+}
+
+// central differences 0.5 (L(x + 1) - L(x - 1)) in float64, NaN on the level's border
+__global__ void __launch_bounds__(256) gradient_kernel(const float *__restrict__ L, int h, int w, double *__restrict__ gx,
+						       double *__restrict__ gy)
+{
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= (long long)h * w) return;
+	const int x = (int)(i % w), y = (int)(i / w);
+	gx[i] = x >= 1 && x + 1 < w ? __dmul_rn(0.5, __dsub_rn((double)L[i + 1], (double)L[i - 1])) : dnan();
+	gy[i] = y >= 1 && y + 1 < h ? __dmul_rn(0.5, __dsub_rn((double)L[i + w], (double)L[i - w])) : dnan();
+}
+
+struct Photo {
+	const float *Is, *Ir;                        // the level's source and reference intensities
+	const double *gx, *gy;                       // the reference's gradients
+	double g2, rho, s;                           // g_min^2, rho, f 2^-l
+};
+
+// P at (x0 + fx, y0 + fy) (k = y0 wl + x0): along x, then y, each a + f (b - a)
+template <typename T>
+__device__ __forceinline__ double bilinear(const T *P, long long k, int wl, double fx, double fy)
+{
+	const double a = (double)P[k], b = (double)P[k + 1], c = (double)P[k + wl], d = (double)P[k + wl + 1];
+	const double top = __dadd_rn(a, __dmul_rn(fx, __dsub_rn(b, a)));
+	const double bot = __dadd_rn(c, __dmul_rn(fx, __dsub_rn(d, c)));
+	return __dadd_rn(top, __dmul_rn(fy, __dsub_rn(bot, top)));
+}
+
+// pixel i's photometric Jacobian row J and residual r (zero, and false, when the pixel is skipped)
+__device__ __forceinline__ bool photo_term(long long i, const Maps &S, const Maps &M, const Pose &T, const Step &st,
+					   const Photo &ph, double *J)
+{
+	for (int k = 0; k < 7; k++) J[k] = 0.0;
+	if (i >= (long long)st.hl * st.wl) return false;
+	const double p0 = S.v[0][i];
+	if (isnan(p0)) return false;                 // no source vertex
+	double q[3];
+	to_world(p0, S.v[1][i], S.v[2][i], T, q);
+	if (!(q[2] > 0.0)) return false;
+	const double xs = __dmul_rn(__dadd_rn(__dmul_rn(__ddiv_rn(q[0], q[2]), st.f), st.cx), st.scale);
+	const double ys = __dmul_rn(__dadd_rn(__dmul_rn(__ddiv_rn(q[1], q[2]), st.f), st.cy), st.scale);
+	const double u = floor(__dadd_rn(xs, 0.5)), v = floor(__dadd_rn(ys, 0.5));
+	if (!(u >= 0.0 && u < st.wl && v >= 0.0 && v < st.hl)) return false;
+	const long long j = (long long)v * st.wl + (long long)u;
+	const double m0 = M.v[0][j];
+	if (isnan(m0)) return false;                 // the reference view sees no surface there
+	const double d[3] = {__dsub_rn(q[0], m0), __dsub_rn(q[1], M.v[1][j]), __dsub_rn(q[2], M.v[2][j])};
+	const double dd = __dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2]));
+	if (!(dd <= st.d2)) return false;            // occluded in the reference view
+	const double x0 = floor(xs), y0 = floor(ys);
+	if (!(x0 >= 1.0 && __dadd_rn(x0, 1.0) <= st.wl - 2 && y0 >= 1.0 && __dadd_rn(y0, 1.0) <= st.hl - 2)) return false;
+	const double fx = __dsub_rn(xs, x0), fy = __dsub_rn(ys, y0);
+	const long long k = (long long)y0 * st.wl + (long long)x0;
+	const double r = __dsub_rn(bilinear(ph.Ir, k, st.wl, fx, fy), (double)ph.Is[i]);
+	const double gx = bilinear(ph.gx, k, st.wl, fx, fy), gy = bilinear(ph.gy, k, st.wl, fx, fy);
+	if (!(__dadd_rn(__dmul_rn(gx, gx), __dmul_rn(gy, gy)) >= ph.g2 && fabs(r) <= ph.rho)) return false;
+	const double a = __ddiv_rn(__dmul_rn(gx, ph.s), q[2]), b = __ddiv_rn(__dmul_rn(gy, ph.s), q[2]);
+	const double c = __ddiv_rn(-__dadd_rn(__dmul_rn(a, q[0]), __dmul_rn(b, q[1])), q[2]);
+	J[0] = __dsub_rn(__dmul_rn(q[1], c), __dmul_rn(q[2], b));
+	J[1] = __dsub_rn(__dmul_rn(q[2], a), __dmul_rn(q[0], c));
+	J[2] = __dsub_rn(__dmul_rn(q[0], b), __dmul_rn(q[1], a));
+	J[3] = a;
+	J[4] = b;
+	J[5] = c;
+	J[6] = r;
+	return true;
+}
+
+// step_kernel's tree over the four pixels' terms of each thread: the first two halvings in registers, strides 128 .. 32
+// through sh, 16 .. 1 through warp shuffles; the chunk's 28 sums to part[k P + chunk]
+__device__ __forceinline__ void reduce_chunk(const double (*J)[7], double *sh, double *__restrict__ part, int P)
+{
+	double s[NS];
+	{
+		int k = 0;
+#pragma unroll
+		for (int a = 0; a < 6; a++)
+#pragma unroll
+			for (int b = a; b < 6; b++, k++) s[k] = quad(J, a, b);
+#pragma unroll
+		for (int a = 0; a < 6; a++) s[21 + a] = quad(J, a, 6);
+		s[27] = quad(J, 6, 6);
+	}
+#pragma unroll
+	for (int stride = 128; stride >= 32; stride >>= 1) {
+		const int t = threadIdx.x;
+		if (t >= stride && t < 2 * stride)
+#pragma unroll
+			for (int k = 0; k < NS; k++) sh[k * stride + t - stride] = s[k];
+		__syncthreads();
+		if (t < stride)
+#pragma unroll
+			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], sh[k * stride + t]);
+		__syncthreads();
+	}
+	if (threadIdx.x < 32) {
+#pragma unroll
+		for (int off = 16; off >= 1; off >>= 1)
+#pragma unroll
+			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], __shfl_down_sync(0xffffffffu, s[k], off));
+		if (threadIdx.x == 0)
+#pragma unroll
+			for (int k = 0; k < NS; k++) part[(long long)k * P + blockIdx.x] = s[k];
+	}
+}
+
+// one block per chunk of 1024 pixels, as step_kernel: the geometric terms (pixel_term) are reduced first, then the
+// photometric ones through the same shared buffer; rows 0 .. 27 of part get the geometric chunk sums, rows 28 .. 55 the
+// photometric ones; inliers[0] and [1] the two inlier counts
+__global__ void __launch_bounds__(RT) step_photometric_kernel(Maps S, Maps M, Pose T, Step st, Photo ph, double *__restrict__ part,
+							      int P, unsigned long long *__restrict__ inliers)
+{
+	__shared__ double sh[NS * 128];
+	const long long base = (long long)blockIdx.x * CH + threadIdx.x;
+	int cg = 0, cp = 0;
+	{
+		double J[4][7];
+#pragma unroll
+		for (int p = 0; p < 4; p++) cg += pixel_term(base + p * RT, S, M, T, st, J[p]);
+		reduce_chunk(J, sh, part, P);
+	}
+	{
+		double J[4][7];
+#pragma unroll
+		for (int p = 0; p < 4; p++) cp += photo_term(base + p * RT, S, M, T, st, ph, J[p]);
+		reduce_chunk(J, sh, part + (long long)NS * P, P);
+	}
+	const int tg = __reduce_add_sync(0xffffffffu, cg), tp = __reduce_add_sync(0xffffffffu, cp);
+	if ((threadIdx.x & 31) == 0) {
+		if (tg) atomicAdd(inliers, (unsigned long long)tg);
+		if (tp) atomicAdd(inliers + 1, (unsigned long long)tp);
+	}
+}
+
+// the 56 rows of chunk sums reduced as chunk_reduce_kernel's; out = the 56 sums, then the geometric and the photometric
+// inliers and the level's source vertices as int64
+__global__ void __launch_bounds__(RED) chunk_reduce_photometric_kernel(double *__restrict__ part, int n, int P,
+								       const unsigned long long *__restrict__ inliers,
+								       const unsigned long long *__restrict__ nvert, double *__restrict__ out)
+{
+	halve_rows(part, 2 * NS, n, P);
+	if (threadIdx.x < 2 * NS) out[threadIdx.x] = part[(long long)threadIdx.x * P];
+	if (threadIdx.x == 0) {
+		((long long *)out)[2 * NS] = (long long)inliers[0];
+		((long long *)out)[2 * NS + 1] = (long long)inliers[1];
+		((long long *)out)[2 * NS + 2] = (long long)*nvert;
 	}
 }
 
@@ -220,6 +413,12 @@ struct mccnn_track {
 	double *host;                                 // pinned: the 30 values read back per step
 	float mf, mcx, mcy;                           // the model's camera
 	bool have_source, have_model;
+	// the photometric term's memory, allocated by the first mccnn_track_intensity
+	long long ioff[LEVELS], npix;                 // each level's first pixel in an intensity pyramid; pixels per pyramid
+	float *imem;                                  // the source's intensity pyramid, then the reference's
+	double *pmem;                                 // the reference's g_x, g_y pyramids, 56 rows of chunk sums, out, counters
+	double *phost;                                // pinned: the 59 values read back per photometric step
+	bool have_intensity[2];
 };
 
 namespace {
@@ -240,6 +439,37 @@ int build_pyramid(mccnn_track *h, int which, const float *src, const Cam &c, cud
 		normal_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(h->hl[l], h->wl[l], m);
 	}
 	ADC_CHECK_LAUNCH();
+	return 0;
+}
+
+// the photometric term's device layout: g_x and g_y pyramids, 2 NS rows of P chunk sums, the 2 NS + 3 outputs, then two
+// counters
+double *photo_part(const mccnn_track *h) { return h->pmem + 2 * h->npix; }
+double *photo_out(const mccnn_track *h) { return photo_part(h) + 2ll * NS * h->P; }
+unsigned long long *photo_ctr(const mccnn_track *h) { return (unsigned long long *)(photo_out(h) + 2 * NS + 3); }
+
+int photo_alloc(mccnn_track *h)
+{
+	if (h->imem) return 0;
+	long long at = 0;
+	for (int l = 0; l < LEVELS; l++) {
+		h->ioff[l] = at;
+		at += (long long)h->hl[l] * h->wl[l];
+	}
+	h->npix = at;
+	float *im = nullptr;
+	double *pm = nullptr, *host = nullptr;
+	cudaError_t e = cudaMalloc(&im, 4 * (size_t)(2 * at));
+	if (e == cudaSuccess) e = cudaMalloc(&pm, 8 * (size_t)(2 * at + 2ll * NS * h->P + 2 * NS + 3 + 2));
+	if (e == cudaSuccess) e = cudaMallocHost(&host, 8 * (2 * NS + 3));
+	if (e != cudaSuccess) {
+		if (im) cudaFree(im);
+		if (pm) cudaFree(pm);
+		return (int)e;
+	}
+	h->imem = im;
+	h->pmem = pm;
+	h->phost = host;
 	return 0;
 }
 
@@ -356,6 +586,85 @@ int mccnn_track_maps(const mccnn_track *h, int which, int level, double *vertice
 	return 0;
 }
 
+int mccnn_track_intensity(mccnn_track *h, int which, const unsigned char *img, int nch, adcensus_stream_t stream)
+{
+	if (!h || !img || which < 0 || which > 1 || (nch != 1 && nch != 3)) return ADCENSUS_EINVAL;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	int rc = photo_alloc(h);
+	if (rc) return rc;
+	cudaStream_t s = adc_stream(stream);
+	float *I = h->imem + which * h->npix;
+	const long long np = (long long)h->H * h->W;
+	grey_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(img, nch, np, I);
+	for (int l = 0; l + 1 < LEVELS; l++) {
+		const long long n2 = (long long)h->hl[l + 1] * h->wl[l + 1];
+		down_kernel<<<adc_div_up(n2, 256), 256, 0, s>>>(I + h->ioff[l], h->hl[l], h->wl[l], I + h->ioff[l + 1], h->hl[l + 1],
+								 h->wl[l + 1]);
+	}
+	if (which == 1)
+		for (int l = 0; l < LEVELS; l++) {
+			const long long np_l = (long long)h->hl[l] * h->wl[l];
+			gradient_kernel<<<adc_div_up(np_l, 256), 256, 0, s>>>(I + h->ioff[l], h->hl[l], h->wl[l], h->pmem + h->ioff[l],
+									     h->pmem + h->npix + h->ioff[l]);
+		}
+	ADC_CHECK_LAUNCH();
+	h->have_intensity[which] = true;
+	return 0;
+}
+
+int mccnn_track_step_photometric(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double g_min,
+				 double rho, double *sums, long long *counts, adcensus_stream_t stream)
+{
+	if (!h || !sums || !counts || level < 0 || level >= LEVELS || !h->have_source || !h->have_model) return ADCENSUS_EINVAL;
+	if (!h->have_intensity[0] || !h->have_intensity[1]) return ADCENSUS_EINVAL;
+	if (!(delta > 0.0 && isfinite(delta) && cos_theta >= -1.0 && cos_theta <= 1.0)) return ADCENSUS_EINVAL;
+	if (!(g_min >= 0.0 && isfinite(g_min) && rho >= 0.0 && isfinite(rho))) return ADCENSUS_EINVAL;
+	Pose T;
+	int rc = check_pose(pose12, &T);
+	if (rc) return rc;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	cudaStream_t s = adc_stream(stream);
+	const int hl = h->hl[level], wl = h->wl[level];
+	const int n = (int)(((long long)hl * wl + CH - 1) / CH);
+	int P = 1;
+	while (P < n) P <<= 1;
+	double *part = photo_part(h), *out = photo_out(h);
+	unsigned long long *ctr = photo_ctr(h);
+	const double scale = ldexp(1.0, -level);
+	const Step st{hl, wl, (double)h->mf, (double)h->mcx, (double)h->mcy, scale, delta * delta, cos_theta};
+	const long long o = h->ioff[level];
+	const Photo ph{h->imem + o, h->imem + h->npix + o, h->pmem + o, h->pmem + h->npix + o, g_min * g_min, rho,
+		       (double)h->mf * scale};
+	ADC_CUDA(cudaMemsetAsync(ctr, 0, 16, s));
+	step_photometric_kernel<<<n, RT, 0, s>>>(level_maps(h, 0, level), level_maps(h, 1, level), T, st, ph, part, P, ctr);
+	chunk_reduce_photometric_kernel<<<1, RED, 0, s>>>(part, n, P, ctr, h->ctr + 1 + level, out);
+	ADC_CHECK_LAUNCH();
+	ADC_CUDA(cudaMemcpyAsync(h->phost, out, 8 * (2 * NS + 3), cudaMemcpyDeviceToHost, s));
+	ADC_CUDA(cudaStreamSynchronize(s));
+	for (int k = 0; k < 2 * NS; k++) sums[k] = h->phost[k];
+	for (int k = 0; k < 3; k++) counts[k] = ((const long long *)h->phost)[2 * NS + k];
+	return 0;
+}
+
+int mccnn_track_intensity_maps(const mccnn_track *h, int which, int level, float *I, double *gx, double *gy,
+			       adcensus_stream_t stream)
+{
+	if (!h || !I || which < 0 || which > 1 || level < 0 || level >= LEVELS || !h->have_intensity[which]) return ADCENSUS_EINVAL;
+	if (which == 1 ? (!gx || !gy) : (gx || gy)) return ADCENSUS_EINVAL;
+	DeviceScope dev(h->device);
+	if (dev.rc) return dev.rc;
+	const long long np = (long long)h->hl[level] * h->wl[level], o = h->ioff[level];
+	cudaStream_t s = adc_stream(stream);
+	ADC_CUDA(cudaMemcpyAsync(I, h->imem + which * h->npix + o, 4 * (size_t)np, cudaMemcpyDeviceToDevice, s));
+	if (which == 1) {
+		ADC_CUDA(cudaMemcpyAsync(gx, h->pmem + o, 8 * (size_t)np, cudaMemcpyDeviceToDevice, s));
+		ADC_CUDA(cudaMemcpyAsync(gy, h->pmem + h->npix + o, 8 * (size_t)np, cudaMemcpyDeviceToDevice, s));
+	}
+	return 0;
+}
+
 void mccnn_track_destroy(mccnn_track *h)
 {
 	if (!h) return;
@@ -364,6 +673,9 @@ void mccnn_track_destroy(mccnn_track *h)
 		if (!dev.rc) {
 			if (h->mem) cudaFree(h->mem);
 			if (h->host) cudaFreeHost(h->host);
+			if (h->imem) cudaFree(h->imem);
+			if (h->pmem) cudaFree(h->pmem);
+			if (h->phost) cudaFreeHost(h->phost);
 		}
 	}
 	delete h;

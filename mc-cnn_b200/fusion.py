@@ -351,7 +351,7 @@ def check_drives(drives, out, mesh=False, tracked=False):
 def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_frames=1, max_depth=None, every=1,
                confidence=False, density=None, disp_max=predict_kitti.DISP_MAX, device=0, prefetch=True, verbose=True,
                mesh=False, trunc=None, score=False, crop="none", min_depth=depth.MIN_DEPTH, poses="oxts", traj=False,
-               **overrides):
+               photometric=0.0, rho=30.0, grad_min=2.0, **overrides):
     """The stereo method over every `every`-th frame of each `_sync` drive in `drives`, in frame order on one device, each
     drive's frames fused into ``out/<drive>/fused.ply`` in its own world frame (dataio.raw_poses: the drive's first fused
     frame).  Prints ``<date>/<drive> <frame>`` per frame and one summary line per drive; returns the
@@ -363,8 +363,10 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
     rendered at the previous frame's pose (track.Tracker, DESIGN §25), predicted by constant velocity ('track', no OXTS
     needed) or by the OXTS increment ('refine'); a lost frame is printed ``<date>/<drive> <frame> lost``, keeps its
     prediction and is not integrated; ``out/<drive>/poses.txt`` gets the poses, and `traj` prints one line of
-    track.trajectory_metrics against the OXTS poses per drive.  Scores are taken at the tracked poses.  Everything that can
-    be refused is refused before any GPU work."""
+    track.trajectory_metrics against the OXTS poses per drive.  Scores are taken at the tracked poses.  `photometric`
+    lambda > 0 (metres per grey level) adds the photometric term (DESIGN §26, gates `rho` and `grad_min`): each frame's
+    left image is aligned to the previous frame's, which stays on the device.  Everything that can be refused is refused
+    before any GPU work."""
     import torch.distributed as dist
 
     from . import depth_eval, track as track_
@@ -389,6 +391,9 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
         raise ValueError("poses %r tracks each frame against the distance field: it needs mesh" % poses)
     if traj and not tracked:
         raise ValueError("traj compares tracked poses with the OXTS poses: it needs poses 'track' or 'refine'")
+    photometric, rho, grad_min = track_.check_photometric(photometric, rho, grad_min)
+    if photometric and not tracked:
+        raise ValueError("photometric weighs a term of the tracking: it needs poses 'track' or 'refine'")
     if mesh:
         trunc = check_trunc(trunc, voxel)
     if score:
@@ -415,7 +420,7 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
                                    cals[predict_raw.date_dir(fr.drive)], *shapes[i], run.dev, min_depth, crop)
 
     out_sums = []
-    fu = tracker = None
+    fu = tracker = ref_left = None
     stereo = []                            # the drive's per-frame stereo counts (score)
     used = oxts if not tracked else {}     # each frame's pose
     try:
@@ -436,10 +441,13 @@ def fuse_drive(dataset, arch, drives, net_fname=None, out="out", voxel=0.1, min_
                     if tracker is None or (tracker.H, tracker.W) != (H, W):
                         if tracker is not None:
                             tracker.close()
-                        tracker = track_.Tracker(H, W, run.dev.index)
+                        tracker = track_.Tracker(H, W, run.dev.index, photometric=photometric, rho=rho, grad_min=grad_min)
                     Z = fu.render(cal, est[-1], H, W, 1, max_depth)
                     O = [oxts[(fr.drive, f.index)] for f in frames[first:i + 1]] if poses == "refine" else None
-                    pose, _, is_lost = tracker.track(pred, cal, Z, est[-1], track_.predict(poses, est, O), max_depth)
+                    images = dict(left=left, ref_left=ref_left) if photometric else {}
+                    pose, _, is_lost = tracker.track(pred, cal, Z, est[-1], track_.predict(poses, est, O), max_depth, **images)
+                if photometric:                # the next frame's reference, lost or not
+                    ref_left = depth._colour(left, *(int(v) for v in shapes[i]), run.dev)[0]
                 est.append(pose)
                 used[(fr.drive, fr.index)] = pose
                 if is_lost:

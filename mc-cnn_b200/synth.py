@@ -607,8 +607,11 @@ def write_mb_eval_gt(unzip, seed=0):
 # world frame is the first frame's rectified left camera (x right, y down, z forward); each plane is (normal, offset):
 # n . x = offset.  Ground, a wall ahead and two side walls.
 POSED_PLANES = (((0.0, 1.0, 0.0), 1.65), ((0.0, 0.0, 1.0), 14.0), ((1.0, 0.0, 0.0), 3.5), ((1.0, 0.0, 0.0), -4.0))
-# the plane's in-plane texture axes (indices of x, y, z)
-_POSED_AXES = ((0, 2), (0, 1), (2, 1), (2, 1))
+# A street (DESIGN §26): the ground and the two side walls, no wall ahead.  Every normal lies across the street, so the
+# geometry alone cannot fix motion along it.
+STREET_PLANES = (POSED_PLANES[0], POSED_PLANES[2], POSED_PLANES[3])
+# a plane's in-plane texture axes (indices of x, y, z) by the axis of its normal
+_POSED_AXES = {1: (0, 2), 2: (0, 1), 0: (2, 1)}
 POSED_B = 0.5
 POSED_LATLON = (49.011212804408, 8.4228850417969, 112.83)         # the first frame's GPS position (Karlsruhe)
 POSED_RPY = (0.021, -0.013, 0.61)                                 # its roll, pitch, yaw
@@ -635,36 +638,44 @@ def _value_noise(a, b, cell, k):
     return (1 - fb) * ((1 - fa) * v(0, 0) + fa * v(1, 0)) + fb * ((1 - fa) * v(0, 1) + fa * v(1, 1))
 
 
-def posed_texture(p, plane):
-    """the grey level in [0, 255] of world points p (..., 3) on plane `plane`: a function of world position only"""
-    a, b = p[..., _POSED_AXES[plane][0]], p[..., _POSED_AXES[plane][1]]
+def posed_texture(p, plane, planes=POSED_PLANES):
+    """the grey level in [0, 255] of world points p (..., 3) on plane number `plane` of `planes`: a function of world
+    position only"""
+    axes = _POSED_AXES[int(np.argmax(np.abs(planes[plane][0])))]
+    a, b = p[..., axes[0]], p[..., axes[1]]
     return 30.0 + 195.0 * (0.6 * _value_noise(a, b, 0.04, 2 * plane) + 0.4 * _value_noise(a, b, 0.15, 2 * plane + 1))
 
 
 def posed_camera_poses(n, step=0.4, yaw=np.radians(1.5)):
     """[4x4 camera-to-world float64] of n frames: the first is I, each next one `step` metres ahead along its heading and
-    turned by `yaw` about the camera's vertical (y) axis"""
+    turned by `yaw` about the camera's vertical (y) axis; `step` may be a sequence of at least n - 1 steps, step k leading
+    from frame k to frame k + 1"""
+    steps = [float(step)] * n if np.ndim(step) == 0 else [float(v) for v in step]
+    if len(steps) < n - 1:
+        raise ValueError("%d frames need at least %d steps, got %d" % (n, n - 1, len(steps)))
     out, R, t = [], np.eye(3), np.zeros(3)
     Ry = np.array([[np.cos(yaw), 0, np.sin(yaw)], [0, 1, 0], [-np.sin(yaw), 0, np.cos(yaw)]])
-    for _ in range(n):
+    for k in range(n):
         M = np.eye(4)
         M[:3, :3], M[:3, 3] = R, t
         out.append(M)
-        t = t + R @ np.array([0.0, 0.0, step])
+        if k + 1 == n:
+            break
+        t = t + R @ np.array([0.0, 0.0, steps[k]])
         R = R @ Ry.T
     return out
 
 
-def posed_render(pose, H, W, f, cx, cy, shift=0.0):
+def posed_render(pose, H, W, f, cx, cy, shift=0.0, planes=POSED_PLANES):
     """(Z (H, W) camera depth of the nearest plane hit, plane id (H, W) int8, grey float) of the camera at `pose` moved by
-    `shift` metres along its own x axis (the right camera: the baseline)"""
+    `shift` metres along its own x axis (the right camera: the baseline), in the world of `planes`"""
     v, u = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
     dc = np.stack([(u - cx) / f, (v - cy) / f, np.ones_like(u)], -1)
     R, t = pose[:3, :3], pose[:3, 3] + pose[:3, :3] @ np.array([shift, 0.0, 0.0])
     dw = dc @ R.T
     Z = np.full((H, W), np.inf)
     pid = np.full((H, W), -1, np.int8)
-    for k, (nrm, off) in enumerate(POSED_PLANES):
+    for k, (nrm, off) in enumerate(planes):
         nrm = np.asarray(nrm)
         den = dw @ nrm
         with np.errstate(divide="ignore", invalid="ignore"):
@@ -673,9 +684,9 @@ def posed_render(pose, H, W, f, cx, cy, shift=0.0):
         Z = np.where(hit, s, Z)
         pid = np.where(hit, k, pid).astype(np.int8)
     grey = np.zeros((H, W))
-    for k in range(len(POSED_PLANES)):
+    for k in range(len(planes)):
         m = pid == k
-        grey[m] = posed_texture(t + dw[m] * Z[m][:, None], k)
+        grey[m] = posed_texture(t + dw[m] * Z[m][:, None], k, planes)
     return Z, pid, grey
 
 
@@ -699,12 +710,12 @@ def posed_oxts(imu_poses, lat0):
     return out
 
 
-def posed_scan(pose, H, W, cal, every=2):
+def posed_scan(pose, H, W, cal, every=2, planes=POSED_PLANES):
     """(N, 4) float32 velodyne scan of the planes seen from the camera at `pose`: one point per `every`-th pixel in each
     direction, on the plane hit along the ray of image coordinate u + 1 (DESIGN §21's projection puts it on pixel u), taken
     through R_rect_00 and RAW_VELO_R into the velodyne frame; reflectance 0.5"""
     cx, cy = cal.cx - 1.0, cal.cy - 1.0
-    Z = posed_render(pose, H, W, cal.f, cx, cy)[0][::every, ::every]
+    Z = posed_render(pose, H, W, cal.f, cx, cy, planes=planes)[0][::every, ::every]
     v, u = np.meshgrid(np.arange(0, H, every, dtype=np.float64), np.arange(0, W, every, dtype=np.float64), indexing="ij")
     ok = np.isfinite(Z)
     z = Z[ok]
@@ -714,9 +725,9 @@ def posed_scan(pose, H, W, cal, every=2):
 
 
 def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, step=0.4, yaw=np.radians(1.5), velodyne=False,
-                            no_oxts=False):
-    """A KITTI raw ``_sync`` drive whose frames view the static world of POSED_PLANES from known poses
-    (:func:`posed_camera_poses`): grey pairs ``image_00`` / ``image_01`` rendered by ray casting (nearest plane hit, the
+                            no_oxts=False, planes=POSED_PLANES):
+    """A KITTI raw ``_sync`` drive whose frames view the static world of `planes` (POSED_PLANES; STREET_PLANES is a street
+    with no wall ahead) from known poses (:func:`posed_camera_poses`, `step` one length or one per frame): grey pairs ``image_00`` / ``image_01`` rendered by ray casting (nearest plane hit, the
     grey level a function of the world position, so the two views agree), the date directory's calibration (f = W,
     baseline POSED_B, a small R_rect_00, velo-to-cam RAW_VELO_R, and calib_imu_to_velo.txt with a rotation and
     translation), and ``oxts/data/%010d.txt`` records whose poses, through dataio.raw_poses, are the camera poses.  With
@@ -750,8 +761,8 @@ def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, 
     disps, pids = [], []
     byte = lambda a: np.clip(np.rint(a), 0, 255).astype(np.uint8)
     for k, P in enumerate(poses):
-        Z, pid, grey = posed_render(P, H, W, cal.f, cal.cx, cal.cy)
-        _, _, grey_r = posed_render(P, H, W, cal.f, cal.cx, cal.cy, shift=cal.baseline)
+        Z, pid, grey = posed_render(P, H, W, cal.f, cal.cx, cal.cy, planes=planes)
+        _, _, grey_r = posed_render(P, H, W, cal.f, cal.cx, cal.cy, shift=cal.baseline, planes=planes)
         Image.fromarray(byte(grey), "L").save(os.path.join(drive_dir, "image_00", "data", "%010d.png" % k), format="PNG")
         Image.fromarray(byte(grey_r), "L").save(os.path.join(drive_dir, "image_01", "data", "%010d.png" % k), format="PNG")
         disps.append((fB / Z).astype(np.float32))
@@ -762,5 +773,5 @@ def write_kitti_posed_drive(root, date="2011_09_26", drive=1, n=4, H=48, W=160, 
     if velodyne:
         os.makedirs(os.path.join(drive_dir, "velodyne_points", "data"), exist_ok=True)
         for k, P in enumerate(poses):
-            posed_scan(P, H, W, cal).astype("<f4").tofile(os.path.join(drive_dir, "velodyne_points", "data", "%010d.bin" % k))
+            posed_scan(P, H, W, cal, planes=planes).astype("<f4").tofile(os.path.join(drive_dir, "velodyne_points", "data", "%010d.bin" % k))
     return drive_dir, disps, pids, poses

@@ -13,6 +13,9 @@ Each frame's vertices and normals (three levels, level l keeping the pixels (2^l
 projective point-to-plane ICP, coarsest level first.  The GPU sums each step's normal equations in a fixed order
 (csrc/track.cu); :func:`run_icp` solves them and updates the pose on the host in float64.  It is the one copy of that loop,
 used by :class:`Tracker` and by the numpy restatement in tests/track_oracle.py alike.
+
+With ``Tracker(H, W, photometric=0.01)`` and ``track(..., left=left, ref_left=prev_left)`` each step also aligns the
+frame's left image to the previous frame's (DESIGN §26), which fixes motion along a street whose normals all lie across it.
 """
 import ctypes
 import math
@@ -31,6 +34,8 @@ LOST_SHARE = 0.1                   # a frame whose level-0 inliers are fewer tha
 EIG_RATIO = 1e-12                  # a solve is degenerate when the smallest eigenvalue is <= this times the largest
 CONVERGED = 1e-6                   # a level ends when |omega| (rad) and |tau| (m) are both below this
 NSUMS = 28
+RHO = 30.0                         # the largest photometric residual of an inlier, grey levels (DESIGN §26)
+GRAD_MIN = 2.0                     # the smallest intensity gradient of a photometric inlier, grey levels per level pixel
 MODES = ("oxts", "track", "refine")
 
 TrajectoryMetrics = namedtuple("TrajectoryMetrics", "ate rpe_t rpe_r t_err r_err segments")
@@ -86,6 +91,12 @@ def solve(sums, count):
     return np.linalg.solve(A, -s[21:27])
 
 
+def solve_joint(sums_g, sums_p, count_g, count_p, lam2):
+    """:func:`solve` of the joint system A_g + lam2 A_p, b_g + lam2 b_p (lam2 = lambda^2, in m^2 per grey level^2) with
+    count = the geometric plus the photometric inliers"""
+    return solve(np.asarray(sums_g, np.float64) + lam2 * np.asarray(sums_p, np.float64), count_g + count_p)
+
+
 def update(T, xi):
     """[Rodrigues(omega) | tau] T"""
     M = np.eye(4)
@@ -94,19 +105,27 @@ def update(T, xi):
     return M @ T
 
 
-def run_icp(step, T, iters=ITERS, delta=DELTA, theta=THETA):
+def run_icp(step, T, iters=ITERS, delta=DELTA, theta=THETA, photometric=0.0):
     """The ICP levels from the coarsest to the finest from the relative pose T (4x4, source camera to model camera).
     step(level, pose12, delta, cos_theta) returns (28 sums, inliers, the level's source vertices).  Returns (T, level-0
-    inliers, lost): lost when a level-0 solve was degenerate or its inliers are fewer than LOST_SHARE of its vertices."""
+    inliers, lost): lost when a level-0 solve was degenerate or its inliers are fewer than LOST_SHARE of its vertices.
+    With `photometric` lambda > 0 (metres per grey level), step returns (56 sums: geometric then photometric,
+    (geometric inliers, photometric inliers), vertices) and each solve is :func:`solve_joint`'s; the inliers of the lost
+    rule stay the geometric ones (DESIGN §26)."""
     cos_t = math.cos(math.radians(theta))
+    lam2 = photometric * photometric
     inliers, vertices, degenerate = 0, 0, False
     for i in range(LEVELS):
         level = LEVELS - 1 - i
         for _ in range(iters[i]):
             sums, inl, nv = step(level, np.ascontiguousarray(T[:3].reshape(12)), delta[i], cos_t)
+            if photometric:
+                xi = solve_joint(sums[:NSUMS], sums[NSUMS:], inl[0], inl[1], lam2)
+                inl = inl[0]
+            else:
+                xi = solve(sums, inl)
             if level == 0:
                 inliers, vertices = inl, nv
-            xi = solve(sums, inl)
             if xi is None:
                 degenerate |= level == 0
                 break
@@ -138,14 +157,25 @@ def check_params(iters, delta, theta):
     return tuple(iters), tuple(float(d) for d in delta), float(theta)
 
 
+def check_photometric(photometric, rho, grad_min):
+    """(lambda, rho, g_min) as floats; each must be a finite number >= 0"""
+    for name, v in (("photometric", photometric), ("rho", rho), ("grad_min", grad_min)):
+        if not (isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v) and v >= 0):
+            raise ValueError("%s must be a finite number >= 0, got %r" % (name, v))
+    return float(photometric), float(rho), float(grad_min)
+
+
 class Tracker:
     """Pyramids of one frame size on CUDA device `device` (mccnn_track_*); :meth:`track` poses one frame against the
-    model's depth map."""
+    model's depth map.  With `photometric` lambda > 0 (metres per grey level; 0, the default, is off), each step also
+    aligns the frame's left image to the previous frame's (DESIGN §26), gated by `rho` (grey levels) and `grad_min`
+    (grey levels per level pixel)."""
 
-    def __init__(self, H, W, device=0, iters=ITERS, delta=DELTA, theta=THETA):
+    def __init__(self, H, W, device=0, iters=ITERS, delta=DELTA, theta=THETA, photometric=0.0, rho=RHO, grad_min=GRAD_MIN):
         if not (isinstance(H, int) and isinstance(W, int) and H >= 1 and W >= 1):
             raise ValueError("H and W must be integers >= 1, got %r, %r" % (H, W))
         self.iters, self.delta, self.theta = check_params(iters, delta, theta)
+        self.photometric, self.rho, self.grad_min = check_photometric(photometric, rho, grad_min)
         self.H, self.W = H, W
         self.dev = torch.device("cuda", int(device))
         self._h = ctypes.c_void_p()
@@ -153,6 +183,8 @@ class Tracker:
             adcensus._check(adcensus.lib().mccnn_track_create(ctypes.byref(self._h), H, W, self.dev.index), "mccnn_track_create")
         self._sums = np.zeros(NSUMS)
         self._counts = np.zeros(2, np.int64)
+        self._psums = np.zeros(2 * NSUMS)
+        self._pcounts = np.zeros(3, np.int64)
 
     def _handle(self):
         if not self._h:
@@ -171,6 +203,43 @@ class Tracker:
                 self._handle(), level, pose12.ctypes.data, delta, cos_t, self._sums.ctypes.data, self._counts.ctypes.data,
                 torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_step")
         return self._sums.copy(), int(self._counts[0]), int(self._counts[1])
+
+    def _step_photometric(self, level, pose12, delta, cos_t, grad_min=None, rho=None):
+        g_min, rho = self.grad_min if grad_min is None else grad_min, self.rho if rho is None else rho
+        with torch.cuda.device(self.dev):
+            adcensus._check(adcensus.lib().mccnn_track_step_photometric(
+                self._handle(), level, pose12.ctypes.data, delta, cos_t, g_min, rho, self._psums.ctypes.data,
+                self._pcounts.ctypes.data, torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_step_photometric")
+        return self._psums.copy(), (int(self._pcounts[0]), int(self._pcounts[1])), int(self._pcounts[2])
+
+    def intensity(self, which, img):
+        """the intensity pyramid of the (H, W) or (H, W, 3) uint8 image `img` (host or device): which is 'source' (the
+        frame's left image) or 'reference' (the previous frame's, with its gradients)"""
+        t, nch = depth._colour(img, self.H, self.W, self.dev)
+        with torch.cuda.device(self.dev):
+            adcensus._check(adcensus.lib().mccnn_track_intensity(self._handle(), ("source", "reference").index(which),
+                                                                 t.data_ptr(), nch, adcensus._stream(t)),
+                            "mccnn_track_intensity")
+
+    def intensity_maps(self, which, level):
+        """(I float32, g_x, g_y float64) of a level, each (ceil(H / 2^l), ceil(W / 2^l)) numpy, the gradients NaN where
+        undefined; the source has no gradients (None)"""
+        hl, wl = -(-self.H // (1 << level)), -(-self.W // (1 << level))
+        k = ("source", "reference").index(which)
+        with torch.cuda.device(self.dev):
+            I = torch.empty((hl, wl), dtype=torch.float32, device=self.dev)
+            G = torch.empty((2, hl, wl), dtype=torch.float64, device=self.dev) if k else None
+            adcensus._check(adcensus.lib().mccnn_track_intensity_maps(
+                self._handle(), k, level, I.data_ptr(), G[0].data_ptr() if k else None, G[1].data_ptr() if k else None,
+                torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_intensity_maps")
+            return (I.cpu().numpy(),) + ((G[0].cpu().numpy(), G[1].cpu().numpy()) if k else (None, None))
+
+    def step_photometric(self, level, pose, delta, cos_theta, grad_min=None, rho=None):
+        """one joint reduce at `level` for the relative pose `pose` (the tracker's gates unless given): (56 sums,
+        geometric then photometric, geometric inliers, photometric inliers, the level's source vertices)"""
+        s, (ng, nph), nv = self._step_photometric(level, fusion.pose12(pose), float(delta), float(cos_theta),
+                                                  None if grad_min is None else float(grad_min), None if rho is None else float(rho))
+        return s, ng, nph, nv
 
     def source(self, disp, cal, max_depth=None):
         """the source pyramid of the CUDA disparity map `disp`"""
@@ -203,13 +272,25 @@ class Tracker:
         """one reduce at `level` for the relative pose `pose`: (28 sums, inliers, the level's source vertices)"""
         return self._step(level, fusion.pose12(pose), float(delta), float(cos_theta))
 
-    def track(self, disp, cal, model_depth, W_prev, W_pred, max_depth=None):
+    def track(self, disp, cal, model_depth, W_prev, W_pred, max_depth=None, left=None, ref_left=None):
         """The pose of the frame of CUDA disparity map `disp`, aligned to `model_depth` (the model rendered at camera-to-world
-        W_prev) from the prediction W_pred: (4x4 pose, level-0 inliers, lost).  A lost frame's pose is W_pred."""
+        W_prev) from the prediction W_pred: (4x4 pose, level-0 inliers, lost).  A lost frame's pose is W_pred.  With the
+        photometric term, `left` is the frame's left image and `ref_left` the left image of the frame posed at W_prev;
+        both are required then, and refused without it."""
+        if self.photometric and (left is None or ref_left is None):
+            raise ValueError("the photometric term aligns the frame's left image to the previous frame's: give left and "
+                             "ref_left")
+        if not self.photometric and (left is not None or ref_left is not None):
+            raise ValueError("left and ref_left are the photometric term's images; the tracker's photometric weight is 0")
         Wp, Wq = as4(W_prev), as4(W_pred)
         self.source(disp, cal, max_depth)
         self.model(model_depth, cal)
-        T, inliers, lost = run_icp(self._step, rigid_inv(Wp) @ Wq, self.iters, self.delta, self.theta)
+        step = self._step
+        if self.photometric:
+            self.intensity("source", left)
+            self.intensity("reference", ref_left)
+            step = self._step_photometric
+        T, inliers, lost = run_icp(step, rigid_inv(Wp) @ Wq, self.iters, self.delta, self.theta, self.photometric)
         return (Wq if lost else Wp @ T), inliers, lost
 
     def close(self):

@@ -33,6 +33,14 @@ drive needs no oxts/.  -poses refine predicts by the OXTS increment instead.  A 
 (KITTI odometry format).  -traj (which needs oxts/) prints one line per drive against the OXTS poses: ate, rpe_t, rpe_r,
 t_err (%) and r_err (deg/m) over 100 .. 800 m segments, and their count.  -score scores renders at the tracked poses.
 Refused as well: -poses track or refine without -mesh, -traj without them, and an existing poses.txt.
+
+    python tools/fuse_raw.py kitti census -drive D -out O -voxel 0.05 -mesh -poses track -photometric 0.01 [-rho 30] \\
+        [-grad_min 2]
+
+-photometric lambda (metres per grey level; 0, the default, is off) adds a photometric term to the tracking (DESIGN §26):
+each frame's left image is aligned to the previous frame's, which fixes motion along a street whose surfaces' normals all
+lie across it.  -rho (grey levels) and -grad_min (grey levels per pixel) gate its pixels.  Refused as well: -photometric
+without -poses track or refine, and a -photometric, -rho or -grad_min that is not a finite number >= 0.
 """
 import argparse
 import math
@@ -65,6 +73,10 @@ def parser():
     ap.add_argument("-poses", choices=("oxts", "track", "refine"), default="oxts",
                     help="the frames' poses: the OXTS records, or tracked against the field (with -mesh)")
     ap.add_argument("-traj", action="store_true", help="with -poses track or refine: print the trajectory's errors against OXTS")
+    ap.add_argument("-photometric", type=float, default=None,
+                    help="with -poses track or refine: the photometric term's weight in metres per grey level (0: off)")
+    ap.add_argument("-rho", type=float, default=30.0, help="with -photometric: the largest residual of an inlier, grey levels")
+    ap.add_argument("-grad_min", type=float, default=2.0, help="with -photometric: the smallest gradient of an inlier")
     return ap
 
 
@@ -104,6 +116,12 @@ def parse_args(argv=None):
         raise SystemExit("fuse_raw.py: -poses %s tracks each frame against the distance field; it needs -mesh" % args.poses)
     if args.traj and args.poses == "oxts":
         raise SystemExit("fuse_raw.py: -traj compares tracked poses with OXTS; it needs -poses track or refine")
+    if args.photometric is not None and args.poses == "oxts":
+        raise SystemExit("fuse_raw.py: -photometric weighs a term of the tracking; it needs -poses track or refine")
+    for name in ("photometric", "rho", "grad_min"):
+        v = getattr(args, name)
+        if v is not None and not (math.isfinite(v) and v >= 0):
+            raise SystemExit("fuse_raw.py: -%s must be a finite number >= 0" % name)
     if args.score and not 0 < args.min_depth <= 80.0:
         raise SystemExit("fuse_raw.py: -min_depth must be in (0, 80]")
     for d in args.drive:
@@ -121,7 +139,8 @@ def main(argv=None):
                min_frames=args.min_frames, max_depth=args.max_depth, every=args.every, confidence=args.confidence,
                density=args.density, disp_max=args.disp_max, device=args.gpu - 1,
                **(dict(mesh=True, trunc=args.trunc, score=args.score, crop=args.crop, min_depth=args.min_depth,
-                       poses=args.poses, traj=args.traj) if args.mesh else {}))
+                       poses=args.poses, traj=args.traj) if args.mesh else {}),
+               **(dict(photometric=args.photometric, rho=args.rho, grad_min=args.grad_min) if args.photometric else {}))
     return 0
 
 
