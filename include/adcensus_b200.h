@@ -891,9 +891,13 @@ void mccnn_tsdf_destroy(mccnn_tsdf *h);
  * projects into the model with this camera.
  * mccnn_track_step: one projective point-to-plane ICP reduce at `level` for the source-to-model pose pose12 ([R | t]):
  * sums (28 host float64) receives the upper triangle of J^T J row by row, J^T r and r^2 over the inlier pixels, summed in
- * DESIGN §25's fixed tree; counts (2 host int64) the inliers and the level's source vertices.  One device-to-host copy;
- * the stream is synchronised.  Refuses (ADCENSUS_EINVAL) a level outside [0, MCCNN_TRACK_LEVELS), a non-finite pose,
- * delta not finite or <= 0, cos_theta outside [-1, 1], NULL outputs, and a handle without both pyramids.
+ * DESIGN §25's fixed tree.  With gates = {g_min, rho} (host), the photometric term of each pixel (DESIGN §26) is reduced
+ * in the same pass and tree: sums (56 host float64) then receives those 28 geometric sums, bit for bit the gate-less
+ * step's, followed by the 28 photometric ones.  counts (3 host int64) gets the geometric inliers, the photometric
+ * inliers (0 without gates) and the level's source vertices.  One device-to-host copy; the stream is synchronised.
+ * Refuses (ADCENSUS_EINVAL) a level outside [0, MCCNN_TRACK_LEVELS), a non-finite pose, delta not finite or <= 0,
+ * cos_theta outside [-1, 1], NULL outputs and a handle without both pyramids; with gates also g_min or rho not finite or
+ * < 0 and a handle without both intensity pyramids.
  * mccnn_track_maps: a level's vertices and normals (`which` 0 source, 1 model) into two DEVICE arrays of 3 planes (x, y,
  * z) of ceil(H / 2^l) ceil(W / 2^l) float64 each.
  * Every argument is checked before any launch; all asynchronous on `stream` except the step's read-back. */
@@ -904,25 +908,18 @@ int mccnn_track_create(mccnn_track **out, int H, int W, int device);
 int mccnn_track_source(mccnn_track *h, const float *disp, float f, float cx, float cy, float fB, float doffs, float max_depth,
 		       adcensus_stream_t stream);
 int mccnn_track_model(mccnn_track *h, const float *depth, float f, float cx, float cy, adcensus_stream_t stream);
-int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double *sums,
-		     long long *counts, adcensus_stream_t stream);
+int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, const double *gates,
+		     double *sums, long long *counts, adcensus_stream_t stream);
 int mccnn_track_maps(const mccnn_track *h, int which, int level, double *vertices, double *normals, adcensus_stream_t stream);
-/* The photometric term (DESIGN §26).  Its memory is allocated by the first mccnn_track_intensity, so a tracker that never
- * uses it is no larger.
+/* The photometric term's pyramids (DESIGN §26).  Their memory is allocated by the first mccnn_track_intensity; a tracker
+ * that never uses them keeps only the step's 28 rows of photometric chunk sums more.
  * mccnn_track_intensity: the intensity pyramid of the DEVICE (H,W) grey (nch 1) or (H,W,3) R, G, B (nch 3) byte image
  * `img`: `which` 0 the source (the frame's left image), 1 the reference (the left image of the frame the model was
  * rendered at), which also gets its g_x and g_y planes.  Refuses which outside {0, 1} and nch outside {1, 3}.
- * mccnn_track_step_photometric: mccnn_track_step's reduce, plus the photometric term of each pixel in the same pass and
- * tree: sums (56 host float64) receives the 28 geometric sums (mccnn_track_step's bits), then the 28 photometric ones;
- * counts (3 host int64) the geometric inliers, the photometric inliers and the level's source vertices.  One
- * device-to-host copy; the stream is synchronised.  Refuses what mccnn_track_step refuses, g_min or rho not finite or < 0,
- * and a handle without both intensity pyramids.
  * mccnn_track_intensity_maps: a level's intensities (ceil(H / 2^l) ceil(W / 2^l) float32) into the DEVICE array I, and for
  * the reference its g_x and g_y (float64 each, NaN on the level's border) into gx and gy, which must be NULL for the
  * source. */
 int mccnn_track_intensity(mccnn_track *h, int which, const unsigned char *img, int nch, adcensus_stream_t stream);
-int mccnn_track_step_photometric(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double g_min,
-				 double rho, double *sums, long long *counts, adcensus_stream_t stream);
 int mccnn_track_intensity_maps(const mccnn_track *h, int which, int level, float *I, double *gx, double *gy,
 			       adcensus_stream_t stream);
 void mccnn_track_destroy(mccnn_track *h);

@@ -23,6 +23,21 @@ static inline cudaStream_t adc_stream(adcensus_stream_t s) { return (cudaStream_
 
 static inline int adc_div_up(long a, long b) { return (int)((a + b - 1) / b); }
 
+// makes `device` current for the scope of one call and restores the caller's device
+struct DeviceScope {
+	int prev = -1;
+	int rc = 0;
+	explicit DeviceScope(int device)
+	{
+		rc = (int)cudaGetDevice(&prev);
+		if (!rc && prev != device) rc = (int)cudaSetDevice(device);
+	}
+	~DeviceScope()
+	{
+		if (prev >= 0) cudaSetDevice(prev);
+	}
+};
+
 // number of SMs of the current device (cached per device; 132 on H100 SXM)
 int adc_num_sms();
 

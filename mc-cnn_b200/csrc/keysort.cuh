@@ -214,19 +214,4 @@ __global__ void __launch_bounds__(THREADS) match_rank_kernel(const u64 *__restri
 
 long grid_for(long long n) { return std::max<long>(1, std::min<long long>((n + THREADS - 1) / THREADS, (long long)adc_num_sms() * 8)); }
 
-// makes `device` current for the scope of one call and restores the caller's device
-struct DeviceScope {
-	int prev = -1;
-	int rc = 0;
-	explicit DeviceScope(int device)
-	{
-		rc = (int)cudaGetDevice(&prev);
-		if (!rc && prev != device) rc = (int)cudaSetDevice(device);
-	}
-	~DeviceScope()
-	{
-		if (prev >= 0) cudaSetDevice(prev);
-	}
-};
-
 }  // namespace

@@ -10,12 +10,11 @@
 // an integer, summed by atomics.  One device-to-host copy per step returns the sums and the counts.
 //
 // The photometric term (DESIGN §26): intensity pyramids of the frame's left image and of the previous frame's (with its
-// gradients), allocated on first use; mccnn_track_step_photometric reduces each pixel's geometric terms and then its
-// photometric ones through the same tree and shared buffer, in one pass and one read-back.
+// gradients), allocated on first use; given gates, the same step kernel reduces each pixel's photometric terms after its
+// geometric ones, through the same tree and shared buffer, in one pass and one read-back.
 #include <math.h>
 
 #include "camera.cuh"
-#include "keysort.cuh"
 
 namespace {
 
@@ -139,18 +138,11 @@ __device__ __forceinline__ double quad(const double (*J)[7], int a, int b)
 			 __dadd_rn(__dmul_rn(J[1][a], J[1][b]), __dmul_rn(J[3][a], J[3][b])));
 }
 
-// one block per chunk of 1024 pixels: thread t holds pixels t, t + 256, t + 512, t + 768 and takes the first two
-// halvings in registers ((a_t + a_t+512) + (a_t+256 + a_t+768)); strides 128, 64 and 32 go through shared memory and
-// 16 .. 1 through warp shuffles.  The chunk's 28 sums go to part[k P + chunk]; the inliers to *inliers.
-__global__ void __launch_bounds__(RT) step_kernel(Maps S, Maps M, Pose T, Step st, double *__restrict__ part, int P,
-						  unsigned long long *__restrict__ inliers)
+// the tree over the four pixels' terms of each thread (pixel p at t + 256 p): the first two halvings in registers
+// ((a_t + a_t+512) + (a_t+256 + a_t+768)), strides 128, 64 and 32 through the shared buffer sh, 16 .. 1 through warp
+// shuffles; the chunk's 28 sums to part[k P + chunk]
+__device__ __forceinline__ void reduce_chunk(const double (*J)[7], double *sh, double *__restrict__ part, int P)
 {
-	__shared__ double sh[NS * 128];
-	const long long base = (long long)blockIdx.x * CH + threadIdx.x;
-	double J[4][7];
-	int cnt = 0;
-#pragma unroll
-	for (int p = 0; p < 4; p++) cnt += pixel_term(base + p * RT, S, M, T, st, J[p]);
 	double s[NS];
 	{
 		int k = 0;
@@ -182,37 +174,6 @@ __global__ void __launch_bounds__(RT) step_kernel(Maps S, Maps M, Pose T, Step s
 		if (threadIdx.x == 0)
 #pragma unroll
 			for (int k = 0; k < NS; k++) part[(long long)k * P + blockIdx.x] = s[k];
-	}
-	const int total = __reduce_add_sync(0xffffffffu, cnt);
-	if ((threadIdx.x & 31) == 0 && total) atomicAdd(inliers, (unsigned long long)total);
-}
-
-// rows of chunk sums (row k at part[k P]) padded with +0.0 from n to P (a power of two), reduced by stride halving in
-// place; one block of RED threads
-__device__ __forceinline__ void halve_rows(double *__restrict__ part, int rows, int n, int P)
-{
-	for (long long e = threadIdx.x; e < (long long)rows * (P - n); e += RED) part[(e / (P - n)) * P + n + e % (P - n)] = 0.0;
-	__syncthreads();
-	for (int stride = P >> 1; stride >= 1; stride >>= 1) {
-		for (long long e = threadIdx.x; e < (long long)rows * stride; e += RED) {
-			const long long k = e / stride, i = e % stride;
-			part[k * P + i] = __dadd_rn(part[k * P + i], part[k * P + i + stride]);
-		}
-		__syncthreads();
-	}
-}
-
-// the chunk sums padded with +0.0 to P (a power of two), reduced by stride halving in place; out = the 28 sums, then the
-// inliers and the level's source vertices as int64
-__global__ void __launch_bounds__(RED) chunk_reduce_kernel(double *__restrict__ part, int n, int P,
-							   const unsigned long long *__restrict__ inliers,
-							   const unsigned long long *__restrict__ nvert, double *__restrict__ out)
-{
-	halve_rows(part, NS, n, P);
-	if (threadIdx.x < NS) out[threadIdx.x] = part[(long long)threadIdx.x * P];
-	if (threadIdx.x == 0) {
-		((long long *)out)[NS] = (long long)*inliers;
-		((long long *)out)[NS + 1] = (long long)*nvert;
 	}
 }
 
@@ -317,49 +278,12 @@ __device__ __forceinline__ bool photo_term(long long i, const Maps &S, const Map
 	return true;
 }
 
-// step_kernel's tree over the four pixels' terms of each thread: the first two halvings in registers, strides 128 .. 32
-// through sh, 16 .. 1 through warp shuffles; the chunk's 28 sums to part[k P + chunk]
-__device__ __forceinline__ void reduce_chunk(const double (*J)[7], double *sh, double *__restrict__ part, int P)
-{
-	double s[NS];
-	{
-		int k = 0;
-#pragma unroll
-		for (int a = 0; a < 6; a++)
-#pragma unroll
-			for (int b = a; b < 6; b++, k++) s[k] = quad(J, a, b);
-#pragma unroll
-		for (int a = 0; a < 6; a++) s[21 + a] = quad(J, a, 6);
-		s[27] = quad(J, 6, 6);
-	}
-#pragma unroll
-	for (int stride = 128; stride >= 32; stride >>= 1) {
-		const int t = threadIdx.x;
-		if (t >= stride && t < 2 * stride)
-#pragma unroll
-			for (int k = 0; k < NS; k++) sh[k * stride + t - stride] = s[k];
-		__syncthreads();
-		if (t < stride)
-#pragma unroll
-			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], sh[k * stride + t]);
-		__syncthreads();
-	}
-	if (threadIdx.x < 32) {
-#pragma unroll
-		for (int off = 16; off >= 1; off >>= 1)
-#pragma unroll
-			for (int k = 0; k < NS; k++) s[k] = __dadd_rn(s[k], __shfl_down_sync(0xffffffffu, s[k], off));
-		if (threadIdx.x == 0)
-#pragma unroll
-			for (int k = 0; k < NS; k++) part[(long long)k * P + blockIdx.x] = s[k];
-	}
-}
-
-// one block per chunk of 1024 pixels, as step_kernel: the geometric terms (pixel_term) are reduced first, then the
-// photometric ones through the same shared buffer; rows 0 .. 27 of part get the geometric chunk sums, rows 28 .. 55 the
-// photometric ones; inliers[0] and [1] the two inlier counts
-__global__ void __launch_bounds__(RT) step_photometric_kernel(Maps S, Maps M, Pose T, Step st, Photo ph, double *__restrict__ part,
-							      int P, unsigned long long *__restrict__ inliers)
+// one block per chunk of 1024 pixels: the geometric terms (pixel_term) go through reduce_chunk into rows 0 .. 27 of
+// part, and with PHOTO the photometric ones (photo_term) then through the same shared buffer into rows 28 .. 55;
+// inliers[0] and [1] get the geometric and the photometric inlier counts
+template <bool PHOTO>
+__global__ void __launch_bounds__(RT) step_kernel(Maps S, Maps M, Pose T, Step st, Photo ph, double *__restrict__ part, int P,
+						  unsigned long long *__restrict__ inliers)
 {
 	__shared__ double sh[NS * 128];
 	const long long base = (long long)blockIdx.x * CH + threadIdx.x;
@@ -370,31 +294,39 @@ __global__ void __launch_bounds__(RT) step_photometric_kernel(Maps S, Maps M, Po
 		for (int p = 0; p < 4; p++) cg += pixel_term(base + p * RT, S, M, T, st, J[p]);
 		reduce_chunk(J, sh, part, P);
 	}
-	{
+	if (PHOTO) {
 		double J[4][7];
 #pragma unroll
 		for (int p = 0; p < 4; p++) cp += photo_term(base + p * RT, S, M, T, st, ph, J[p]);
 		reduce_chunk(J, sh, part + (long long)NS * P, P);
 	}
-	const int tg = __reduce_add_sync(0xffffffffu, cg), tp = __reduce_add_sync(0xffffffffu, cp);
+	const int tg = __reduce_add_sync(0xffffffffu, cg), tp = PHOTO ? __reduce_add_sync(0xffffffffu, cp) : 0;
 	if ((threadIdx.x & 31) == 0) {
 		if (tg) atomicAdd(inliers, (unsigned long long)tg);
 		if (tp) atomicAdd(inliers + 1, (unsigned long long)tp);
 	}
 }
 
-// the 56 rows of chunk sums reduced as chunk_reduce_kernel's; out = the 56 sums, then the geometric and the photometric
-// inliers and the level's source vertices as int64
-__global__ void __launch_bounds__(RED) chunk_reduce_photometric_kernel(double *__restrict__ part, int n, int P,
-								       const unsigned long long *__restrict__ inliers,
-								       const unsigned long long *__restrict__ nvert, double *__restrict__ out)
+// `rows` rows of chunk sums (row k at part[k P]) padded with +0.0 from n to P (a power of two), reduced by stride halving
+// in place; out = the rows' sums, then the geometric and the photometric inliers and the level's source vertices as int64
+__global__ void __launch_bounds__(RED) chunk_reduce_kernel(double *__restrict__ part, int rows, int n, int P,
+							   const unsigned long long *__restrict__ inliers,
+							   const unsigned long long *__restrict__ nvert, double *__restrict__ out)
 {
-	halve_rows(part, 2 * NS, n, P);
-	if (threadIdx.x < 2 * NS) out[threadIdx.x] = part[(long long)threadIdx.x * P];
+	for (long long e = threadIdx.x; e < (long long)rows * (P - n); e += RED) part[(e / (P - n)) * P + n + e % (P - n)] = 0.0;
+	__syncthreads();
+	for (int stride = P >> 1; stride >= 1; stride >>= 1) {
+		for (long long e = threadIdx.x; e < (long long)rows * stride; e += RED) {
+			const long long k = e / stride, i = e % stride;
+			part[k * P + i] = __dadd_rn(part[k * P + i], part[k * P + i + stride]);
+		}
+		__syncthreads();
+	}
+	if (threadIdx.x < rows) out[threadIdx.x] = part[(long long)threadIdx.x * P];
 	if (threadIdx.x == 0) {
-		((long long *)out)[2 * NS] = (long long)inliers[0];
-		((long long *)out)[2 * NS + 1] = (long long)inliers[1];
-		((long long *)out)[2 * NS + 2] = (long long)*nvert;
+		((long long *)out)[rows] = (long long)inliers[0];
+		((long long *)out)[rows + 1] = (long long)inliers[1];
+		((long long *)out)[rows + 2] = (long long)*nvert;
 	}
 }
 
@@ -408,16 +340,15 @@ struct mccnn_track {
 	long long off[LEVELS];                        // each level's first double in a pyramid
 	long long pyr;                                // doubles per pyramid
 	int P;                                        // chunk sums per term: the level-0 chunk count rounded up to 2^k
-	double *mem;                                  // source pyramid, model pyramid, chunk sums, out
-	unsigned long long *ctr;                      // inliers, then the source vertices per level
-	double *host;                                 // pinned: the 30 values read back per step
+	double *mem;                                  // source pyramid, model pyramid, 2 NS rows of P chunk sums, out
+	unsigned long long *ctr;                      // geometric and photometric inliers, then the source vertices per level
+	double *host;                                 // pinned: the up to 2 NS + 3 values read back per step
 	float mf, mcx, mcy;                           // the model's camera
 	bool have_source, have_model;
-	// the photometric term's memory, allocated by the first mccnn_track_intensity
+	// the photometric term's pyramids, allocated by the first mccnn_track_intensity
 	long long ioff[LEVELS], npix;                 // each level's first pixel in an intensity pyramid; pixels per pyramid
 	float *imem;                                  // the source's intensity pyramid, then the reference's
-	double *pmem;                                 // the reference's g_x, g_y pyramids, 56 rows of chunk sums, out, counters
-	double *phost;                                // pinned: the 59 values read back per photometric step
+	double *pmem;                                 // the reference's g_x, g_y pyramids
 	bool have_intensity[2];
 };
 
@@ -430,23 +361,17 @@ Maps level_maps(const mccnn_track *h, int which, int l)
 
 int build_pyramid(mccnn_track *h, int which, const float *src, const Cam &c, cudaStream_t s)
 {
-	if (which == 0) ADC_CUDA(cudaMemsetAsync(h->ctr + 1, 0, 8 * LEVELS, s));
+	if (which == 0) ADC_CUDA(cudaMemsetAsync(h->ctr + 2, 0, 8 * LEVELS, s));
 	for (int l = 0; l < LEVELS; l++) {
 		const long long np = (long long)h->hl[l] * h->wl[l];
 		const Maps m = level_maps(h, which, l);
 		vertex_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(src, which, h->W, l, h->hl[l], h->wl[l], c, m,
-								  which == 0 ? h->ctr + 1 + l : nullptr);
+								  which == 0 ? h->ctr + 2 + l : nullptr);
 		normal_kernel<<<adc_div_up(np, 256), 256, 0, s>>>(h->hl[l], h->wl[l], m);
 	}
 	ADC_CHECK_LAUNCH();
 	return 0;
 }
-
-// the photometric term's device layout: g_x and g_y pyramids, 2 NS rows of P chunk sums, the 2 NS + 3 outputs, then two
-// counters
-double *photo_part(const mccnn_track *h) { return h->pmem + 2 * h->npix; }
-double *photo_out(const mccnn_track *h) { return photo_part(h) + 2ll * NS * h->P; }
-unsigned long long *photo_ctr(const mccnn_track *h) { return (unsigned long long *)(photo_out(h) + 2 * NS + 3); }
 
 int photo_alloc(mccnn_track *h)
 {
@@ -458,18 +383,15 @@ int photo_alloc(mccnn_track *h)
 	}
 	h->npix = at;
 	float *im = nullptr;
-	double *pm = nullptr, *host = nullptr;
+	double *pm = nullptr;
 	cudaError_t e = cudaMalloc(&im, 4 * (size_t)(2 * at));
-	if (e == cudaSuccess) e = cudaMalloc(&pm, 8 * (size_t)(2 * at + 2ll * NS * h->P + 2 * NS + 3 + 2));
-	if (e == cudaSuccess) e = cudaMallocHost(&host, 8 * (2 * NS + 3));
+	if (e == cudaSuccess) e = cudaMalloc(&pm, 8 * (size_t)(2 * at));
 	if (e != cudaSuccess) {
 		if (im) cudaFree(im);
-		if (pm) cudaFree(pm);
 		return (int)e;
 	}
 	h->imem = im;
 	h->pmem = pm;
-	h->phost = host;
 	return 0;
 }
 
@@ -503,15 +425,15 @@ int mccnn_track_create(mccnn_track **out, int H, int W, int device)
 	const long long chunks = ((long long)H * W + CH - 1) / CH;
 	h->P = 1;
 	while (h->P < chunks) h->P <<= 1;
-	const size_t bytes = 8 * (size_t)(2 * h->pyr + (long long)NS * h->P + NS + 2) + 8 * (1 + LEVELS);
-	cudaError_t e = cudaMalloc(&h->mem, bytes);
-	if (e == cudaSuccess) e = cudaMallocHost(&h->host, 8 * (NS + 2));
+	const long long out_at = 2 * h->pyr + 2ll * NS * h->P;
+	cudaError_t e = cudaMalloc(&h->mem, 8 * (size_t)(out_at + 2 * NS + 3) + 8 * (2 + LEVELS));
+	if (e == cudaSuccess) e = cudaMallocHost(&h->host, 8 * (2 * NS + 3));
 	if (e != cudaSuccess) {
 		if (h->mem) cudaFree(h->mem);
 		delete h;
 		return (int)e;
 	}
-	h->ctr = (unsigned long long *)(h->mem + 2 * h->pyr + (long long)NS * h->P + NS + 2);
+	h->ctr = (unsigned long long *)(h->mem + out_at + 2 * NS + 3);
 	*out = h;
 	return 0;
 }
@@ -543,11 +465,13 @@ int mccnn_track_model(mccnn_track *h, const float *depth, float f, float cx, flo
 	return rc;
 }
 
-int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double *sums,
-		     long long *counts, adcensus_stream_t stream)
+int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, const double *gates,
+		     double *sums, long long *counts, adcensus_stream_t stream)
 {
 	if (!h || !sums || !counts || level < 0 || level >= LEVELS || !h->have_source || !h->have_model) return ADCENSUS_EINVAL;
 	if (!(delta > 0.0 && isfinite(delta) && cos_theta >= -1.0 && cos_theta <= 1.0)) return ADCENSUS_EINVAL;
+	if (gates && !(h->have_intensity[0] && h->have_intensity[1])) return ADCENSUS_EINVAL;
+	if (gates && !(gates[0] >= 0.0 && isfinite(gates[0]) && gates[1] >= 0.0 && isfinite(gates[1]))) return ADCENSUS_EINVAL;
 	Pose T;
 	int rc = check_pose(pose12, &T);
 	if (rc) return rc;
@@ -558,17 +482,26 @@ int mccnn_track_step(mccnn_track *h, int level, const double *pose12, double del
 	const int n = (int)(((long long)hl * wl + CH - 1) / CH);
 	int P = 1;
 	while (P < n) P <<= 1;
-	double *part = h->mem + 2 * h->pyr, *out = part + (long long)NS * h->P;
-	const Step st{hl, wl, (double)h->mf, (double)h->mcx, (double)h->mcy, ldexp(1.0, -level), delta * delta, cos_theta};
-	ADC_CUDA(cudaMemsetAsync(h->ctr, 0, 8, s));
-	step_kernel<<<n, RT, 0, s>>>(level_maps(h, 0, level), level_maps(h, 1, level), T, st, part, P, h->ctr);
-	chunk_reduce_kernel<<<1, RED, 0, s>>>(part, n, P, h->ctr, h->ctr + 1 + level, out);
+	const int rows = gates ? 2 * NS : NS;
+	double *part = h->mem + 2 * h->pyr, *out = part + 2ll * NS * h->P;
+	const double scale = ldexp(1.0, -level);
+	const Step st{hl, wl, (double)h->mf, (double)h->mcx, (double)h->mcy, scale, delta * delta, cos_theta};
+	const Maps S = level_maps(h, 0, level), M = level_maps(h, 1, level);
+	ADC_CUDA(cudaMemsetAsync(h->ctr, 0, 16, s));
+	if (gates) {
+		const long long o = h->ioff[level];
+		const Photo ph{h->imem + o, h->imem + h->npix + o, h->pmem + o, h->pmem + h->npix + o, gates[0] * gates[0], gates[1],
+			       (double)h->mf * scale};
+		step_kernel<true><<<n, RT, 0, s>>>(S, M, T, st, ph, part, P, h->ctr);
+	} else {
+		step_kernel<false><<<n, RT, 0, s>>>(S, M, T, st, Photo{}, part, P, h->ctr);
+	}
+	chunk_reduce_kernel<<<1, RED, 0, s>>>(part, rows, n, P, h->ctr, h->ctr + 2 + level, out);
 	ADC_CHECK_LAUNCH();
-	ADC_CUDA(cudaMemcpyAsync(h->host, out, 8 * (NS + 2), cudaMemcpyDeviceToHost, s));
+	ADC_CUDA(cudaMemcpyAsync(h->host, out, 8 * (rows + 3), cudaMemcpyDeviceToHost, s));
 	ADC_CUDA(cudaStreamSynchronize(s));
-	for (int k = 0; k < NS; k++) sums[k] = h->host[k];
-	counts[0] = ((const long long *)h->host)[NS];
-	counts[1] = ((const long long *)h->host)[NS + 1];
+	for (int k = 0; k < rows; k++) sums[k] = h->host[k];
+	for (int k = 0; k < 3; k++) counts[k] = ((const long long *)h->host)[rows + k];
 	return 0;
 }
 
@@ -613,41 +546,6 @@ int mccnn_track_intensity(mccnn_track *h, int which, const unsigned char *img, i
 	return 0;
 }
 
-int mccnn_track_step_photometric(mccnn_track *h, int level, const double *pose12, double delta, double cos_theta, double g_min,
-				 double rho, double *sums, long long *counts, adcensus_stream_t stream)
-{
-	if (!h || !sums || !counts || level < 0 || level >= LEVELS || !h->have_source || !h->have_model) return ADCENSUS_EINVAL;
-	if (!h->have_intensity[0] || !h->have_intensity[1]) return ADCENSUS_EINVAL;
-	if (!(delta > 0.0 && isfinite(delta) && cos_theta >= -1.0 && cos_theta <= 1.0)) return ADCENSUS_EINVAL;
-	if (!(g_min >= 0.0 && isfinite(g_min) && rho >= 0.0 && isfinite(rho))) return ADCENSUS_EINVAL;
-	Pose T;
-	int rc = check_pose(pose12, &T);
-	if (rc) return rc;
-	DeviceScope dev(h->device);
-	if (dev.rc) return dev.rc;
-	cudaStream_t s = adc_stream(stream);
-	const int hl = h->hl[level], wl = h->wl[level];
-	const int n = (int)(((long long)hl * wl + CH - 1) / CH);
-	int P = 1;
-	while (P < n) P <<= 1;
-	double *part = photo_part(h), *out = photo_out(h);
-	unsigned long long *ctr = photo_ctr(h);
-	const double scale = ldexp(1.0, -level);
-	const Step st{hl, wl, (double)h->mf, (double)h->mcx, (double)h->mcy, scale, delta * delta, cos_theta};
-	const long long o = h->ioff[level];
-	const Photo ph{h->imem + o, h->imem + h->npix + o, h->pmem + o, h->pmem + h->npix + o, g_min * g_min, rho,
-		       (double)h->mf * scale};
-	ADC_CUDA(cudaMemsetAsync(ctr, 0, 16, s));
-	step_photometric_kernel<<<n, RT, 0, s>>>(level_maps(h, 0, level), level_maps(h, 1, level), T, st, ph, part, P, ctr);
-	chunk_reduce_photometric_kernel<<<1, RED, 0, s>>>(part, n, P, ctr, h->ctr + 1 + level, out);
-	ADC_CHECK_LAUNCH();
-	ADC_CUDA(cudaMemcpyAsync(h->phost, out, 8 * (2 * NS + 3), cudaMemcpyDeviceToHost, s));
-	ADC_CUDA(cudaStreamSynchronize(s));
-	for (int k = 0; k < 2 * NS; k++) sums[k] = h->phost[k];
-	for (int k = 0; k < 3; k++) counts[k] = ((const long long *)h->phost)[2 * NS + k];
-	return 0;
-}
-
 int mccnn_track_intensity_maps(const mccnn_track *h, int which, int level, float *I, double *gx, double *gy,
 			       adcensus_stream_t stream)
 {
@@ -675,7 +573,6 @@ void mccnn_track_destroy(mccnn_track *h)
 			if (h->host) cudaFreeHost(h->host);
 			if (h->imem) cudaFree(h->imem);
 			if (h->pmem) cudaFree(h->pmem);
-			if (h->phost) cudaFreeHost(h->phost);
 		}
 	}
 	delete h;

@@ -107,25 +107,24 @@ def update(T, xi):
 
 def run_icp(step, T, iters=ITERS, delta=DELTA, theta=THETA, photometric=0.0):
     """The ICP levels from the coarsest to the finest from the relative pose T (4x4, source camera to model camera).
-    step(level, pose12, delta, cos_theta) returns (28 sums, inliers, the level's source vertices).  Returns (T, level-0
-    inliers, lost): lost when a level-0 solve was degenerate or its inliers are fewer than LOST_SHARE of its vertices.
-    With `photometric` lambda > 0 (metres per grey level), step returns (56 sums: geometric then photometric,
-    (geometric inliers, photometric inliers), vertices) and each solve is :func:`solve_joint`'s; the inliers of the lost
-    rule stay the geometric ones (DESIGN §26)."""
+    step(level, pose12, delta, cos_theta) returns (sums, geometric inliers, photometric inliers, the level's source
+    vertices), as :meth:`Tracker.step`.  Returns (T, level-0 inliers, lost): lost when a level-0 solve was degenerate or
+    its inliers are fewer than LOST_SHARE of its vertices.  Each solve is :func:`solve`'s of the 28 geometric sums, or
+    with `photometric` lambda > 0 (metres per grey level) :func:`solve_joint`'s of the 56 sums, geometric then
+    photometric; the inliers of the lost rule stay the geometric ones (DESIGN §26)."""
     cos_t = math.cos(math.radians(theta))
     lam2 = photometric * photometric
     inliers, vertices, degenerate = 0, 0, False
     for i in range(LEVELS):
         level = LEVELS - 1 - i
         for _ in range(iters[i]):
-            sums, inl, nv = step(level, np.ascontiguousarray(T[:3].reshape(12)), delta[i], cos_t)
+            sums, ng, nph, nv = step(level, np.ascontiguousarray(T[:3].reshape(12)), delta[i], cos_t)
             if photometric:
-                xi = solve_joint(sums[:NSUMS], sums[NSUMS:], inl[0], inl[1], lam2)
-                inl = inl[0]
+                xi = solve_joint(sums[:NSUMS], sums[NSUMS:], ng, nph, lam2)
             else:
-                xi = solve(sums, inl)
+                xi = solve(sums[:NSUMS], ng)
             if level == 0:
-                inliers, vertices = inl, nv
+                inliers, vertices = ng, nv
             if xi is None:
                 degenerate |= level == 0
                 break
@@ -181,10 +180,9 @@ class Tracker:
         self._h = ctypes.c_void_p()
         with torch.cuda.device(self.dev):
             adcensus._check(adcensus.lib().mccnn_track_create(ctypes.byref(self._h), H, W, self.dev.index), "mccnn_track_create")
-        self._sums = np.zeros(NSUMS)
-        self._counts = np.zeros(2, np.int64)
-        self._psums = np.zeros(2 * NSUMS)
-        self._pcounts = np.zeros(3, np.int64)
+        # the step's host buffers, and their addresses taken once: ndarray.ctypes costs microseconds on every access
+        self._sums, self._counts, self._gates = np.zeros(2 * NSUMS), np.zeros(3, np.int64), np.zeros(2)
+        self._ptrs = (self._sums.ctypes.data, self._counts.ctypes.data, self._gates.ctypes.data)
 
     def _handle(self):
         if not self._h:
@@ -197,20 +195,15 @@ class Tracker:
             raise ValueError("%s: %s is %dx%d on %s, the tracker %dx%d on %s" % (fn, name, H, W, m.device, self.H, self.W, self.dev))
         return m
 
-    def _step(self, level, pose12, delta, cos_t):
+    def _step(self, level, pose12, delta, cos_t, gates=None):
+        sums, counts, g = self._ptrs
+        if gates is not None:
+            self._gates[:] = gates
         with torch.cuda.device(self.dev):
             adcensus._check(adcensus.lib().mccnn_track_step(
-                self._handle(), level, pose12.ctypes.data, delta, cos_t, self._sums.ctypes.data, self._counts.ctypes.data,
+                self._handle(), level, pose12.ctypes.data, delta, cos_t, None if gates is None else g, sums, counts,
                 torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_step")
-        return self._sums.copy(), int(self._counts[0]), int(self._counts[1])
-
-    def _step_photometric(self, level, pose12, delta, cos_t, grad_min=None, rho=None):
-        g_min, rho = self.grad_min if grad_min is None else grad_min, self.rho if rho is None else rho
-        with torch.cuda.device(self.dev):
-            adcensus._check(adcensus.lib().mccnn_track_step_photometric(
-                self._handle(), level, pose12.ctypes.data, delta, cos_t, g_min, rho, self._psums.ctypes.data,
-                self._pcounts.ctypes.data, torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_step_photometric")
-        return self._psums.copy(), (int(self._pcounts[0]), int(self._pcounts[1])), int(self._pcounts[2])
+        return (self._sums[:NSUMS if gates is None else 2 * NSUMS].copy(), *self._counts.tolist())
 
     def intensity(self, which, img):
         """the intensity pyramid of the (H, W) or (H, W, 3) uint8 image `img` (host or device): which is 'source' (the
@@ -233,13 +226,6 @@ class Tracker:
                 self._handle(), k, level, I.data_ptr(), G[0].data_ptr() if k else None, G[1].data_ptr() if k else None,
                 torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_intensity_maps")
             return (I.cpu().numpy(),) + ((G[0].cpu().numpy(), G[1].cpu().numpy()) if k else (None, None))
-
-    def step_photometric(self, level, pose, delta, cos_theta, grad_min=None, rho=None):
-        """one joint reduce at `level` for the relative pose `pose` (the tracker's gates unless given): (56 sums,
-        geometric then photometric, geometric inliers, photometric inliers, the level's source vertices)"""
-        s, (ng, nph), nv = self._step_photometric(level, fusion.pose12(pose), float(delta), float(cos_theta),
-                                                  None if grad_min is None else float(grad_min), None if rho is None else float(rho))
-        return s, ng, nph, nv
 
     def source(self, disp, cal, max_depth=None):
         """the source pyramid of the CUDA disparity map `disp`"""
@@ -268,9 +254,11 @@ class Tracker:
                                                             torch.cuda.current_stream(self.dev).cuda_stream), "mccnn_track_maps")
             return V.cpu().numpy(), N.cpu().numpy()
 
-    def step(self, level, pose, delta, cos_theta):
-        """one reduce at `level` for the relative pose `pose`: (28 sums, inliers, the level's source vertices)"""
-        return self._step(level, fusion.pose12(pose), float(delta), float(cos_theta))
+    def step(self, level, pose, delta, cos_theta, gates=None):
+        """one reduce at `level` for the relative pose `pose`: (sums, geometric inliers, photometric inliers, the level's
+        source vertices).  Without `gates` the 28 geometric sums and 0 photometric inliers; with gates = (g_min, rho) the
+        joint reduce's 56 sums, geometric then photometric (both intensity pyramids are needed)"""
+        return self._step(level, fusion.pose12(pose), float(delta), float(cos_theta), gates)
 
     def track(self, disp, cal, model_depth, W_prev, W_pred, max_depth=None, left=None, ref_left=None):
         """The pose of the frame of CUDA disparity map `disp`, aligned to `model_depth` (the model rendered at camera-to-world
@@ -285,12 +273,13 @@ class Tracker:
         Wp, Wq = as4(W_prev), as4(W_pred)
         self.source(disp, cal, max_depth)
         self.model(model_depth, cal)
-        step = self._step
+        gates = None
         if self.photometric:
             self.intensity("source", left)
             self.intensity("reference", ref_left)
-            step = self._step_photometric
-        T, inliers, lost = run_icp(step, rigid_inv(Wp) @ Wq, self.iters, self.delta, self.theta, self.photometric)
+            gates = (self.grad_min, self.rho)
+        T, inliers, lost = run_icp(lambda *a: self._step(*a, gates), rigid_inv(Wp) @ Wq, self.iters, self.delta, self.theta,
+                                   self.photometric)
         return (Wq if lost else Wp @ T), inliers, lost
 
     def close(self):

@@ -111,7 +111,7 @@ def test_sums_and_counts_are_the_oracle():
                     assert got[1:] == want[1:], "%s: counts %s vs %s" % (what, got[1:], want[1:])
                     assert np.array_equal(got[0].view(np.uint64), want[0].view(np.uint64)), what
                     if model == "rendered" and k == 0:
-                        assert got[1] > 0.3 * got[2], what
+                        assert got[1] > 0.3 * got[3], what
                     if model == "empty" or k >= 5:
                         assert got[1] == 0 and not got[0].any(), what
 
@@ -124,9 +124,9 @@ def test_abi_refusals():
     assert lib.mccnn_track_create(ctypes.byref(h), 1 << 16, 1 << 15, 0) == -2
     assert lib.mccnn_track_create(ctypes.byref(h), 4, 5, 0) == 0
     s = torch.cuda.current_stream().cuda_stream
-    sums, counts = np.zeros(28), np.zeros(2, np.int64)
+    sums, counts = np.zeros(28), np.zeros(3, np.int64)
     pose = np.eye(4)[:3].reshape(-1).copy()
-    step = (h, 0, pose.ctypes.data, 0.5, 0.5, sums.ctypes.data, counts.ctypes.data, s)
+    step = (h, 0, pose.ctypes.data, 0.5, 0.5, None, sums.ctypes.data, counts.ctypes.data, s)
     assert lib.mccnn_track_step(*step) == -1                      # no pyramids yet
     d = torch.ones((4, 5), device="cuda")
     V = torch.empty(3 * 20, dtype=torch.float64, device="cuda")
@@ -146,7 +146,7 @@ def test_abi_refusals():
     bad_pose = pose.copy()
     bad_pose[3] = np.nan
     for k, v in ((0, None), (1, -1), (1, 3), (2, None), (2, bad_pose.ctypes.data), (3, 0.0), (3, float("inf")), (4, 1.5),
-                 (4, float("nan")), (5, None), (6, None)):
+                 (4, float("nan")), (6, None), (7, None)):
         args = list(step)
         args[k] = v
         assert lib.mccnn_track_step(*args) == -1, "step argument %d = %r" % (k, v)

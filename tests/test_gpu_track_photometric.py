@@ -1,6 +1,6 @@
-"""GPU: the photometric term of tracking (DESIGN §26) -- mccnn_track_intensity / _step_photometric bit for bit against the
-numpy restatement (tests/track_photometric_oracle.py): intensity pyramids and gradients, the 56 sums and 3 counts at
-every level, the geometric half against mccnn_track_step, a whole tracked street drive twice; tools/fuse_raw.py
+"""GPU: the photometric term of tracking (DESIGN §26) -- mccnn_track_intensity / mccnn_track_step with gates bit for bit
+against the numpy restatement (tests/track_photometric_oracle.py): intensity pyramids and gradients, the 56 sums and 3
+counts at every level, the geometric half against the gate-less step, a whole tracked street drive twice; tools/fuse_raw.py
 -photometric with census against the oracle loop, and -photometric 0 against no flag; the accuracy on a street, where
 geometry alone cannot fix motion along it, and on the default drive."""
 import ctypes
@@ -121,14 +121,14 @@ def test_sums_and_counts_are_the_oracle():
             tr.model(cu(Zm if model == "rendered" else np.full_like(Zm, np.nan)), cal)
             for k, (T, delta, cos_t, g_min, rho) in enumerate(cases):
                 for level in range(3):
-                    got = tr.step_photometric(level, T, delta, cos_t, g_min, rho)
+                    got = tr.step(level, T, delta, cos_t, (g_min, rho))
                     want = po.step(src, mref, isrc, iref, cal, level, T[:3].reshape(12), delta, cos_t, g_min, rho)
                     what = "%s model case %d level %d" % (model, k, level)
                     assert got[1:] == want[1:], "%s: counts %s vs %s" % (what, got[1:], want[1:])
                     assert np.array_equal(got[0].view(np.uint64), want[0].view(np.uint64)), what
                     geo = tr.step(level, T, delta, cos_t)
                     assert np.array_equal(got[0][:28].view(np.uint64), geo[0].view(np.uint64)), what + ": geometric half"
-                    assert (got[1], got[3]) == geo[1:], what
+                    assert (got[1], 0, got[3]) == geo[1:], what
                     if model == "rendered" and k == 0:
                         assert got[2] > 0.2 * got[3], what
                     if model == "empty" or k >= 6:
@@ -140,9 +140,9 @@ def test_abi_refusals():
     h = ctypes.c_void_p()
     assert lib.mccnn_track_create(ctypes.byref(h), 6, 7, 0) == 0
     s = torch.cuda.current_stream().cuda_stream
-    sums, counts = np.zeros(56), np.zeros(3, np.int64)
+    sums, counts, gates = np.zeros(56), np.zeros(3, np.int64), np.array([2.0, 30.0])
     pose = np.eye(4)[:3].reshape(-1).copy()
-    step = (h, 0, pose.ctypes.data, 0.5, 0.5, 2.0, 30.0, sums.ctypes.data, counts.ctypes.data, s)
+    step = (h, 0, pose.ctypes.data, 0.5, 0.5, gates.ctypes.data, sums.ctypes.data, counts.ctypes.data, s)
     img = torch.zeros((6, 7, 3), dtype=torch.uint8, device="cuda")
     I = torch.empty(42, dtype=torch.float32, device="cuda")
     G = torch.empty(42, dtype=torch.float64, device="cuda")
@@ -153,19 +153,20 @@ def test_abi_refusals():
     d = torch.ones((6, 7), device="cuda")
     assert lib.mccnn_track_source(h, d.data_ptr(), 2.0, 2.0, 2.0, 1.0, 0.0, float("inf"), s) == 0
     assert lib.mccnn_track_model(h, d.data_ptr(), 2.0, 2.0, 2.0, s) == 0
-    assert lib.mccnn_track_step_photometric(*step) == -1                   # no intensity pyramids
+    assert lib.mccnn_track_step(*step) == -1                               # no intensity pyramids
     assert lib.mccnn_track_intensity(h, 0, img.data_ptr(), 3, s) == 0
-    assert lib.mccnn_track_step_photometric(*step) == -1                   # no reference
+    assert lib.mccnn_track_step(*step) == -1                               # no reference
     assert lib.mccnn_track_intensity(h, 1, img.data_ptr(), 1, s) == 0
     bad_pose = pose.copy()
     bad_pose[5] = np.inf
-    for k, v in ((0, None), (1, -1), (1, 3), (2, None), (2, bad_pose.ctypes.data), (3, 0.0), (3, float("nan")), (4, 1.5),
-                 (5, -1.0), (5, float("inf")), (5, float("nan")), (6, -0.5), (6, float("inf")), (6, float("nan")), (7, None),
-                 (8, None)):
+    inf, nan = float("inf"), float("nan")
+    bad_gates = [np.array(g) for g in ((-1.0, 30.0), (inf, 30.0), (nan, 30.0), (2.0, -0.5), (2.0, inf), (2.0, nan))]
+    for k, v in ((0, None), (1, -1), (1, 3), (2, None), (2, bad_pose.ctypes.data), (3, 0.0), (3, nan), (4, 1.5),
+                 *((5, g.ctypes.data) for g in bad_gates), (6, None), (7, None)):
         args = list(step)
         args[k] = v
-        assert lib.mccnn_track_step_photometric(*args) == -1, "step argument %d = %r" % (k, v)
-    assert lib.mccnn_track_step_photometric(*step) == 0
+        assert lib.mccnn_track_step(*args) == -1, "step argument %d = %r" % (k, v)
+    assert lib.mccnn_track_step(*step) == 0
     assert lib.mccnn_track_intensity_maps(h, 0, 0, I.data_ptr(), G.data_ptr(), G.data_ptr(), s) == -1   # the source has no g
     assert lib.mccnn_track_intensity_maps(h, 1, 0, I.data_ptr(), None, G.data_ptr(), s) == -1
     assert lib.mccnn_track_intensity_maps(h, 1, 3, I.data_ptr(), G.data_ptr(), G.data_ptr(), s) == -1

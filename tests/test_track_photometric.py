@@ -206,8 +206,7 @@ def test_run_icp_default_is_geometric():
     T0[:3, 3] = [0.02, -0.01, 0.03]
     a = track.run_icp(geo, T0)
     isrc = iref = po.pyramid(img)
-    joint = lambda level, p12, delta, cos_t: (lambda s: (s[0], (s[1], s[2]), s[3]))(
-        po.step(src, mod, isrc, iref, cal, level, p12, delta, cos_t, 2.0, 30.0))
+    joint = lambda level, p12, delta, cos_t: po.step(src, mod, isrc, iref, cal, level, p12, delta, cos_t, 2.0, 30.0)
     b = track.run_icp(joint, T0, photometric=0.01)
     assert a[1] == b[1] or abs(a[1] - b[1]) < 0.05 * a[1]
     assert not a[2] and not b[2]

@@ -141,9 +141,9 @@ def tree_sum(t):
 
 
 def step(src, mod, cal, level, pose12, delta, cos_t):
-    """(28 sums, inliers, the level's source vertices), as mccnn_track_step"""
+    """(28 sums, inliers, 0 photometric inliers, the level's source vertices), as mccnn_track_step without gates"""
     t, ok = terms(src, mod, cal, level, pose12, delta, cos_t)
-    return tree_sum(t), int(ok.sum()), int((~np.isnan(src[level][0][2])).sum())
+    return tree_sum(t), int(ok.sum()), 0, int((~np.isnan(src[level][0][2])).sum())
 
 
 def track(track_mod, disp, cal, Z, W_prev, W_pred, max_depth=None, **params):

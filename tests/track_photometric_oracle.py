@@ -135,7 +135,7 @@ def photometric_terms(src, mod, isrc, iref, cal, level, pose12, delta, g_min, rh
 
 def step(src, mod, isrc, iref, cal, level, pose12, delta, cos_t, g_min, rho):
     """(56 sums: geometric then photometric, geometric inliers, photometric inliers, the level's source vertices), as
-    mccnn_track_step_photometric"""
+    mccnn_track_step with gates {g_min, rho}"""
     tg, okg = track_oracle.terms(src, mod, cal, level, pose12, delta, cos_t)
     tp, okp = photometric_terms(src, mod, isrc, iref, cal, level, pose12, delta, g_min, rho)
     sums = np.concatenate([track_oracle.tree_sum(tg), track_oracle.tree_sum(tp)])
@@ -148,11 +148,7 @@ def track(track_mod, disp, cal, Z, W_prev, W_pred, left, ref_left, photometric, 
     src, mod = track_oracle.source_pyramid(disp, cal, max_depth), track_oracle.model_pyramid(Z, cal)
     isrc, iref = pyramid(left), pyramid(ref_left)
     Wp, Wq = track_mod.as4(W_prev), track_mod.as4(W_pred)
-
-    def fn(level, p12, delta, cos_t):
-        s, ng, nph, nv = step(src, mod, isrc, iref, cal, level, p12, delta, cos_t, grad_min, rho)
-        return s, (ng, nph), nv
-
+    fn = lambda level, p12, delta, cos_t: step(src, mod, isrc, iref, cal, level, p12, delta, cos_t, grad_min, rho)
     T, inliers, lost = track_mod.run_icp(fn, track_mod.rigid_inv(Wp) @ Wq, photometric=photometric, **params)
     return (Wq if lost else Wp @ T), inliers, lost
 

@@ -3,12 +3,12 @@
     python tools/time_track.py [--rounds 20] [--frames 8] [--json out.json]
 
 Reported, on a synthetic posed drive of --frames 375 x 1242 frames (synth.write_kitti_posed_drive), voxel 0.05 m and the
-default truncation: the median time of one mccnn_track_step reduce at each level (its read-back included); the median
-tracking cost of a frame, TSDF.render at the previous pose plus Tracker.track (both pyramids and every ICP step); and the
-frames per second of fuse_raw -mesh -poses track's loop against -poses oxts's (fusion.fuse_drive) with census at D 228,
-each over the whole drive after one warm-up pass, with the tracked drive's errors against its OXTS poses.  Each call is
-timed on the host clock around work that ends in a device synchronise.  The card's name and power limit are read in the
-same run.
+default truncation: the median time of one gate-less (geometric) mccnn_track_step reduce at each level (its read-back
+included); the median tracking cost of a frame, TSDF.render at the previous pose plus Tracker.track (both pyramids and
+every ICP step); and the frames per second of fuse_raw -mesh -poses track's loop against -poses oxts's (fusion.fuse_drive)
+with census at D 228, each over the whole drive after one warm-up pass, with the tracked drive's errors against its OXTS
+poses.  Each call is timed on the host clock around work that ends in a device synchronise.  The card's name and power
+limit are read in the same run.
 """
 import argparse
 import contextlib

@@ -3,12 +3,12 @@
     python tools/time_track_photometric.py [--rounds 20] [--frames 8] [--json out.json]
 
 Reported, on a synthetic posed drive of --frames 375 x 1242 frames (synth.write_kitti_posed_drive), voxel 0.05 m and the
-default truncation: the median time of one mccnn_track_step_photometric reduce at each level against mccnn_track_step's
-(read-backs included); the median tracking cost of a frame, TSDF.render at the previous pose plus Tracker.track, without
-and with the term (lambda 0.01, both intensity pyramids included); and the frames per second of fuse_raw -mesh -poses
-track's loop (fusion.fuse_drive) with census at D 228, without and with -photometric 0.01, each over the whole drive
-after one warm-up pass.  Each call is timed on the host clock around work that ends in a device synchronise.  The card's
-name and power limit are read in the same run.
+default truncation: the median time of one mccnn_track_step reduce at each level with gates (the joint step) against one
+without (read-backs included); the median tracking cost of a frame, TSDF.render at the previous pose plus Tracker.track,
+without and with the term (lambda 0.01, both intensity pyramids included); and the frames per second of fuse_raw -mesh
+-poses track's loop (fusion.fuse_drive) with census at D 228, without and with -photometric 0.01, each over the whole
+drive after one warm-up pass.  Each call is timed on the host clock around work that ends in a device synchronise.  The
+card's name and power limit are read in the same run.
 """
 import argparse
 import json
@@ -71,10 +71,11 @@ def main(argv=None):
             pho.intensity("reference", L[last - 1])
             T = track.rigid_inv(poses[last - 1]) @ poses[last]
             cos_t = math.cos(math.radians(track.THETA))
+            gates = (track.GRAD_MIN, track.RHO)
             for level in range(track.LEVELS):
                 delta = track.DELTA[track.LEVELS - 1 - level]
                 for key, fn in (("step_ms", lambda: geo.step(level, T, delta, cos_t)),
-                                ("step_photometric_ms", lambda: pho.step_photometric(level, T, delta, cos_t))):
+                                ("step_joint_ms", lambda: pho.step(level, T, delta, cos_t, gates))):
                     fn()
                     out["%s_level%d" % (key, level)] = statistics.median(host_ms(fn) for _ in range(a.rounds))
             pred = track.predict("track", poses[:last])
@@ -101,7 +102,7 @@ def main(argv=None):
     print("card: %s, power limit %s" % (name, power))
     for level in range(track.LEVELS):
         print("reduce step at %dx%d level %d: geometric %.3f ms, joint %.3f ms" % (
-            H, W, level, out["step_ms_level%d" % level], out["step_photometric_ms_level%d" % level]))
+            H, W, level, out["step_ms_level%d" % level], out["step_joint_ms_level%d" % level]))
     print("tracking one frame, render included: %.3f ms geometric, %.3f ms with the photometric term" % (
         out["track_frame_ms"], out["track_frame_photometric_ms"]))
     print("census D 228, %d-frame posed drive, fuse_raw -mesh -poses track: %.2f frames/s, -photometric %g %.2f frames/s" % (
