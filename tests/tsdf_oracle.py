@@ -334,6 +334,22 @@ class Field:
         return out.reshape(H, W)
 
 
+def sampled_bricks(keys, frames, tables, voxel, trunc=None, max_depth=None):
+    """the Field of the sorted bricks `keys` alone, each voxel integrated by the per-voxel rule over `frames` [(disp, cal,
+    rgb, pose)] while its brick is in the table: `tables` holds the sorted keys of the table after each frame's allocation.
+    These are the values those bricks hold in the whole field of the frames, at the cost of the sample."""
+    keys = np.asarray(keys, np.uint64)
+    f = Field(voxel, trunc)
+    f.allocate(keys)
+    for (disp, cal, rgb, pose), table in zip(frames, tables):
+        have = np.isin(keys, table)
+        g = Field(voxel, trunc)
+        g.keys, g.S, g.n, g.nc, g.col = keys[have], f.S[have], f.n[have], f.nc[have], f.col[have]
+        g.integrate(disp, cal, rgb, pose, max_depth)
+        f.S[have], f.n[have], f.nc[have], f.col[have] = g.S, g.n, g.nc, g.col
+    return f
+
+
 MESH_HEADER = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
                "property uchar red\nproperty uchar green\nproperty uchar blue\nelement face %d\n"
                "property list uchar int vertex_indices\nend_header\n")
