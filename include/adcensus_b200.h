@@ -46,6 +46,11 @@ typedef void *adcensus_stream_t;   /* cudaStream_t */
 /* "libadcensus_b200 <version>"; replaces adcensus.version (adcensus.cu:2055-2059) */
 const char *adcensus_version(void);
 
+/* the SM count every launch sized by the SM count uses on the current device: the device's own, or the value of the
+ * environment variable ADCENSUS_NUM_SMS (a decimal integer in 1..1024, read once) that tests set to run those launches at
+ * other grid sizes.  No output depends on it (DESIGN.md §4). */
+int adcensus_num_sms(void);
+
 /* ---- operators of the hot path (one per Lua function) ------------------- */
 
 /* adcensus.StereoJoin(input_L, input_R, output_L, output_R)  adcensus.cu:1455-1498

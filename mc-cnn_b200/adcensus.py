@@ -82,6 +82,11 @@ def version():
     return lib().adcensus_version().decode()
 
 
+def num_sms():
+    """the SM count the launches sized by it use on the current device (ADCENSUS_NUM_SMS when set, DESIGN §4)"""
+    return lib().adcensus_num_sms()
+
+
 def _check(rc, what):
     if rc == 0:
         return

@@ -1,9 +1,28 @@
 // common.cu -- device properties cache, stream-ordered scratch, shared-memory opt-in, version string
+#include <cstdlib>
+#include <cstring>
 #include <map>
 #include <mutex>
 #include <utility>
 
 #include "common.cuh"
+
+namespace {
+
+// ADCENSUS_NUM_SMS as a decimal integer in 1..1024, or 0 when it is unset or anything else (DESIGN §4)
+int forced_num_sms()
+{
+	const char *v = getenv("ADCENSUS_NUM_SMS");
+	if (!v || !*v || strlen(v) > 4) return 0;
+	int n = 0;
+	for (const char *c = v; *c; c++) {
+		if (*c < '0' || *c > '9') return 0;
+		n = 10 * n + (*c - '0');
+	}
+	return n >= 1 && n <= 1024 ? n : 0;
+}
+
+}  // namespace
 
 int adc_num_sms()
 {
@@ -11,8 +30,9 @@ int adc_num_sms()
 	int dev = 0;
 	if (cudaGetDevice(&dev) != cudaSuccess) return 132;
 	if (!sms[dev & 63]) {
-		int n = 0;
-		if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+		static const int forced = forced_num_sms();
+		int n = forced;
+		if (!n && (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)) n = 132;
 		sms[dev & 63] = n;
 	}
 	return sms[dev & 63];
@@ -80,6 +100,8 @@ extern "C" int adcensus_trim_scratch(void)
 }
 
 extern "C" const char *adcensus_version(void) { return "libadcensus_b200 0.1.0 (sm_90a)"; }
+
+extern "C" int adcensus_num_sms(void) { return adc_num_sms(); }
 
 // ---------------------------------------------------------------- TMA tensor maps
 #include "tma.cuh"

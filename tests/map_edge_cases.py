@@ -68,6 +68,96 @@ def hash_bits(n):
     return bits
 
 
+# ------------------------------------------------------------------------------------------ launches sized by the SM count
+#
+# Every grid that follows the SM count s (adc_num_sms, csrc/common.cu) is capped at a multiple of s, and the kernel covers
+# the rest of its work with a grid-stride or persistent loop.  One row per cap: the C expression it restates, the blocks it
+# launches, the elements one pass of the grid covers, and the launches it sizes.  tests/test_map_edge_cases.py checks the
+# rows against every use of adc_num_sms in csrc/; tests/test_gpu_sm_counts.py runs each launch at forced SM counts.
+
+def grid16(n, sms):
+    """preprocess.cu / preprocess_mb.cu elementwise_grid: ceil(n / 256) blocks, at most 16 per SM"""
+    return min(-(-n // THREADS), sms * 16)
+
+
+def fill_nan_blocks(n, sms):
+    """post.cu mccnn_fill_nan: the float4 body's blocks for n floats from a 16-byte aligned start, at least 1, at most 16 per SM"""
+    return max(1, min(-(-(n // 4) // THREADS), sms * 16))
+
+
+SEL_THREADS = 256                # confidence.cu SEL_THREADS
+
+
+def sel_blocks(n, sms):
+    """confidence.cu sel_blocks: ceil(n / 2048) blocks, at least 1, at most 4 per SM"""
+    return max(1, min(-(-n // (SEL_THREADS * 8)), sms * 4))
+
+
+def resident_ctas(ntile, sms):
+    """feature_tower.cu: the resident conv's persistent CTAs, one per SM at most; each runs ceil(ntile / CTAs) tiles"""
+    return min(ntile, sms)
+
+
+# name; blocks(n, s); the elements one block covers in one pass; the elements per block of the uncapped grid; the (csrc
+# file, sizing-line regex) of each use of adc_num_sms the row restates; the launches it sizes, as (file, kernel)
+SmCap = namedtuple("SmCap", "name blocks per_block uncapped sites launches")
+
+SM_CAPS = [
+    SmCap("grid8", grid_for, THREADS, THREADS,
+          [("keysort.cuh", r"long grid_for\(long long n\).*adc_num_sms\(\) \* 8"),
+           ("depth.cu", r"long grid_for\(long n\).*adc_num_sms\(\) \* 8"),
+           ("render.cu", r"long grid_for\(long n\).*adc_num_sms\(\) \* 8"),
+           ("kitti_eval.cu", r"long grid_for\(long n\).*adc_num_sms\(\) \* 8"),
+           ("rectify.cu", r"const int grid = .*adc_num_sms\(\) \* 8"),
+           ("frontend.cu", r"const dim3 grid\(.*adc_num_sms\(\) \* 8\), 2\)"),
+           ("frontend.cu", r"const int grid = .*adc_num_sms\(\) \* 8")],
+          [("fusion.cu", "merge_table_kernel"), ("fusion.cu", "merge_frame_kernel"), ("tsdf.cu", "merge_table_kernel"),
+           ("tsdf.cu", "merge_frame_kernel"), ("tsdf.cu", "hash_build_kernel"),
+           ("depth.cu", "depth_kernel"), ("depth.cu", "velo_key_kernel"), ("depth.cu", "velo_decode_kernel"),
+           ("render.cu", "volume_grey_kernel"), ("render.cu", "map_grey_kernel"), ("render.cu", "jet_kernel"),
+           ("render.cu", "error_kernel"), ("kitti_eval.cu", "quantise_kernel"), ("kitti_eval.cu", "column_kernel"),
+           ("rectify.cu", "rectify_kernel"), ("frontend.cu", "normalise_kernel"), ("frontend.cu", "error_count_kernel")]),
+    SmCap("grid16", grid16, THREADS, THREADS,
+          [("preprocess.cu", r"int elementwise_grid\(size_t n\).*adc_num_sms\(\) \* 16"),
+           ("preprocess_mb.cu", r"int elementwise_grid\(long n\).*adc_num_sms\(\) \* 16")],
+          [("preprocess.cu", "nonvisible_kernel"), ("preprocess.cu", "white_kernel"), ("preprocess_mb.cu", "half_rows_kernel"),
+           ("preprocess_mb.cu", "half_cols_kernel"), ("preprocess_mb.cu", "half_disp_kernel"),
+           ("preprocess_mb.cu", "mask_kernel")]),
+    SmCap("fill_nan", fill_nan_blocks, 4 * THREADS, 4 * THREADS,
+          [("post.cu", r"int cap = adc_num_sms\(\) \* 16;")],
+          [("post.cu", "fill_nan_kernel")]),
+    SmCap("sel", sel_blocks, SEL_THREADS, 8 * SEL_THREADS,
+          [("confidence.cu", r"const long cap = \(long\)adc_num_sms\(\) \* 4;")],
+          [("confidence.cu", "sparsify_write_kernel"), ("confidence.cu", "counts_mb_kernel"),
+           ("confidence.cu", "counts_bad_kernel"), ("confidence.cu", "sel_hist_kernel")]),
+    SmCap("resident", resident_ctas, 1, 1,
+          [("feature_tower.cu", r"const int nb = ntile < adc_num_sms\(\) \? ntile : adc_num_sms\(\);")],
+          [("feature_tower.cu", "conv3x3_resident_kernel")]),
+]
+
+# launches whose grids do not follow the SM count: mb_eval.cu sizes its grids from the pixel count, track.cu from the
+# pyramid's chunks
+SM_FREE = ("mb_eval.cu", "track.cu")
+
+
+def sm_cap(name):
+    return next(c for c in SM_CAPS if c.name == name)
+
+
+def sm_passes(cap, n, s):
+    """the passes of cap's grid-stride (or persistent) loop over n elements (tiles for the resident conv) at s SMs: above 1
+    the loop wraps"""
+    c = sm_cap(cap)
+    return max(1, -(-n // (c.blocks(n, s) * c.per_block)))
+
+
+def sm_cap_elements(cap, s):
+    """the most elements at which cap's grid is still the uncapped one at s SMs: with one more the cap binds, and the loop
+    takes one more pass (the selection's blocks loop over 2048 pixels each before the cap binds)"""
+    c = sm_cap(cap)
+    return c.blocks(1 << 40, s) * c.uncapped
+
+
 # the KITTI-like camera of the full-size cases (2011_09_26's rectified left camera), and a proportional one otherwise
 KITTI_H, KITTI_W = 375, 1242
 

@@ -62,6 +62,7 @@ def test_loader_prototypes_pinned(lib):
     assert lib.mccnn_fill_nan.argtypes == [p, ctypes.c_size_t, p]
     assert lib.mccnn_pipeline_destroy.restype is None
     assert lib.adcensus_version.restype is ctypes.c_char_p and lib.adcensus_version.argtypes == []
+    assert lib.adcensus_num_sms.restype is i and lib.adcensus_num_sms.argtypes == []
     assert lib.mccnn_mb_sample_starts.argtypes == [p, ctypes.c_longlong, i, ctypes.c_double, p, ctypes.c_longlong, p, p]
 
 

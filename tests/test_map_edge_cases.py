@@ -5,6 +5,7 @@ numpy oracles, so a kernel that reordered a sum or dropped a run of a grid-strid
 import importlib.util
 import math
 import os
+import re
 
 import numpy as np
 import pytest
@@ -186,3 +187,107 @@ def test_sums_are_order_sensitive(case):
                 assert _differs(seq_chunk_sums(t), want), what + ": chunk sums in order"
             if n != mc.pad(n) and n > 4:
                 assert _differs(pad_to_n(t), want), what + ": chunk sums padded to n"
+
+
+# ------------------------------------------------------------------------------------------ launches sized by the SM count
+
+CSRC = os.path.join(ROOT, "mc-cnn_b200", "csrc")
+# the name a file launches its SM-capped grids by: its helper, or the variable its use of adc_num_sms sets
+CAPPED_GRID = {"keysort.cuh": r"grid_for\(", "fusion.cu": r"grid_for\(", "tsdf.cu": r"grid_for\(",
+               "depth.cu": r"grid_for\(", "render.cu": r"grid_for\(", "kitti_eval.cu": r"grid_for\(",
+               "preprocess.cu": r"elementwise_grid\(", "preprocess_mb.cu": r"elementwise_grid\(",
+               "rectify.cu": r"dim3\(grid, 2\)$", "frontend.cu": r"grid$", "post.cu": r"blocks$",
+               "confidence.cu": r"(sel_blocks\(|blocks$)", "feature_tower.cu": r"nb$"}
+
+
+def _src(name):
+    with open(os.path.join(CSRC, name)) as f:
+        return f.read()
+
+
+def _launches(src):
+    """[(kernel, grid expression)] of every <<<...>>> launch in a source"""
+    out = []
+    for m in re.finditer(r"(\w+)(?:<[^<>;]*>)?\s*<<<", src):
+        depth, i = 0, m.end()
+        while depth or src[i] != ",":
+            depth += {"(": 1, ")": -1}.get(src[i], 0)
+            i += 1
+        out.append((m.group(1), src[m.end():i].strip()))
+    return out
+
+
+def test_sm_caps_are_every_use_of_adc_num_sms():
+    """each line of csrc/ that uses adc_num_sms is one site of one row of the table, and each site is such a line"""
+    lines = []
+    for name in sorted(os.listdir(CSRC)):
+        if name in ("common.cu", "common.cuh"):                    # the definition and its declaration
+            continue
+        lines += [(name, l.strip()) for l in _src(name).splitlines() if "adc_num_sms" in l]
+    sites = [(f, rx, c.name) for c in mc.SM_CAPS for f, rx in c.sites]
+    for f, l in lines:
+        hit = [s for s in sites if s[0] == f and re.search(s[1], l)]
+        assert len(hit) == 1, "%s: '%s' is not one row's site of map_edge_cases.SM_CAPS" % (f, l)
+    for f, rx, cap in sites:
+        assert sum(1 for g, l in lines if g == f and re.search(rx, l)) == 1, "%s site %s of %s is not in csrc" % (cap, rx, f)
+    assert len(lines) == len(sites)
+
+
+def test_sm_caps_list_every_capped_launch():
+    """the launches a file sizes by its capped grid are the ones its rows list, and the SM-free files use no SM count"""
+    listed = {}
+    for c in mc.SM_CAPS:
+        for f, k in c.launches:
+            listed.setdefault(f, set()).add(k)
+    assert set(listed) | {"keysort.cuh"} == set(CAPPED_GRID)
+    for f, rx in CAPPED_GRID.items():
+        got = {k for k, g in _launches(_src(f)) if re.search(rx, g)}
+        assert got == listed.get(f, set()), "%s: capped launches %s, the table lists %s" % (f, sorted(got), sorted(listed.get(f, ())))
+    for f in sorted(os.listdir(CSRC)):
+        if "grid_for(" in _src(f) and f != "keysort.cuh":
+            assert f in CAPPED_GRID, "%s launches on a grid_for grid the table does not list" % f
+    for f in mc.SM_FREE:
+        src = _src(f)
+        assert "adc_num_sms" not in src and "keysort.cuh" not in src, f
+        assert _launches(src), f
+
+
+def test_sm_cap_rules():
+    """the issue's table: the elements each cap's largest grid takes before the cap binds, at s SMs"""
+    s = 132
+    assert [mc.sm_cap_elements(c, s) for c in ("grid8", "grid16", "fill_nan", "sel", "resident")] == \
+        [2048 * s, 4096 * s, 16384 * s, 8192 * s, s]
+    for c in mc.SM_CAPS:
+        for s in (1, 7, 114, 132):
+            e = mc.sm_cap_elements(c.name, s)
+            assert c.blocks(e, s) == -(-e // c.uncapped) and c.blocks(e + 1, s) < -(-(e + 1) // c.uncapped)
+            assert mc.sm_passes(c.name, e + 1, s) > mc.sm_passes(c.name, e, s) or c.name == "sel"
+    assert mc.sel_blocks(1, 1) == 1 and mc.sel_blocks(2049, 1) == 2 and mc.sel_blocks(8193, 1) == 4
+    assert mc.sm_passes("sel", 2048, 132) == 8 and mc.sm_passes("sel", 8193, 1) == 9
+    assert mc.fill_nan_blocks(3, 1) == 1 and mc.fill_nan_blocks(16388, 1) == 16
+    assert mc.resident_ctas(7500, 114) == 114 and mc.resident_ctas(24, 114) == 24
+
+
+smr = _load("sm_count_runs")
+
+
+def test_sm_count_cases_wrap_every_cap():
+    """at one SM every row's loop wraps at least twice in some case and goes one block's elements past its cap in another;
+    the fusion merges wrap at 1 and 7 SMs, the TSDF merges and the render's hash build at 1; 114 SMs run the full sizes"""
+    passes = {}                                       # (cap, launch) -> [(case, passes at 1, 7, 114 SMs, elements)]
+    for c in smr.CASES:
+        inp = smr.inputs(c)
+        sizes = smr.map_sizes(c, inp) if c.kind in ("fusion", "tsdf") else None
+        for cap, launch, n in smr.loops(c, inp, sizes):
+            passes.setdefault(cap, []).append((c.name, launch, [mc.sm_passes(cap, n, s) for s in (1, 7, 114)], n))
+    assert set(passes) == {c.name for c in mc.SM_CAPS}
+    for cap, rows in passes.items():
+        assert any(p[0] >= 3 for _, _, p, _ in rows), cap
+        past = mc.sm_cap_elements(cap, 1)
+        assert any(past < n <= past + mc.sm_cap(cap).uncapped for _, _, _, n in rows), "%s: no case one past the cap" % cap
+    p = {launch: ps for rows in passes.values() for _, launch, ps, _ in rows}
+    assert p["fusion merge_frame"][1] >= 2 and p["fusion merge_table"][1] >= 2
+    assert min(p["tsdf merge_frame"][0], p["tsdf merge_table"][0], p["tsdf hash_build"][0]) >= 3
+    names = {c.name for c in smr.CASES}
+    assert {"frontend_kitti_grey", "frontend_kitti_rgb", "rectify_raw_grey", "rectify_raw_rgb", "render_mb", "confidence_mb",
+            "depth_mb", "tower_kitti"} <= names
